@@ -275,6 +275,74 @@ class GaussianProcess:
         return res[0] if len(res) == 1 else tuple(res)
 
 
+    def sample_joint(self, sets, derivs_s=None, seed=0, first_draw=0, table=None, jitter=0.0,
+                     want=("samples", "argmin")):
+        """cmoe_gp_sample_joint: one joint posterior draw per point set.  sets: [num_sets, num_pts, dim].  Set b uses
+        Philox draw first_draw + b, or row b of ``table`` [num_sets, Q].  Returns a dict with any of samples
+        [num_sets, Q], argmin [num_sets], mean [num_sets, Q], chol [num_sets, Q, Q] (lower, as a [row, col] array)."""
+        sets = _f64(sets)
+        if sets.ndim == 2:
+            sets = sets[None]
+        ns, num, _ = sets.shape
+        ds = _i32(derivs_s)
+        Q = num * (1 + len(ds))
+        table = _f64(table).ravel() if table is not None else None
+        if table is not None and table.size != ns * Q:
+            raise BoundsError(ERR_BOUNDS, f"normals table needs num_sets*Q = {ns * Q} values, got {table.size}")
+        bufs = {"samples": np.empty((ns, Q)) if "samples" in want else None,
+                "argmin": np.empty(ns, dtype=np.int32) if "argmin" in want else None,
+                "mean": np.empty((ns, Q)) if "mean" in want else None,
+                "chol": np.empty((ns, Q, Q)) if "chol" in want else None}
+        info = ctypes.c_int(0)
+        rc = lib().cmoe_gp_sample_joint(self.h, _d(sets), ns, num, _i(ds), len(ds), ctypes.c_uint64(seed),
+                                        ctypes.c_uint64(first_draw), _d(table), ctypes.c_double(jitter),
+                                        _d(bufs["samples"]), _i(bufs["argmin"]), _d(bufs["mean"]), _d(bufs["chol"]),
+                                        ctypes.byref(info))
+        _check(rc, info.value)
+        if bufs["chol"] is not None:
+            bufs["chol"] = np.ascontiguousarray(bufs["chol"].transpose(0, 2, 1))  # column-major -> [row, col]
+        return {k: v for k, v in bufs.items() if v is not None}
+
+    def sample_global_optima(self, num_optima, inner_number, domain_bounds, seed=0, first_draw=0, jitter=0.0):
+        """cmoe_gp_sample_global_optima: [num_optima, dim] minimisers of joint draws over Latin hypercubes."""
+        bounds = _f64(domain_bounds).ravel()
+        if bounds.size != 2 * self.dim:
+            raise BoundsError(ERR_BOUNDS, f"domain_bounds needs 2*dim = {2 * self.dim} values, got {bounds.size}")
+        out = np.empty((int(num_optima), self.dim))
+        info = ctypes.c_int(0)
+        rc = lib().cmoe_gp_sample_global_optima(self.h, int(num_optima), int(inner_number), _d(bounds),
+                                                ctypes.c_uint64(seed), ctypes.c_uint64(first_draw),
+                                                ctypes.c_double(jitter), _d(out), ctypes.byref(info))
+        _check(rc, info.value)
+        return out
+
+
+def latin_hypercube(num_sets, num_pts, domain_bounds, seed=0, first_draw=0, device=0):
+    """cmoe_latin_hypercube: [num_sets, num_pts, dim] points; set b is a pure function of (seed, first_draw + b).
+    domain_bounds: [dim, 2] (min, max) or the flat list."""
+    bounds = _f64(domain_bounds).ravel()
+    if bounds.size % 2:
+        raise BoundsError(ERR_BOUNDS, "domain_bounds needs (min, max) per dimension")
+    dim = bounds.size // 2
+    out = np.empty((int(num_sets), int(num_pts), max(dim, 0)))
+    _check(lib().cmoe_latin_hypercube(ctypes.c_uint64(seed), ctypes.c_uint64(first_draw), int(num_sets), int(num_pts),
+                                      int(dim), _d(bounds), _d(out), int(device)))
+    return out
+
+
+def bench_cholesky_batched(mats, repeats=3, device=0):
+    """cmoe_bench_cholesky_batched: (usec per batched call, usec per loop of the single-matrix Cholesky) for the
+    [num_mats, Q, Q] symmetric positive definite matrices ``mats``."""
+    mats = np.ascontiguousarray(np.asarray(mats, dtype=np.float64).transpose(0, 2, 1))
+    nm, Q, _ = mats.shape
+    tb, tl = ctypes.c_double(), ctypes.c_double()
+    info = ctypes.c_int(0)
+    rc = lib().cmoe_bench_cholesky_batched(_d(mats), nm, Q, int(repeats), int(device), ctypes.byref(tb),
+                                           ctypes.byref(tl), ctypes.byref(info))
+    _check(rc, info.value)
+    return tb.value, tl.value
+
+
 def log_marginal_likelihood(kernel, alpha, lengths, X, y, noise, derivs=None, device=0):
     """cmoe_log_marginal_likelihood (gpp_model_selection.cpp:540-612): one device fit + two host reductions."""
     X = _f64(X)

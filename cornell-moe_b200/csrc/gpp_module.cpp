@@ -174,6 +174,33 @@ struct GaussianProcess {
           info);
   }
   ~GaussianProcess() { cmoe_gp_destroy(h); }
+  // Randomness of the sampling methods: Philox key `seed_`, next unused draw `next_draw_`.  Construction behaves like
+  // set_randomized_seed(0), as the reference's constructor does (gpp_python_gaussian_process.cpp:60).
+  uint64_t seed_ = RandomnessSourceContainer::mix(0, 0), next_draw_ = 0;
+  void set_explicit_seed(uint32_t s) { seed_ = s; next_draw_ = 0; }
+  void set_randomized_seed(uint32_t s) { seed_ = RandomnessSourceContainer::mix(s, 0); next_draw_ = 0; }
+  void reset_to_most_recent_seed() { next_draw_ = 0; }
+  // SamplePointFromGPWrapper (gpp_python_gaussian_process.cpp:255-269): one joint draw of the value and the GP's
+  // derivative rows at one point, without noise; uses one draw.
+  py::list sample_point_from_gp(const py::list& point_to_sample) {
+    const auto P = to_vec(point_to_sample, dim_);
+    std::vector<double> out(1 + num_derivatives_);
+    int info = 0;
+    check(cmoe_gp_sample_joint(h, P.data(), 1, 1, derivatives_.data(), num_derivatives_, seed_, next_draw_, nullptr,
+                               0.0, out.data(), nullptr, nullptr, nullptr, &info), info);
+    ++next_draw_;
+    return to_list(out);
+  }
+  // SampleGlobalOptimaFromGPWrapper (:271-286): num_optima * dim values; uses num_optima draws.
+  py::list sample_global_optima(int num_optima, int inner_number, const py::list& domain_bounds) {
+    const auto B = to_vec(domain_bounds, 2 * static_cast<size_t>(dim_));
+    std::vector<double> out(static_cast<size_t>(std::max(num_optima, 0)) * dim_);
+    int info = 0;
+    check(cmoe_gp_sample_global_optima(h, num_optima, inner_number, B.data(), seed_, next_draw_, 0.0, out.data(),
+                                       &info), info);
+    next_draw_ += static_cast<uint64_t>(num_optima);
+    return to_list(out);
+  }
   GaussianProcess(const GaussianProcess&) = delete;
   GaussianProcess& operator=(const GaussianProcess&) = delete;
   int dim() const { return dim_; }
@@ -890,11 +917,12 @@ PYBIND11_MODULE(GPP, m) {
       .def("compute_grad_cholesky_variance_of_points",
            [](const GaussianProcess& g, const py::list& pts, int n, int nd) { return g.grad_variance(pts, n, nd, true); })
       .def("add_sampled_points", &GaussianProcess::add_sampled_points)
-      .def("sample_point_from_gp", [](GaussianProcess&, const py::list&) -> py::list { not_on_path("sample_point_from_gp"); })
-      .def("sample_global_optima", [](GaussianProcess&, int, int, const py::list&) -> py::list { not_on_path("sample_global_optima"); })
-      .def("set_explicit_seed", [](GaussianProcess&, uint32_t) {})
-      .def("set_randomized_seed", [](GaussianProcess&, uint32_t) {})
-      .def("reset_to_most_recent_seed", [](GaussianProcess&) {})
+      .def("sample_point_from_gp", &GaussianProcess::sample_point_from_gp, py::arg("point_to_sample"))
+      .def("sample_global_optima", &GaussianProcess::sample_global_optima, py::arg("num_optima"),
+           py::arg("inner_number"), py::arg("domain_bounds"))
+      .def("set_explicit_seed", &GaussianProcess::set_explicit_seed, py::arg("seed"))
+      .def("set_randomized_seed", &GaussianProcess::set_randomized_seed, py::arg("seed"))
+      .def("reset_to_most_recent_seed", &GaussianProcess::reset_to_most_recent_seed)
       .def("print_historical_data", [](GaussianProcess&) {});
 
   m.def("compute_expected_improvement", &compute_expected_improvement);

@@ -149,6 +149,8 @@ struct cmoe_gp {
   mutable struct cmoe_kg_plan* cached_plan = nullptr;
   // replicas of this GP on other devices (multi-GPU multistart inside one call); rebuilt when the generation changes
   mutable std::vector<cmoe_gp*> replicas;
+  // device workspace of the joint-sampling calls (sample.cu), grown on demand and kept until the handle is destroyed
+  mutable std::shared_ptr<void> sample_ws;
   mutable uint64_t replicas_generation = 0;
   ~cmoe_gp();
 };
@@ -202,6 +204,11 @@ struct PosteriorBatch {
   void run(const cmoe_gp& gp, int diag_mode, bool want_chol, bool want_grad_chol, cudaStream_t s);
   int first_failure(cudaStream_t s, int* which_set);
 };
+
+// Mean (and, if gmu != NULL, its gradient) at npts independent points of P [npts][dim] with the derivative rows
+// dPs[gs] (device): mu [npts][1+gs], gmu [npts][1+gs][dim].  No K^-1 K*, no bound on the number of points.
+void posterior_mean_points(const cmoe_gp& gp, const double* P, size_t npts, const int* dPs, int gs, double* mu,
+                           double* gmu, cudaStream_t s);
 
 // ---- ei.cu ---------------------------------------------------------------------------------------------------
 void upload_union_sets(PosteriorBatch& pb, const double* candidates, int nc, int q, const double* Xp, int p, int dim,

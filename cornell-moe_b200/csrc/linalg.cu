@@ -23,61 +23,6 @@ namespace cmoe {
 
 namespace {
 
-// Factor the 64x64 block in shared memory S (row r, col c at S[r][c]; rows/cols beyond the matrix padded with the
-// identity): [L11 0; L21 L22] via chol32(A11), L21 = A21 L11^-T, A22 -= L21 L21^T, chol32(A22).  The factor is left
-// in LT (transposed) with rd[k] = 1/L_kk (FAST) or L_kk.  Called by all PT threads; returns 0 or the failing 1-based
-// pivot index.
-template <bool FAST>
-__device__ __forceinline__ int factor_block64(double (*S)[NB + 1], double* LT, double* rd,
-                                              double* colbuf, volatile int* sfail) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (warp == 0) {
-    double a[32];
-#pragma unroll
-    for (int c = 0; c < 32; ++c) a[c] = S[lane][c];
-    const int f = chol32_warp<FAST>(a, lane, colbuf, LT, rd, 0);
-    if (lane == 0) *sfail = f;
-    __syncwarp();
-    if (!f) {
-      // L21 = A21 L11^-T: lane r solves row 32+r; the result goes to S (row access for the SYRK) and LT
-      double x[32];
-#pragma unroll
-      for (int c = 0; c < 32; ++c) x[c] = S[32 + lane][c];
-      solve_steps_rot<32, 32, 4, FAST>(x, LT, rd, 0, [&](int k, double v) {
-        S[32 + lane][k] = v;
-        LT[k * LTS + 32 + lane] = v;
-      });
-    }
-  }
-  __syncthreads();
-  if (*sfail) return *sfail;
-  {
-    // A22 -= L21 L21^T: warp w owns columns 8w..8w+7, lane r row 32+r
-    constexpr int CW = 32 / (PT / 32);
-    double acc[CW];
-#pragma unroll
-    for (int cc = 0; cc < CW; ++cc) acc[cc] = S[32 + lane][32 + warp * CW + cc];
-#pragma unroll 4
-    for (int k = 0; k < 32; ++k) {
-      const double xr = S[32 + lane][k];
-#pragma unroll
-      for (int cc = 0; cc < CW; ++cc) acc[cc] = fma(-xr, LT[k * LTS + 32 + warp * CW + cc], acc[cc]);
-    }
-#pragma unroll
-    for (int cc = 0; cc < CW; ++cc) S[32 + lane][32 + warp * CW + cc] = acc[cc];
-  }
-  __syncthreads();
-  if (warp == 0) {
-    double a[32];
-#pragma unroll
-    for (int c = 0; c < 32; ++c) a[c] = S[32 + lane][32 + c];
-    const int f = chol32_warp<FAST>(a, lane, colbuf, LT, rd, 32);
-    if (lane == 0) *sfail = f ? 32 + f : 0;
-  }
-  __syncthreads();
-  return *sfail;
-}
-
 // One launch per 64-column block step: CTA 0 factors the diagonal block and writes it back; every other CTA owns PT
 // rows of the panel below it (one row per thread, held in registers), factors the (L2-resident) diagonal block
 // redundantly in its own shared memory — cheaper than a second dependent launch — and then solves  X L_kk^T = A_ik

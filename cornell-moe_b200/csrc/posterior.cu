@@ -361,6 +361,15 @@ void PosteriorBatch::run(const cmoe_gp& gp, int diag_mode, bool want_chol, bool 
   CMOE_CUDA(cudaGetLastError());
 }
 
+void posterior_mean_points(const cmoe_gp& gp, const double* P, size_t npts, const int* dPs, int gs, double* mu,
+                           double* gmu, cudaStream_t s) {
+  if (npts == 0) return;
+  post_mean_only_kernel<<<static_cast<unsigned>(npts), kMeanThreads, 0, s>>>(gp.spec, gp.N, gp.mean, gp.dX.p,
+                                                                             gp.dKinvY.p, P, dPs, gs, mu, gmu);
+  count_launch();
+  CMOE_CUDA(cudaGetLastError());
+}
+
 int PosteriorBatch::first_failure(cudaStream_t s, int* which_set) {
   std::vector<int> h(nc);
   fail.download(h.data(), nc, s);
@@ -396,10 +405,7 @@ extern "C" int cmoe_gp_posterior(const cmoe_gp* gp, const double* sets, int num_
       DevBuf<int> dd(g_s > 0 ? g_s : 1);
       dP.upload(sets, npts * dim, s);
       if (g_s > 0) dd.upload(derivs_s, g_s, s);
-      post_mean_only_kernel<<<static_cast<unsigned>(npts), kMeanThreads, 0, s>>>(
-          gp->spec, gp->N, gp->mean, gp->dX.p, gp->dKinvY.p, dP.p, dd.p, g_s, dmu.p, grad_mean ? dgmu.p : nullptr);
-      count_launch();
-      CMOE_CUDA(cudaGetLastError());
+      posterior_mean_points(*gp, dP.p, npts, dd.p, g_s, dmu.p, grad_mean ? dgmu.p : nullptr, s);
       if (mean) dmu.download(mean, npts * bs, s);
       if (grad_mean) dgmu.download(grad_mean, npts * bs * dim, s);
       CMOE_CUDA(cudaStreamSynchronize(s));

@@ -132,6 +132,37 @@ int cmoe_gp_posterior(const cmoe_gp* gp, const double* sets, int num_sets, int n
                       double* mean, double* grad_mean, double* var, double* chol_var, double* grad_var,
                       double* grad_chol, int* info);
 
+/* ---- joint posterior draws, batched over point sets ------------------------------------------------------------
+ * Joint posterior draws over point sets: GaussianProcess::SamplePointsFromGP (gpp_math.cpp:1803-1848) batched over sets;
+ * SamplePointFromGP (:1761-1798) is the one-point case carrying the GP's derivative rows.  Python boundary
+ * SamplePointFromGPWrapper (gpp_python_gaussian_process.cpp:255-269).
+ * sets [num_sets][num_pts][dim]; each point carries derivative rows derivs_s[g_s]; Q = num_pts*(1+g_s) <= 8192.
+ * Set b draws Q normals: Philox draw (first_draw + b), exactly cmoe_philox_normals(seed, first_draw + b, 1, Q),
+ * or row b of normals_table [num_sets][Q] when it is not NULL (NormalRNG replay for parity).
+ * jitter >= 0 is added to the diagonal before factorisation (0 = the reference).
+ * samples [num_sets][Q]; argmin [num_sets] = index of the point with the smallest value row (ties: lowest index);
+ * mean [num_sets][Q]; chol [num_sets][Q*Q] (lower, upper zeroed). Every output may be NULL.
+ * The posterior covariance is K(P,P) - V^T V with V = L^-1 K(X,P) (one triangular solve; the reference uses
+ * (K^-1 K*)^T K*, which differs by rounding).  Sets are processed in chunks that fit a 2 GiB device workspace (or one
+ * set, if larger); a set's result does not depend on the chunking.  The workspace is kept on the handle (grown on demand,
+ * released by cmoe_gp_destroy), as the q-KG workspace is.
+ * A failed factorisation (pivot <= 1e-16) -> CMOE_ERR_SINGULAR, *info = leading minor of the first failing set.
+ * (The reference ignores the failure and applies the partial factor; its argmin starts at -1 with a strict `<`, so a
+ * minimum at point 0 yields -1 there and 0 here.) */
+int cmoe_gp_sample_joint(const cmoe_gp* gp, const double* sets, int num_sets, int num_pts, const int* derivs_s, int g_s,
+                         uint64_t seed, uint64_t first_draw, const double* normals_table, double jitter,
+                         double* samples, int* argmin, double* mean, double* chol, int* info);
+/* Latin hypercube in a box (ComputeLatinHypercubePointsInDomain, gpp_random.cpp:173-194): out [num_sets][num_pts][dim].
+ * domain_bounds [dim][2] = (min, max), min <= max; num_pts <= 8192.  Set b is a pure function of (seed, first_draw + b):
+ * the strata of each dimension are permuted by ranking Philox uniforms (counter word 3 = 1, the normals use 0). */
+int cmoe_latin_hypercube(uint64_t seed, uint64_t first_draw, int num_sets, int num_pts, int dim,
+                         const double* domain_bounds, double* out, int device);
+/* SampleGlobalOptimaFromGP (gpp_math.cpp:1854-1870): optimum b = argmin of one joint draw over the Latin hypercube
+ * cmoe_latin_hypercube(seed, first_draw + b, 1, inner_number, ...). points_optima [num_optima][dim].
+ * Python boundary SampleGlobalOptimaFromGPWrapper (gpp_python_gaussian_process.cpp:271-286). */
+int cmoe_gp_sample_global_optima(const cmoe_gp* gp, int num_optima, int inner_number, const double* domain_bounds,
+                                 uint64_t seed, uint64_t first_draw, double jitter, double* points_optima, int* info);
+
 /* ---- q-EI Monte Carlo, batched over candidates ----------------------------------------------------------------
  * Replaces ExpectedImprovementEvaluator::ComputeExpectedImprovement / ComputeGradExpectedImprovement
  * (gpp_math.cpp:1991-2126); Python boundary compute_expected_improvement / compute_grad_expected_improvement /
@@ -340,6 +371,11 @@ int cmoe_posterior_mean_optimization(const cmoe_gp* gp, int num_fidelity, const 
 int cmoe_bench_cov_build(const cmoe_gp* gp, int repeats, double* usec_per_build);
 /* Blocked Cholesky alone (re-factors a fresh copy of K each repeat). */
 int cmoe_bench_cholesky(const cmoe_gp* gp, int repeats, double* usec_per_factor);
+/* The batched Cholesky of cmoe_gp_sample_joint alone on num_mats device-resident Q x Q matrices (mats
+ * [num_mats][Q*Q] column-major, uploaded once), against a loop of the single-matrix blocked Cholesky over the same
+ * matrices: device time per call of each, averaged over `repeats` after one warm-up. */
+int cmoe_bench_cholesky_batched(const double* mats, int num_mats, int Q, int repeats, int device, double* usec_batched,
+                                double* usec_loop, int* info);
 /* Measured FP64 peaks of this GPU: tflops[0] = DFMA vector pipe, tflops[1] = DMMA tensor pipe (m8n8k4). */
 int cmoe_bench_fp64_peaks(int device, double* tflops);
 /* tflops[0] = total FP64 TFLOP/s when every warp interleaves DFMA and DMMA 1:1 by flops (do the vector pipe and the
