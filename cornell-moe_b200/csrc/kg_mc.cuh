@@ -19,10 +19,12 @@
 #pragma once
 
 #include <algorithm>
+#include <type_traits>
 
 #include "device_math.cuh"
 #include "internal.cuh"
 
+#include "linalg_dev.cuh"
 #include "ptx_util.cuh"
 
 namespace cmoe {
@@ -187,8 +189,188 @@ __device__ __forceinline__ double weight_row(const double* __restrict__ pk, doub
   return a;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Tile evaluation of the training rows (shared-memory fast path, DESIGN.md K6).  A round is warp-uniform, so the
+// three small contractions of a round — x~ . X~_j (and a_min g~ . X~_j on LINE rounds), a_j = beta_j - B_j . c and, on
+// POINT rounds, the gradient sums s_d = sum_j w_j X~_jd — are, for one block of 8 training rows, products of shape
+// 32 samples x 8 rows x K.  They run on FP64 DMMA m16n8k4 (M = 16 samples: the warp's lanes in two halves run one after
+// the other, N = 8 rows, K = DIM or QP in steps of 4, K tails zero-filled); only the exps and the trial arithmetic stay
+// element-wise, in the accumulator layout.  Fragment layout (PTX ISA, f64, lane = 4 g + t):
+//   A: a0 = A[g][t], a1 = A[g+8][t];   B: b = B[t][g];   C: c0 = C[g][2t], c1 = C[g][2t+1], c2 = C[g+8][2t], c3 = C[g+8][2t+1]
+// A sample's row of every product depends on that sample's operands only, and its partial sums over the 8 columns of a
+// block are reduced across the quad in a fixed order, so a result does not depend on which lane holds the sample.
+// Columns past N (last block) read row N-1 and get weight 0 (and p_j = 0 on LINE rounds): exact zeros, never 0 x inf.
+// ---------------------------------------------------------------------------------------------------------------
+
+// Which instantiations run the tile path: the ones measured to gain, SquareExponential at DIM = 8, QP = 8.  All the
+// others keep the scalar row loops (DESIGN.md K6 lists both groups).  The LINE tile needs ~240 registers per thread
+// against the 168 that 3 CTAs of 128 threads leave; the spill code grows with DIM and QP, and Matern-5/2's LINE rounds
+// are dominated by the per-trial sqrt and exp.
+template <int KERNEL, int DIM, int QP>
+constexpr bool kg_tile_path() {
+  return KERNEL == CMOE_KERNEL_SQUARE_EXPONENTIAL && DIM == 8 && QP == 8;
+}
+
+// A fragments of the half h (samples 16h .. 16h+15) from the lanes' own rows v[0..W): element k is -v[k] (NEG),
+// v[k] * scale[k] or, with row factors r0 / r1 (rows g / g+8), r * (v[k] * scale[k]) — the scaling is done after the
+// shuffle, so that the lanes keep only their state arrays live, and in the order the scalar path rounds it.
+template <int W, bool NEG, bool ROWF = false>
+__device__ __forceinline__ void tile_frag(const double (&v)[W], const double* scale, int h, double (&f)[(W + 3) / 4][2],
+                                          double r0 = 1.0, double r1 = 1.0) {
+  const int lane = threadIdx.x & 31, src = 16 * h + (lane >> 2), t = lane & 3;
+#pragma unroll
+  for (int ks = 0; ks < (W + 3) / 4; ++ks) {
+    f[ks][0] = 0.0;
+    f[ks][1] = 0.0;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int k = 4 * ks + e;
+      if (k < W) {
+        double x0 = __shfl_sync(0xffffffffu, v[k], src);
+        double x1 = __shfl_sync(0xffffffffu, v[k], src + 8);
+        if (t == e) {
+          if (NEG) {
+            x0 = -x0;
+            x1 = -x1;
+          } else if (scale != nullptr) {
+            x0 *= scale[k];
+            x1 *= scale[k];
+          }
+          if (ROWF) {
+            x0 *= r0;
+            x1 *= r1;
+          }
+          f[ks][0] = x0;
+          f[ks][1] = x1;
+        }
+      }
+    }
+  }
+}
+
+// per-sample scalar of the half h in the C layout: rows g (lo) and g + 8 (hi)
+__device__ __forceinline__ void tile_rows(double v, int h, double& lo, double& hi) {
+  const int src = 16 * h + ((threadIdx.x & 31) >> 2);
+  lo = __shfl_sync(0xffffffffu, v, src);
+  hi = __shfl_sync(0xffffffffu, v, src + 8);
+}
+
+// fixed-order sum over the quad (the butterfly gives the same bits on all four lanes)
+__device__ __forceinline__ double quad_sum(double v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+// hands the quad-uniform values of rows (g, g + 8) of half h to the owning lanes 16h + g and 16h + g + 8 (ADD: added
+// to the owner's value)
+template <bool ADD = false>
+__device__ __forceinline__ double tile_to_owner(double lo, double hi, int h, double mine) {
+  const int lane = threadIdx.x & 31, src = 4 * (lane & 7);
+  const double vl = __shfl_sync(0xffffffffu, lo, src), vh = __shfl_sync(0xffffffffu, hi, src);
+  const double v = (lane & 8) ? vh : vl;
+  return (lane >> 4) != h ? mine : (ADD ? mine + v : v);
+}
+
+// Row operands of one block, shared by all tile rounds: the B-operand row of the dot / weight products (jb = j0 + g)
+// and the two C columns of this lane (je0 = j0 + 2t, je1 = j0 + 2t + 1) with their (e_j, beta_j).
+template <int QP, bool TAIL>
+struct TileRows {
+  int jb, je0, je1;
+  bool v0, v1;  // columns inside [0, N)
+  double2 h0, h1;
+  __device__ __forceinline__ TileRows(const double* __restrict__ Pk, int N, int j0) {
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    jb = j0 + g;
+    je0 = j0 + 2 * t;
+    je1 = je0 + 1;
+    v0 = !TAIL || je0 < N;
+    v1 = !TAIL || je1 < N;
+    if (TAIL) {
+      jb = min(jb, N - 1);
+      je0 = min(je0, N - 1);
+      je1 = min(je1, N - 1);
+    }
+    h0 = *reinterpret_cast<const double2*>(Pk + je0 * (QP + 2));
+    h1 = *reinterpret_cast<const double2*>(Pk + je1 * (QP + 2));
+  }
+};
+
+// acc[4] (C layout) += A (K = W, fragments f) x B, B[k][n] = src[(row n) * stride + k] of the lane's row jb
+template <int W>
+__device__ __forceinline__ void tile_mma(double (&acc)[4], const double (&f)[(W + 3) / 4][2], const double* row) {
+  const int t = threadIdx.x & 3;
+#pragma unroll
+  for (int ks = 0; ks < (W + 3) / 4; ++ks) {
+    const double b = (4 * ks + t < W) ? row[4 * ks + t] : 0.0;
+    dmma_m16n8k4(acc[0], acc[1], acc[2], acc[3], f[ks][0], f[ks][1], b);
+  }
+}
+
+// POINT round (SquareExponential) over the training rows: S0 = sum_j a_j k_j and s_d = sum_j a_j k_j X~_jd of every
+// lane's query point xq (hq = -|xq|^2 / 2).
+template <int DIM, int QP>
+__device__ __forceinline__ void tile_posterior(const double* __restrict__ Xt, const double* __restrict__ Pk, int N,
+                                               const double (&xq)[DIM], const double (&c)[QP], double hq, double& S0,
+                                               double (&s)[DIM]) {
+  constexpr int KD = (DIM + 3) / 4, KQ = (QP + 3) / 4, ND = (DIM + 7) / 8;
+  const int lane = threadIdx.x & 31, g = lane >> 2;
+  S0 = 0.0;
+#pragma unroll
+  for (int d = 0; d < DIM; ++d) s[d] = 0.0;
+#pragma unroll 1
+  for (int h = 0; h < 2; ++h) {
+    double xa[KD][2], ca[KQ][2];
+    tile_frag<DIM, false>(xq, nullptr, h, xa);
+    tile_frag<QP, true>(c, nullptr, h, ca);  // a = beta + (-c) . B: the negation is exact, each product is the scalar one
+    double hq0, hq1;
+    tile_rows(hq, h, hq0, hq1);
+    double s0[2] = {0.0, 0.0}, sacc[ND][4];
+#pragma unroll
+    for (int n = 0; n < ND; ++n) sacc[n][0] = sacc[n][1] = sacc[n][2] = sacc[n][3] = 0.0;
+    auto block = [&](int j0, auto tail) {
+      constexpr bool TAIL = decltype(tail)::value;
+      const TileRows<QP, TAIL> r(Pk, N, j0);
+      // the exponent's e_j enters as the accumulator seed
+      double dot[4] = {r.h0.x, r.h1.x, r.h0.x, r.h1.x};
+      double a[4] = {r.h0.y, r.h1.y, r.h0.y, r.h1.y};
+      tile_mma<DIM>(dot, xa, Xt + r.jb * DIM);
+      tile_mma<QP>(a, ca, Pk + r.jb * (QP + 2) + 2);
+      double w[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const double ai = ((i & 1) ? r.v1 : r.v0) ? a[i] : 0.0;
+        const double kv = exp_tab(dot[i] + ((i < 2) ? hq0 : hq1));
+        s0[i >> 1] = fma(ai, kv, s0[i >> 1]);
+        w[i] = ai * kv;
+      }
+      // s += W X~: k-step 0 takes the even columns (rows je0: A = (w0, w2)), k-step 1 the odd ones (rows je1)
+#pragma unroll
+      for (int n = 0; n < ND; ++n) {
+        const int d = 8 * n + g;
+        const double b0 = (d < DIM) ? Xt[r.je0 * DIM + d] : 0.0;
+        const double b1 = (d < DIM) ? Xt[r.je1 * DIM + d] : 0.0;
+        dmma_m16n8k4(sacc[n][0], sacc[n][1], sacc[n][2], sacc[n][3], w[0], w[2], b0);
+        dmma_m16n8k4(sacc[n][0], sacc[n][1], sacc[n][2], sacc[n][3], w[1], w[3], b1);
+      }
+    };
+    const int nfull = N & ~7;
+#pragma unroll 1
+    for (int j0 = 0; j0 < nfull; j0 += 8) block(j0, std::false_type());
+    if (nfull < N) block(nfull, std::true_type());
+    S0 = tile_to_owner(quad_sum(s0[0]), quad_sum(s0[1]), h, S0);
+#pragma unroll
+    for (int d = 0; d < DIM; ++d) {
+      // s[row][d] sits in lane 4 (row & 7) + ((d & 7) >> 1) of the row's quad, register (d & 1) (+ 2 for rows 8..15)
+      const int src = 4 * (lane & 7) + ((d & 7) >> 1);
+      const double vl = __shfl_sync(0xffffffffu, sacc[d / 8][d & 1], src);
+      const double vh = __shfl_sync(0xffffffffu, sacc[d / 8][2 + (d & 1)], src);
+      if ((lane >> 4) == h) s[d] = (lane & 8) ? vh : vl;
+    }
+  }
+}
+
 // mu+(xq) - m  and  the scaled-gradient accumulators, for one query point (scaled coordinates xq).
-template <int KERNEL, int DIM, int QP, bool SMEM>
+template <int KERNEL, int DIM, int QP, bool SMEM, bool TILE = false>
 __device__ __forceinline__ void eval_posterior(const double* __restrict__ Xt, const double* __restrict__ Pk,
                                                const double* __restrict__ Xu, int N, int U, double alpha,
                                                const double (&xq)[DIM], const double (&c)[QP], double& S0, double& SB,
@@ -202,8 +384,10 @@ __device__ __forceinline__ void eval_posterior(const double* __restrict__ Xt, co
   SB = 0.0;
 #pragma unroll
   for (int d = 0; d < DIM; ++d) s[d] = 0.0;
+  static_assert(!TILE || KERNEL == CMOE_KERNEL_SQUARE_EXPONENTIAL, "the tile path is SquareExponential only");
+  if (TILE) tile_posterior<DIM, QP>(Xt, Pk, N, xq, c, hq, S0, s);
 #pragma unroll 2
-  for (int j = 0; j < N; ++j) {
+  for (int j = 0; j < (TILE ? 0 : N); ++j) {
     const double* xj = Xt + j * DIM;
     const double* pk = Pk + j * (QP + 2);
     double xv[DIM];
@@ -269,11 +453,76 @@ __device__ __forceinline__ void eval_posterior(const double* __restrict__ Xt, co
 // batches whose factors could leave the double range (it then falls back to one-at-a-time evaluations).
 constexpr int kLineBatch = 8;  // trial step sizes per batch (6 measured +1.5 %, but a second batch costs a whole pass)
 
-template <int DIM, int QP, bool SMEM>
+// LINE round (SquareExponential) over the training rows, added to S[k] and pmax_hi as eval_line computes them.  The
+// lanes' operands come from their unscaled state: base point xr, gradient gr (x~ = xr / l, a_min g~ = a_min (gr / l)),
+// with hq = -|x~|^2 / 2 and xga = -a_min x~ . g~.
+template <int DIM, int QP>
+__device__ __forceinline__ void tile_line(const double* __restrict__ Xt, const double* __restrict__ Pk, int N,
+                                          const double (&xr)[DIM], const double (&gr)[DIM], const double* inv_len,
+                                          double alpha_min, const double (&c)[QP], double hq, double xga,
+                                          double (&S)[kLineBatch], int& pmax_hi) {
+  constexpr int KD = (DIM + 3) / 4, KQ = (QP + 3) / 4, KB = kLineBatch;
+#pragma unroll 1
+  for (int h = 0; h < 2; ++h) {
+    double xa[KD][2], gf[KD][2], ca[KQ][2];
+    double hq0, hq1, xg0, xg1, am0, am1;
+    tile_rows(hq, h, hq0, hq1);
+    tile_rows(xga, h, xg0, xg1);
+    tile_rows(alpha_min, h, am0, am1);
+    tile_frag<DIM, false>(xr, inv_len, h, xa);
+    tile_frag<DIM, false, true>(gr, inv_len, h, gf, am0, am1);
+    tile_frag<QP, true>(c, nullptr, h, ca);
+    double Sp[2][KB];
+#pragma unroll
+    for (int k = 0; k < KB; ++k) Sp[0][k] = Sp[1][k] = 0.0;
+    int pm[2] = {0, 0};
+    auto block = [&](int j0, auto tail) {
+      constexpr bool TAIL = decltype(tail)::value;
+      const TileRows<QP, TAIL> r(Pk, N, j0);
+      double dot[4] = {r.h0.x, r.h1.x, r.h0.x, r.h1.x};
+      double p[4] = {xg0, xg0, xg1, xg1};
+      double a[4] = {r.h0.y, r.h1.y, r.h0.y, r.h1.y};
+      const double* xj = Xt + r.jb * DIM;
+      tile_mma<DIM>(dot, xa, xj);
+      tile_mma<DIM>(p, gf, xj);
+      tile_mma<QP>(a, ca, Pk + r.jb * (QP + 2) + 2);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const bool v = (i & 1) ? r.v1 : r.v0;
+        const double pj = v ? p[i] : 0.0;
+        pm[i >> 1] = max(pm[i >> 1], __double2hiint(pj) & 0x7fffffff);
+        const double w = (v ? a[i] : 0.0) * exp_tab(dot[i] + ((i < 2) ? hq0 : hq1));
+        double G = exp_tab(pj);
+#pragma unroll
+        for (int k = KB - 1; k >= 0; --k) {
+          Sp[i >> 1][k] = fma(w, G, Sp[i >> 1][k]);
+          if (k > 0) G *= G;
+        }
+      }
+    };
+    const int nfull = N & ~7;
+#pragma unroll 1
+    for (int j0 = 0; j0 < nfull; j0 += 8) block(j0, std::false_type());
+    if (nfull < N) block(nfull, std::true_type());
+#pragma unroll
+    for (int k = 0; k < KB; ++k) S[k] = tile_to_owner<true>(quad_sum(Sp[0][k]), quad_sum(Sp[1][k]), h, S[k]);
+#pragma unroll
+    for (int m = 1; m < 4; m <<= 1) {
+      pm[0] = max(pm[0], __shfl_xor_sync(0xffffffffu, pm[0], m));
+      pm[1] = max(pm[1], __shfl_xor_sync(0xffffffffu, pm[1], m));
+    }
+    const int lane = threadIdx.x & 31, src = 4 * (lane & 7);
+    const int vl = __shfl_sync(0xffffffffu, pm[0], src), vh = __shfl_sync(0xffffffffu, pm[1], src);
+    if ((lane >> 4) == h) pmax_hi = max(pmax_hi, (lane & 8) ? vh : vl);
+  }
+}
+
+template <int DIM, int QP, bool SMEM, bool TILE = false>
 __device__ __forceinline__ void eval_line(const double* __restrict__ Xt, const double* __restrict__ Pk,
                                           const double* __restrict__ Xu, int N, int U, const double (&xb)[DIM],
                                           const double (&gt)[DIM], const double (&c)[QP], double alpha_min,
-                                          double (&S)[kLineBatch], int& pmax_hi) {
+                                          double (&S)[kLineBatch], int& pmax_hi, const double (&xr)[DIM],
+                                          const double (&gr)[DIM], const double* inv_len) {
   double nq = 0.0, xg = 0.0;
 #pragma unroll
   for (int d = 0; d < DIM; ++d) {
@@ -289,7 +538,7 @@ __device__ __forceinline__ void eval_line(const double* __restrict__ Xt, const d
   for (int k = 0; k < kLineBatch; ++k) S[k] = 0.0;
   pmax_hi = 0;  // max over rows of the high word of |a_min p_j| (integer ALU; monotone in |p|, NaN/inf sort last)
 #pragma unroll 2
-  for (int j = 0; j < N; ++j) {
+  for (int j = 0; j < (TILE ? 0 : N); ++j) {
     const double* xj = Xt + j * DIM;
     const double* pk = Pk + j * (QP + 2);
     double xv[DIM];
@@ -341,6 +590,8 @@ __device__ __forceinline__ void eval_line(const double* __restrict__ Xt, const d
       if (k > 0) G *= G;
     }
   }
+  // tile path: the training rows last, so that the scaled operands above are dead during the row loop
+  if (TILE) tile_line<DIM, QP>(Xt, Pk, N, xr, gr, inv_len, alpha_min, c, hq, xga, S, pmax_hi);
 }
 
 // Batched backtracking for the Matern-5/2 kernel.  No factorisation along the line here, but the trial points
@@ -801,6 +1052,7 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
   constexpr bool LINE = SE || !GEN;  // Matern-5/2 batches its trials too (eval_line_matern) unless derivative rows exist
   constexpr int KB = SE ? kLineBatch : kLineBatchM;  // trial step sizes per LINE round
   constexpr int ST_SEARCH = LINE ? ST_LINE : ST_TRIAL;  // how a step's backtracking starts
+  constexpr bool TILE = SMEM && !GEN && kg_tile_path<KERNEL, DIM, QP>();  // DMMA tiles for the training rows
   const int N = prm.N, U = prm.U;
   const double* A = prm.A + static_cast<size_t>(cand) * prm.M * DIM;
   const double* recC = prm.recC + static_cast<size_t>(cand) * prm.num_mc * QP;
@@ -892,6 +1144,11 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
         gt[d] = gb[d] * prm.inv_len[d];
         gg = fma(gt[d], gt[d], gg);
       }
+      double nb2 = 0.0;  // tile path: formed before the evaluation, so that xt is dead during it
+      if (TILE) {
+#pragma unroll
+        for (int d = 0; d < DIM; ++d) nb2 = fma(xt[d], xt[d], nb2);
+      }
       constexpr double kTop = static_cast<double>(1 << (KB - 1));
       double T[GEN ? kLineBatch : 1];
       if (!SE) {
@@ -901,14 +1158,16 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
         eval_line_gen<DIM, QP, SMEM>(prm, Xt, Pk, Xu, xt, gt, aw, ring, cl, alpha_n * (1.0 / kTop), S,
                                reinterpret_cast<double (&)[kLineBatch]>(T), pmax_hi);
       } else {
-        eval_line<DIM, QP, SMEM>(Xt, Pk, Xu, N, U, xt, gt, c, alpha_n * (1.0 / kTop), S, pmax_hi);
+        eval_line<DIM, QP, SMEM, TILE>(Xt, Pk, Xu, N, U, xt, gt, c, alpha_n * (1.0 / kTop), S, pmax_hi, xb, gb,
+                                        prm.inv_len);
       }
       if (state == ST_LINE) {
         n_line += 1;
         // safe iff a_0 |p_j| = 2^(KB-1) |a_min p_j| < 512 for every row: every factor exp(a_k p_j) stays in range
-        double nb2 = 0.0;
+        if (!TILE) {
 #pragma unroll
-        for (int d = 0; d < DIM; ++d) nb2 = fma(xt[d], xt[d], nb2);
+          for (int d = 0; d < DIM; ++d) nb2 = fma(xt[d], xt[d], nb2);
+        }
         if (pmax_hi >= __double2hiint(512.0 / kTop) || !(nb2 <= kFarRadius * kFarRadius)) {
           state = ST_TRIAL;  // factors could leave the double range: this step backtracks one evaluation at a time
         } else {
@@ -965,7 +1224,7 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
               if (d == prm.derivs[m]) s[d] += em[m];
           }
       } else {
-        eval_posterior<KERNEL, DIM, QP, SMEM>(Xt, Pk, Xu, N, U, prm.alpha, xq, c, S0, SB, s);
+        eval_posterior<KERNEL, DIM, QP, SMEM, TILE>(Xt, Pk, Xu, N, U, prm.alpha, xq, c, S0, SB, s);
       }
       if (state == ST_INIT || state == ST_TRIAL || state == ST_LIMIT) {
         n_evals += 1;
