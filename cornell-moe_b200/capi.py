@@ -734,3 +734,66 @@ class GaussianProcessEnsemble:
                                                  _d(vals), _d(pts), ctypes.byref(info))
         _check(rc, info.value)
         return vals, pts
+
+    @classmethod
+    def from_members(cls, members):
+        """An ensemble over existing GaussianProcess handles (same dim, derivative observations and device; the number
+        of sampled points may differ, e.g. after add_sampled_points on some of them)."""
+        self = cls.__new__(cls)
+        self.members = list(members)
+        self.dim = self.members[0].dim
+        return self
+
+    def posterior_mean(self, points, num_fidelity=0, grad=False, per_member=False):
+        """cmoe_posterior_mean_mcmc: f = -(1/M) sum_m mu_m at points [P, dim - num_fidelity] (PosteriorMeanMCMC's sign;
+        fidelity coordinates pinned to 1.0).  Returns values [P], followed by grads [P, dim - num_fidelity] if grad and
+        by member values -mu_m [M, P] if per_member."""
+        ps = self.dim - num_fidelity
+        pts = _f64(points).reshape(-1, ps)
+        P, M = pts.shape[0], len(self.members)
+        vals = np.empty(P)
+        g = np.empty((P, ps)) if grad else None
+        mv = np.empty((M, P)) if per_member else None
+        info = ctypes.c_int()
+        _check(lib().cmoe_posterior_mean_mcmc(self._handles(), M, int(num_fidelity), _d(pts), P, _d(vals), _d(g), _d(mv),
+                                              ctypes.byref(info)), info.value)
+        out = (vals,) + ((g,) if grad else ()) + ((mv,) if per_member else ())
+        return out[0] if len(out) == 1 else out
+
+    def posterior_mean_optimization(self, starts, params, domain_bounds, num_fidelity=0):
+        """cmoe_posterior_mean_mcmc_optimization: the Python fixed-step gradient descent with Polyak-Ruppert averaging
+        on the ensemble mean from every start [S, dim - num_fidelity].  `params` is a GDParams, an 8-sequence in its
+        field order, or any object with its attributes (e.g. the reference's python_version GradientDescentParameters).
+        Returns (best_point [dim - nf], best_value, points [S, dim - nf], values [S])."""
+        ps = self.dim - num_fidelity
+        starts = _f64(starts).reshape(-1, ps)
+        ns, M = starts.shape[0], len(self.members)
+        params = _gd_params_any(params)
+        db = _f64(domain_bounds).ravel()
+        pts, vals, best = np.empty((ns, ps)), np.empty(ns), np.empty(ps)
+        bv, info = ctypes.c_double(), ctypes.c_int()
+        _check(lib().cmoe_posterior_mean_mcmc_optimization(self._handles(), M, int(num_fidelity), ctypes.byref(params),
+                                                           _d(db), _d(starts), ns, _d(pts), _d(vals), _d(best),
+                                                           ctypes.byref(bv), ctypes.byref(info)), info.value)
+        return best, bv.value, pts, vals
+
+    def recommend_point(self, eval_pts, params, domain_bounds, num_fidelity=0):
+        """The recommendation step of the reference's examples/main.py:243-260 in two device calls: screen eval_pts,
+        descend from the point of least ensemble mean, and keep the screened point if the descended one is strictly
+        worse.  Returns the point [dim - num_fidelity]."""
+        ps = self.dim - num_fidelity
+        pts = _f64(eval_pts).reshape(-1, ps)
+        test = -self.posterior_mean(pts, num_fidelity)  # the ensemble's mean posterior mean, as main.py's `test`
+        initial = pts[int(np.argmin(test))]
+        point, value, _, _ = self.posterior_mean_optimization(initial[None], params, domain_bounds, num_fidelity)
+        return initial.copy() if -value > np.min(test) else point
+
+
+def _gd_params_any(p):
+    if isinstance(p, GDParams):
+        return p
+    if all(hasattr(p, f) for f in ("max_num_steps", "num_steps_averaged", "gamma", "pre_mult", "max_relative_change")):
+        return GDParams(int(getattr(p, "num_multistarts", 0)), int(p.max_num_steps), int(getattr(p, "max_num_restarts", 0)),
+                        int(p.num_steps_averaged), float(p.gamma), float(p.pre_mult), float(p.max_relative_change),
+                        float(getattr(p, "tolerance", 0.0)))
+    return GDParams.from_seq(p)

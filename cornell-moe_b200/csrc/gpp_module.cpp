@@ -17,6 +17,8 @@
 //   evaluate_KG_mcmc_at_point_list                                        gpp_python_knowledge_gradient_mcmc.cpp:49-384
 //   compute_{,grad_}expected_improvement_mcmc, multistart_expected_improvement_mcmc_optimization,
 //   evaluate_EI_mcmc_at_point_list                                        gpp_python_expected_improvement_mcmc.cpp:46-300
+//   compute_posterior_mean_of_points, compute_{,grad_}posterior_mean_mcmc_of_points, posterior_mean_mcmc_optimization
+//                                                                         batched forms, not in the reference module
 //   GradientDescentParameters, NewtonParameters, RandomnessSourceContainer, OptimizerTypes, DomainTypes,
 //   LogLikelihoodTypes                                                    gpp_python_common.cpp:201-370
 //   OptimalLearningException, BoundsException, InvalidValueException, SingularMatrixException   gpp_python.cpp:189-206
@@ -838,6 +840,81 @@ py::list evaluate_EI_mcmc_at_point_list(const GaussianProcessMCMC& gp, const py:
 
 }  // namespace
 
+// ---- ensemble posterior mean (not in the reference module) ------------------------------------------------------------
+// The recommendation step of examples/main.py:243-260 evaluates PosteriorMeanMCMC point by point and runs the Python
+// GradientDescentOptimizer on it.  These names do both in one device call each.  `gps` is a GaussianProcessMCMC or a
+// Python list of GaussianProcess (what PosteriorMeanMCMC holds, as gp._gaussian_process; the wrapper objects themselves
+// are accepted too).
+std::vector<const cmoe_gp*> ensemble_handles(const py::object& gps) {
+  if (py::isinstance<GaussianProcessMCMC>(gps)) {
+    const auto& e = gps.cast<const GaussianProcessMCMC&>();
+    return std::vector<const cmoe_gp*>(e.members.begin(), e.members.end());
+  }
+  std::vector<const cmoe_gp*> h;
+  for (const py::handle& item : gps) {
+    py::object o = py::reinterpret_borrow<py::object>(item);
+    if (!py::isinstance<GaussianProcess>(o) && py::hasattr(o, "_gaussian_process")) o = o.attr("_gaussian_process");
+    h.push_back(o.cast<const GaussianProcess&>().h);
+  }
+  return h;
+}
+
+// GPP.GradientDescentParameters or the reference's python_version GradientDescentParameters namedtuple, by attribute
+cmoe_gd_params gd_by_attr(const py::object& p) {
+  auto get_int = [&](const char* n) { return py::hasattr(p, n) ? p.attr(n).cast<int>() : 0; };
+  auto get_dbl = [&](const char* n) { return py::hasattr(p, n) ? p.attr(n).cast<double>() : 0.0; };
+  return cmoe_gd_params{get_int("num_multistarts"), p.attr("max_num_steps").cast<int>(), get_int("max_num_restarts"),
+                        p.attr("num_steps_averaged").cast<int>(), p.attr("gamma").cast<double>(),
+                        p.attr("pre_mult").cast<double>(), p.attr("max_relative_change").cast<double>(),
+                        get_dbl("tolerance")};
+}
+
+int ensemble_dim(const std::vector<const cmoe_gp*>& h) { return h.empty() ? 0 : cmoe_gp_dim(h[0]); }
+
+// values of PosteriorMeanMCMC.compute_objective_function, -(1/M) sum_m mu_m, at num_points points [num_points][dim-nf]
+py::list compute_posterior_mean_mcmc_of_points(const py::object& gps, int num_fidelity, const py::list& pts,
+                                               int num_points) {
+  const auto h = ensemble_handles(gps);
+  const auto flat = to_vec(pts, static_cast<size_t>(std::max(num_points, 0)) * std::max(ensemble_dim(h) - num_fidelity, 0));
+  std::vector<double> v(std::max(num_points, 0));
+  int info = 0;
+  check(cmoe_posterior_mean_mcmc(h.data(), static_cast<int>(h.size()), num_fidelity, flat.data(), num_points, v.data(),
+                                 nullptr, nullptr, &info), info);
+  return to_list(v);
+}
+
+// compute_grad_objective_function of PosteriorMeanMCMC at every point, flat [num_points][dim-nf]
+py::list compute_grad_posterior_mean_mcmc_of_points(const py::object& gps, int num_fidelity, const py::list& pts,
+                                                    int num_points) {
+  const auto h = ensemble_handles(gps);
+  const size_t ps = std::max(ensemble_dim(h) - num_fidelity, 0), n = std::max(num_points, 0);
+  const auto flat = to_vec(pts, n * ps);
+  std::vector<double> v(n), g(n * ps);
+  int info = 0;
+  check(cmoe_posterior_mean_mcmc(h.data(), static_cast<int>(h.size()), num_fidelity, flat.data(), num_points, v.data(),
+                                 g.data(), nullptr, &info), info);
+  return to_list(g);
+}
+
+// multistart_optimize(GradientDescentOptimizer(RepeatedDomain(1, box), PosteriorMeanMCMC, params), starts):
+// (best_point [dim-nf], function_values [num_starts]), as python_version.optimization.multistart_optimize returns them
+py::tuple posterior_mean_mcmc_optimization(const py::object& gps, int num_fidelity, const py::object& optimizer_parameters,
+                                           const py::list& domain_bounds, const py::list& starting_points,
+                                           int num_starts) {
+  const auto h = ensemble_handles(gps);
+  const size_t ps = std::max(ensemble_dim(h) - num_fidelity, 0), n = std::max(num_starts, 0);
+  const auto bounds = to_vec(domain_bounds, 2 * ps);
+  const auto starts = to_vec(starting_points, n * ps);
+  const cmoe_gd_params gd = gd_by_attr(optimizer_parameters);
+  std::vector<double> vals(n), best(ps);
+  double best_value = 0.0;
+  int info = 0;
+  check(cmoe_posterior_mean_mcmc_optimization(h.data(), static_cast<int>(h.size()), num_fidelity, &gd, bounds.data(),
+                                              starts.data(), num_starts, nullptr, vals.data(), best.data(), &best_value,
+                                              &info), info);
+  return py::make_tuple(to_list(best), to_list(vals));
+}
+
 PYBIND11_MODULE(GPP, m) {
   m.doc() = "H100-native drop-in for moe.build.GPP (GP posterior + MC acquisition hot path)";
   g_exc_base = PyErr_NewExceptionWithDoc("GPP.OptimalLearningException",
@@ -968,6 +1045,12 @@ PYBIND11_MODULE(GPP, m) {
   m.def("compute_grad_expected_improvement_mcmc", &compute_grad_expected_improvement_mcmc);
   m.def("multistart_expected_improvement_mcmc_optimization", &multistart_expected_improvement_mcmc_optimization);
   m.def("evaluate_EI_mcmc_at_point_list", &evaluate_EI_mcmc_at_point_list);
+  m.def("compute_posterior_mean_mcmc_of_points", &compute_posterior_mean_mcmc_of_points, py::arg("gps"),
+        py::arg("num_fidelity"), py::arg("points"), py::arg("num_points"));
+  m.def("compute_grad_posterior_mean_mcmc_of_points", &compute_grad_posterior_mean_mcmc_of_points, py::arg("gps"),
+        py::arg("num_fidelity"), py::arg("points"), py::arg("num_points"));
+  m.def("posterior_mean_mcmc_optimization", &posterior_mean_mcmc_optimization, py::arg("gps"), py::arg("num_fidelity"),
+        py::arg("optimizer_parameters"), py::arg("domain_bounds"), py::arg("starting_points"), py::arg("num_starts"));
   // names of the reference module that are outside the hot path (model selection, heuristic EI): present, so that an
   // unmodified front end fails with the library's own exception class and a clear message rather than AttributeError
   // compute_log_likelihood(points_sampled, points_sampled_value, dim, num_sampled, objective_type, hyperparameters,

@@ -210,6 +210,10 @@ struct PosteriorBatch {
 void posterior_mean_points(const cmoe_gp& gp, const double* P, size_t npts, const int* dPs, int gs, double* mu,
                            double* gmu, cudaStream_t s);
 
+// ---- multistart.cu -------------------------------------------------------------------------------------------
+// An ensemble (one GP per hyper-parameter sample) is non-empty and its members share dim, g and device.
+void check_ensemble(const cmoe_gp* const* gps, int num_gp);
+
 // ---- ei.cu ---------------------------------------------------------------------------------------------------
 void upload_union_sets(PosteriorBatch& pb, const double* candidates, int nc, int q, const double* Xp, int p, int dim,
                        cudaStream_t s);

@@ -446,7 +446,9 @@ struct KgEnsembleEvaluator {
   }
 };
 
-void check_ensemble(const cmoe_gp* const* gps, int num_gp) {
+}  // namespace
+
+void cmoe::check_ensemble(const cmoe_gp* const* gps, int num_gp) {
   CMOE_REQUIRE(gps != nullptr && num_gp >= 1, CMOE_ERR_BOUNDS, "an ensemble needs at least one GP");
   for (int m = 0; m < num_gp; ++m) {
     CMOE_REQUIRE(gps[m] != nullptr, CMOE_ERR_INVALID_VALUE, "NULL GP in ensemble");
@@ -455,6 +457,8 @@ void check_ensemble(const cmoe_gp* const* gps, int num_gp) {
                  CMOE_ERR_INVALID_VALUE, "ensemble members must share dim, derivative observations and device");
   }
 }
+
+namespace {
 
 void make_kg_ensemble(KgEnsembleEvaluator& ens, const cmoe_gp* const* gps, int num_gp, int nf,
                       const cmoe_gd_params* inner, const double* inner_bounds, const double* discrete_pts, int num_pts,

@@ -366,6 +366,32 @@ int cmoe_posterior_mean_optimization(const cmoe_gp* gp, int num_fidelity, const 
                                      const double* domain_bounds, const double* initial_guess, double* best_point,
                                      double* best_value, int* found_flag);
 
+/* ---- ensemble posterior mean: the recommendation step of the MCMC loop ---------------------------------------------
+ * PosteriorMeanMCMC (moe/optimal_learning/python/cpp_wrappers/knowledge_gradient_mcmc.py:25-157) over an ensemble
+ * (gps[num_gp], as for the *_mcmc calls above): f(x) = -(1/M) sum_m mu_m(x), the members summed in ascending order and
+ * then divided by M; fidelity coordinates are pinned to 1.0.  Members may have different numbers of sampled points.
+ *
+ * cmoe_posterior_mean_mcmc   f at num_points points [num_points][dim-num_fidelity] in one call (the screening loop of
+ *                            examples/main.py:243-252): values[num_points]; grads[num_points][dim-num_fidelity] (grad f
+ *                            on the free coordinates) or NULL; member_values[num_gp][num_points] = -mu_m or NULL.
+ * cmoe_posterior_mean_mcmc_optimization
+ *                            The Python GradientDescentOptimizer (python_version/optimization.py:392-528) on f from every
+ *                            start (MultistartOptimizer, :565-610): for k = 1..max_num_steps, s = pre_mult k^-gamma grad f,
+ *                            each coordinate limited by TensorProductDomain.compute_update_restricted_to_domain
+ *                            (python_version/domain.py:158-202, no half-step fallback), x += s; then the Polyak-Ruppert
+ *                            average over _get_averaging_range (:415-442).  points_out[num_starts][dim-num_fidelity] and
+ *                            values_out[num_starts] (f at the average) may be NULL.  best: strict > in start order from
+ *                            -inf, best_point starting as starts[0].  max_num_restarts, tolerance and num_multistarts are
+ *                            ignored, as the Python optimiser ignores them.  max_num_steps < 1 (where the Python optimiser
+ *                            averages an empty range), an empty box, num_fidelity outside [0, dim) and num_starts < 1 are
+ *                            CMOE_ERR_BOUNDS.  One CTA per start; a start's result does not depend on the batch. */
+int cmoe_posterior_mean_mcmc(const cmoe_gp* const* gps, int num_gp, int num_fidelity, const double* points,
+                             int num_points, double* values, double* grads, double* member_values, int* info);
+int cmoe_posterior_mean_mcmc_optimization(const cmoe_gp* const* gps, int num_gp, int num_fidelity,
+                                          const cmoe_gd_params* params, const double* domain_bounds,
+                                          const double* starts, int num_starts, double* points_out,
+                                          double* values_out, double* best_point, double* best_value, int* info);
+
 /* ---- building blocks exposed for parity tests and micro-benchmarks ------------------------------------------------ */
 /* Covariance build alone on device-resident inputs: returns device time (usec) of `repeats` builds of the n*n matrix. */
 int cmoe_bench_cov_build(const cmoe_gp* gp, int repeats, double* usec_per_build);
