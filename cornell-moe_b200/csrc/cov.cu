@@ -330,15 +330,16 @@ __global__ void __launch_bounds__(256) cov_build_generic_kernel(const __grid_con
   }
 }
 
-// K(X, P): thread per (sampled point i, P point j), writes the (1+g)x(1+gs) block; rows fastest.
+// K(X, P): thread per (sampled point i, P point j), writes the (1+g)x(1+gs) block; rows fastest.  The P points run
+// along grid.x (8 per CTA), so their number is not bounded by grid.y's 65535; the training rows take grid.y.
 __global__ void __launch_bounds__(256) mix_cov_kernel(const __grid_constant__ KernelSpec spec,
                                                       const double* __restrict__ X, int N,
                                                       const double* __restrict__ P, int num,
                                                       const int* __restrict__ dPs, int gs,
                                                       double* __restrict__ out) {
   const int dim = spec.dim, b = 1 + spec.g, bs = 1 + gs, n = N * b;
-  const int i = blockIdx.x * 32 + (threadIdx.x & 31);
-  const int j = blockIdx.y * 8 + (threadIdx.x >> 5);
+  const int i = blockIdx.y * 32 + (threadIdx.x & 31);
+  const int j = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (i >= N || j >= num) return;
   const double* p1 = X + static_cast<size_t>(i) * dim;
   const double* p2 = P + static_cast<size_t>(j) * dim;
@@ -398,10 +399,16 @@ void build_covariance(const KernelSpec& spec, const double* X, const double* Xs,
   if (spec.g == 0) {
     const int trows = (N + TR - 1) / TR;
     dim3 grid(trows * (trows + 1) / 2 * (TR / TCW));
+    // the staged slabs take (TR + TCW)(dim + 1) + 64 doubles: past the default 48 KiB for dim >= 31
     const size_t smem = (static_cast<size_t>(TR + TCW) * (spec.dim + 1) + 64) * sizeof(double);
+    constexpr int kMaxSmem = ((TR + TCW) * (CMOE_MAX_DIM + 1) + 64) * sizeof(double);
     if (spec.kernel == CMOE_KERNEL_SQUARE_EXPONENTIAL) {
+      CMOE_CUDA(cudaFuncSetAttribute(cov_build_g0_kernel<CMOE_KERNEL_SQUARE_EXPONENTIAL>,
+                                     cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
       cov_build_g0_kernel<CMOE_KERNEL_SQUARE_EXPONENTIAL><<<grid, 256, smem, s>>>(spec, Xs, N, noise, K);
     } else {
+      CMOE_CUDA(cudaFuncSetAttribute(cov_build_g0_kernel<CMOE_KERNEL_MATERN_NU_2P5>,
+                                     cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
       cov_build_g0_kernel<CMOE_KERNEL_MATERN_NU_2P5><<<grid, 256, smem, s>>>(spec, Xs, N, noise, K);
     }
   } else {
@@ -415,7 +422,7 @@ void build_covariance(const KernelSpec& spec, const double* X, const double* Xs,
 void build_mix_covariance(const KernelSpec& spec, const double* X, int N, const double* P, int num, const int* dPs,
                           int gs, double* out, cudaStream_t s) {
   if (num == 0 || N == 0) return;
-  dim3 grid((N + 31) / 32, (num + 7) / 8);
+  dim3 grid((num + 7) / 8, (N + 31) / 32);
   mix_cov_kernel<<<grid, 256, 0, s>>>(spec, X, N, P, num, dPs, gs, out);
   count_launch();
   CMOE_CUDA(cudaGetLastError());

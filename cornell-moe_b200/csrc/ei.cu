@@ -145,7 +145,11 @@ void ei_eval_chunk(const cmoe_gp& gp, const double* candidates, int nc, int q, c
   DevBuf<double> zbuf(static_cast<size_t>(nc) * num_mc * U), imp(static_cast<size_t>(nc) * num_mc);
   DevBuf<int> win(static_cast<size_t>(nc) * num_mc);
   DevBuf<double> dei(nc), dgrad(want_grad ? static_cast<size_t>(nc) * q * dim : 1);
+  // (U^2 + U) doubles: past the default 48 KiB from U = 78 on, 74.5 KB at U = kMaxQ = 96
   const size_t smem1 = (static_cast<size_t>(U) * U + U) * sizeof(double);
+  constexpr int kMaxSmem = (kMaxQ * kMaxQ + kMaxQ) * sizeof(double);
+  CMOE_CUDA(cudaFuncSetAttribute(ei_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
+  CMOE_CUDA(cudaFuncSetAttribute(ei_reduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
   ei_sample_kernel<<<dim3((num_mc + 255) / 256, nc), 256, smem1, s>>>(U, num_mc, best_so_far, seed, dtable, pb.mu.p,
                                                                       pb.chol.p, pb.fail.p, zbuf.p, imp.p, win.p);
   ei_reduce_kernel<<<nc, 256, smem1, s>>>(U, q, dim, want_grad ? q : 0, num_mc, zbuf.p, imp.p, win.p, pb.gmu.p,
@@ -158,13 +162,14 @@ void ei_eval_chunk(const cmoe_gp& gp, const double* candidates, int nc, int q, c
 }
 }  // namespace
 
-// any number of candidates: the per-sample scratch (z, improvement, winner) is bounded to ~2 GiB per chunk — for the C
-// entry point and for the multistart drivers alike
+// any number of candidates: the per-sample scratch (z, improvement, winner) is bounded to ~2 GiB per chunk, and a chunk
+// holds at most 65535 candidates (grid.y of ei_sample_kernel) — for the C entry point and the multistart drivers alike
 void ei_eval_batch(const cmoe_gp& gp, const double* candidates, int nc, int q, const double* Xp, int p, int num_mc,
                    double best_so_far, uint64_t seed, const double* dtable, double* ei_host, double* grad_host) {
   const int U = q + p, dim = gp.spec.dim;
   const size_t per_cand = static_cast<size_t>(num_mc) * (U + 2) * sizeof(double);
-  const int batch = static_cast<int>(std::max<size_t>(1, std::min<size_t>(nc, (size_t(2) << 30) / per_cand)));
+  const int batch = static_cast<int>(
+      std::max<size_t>(1, std::min<size_t>({static_cast<size_t>(nc), (size_t(2) << 30) / per_cand, kMaxGridY})));
   for (int c0 = 0; c0 < nc; c0 += batch) {
     const int nb = std::min(batch, nc - c0);
     ei_eval_chunk(gp, candidates + static_cast<size_t>(c0) * q * dim, nb, q, Xp, p, num_mc, best_so_far, seed, dtable,

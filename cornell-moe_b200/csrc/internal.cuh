@@ -158,6 +158,8 @@ struct cmoe_gp {
 namespace cmoe {
 
 constexpr int kTrsmNB = 32;
+// largest grid.y (and grid.z) of a launch; the batched drivers that put one candidate per blockIdx.y split at this size
+constexpr size_t kMaxGridY = 65535;
 
 // ---- gp.cu ----
 void fit_gp(cmoe_gp* gp, bool mean_change);

@@ -679,10 +679,12 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
       }
     }
     pl->use_smem = pl->smem_fits && pl->rmax_static < kFastPathRadius;
-    // candidates per batch bounded by ~3 GiB of per-sample records
+    // candidates per batch bounded by ~3 GiB of per-sample records, and by grid.y of the per-candidate launches
+    // (kg_prep_kernel, the MC and accumulation kernels)
     const size_t per_cand = static_cast<size_t>(num_mc) * (QP + DIMP + 2) * sizeof(double) +
                             static_cast<size_t>(n) * Q * 4 * sizeof(double);
-    pl->batch = static_cast<int>(std::max<size_t>(1, std::min<size_t>(max_candidates, (size_t(3) << 30) / per_cand)));
+    pl->batch = static_cast<int>(std::max<size_t>(
+        1, std::min<size_t>({static_cast<size_t>(max_candidates), (size_t(3) << 30) / per_cand, kMaxGridY})));
     // samples per CTA: aim for >= ~8 waves of CTAs over the whole batch, between 2 and 16 samples per lane
     {
       const long long target_ctas = 8LL * sms * 3;

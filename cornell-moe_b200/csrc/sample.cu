@@ -34,7 +34,10 @@ namespace {
 
 constexpr int kMaxSampleQ = 8192;                          // rows of one set's joint draw
 constexpr size_t kSampleWorkspaceBytes = size_t(2) << 30;  // device workspace of one chunk (or of one set, if larger)
-constexpr int kMaxChunkSets = 4096;                        // grid.y / grid.z of the per-set launches
+// sets per chunk: one CTA row per set on grid.y / grid.z of the per-set launches (cov_tile, batched Cholesky,
+// sample_rows, lhs), well inside their 65535.  It does not bound the chunk's points: build_mix_covariance puts those on
+// grid.x.
+constexpr int kMaxChunkSets = 4096;
 constexpr int kTileThreads = 128;
 constexpr int kRowThreads = 256;
 

@@ -212,24 +212,6 @@ def test_dkg_config4_full_size(capi):
         np.testing.assert_allclose(grad[c], g, rtol=1e-4, atol=1e-7)
 
 
-@pytest.mark.parametrize("dim,q", [(2, 2), (5, 3), (6, 4), (10, 2), (13, 1)])
-def test_kg_other_dimensions(capi, dim, q):
-    """Every compiled padded-dimension variant (2, 4, 6, 8, 12, 16, 32) against the checker."""
-    prob = make_problem(20, dim, seed=dim, noise=0.05)
-    gp, ref = _pair(capi, dim % 2, prob)
-    rng = np.random.default_rng(dim)
-    cands = rng.uniform(size=(2, q, dim))
-    disc = rng.uniform(size=(6, dim))
-    mc = 32
-    table = rng.standard_normal((mc // 2) * q)
-    best = float(ref.mean_additional(disc).min())
-    kg, grad = gp.kg(cands, None, mc, best, EXAMPLE_INNER_GD, unit_bounds(dim), disc, table=table, grad=True)
-    for c in range(2):
-        v, g = ref.kg(cands[c], None, mc, best, table, EXAMPLE_INNER_GD, unit_bounds(dim), disc, grad=True)
-        np.testing.assert_allclose(kg[c], v, rtol=1e-7, atol=1e-10)
-        np.testing.assert_allclose(grad[c], g, rtol=1e-5, atol=1e-8)
-
-
 @pytest.mark.parametrize("case", ["second_batch", "out_of_range_factors", "exhausted_search", "tiny_length_scale"])
 def test_kg_line_batch_edge_paths(capi, case):
     """The SquareExponential fast path evaluates all backtracking trials of a step in one pass (8 step sizes per batch).
