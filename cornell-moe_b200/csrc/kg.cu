@@ -119,6 +119,98 @@ __global__ void __launch_bounds__(256) kg_pack_kernel(const __grid_constant__ Ke
   }
 }
 
+// Start-point table (g == 0), one CTA per (discretisation point m, candidate).  The fused MC kernel starts every sample's
+// inner descent at A_m = A[recStart]; there mu+ - m and the sums of its POINT round are affine in c = L^-T z:
+//     S0 = sum_j beta_j k_j + sum_u c_u (k(a, Xu_u) - sum_j B_ju k_j),  k_j = k(a, X_j)
+// and likewise SB (kb in place of k) and s_d (kb X~_jd).  Out[m][r][col], r = 0 (beta part) or 1 + u, col = S0, SB, s_d:
+// row r's weights are w_j = beta_j (r = 0) or -B_ju, and 1 on union row u (r = 1 + u).  The kernel values come from the
+// MC kernel's own operands (Xt, Pk, Xu: the same e_j and the same exp); every sum runs over the training rows, then the
+// union rows, in ascending order, with the POINT round's per-row rounding, so a candidate's table does not depend on its
+// batch.  fast: the MC kernel's shared-memory fast path (table exp, and all kernel values 0 beyond kFarRadius).
+constexpr int kStartThreads = 256;
+constexpr int kStartOuts = 5;  // outputs per thread: (1 + QP)(DIMP + 2) <= 33 x 34 = 1122 <= 5 x 256
+static_assert(kStartOuts * kStartThreads >= (1 + 32) * (CMOE_MAX_DIM + 2), "start table outputs per CTA (QP <= 32)");
+__global__ void __launch_bounds__(kStartThreads) kg_start_kernel(const __grid_constant__ KernelSpec spec, int N, int U,
+                                                                 int M, int DIMP, int QP, int fast,
+                                                                 const double* __restrict__ Xt,
+                                                                 const double* __restrict__ Pk,
+                                                                 const double* __restrict__ Xu,
+                                                                 const double* __restrict__ A,
+                                                                 double* __restrict__ Out) {
+  __shared__ double s_kv[kStartThreads], s_kb[kStartThreads];
+  const int m = blockIdx.x, c = blockIdx.y, tid = threadIdx.x, W = DIMP + 2, nout = (1 + QP) * W;
+  const bool se = spec.kernel == CMOE_KERNEL_SQUARE_EXPONENTIAL;
+  if (fast) exp_table_stage();
+  const double* a = A + (static_cast<size_t>(c) * M + m) * DIMP;
+  const double* pk = Pk + static_cast<size_t>(c) * N * (QP + 2);
+  const double* xu = Xu + static_cast<size_t>(c) * U * (DIMP + 2);
+  double nq = 0.0;
+  for (int d = 0; d < spec.dim; ++d) {  // the padding coordinates are 0 in every operand
+    const double x = a[d] * spec.inv_len[d];
+    nq = fma(x, x, nq);
+  }
+  const double hq = -0.5 * nq;
+  double acc[kStartOuts];
+#pragma unroll
+  for (int k = 0; k < kStartOuts; ++k) acc[k] = 0.0;
+  for (int j0 = 0; j0 < N + U; j0 += kStartThreads) {
+    const int j = j0 + tid;
+    if (j < N + U) {
+      const double* xj = (j < N) ? Xt + static_cast<size_t>(j) * DIMP : xu + static_cast<size_t>(j - N) * (DIMP + 2);
+      const double pk0 = (j < N) ? pk[static_cast<size_t>(j) * (QP + 2)] : xj[DIMP];
+      double dot = 0.0;
+      for (int d = 0; d < spec.dim; ++d) dot = fma(a[d] * spec.inv_len[d], xj[d], dot);
+      double kv, kb;
+      if (!se) {
+        kernel_pair<CMOE_KERNEL_MATERN_NU_2P5>(dot, pk0, hq, spec.alpha, kv, kb);
+      } else if (fast) {
+        kernel_pair<CMOE_KERNEL_SQUARE_EXPONENTIAL, true>(dot, pk0, hq, spec.alpha, kv, kb);
+      } else {
+        kernel_pair<CMOE_KERNEL_SQUARE_EXPONENTIAL, false>(dot, pk0, hq, spec.alpha, kv, kb);
+      }
+      s_kv[tid] = kv;
+      s_kb[tid] = kb;
+    }
+    __syncthreads();
+    const int jn = min(kStartThreads, N + U - j0);
+#pragma unroll
+    for (int k = 0; k < kStartOuts; ++k) {
+      const int o = tid + k * kStartThreads;
+      if (o < nout) {
+        const int r = o / W, col = o % W;
+        for (int i = 0; i < jn; ++i) {
+          const int jj = j0 + i;
+          double w;
+          const double* xj;
+          if (jj < N) {
+            const double* pr = pk + static_cast<size_t>(jj) * (QP + 2);
+            w = (r == 0) ? pr[1] : -pr[1 + r];
+            xj = Xt + static_cast<size_t>(jj) * DIMP;
+          } else {
+            w = (r == 1 + (jj - N)) ? 1.0 : 0.0;
+            xj = xu + static_cast<size_t>(jj - N) * (DIMP + 2);
+          }
+          if (col == 0 || (se && col == 1)) {  // SquareExponential: SB = S0, as the POINT round sets it
+            acc[k] = fma(w, s_kv[i], acc[k]);
+          } else if (col == 1) {
+            acc[k] += w * s_kb[i];
+          } else {
+            acc[k] = fma(w * s_kb[i], xj[col - 2], acc[k]);
+          }
+        }
+      }
+    }
+    __syncthreads();
+  }
+  double* out = Out + (static_cast<size_t>(c) * M + m) * nout;
+  const bool far = fast && nq > kFarRadius * kFarRadius;  // see kFastPathRadius: every kernel value is exactly 0
+#pragma unroll
+  for (int k = 0; k < kStartOuts; ++k) {
+    const int o = tid + k * kStartThreads;
+    if (o < nout) out[o] = far ? 0.0 : acc[k];
+  }
+}
+
 // W = L^-1 Cov_n(Xu rows, A), mu_n(A), best_posterior and its arg-min, one CTA per candidate.
 // KAu = K(X rows, A_union part) [n][nc*U], KD = K(X rows, D) [n][num_pts] (shared by all candidates), muD = mu_n(D).
 __global__ void __launch_bounds__(256) kg_discrete_kernel(const __grid_constant__ KernelSpec spec, int n, int U,
@@ -199,7 +291,15 @@ __global__ void __launch_bounds__(256) kg_prep_kernel(int Q, int M, int QP, int 
                                                       int* __restrict__ recStart) {
   extern __shared__ double sm[];
   const int c = blockIdx.y;
-  if (fail[c] != 0) return;
+  if (fail[c] != 0) {
+    // singular candidate: its KG is NaN, but the MC kernel still runs over its samples; keep their records in range
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s < num_mc) {
+      recStart[static_cast<size_t>(c) * num_mc + s] = 0;
+      for (int a = 0; a < QP; ++a) recC[(static_cast<size_t>(c) * num_mc + s) * QP + a] = 0.0;
+    }
+    return;
+  }
   double* Ls = sm;
   double* Ws = sm + Q * Q;
   double* ms = Ws + (w_in_smem ? static_cast<size_t>(M) * QP : 0);
@@ -445,6 +545,7 @@ struct cmoe_kg_plan {
   DevBuf<double> dPk, dXu, dA, dAfull, dKAu, dW, dMuA, dBestPost, dRecC, dOutVal, dOutX, dOutH, dR, dGu, dGkB, dTp, dG1;
   DevBuf<int> dWinner, dRecStart, dWork;
   DevBuf<double> dWt, dAw;  // general path: weight table per candidate, per-lane weight columns per resident CTA
+  DevBuf<double> dStart;    // g == 0: start-point table [batch][M][1+QP][DIMP+2] (kg_start_kernel)
   int aw_slots = 0;
   DevBuf<unsigned long long> dStats;
   // results
@@ -486,6 +587,11 @@ void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
                                     pl.dD.p, pl.dPk.p, pl.dXu.p, pl.dA.p, pl.dAfull.p,
                                     pl.dStale.count ? pl.dStale.p : nullptr, q, gen ? pl.dWt.p : nullptr);
   count_launch();
+  if (!gen) {
+    kg_start_kernel<<<dim3(M, nb), kStartThreads, 0, s>>>(spec, N, U, M, DIMP, QP, pl.use_smem ? 1 : 0, pl.dXt.p,
+                                                         pl.dPk.p, pl.dXu.p, pl.dA.p, pl.dStart.p);
+    count_launch();
+  }
   // K(X, A_union) for all candidates of the batch (value rows only)
   build_mix_covariance(spec, gp.dX.p, N, pl.dAfull.p, nb * U, nullptr, 0, pl.dKAu.p, s);
   const size_t smem_d = static_cast<size_t>(Q) * Q * sizeof(double);
@@ -509,6 +615,7 @@ void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
   prm.A = pl.dA.p;
   prm.recC = pl.dRecC.p;
   prm.recStart = pl.dRecStart.p;
+  prm.Start = gen ? nullptr : pl.dStart.p;
   prm.outVal = pl.dOutVal.p;
   prm.outX = pl.dOutX.p;
   prm.outH = pl.dOutH.p;
@@ -679,10 +786,11 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
       }
     }
     pl->use_smem = pl->smem_fits && pl->rmax_static < kFastPathRadius;
-    // candidates per batch bounded by ~3 GiB of per-sample records, and by grid.y of the per-candidate launches
-    // (kg_prep_kernel, the MC and accumulation kernels)
+    // candidates per batch bounded by ~3 GiB of per-sample records and start-point tables, and by grid.y of the
+    // per-candidate launches (kg_start_kernel, kg_prep_kernel, the MC and accumulation kernels)
     const size_t per_cand = static_cast<size_t>(num_mc) * (QP + DIMP + 2) * sizeof(double) +
-                            static_cast<size_t>(n) * Q * 4 * sizeof(double);
+                            static_cast<size_t>(n) * Q * 4 * sizeof(double) +
+                            (spec.g == 0 ? static_cast<size_t>(pl->M) * (1 + QP) * (DIMP + 2) * sizeof(double) : 0);
     pl->batch = static_cast<int>(std::max<size_t>(
         1, std::min<size_t>({static_cast<size_t>(max_candidates), (size_t(3) << 30) / per_cand, kMaxGridY})));
     // samples per CTA: aim for >= ~8 waves of CTAs over the whole batch, between 2 and 16 samples per lane
@@ -717,6 +825,8 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
       pl->dAw.alloc(slot * pl->aw_slots);
       pl->dWt.alloc(static_cast<size_t>(B) * (1 + QP) * n);
       pl->dWork.alloc(1);
+    } else {
+      pl->dStart.alloc(static_cast<size_t>(B) * pl->M * (1 + QP) * (DIMP + 2));
     }
     if (pl->want_grad) {
       pl->dR.alloc(static_cast<size_t>(B) * QP * (n + Q));

@@ -66,6 +66,7 @@ struct KgMcParams {
   const double* A;       // [nc][M][DIM]   unscaled start points (fidelity coords = 1, padding = 0)
   const double* recC;    // [nc][num_mc][QP]
   const int* recStart;   // [nc][num_mc]
+  const double* Start;   // g == 0: [nc][M][1+QP][DIM+2] start-point table (kg_start_kernel)
   const double* alpha0;  // [max_steps]  pre_mult * (i+1)^-gamma
   double* outVal;        // [nc][num_mc]   -mu+(x*)  (the reference's best_function_value)
   double* outX;          // [nc][num_mc][DIM] scaled minimiser
@@ -1033,6 +1034,37 @@ __device__ __forceinline__ void fill_own_weights(const double* __restrict__ Wt, 
   }
 }
 
+// Value and gradient of mu+ at a sample's start point, from the start-point table instead of a POINT round (g == 0).
+// mu+ - m and the POINT round's sums S0, SB, s_d are affine in c, so kg_start_kernel tabulates, per discretisation
+// point, row 0 (the beta part) and rows 1+u (the union point u's part: k(a, Xu_u) - sum_j B_ju k(a, X_j)), columns
+// (S0, SB, s_0 .. s_DIM-1); a sample combines them with its c in ascending u.  xb is the (unscaled) start point; returns
+// f = -mu+ and the gradient the INIT transition forms.
+template <int DIM, int QP>
+__device__ __forceinline__ void start_from_table(const KgMcParams& prm, const double* __restrict__ row,
+                                                 const double (&c)[QP], const double (&xb)[DIM], double& fb,
+                                                 double (&gb)[DIM]) {
+  constexpr int W = DIM + 2;
+  // one pair of columns at a time (S0 and SB first), so that only two sums are live next to the lane's state
+  auto pair = [&](int k) {
+    double2 t = __ldg(reinterpret_cast<const double2*>(row + k));
+#pragma unroll
+    for (int u = 0; u < QP; ++u) {
+      const double2 v = __ldg(reinterpret_cast<const double2*>(row + (1 + u) * W + k));
+      t.x = fma(c[u], v.x, t.x);
+      t.y = fma(c[u], v.y, t.y);
+    }
+    return t;
+  };
+  const double2 t0 = pair(0);  // (S0, SB)
+  fb = -(prm.mean + t0.x);
+#pragma unroll
+  for (int d = 0; d < DIM; d += 2) {
+    const double2 s = pair(2 + d);
+    gb[d] = (d < prm.ps) ? -prm.inv_len[d] * (s.x - (xb[d] * prm.inv_len[d]) * t0.y) : 0.0;
+    gb[d + 1] = (d + 1 < prm.ps) ? -prm.inv_len[d + 1] * (s.y - (xb[d + 1] * prm.inv_len[d + 1]) * t0.y) : 0.0;
+  }
+}
+
 enum : int { ST_FETCH = 0, ST_INIT = 1, ST_TRIAL = 2, ST_LIMIT = 3, ST_DONE = 4, ST_LINE = 5 };
 
 
@@ -1042,7 +1074,10 @@ enum : int { ST_FETCH = 0, ST_INIT = 1, ST_TRIAL = 2, ST_LIMIT = 3, ST_DONE = 4,
 // A round of the warp is either a POINT round (mu+ and its gradient at one query point per lane: INIT / TRIAL / LIMIT
 // lanes) or, for the SquareExponential fast path, a LINE round (all backtracking trials of a step at once, eval_line).
 // Which one runs is a warp vote; lanes waiting for the other kind idle for that round and are in phase again after it
-// (a sample alternates LINE, POINT, LINE, ... so the vote keeps a warp in lock-step once it is).
+// (a sample alternates LINE, POINT, LINE, ... so the vote keeps a warp in lock-step once it is).  Without derivative
+// observations a sample's start evaluation comes from the start-point table (start_from_table) when the lane takes the
+// sample, so a new sample's first round is a LINE round, in phase with the lanes that continue; only the general path
+// (GEN) spends a POINT round on it (ST_INIT).
 template <int KERNEL, int DIM, int QP, bool SMEM, bool GEN>
 __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* __restrict__ Xt,
                                            const double* __restrict__ Pk, const double* __restrict__ Xu, int cand,
@@ -1075,6 +1110,7 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
 
   while (true) {
     bool took_sample = false;
+    bool finish_run = false;
     if (state == ST_FETCH) {
       if (sample < s_end) {
         if (prm.max_restarts > 0) {
@@ -1093,7 +1129,26 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
           }
           step_i = 0;
           restart_i = 0;
-          state = ST_INIT;
+          if (GEN) {
+            state = ST_INIT;
+          } else {
+            // the start evaluation from the table, then the INIT transition: the sample's first round is a LINE round
+            start_from_table<DIM, QP>(prm,
+                                      prm.Start + (static_cast<size_t>(cand) * prm.M + recStart[sample]) *
+                                                      (1 + QP) * (DIM + 2),
+                                      c, xb, fb, gb);
+            n_evals += 1;
+            if (prm.max_steps <= 0) {
+              finish_run = true;  // the lane stays in ST_FETCH, so it sits out this iteration's round
+            } else {
+              alpha_n = prm.alpha0[0];
+              search = 0;
+              gnorm = 0.0;
+#pragma unroll
+              for (int d = 0; d < DIM; ++d) gnorm = fma(gb[d], gb[d], gnorm);
+              state = ST_SEARCH;
+            }
+          }
         } else {
           // ComputeOptimalPosteriorMean returns without touching its outputs (...optimization.cpp:424-426):
           // best_function_value stays 0 and the best point keeps its fill value 1.0
@@ -1131,7 +1186,6 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
       const unsigned wp = __ballot_sync(0xffffffffu, state == ST_INIT || state == ST_TRIAL || state == ST_LIMIT);
       line_round = __popc(wl) > __popc(wp);
     }
-    bool finish_run = false;
 
     if (LINE && line_round) {
       // ---- all backtracking trials of this step in one pass (warp-uniform) ----
