@@ -504,10 +504,12 @@ void register_kg_entries(const KgDispatchEntry* entries, int count) {
   for (int i = 0; i < count; ++i) kg_table().push_back(entries[i]);
 }
 
-const KgDispatchEntry* find_kg_entry(int kernel, int dim, int Q, bool need_gen) {
+const KgDispatchEntry* find_kg_entry(int kernel, int dim, int Q, int g) {
+  const bool need_gen = g > 0, wide = g > kMaxG;
   const KgDispatchEntry* best = nullptr;
   for (const auto& e : kg_table()) {
     if (e.kernel != kernel || e.dim < dim || e.qp < Q) continue;
+    if (e.wide != wide) continue;
     if (need_gen && e.mc_gen == nullptr) continue;
     if (!best || e.dim < best->dim || (e.dim == best->dim && e.qp < best->qp)) best = &e;
   }
@@ -661,7 +663,7 @@ void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
     CMOE_CUDA(cudaMemsetAsync(pl.dR.p, 0, static_cast<size_t>(nb) * QP * (n + Q) * sizeof(double), s));
     if (gen) {
       ap.g = spec.g;
-      for (int k = 0; k < 8; ++k) ap.derivs[k] = (k < spec.g) ? spec.derivs[k] : 0;
+      for (int k = 0; k < CMOE_MAX_DIM; ++k) ap.derivs[k] = (k < spec.g) ? spec.derivs[k] : 0;
       for (int d = 0; d < CMOE_MAX_DIM; ++d) ap.inv_len[d] = (d < dim) ? spec.inv_len[d] : 0.0;
       ap.fast_exp = 0;
       pl.entry->acc_gen(ap, dim3((n + Q + 127) / 128, nb), s);
@@ -699,7 +701,15 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     const KernelSpec& spec = gp->spec;
     const int dim = spec.dim;
     CMOE_REQUIRE(num_fidelity >= 0 && num_fidelity < dim, CMOE_ERR_BOUNDS, "num_fidelity out of range");
-    CMOE_REQUIRE(spec.g <= kMaxG, CMOE_ERR_BOUNDS, "at most 8 derivative observations per point in the q-KG kernel");
+    CMOE_REQUIRE(spec.g <= kMaxGWide, CMOE_ERR_BOUNDS,
+                 "at most 31 derivative observations per point in the q-KG kernel");
+    if (spec.g > kMaxG) {
+      // the wide kernel visits the derivative rows by coordinate (KgMcParams::drow)
+      for (int a = 0; a < spec.g; ++a)
+        for (int b = 0; b < a; ++b)
+          CMOE_REQUIRE(spec.derivs[a] != spec.derivs[b], CMOE_ERR_BOUNDS,
+                       "a partial derivative is observed twice per point (q-KG with more than 8 derivative observations)");
+    }
     CMOE_REQUIRE(inner->max_num_steps <= 4096, CMOE_ERR_BOUNDS, "inner max_num_steps must be <= 4096");
     require_device(gp->device);
     std::unique_ptr<cmoe_kg_plan> pl(new cmoe_kg_plan());
@@ -725,7 +735,7 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     for (int d = 0; d < ps; ++d)
       CMOE_REQUIRE(inner_bounds[2 * d] <= inner_bounds[2 * d + 1], CMOE_ERR_BOUNDS, "Tensor product region is EMPTY.");
     pl->Q = pl->U * (1 + spec.g);
-    pl->entry = find_kg_entry(spec.kernel, dim, pl->Q, spec.g > 0);
+    pl->entry = find_kg_entry(spec.kernel, dim, pl->Q, spec.g);
     CMOE_REQUIRE(pl->entry != nullptr, CMOE_ERR_BOUNDS,
                  "(q+p)*(1+num_derivatives) or dim exceeds the largest compiled q-KG kernel (32 rows, 32 dims)");
     pl->DIMP = pl->entry->dim;
@@ -861,7 +871,11 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     // for two CTAs per SM (2 x (90 KB ring + 20 KB) < 227 KB)
     m.stage_ops = (spec.g > 0 && static_cast<size_t>(N) * (DIMP + 2) * sizeof(double) <= 20 * 1024) ? 1 : 0;
     if (const char* e = std::getenv("CMOE_GEN_STAGE")) m.stage_ops = m.stage_ops && std::atoi(e) != 0;
-    for (int k = 0; k < 8; ++k) m.derivs[k] = (k < spec.g) ? spec.derivs[k] : 0;
+    for (int k = 0; k < CMOE_MAX_DIM; ++k) {
+      m.derivs[k] = (k < spec.g) ? spec.derivs[k] : 0;
+      m.drow[k] = 0;
+    }
+    for (int k = 0; k < spec.g; ++k) m.drow[spec.derivs[k]] = 1 + k;
     m.max_steps = inner->max_num_steps;
     m.max_restarts = inner->max_num_restarts;
     m.mean = gp->mean;

@@ -57,7 +57,8 @@ struct KgMcParams {
   int g;          // derivative observations per point (0 on the fast path)
   int Q;          // rows of the union block = U * (1 + g)
   int pk_stride;  // doubles per training point in Pk: QP + 2 (g == 0) or 2 (g > 0: e_j only, the weights live in Wt)
-  int derivs[8];  // observed partial-derivative indices (g <= 8 on the general path)
+  int derivs[CMOE_MAX_DIM];  // observed partial-derivative indices (g <= 8 on the narrow general path, <= 31 wide)
+  int drow[CMOE_MAX_DIM];    // wide general path: row 1 + m of coordinate d = derivs[m] in a point's block, else 0
   int max_steps, max_restarts;
   double mean, mrc, tol, step_tol, alpha;
   const double* Xt;      // [N][DIM] scaled training points (zero padded)
@@ -87,7 +88,7 @@ struct KgAccParams {
   int N, U, dim, num_mc;
   int fast_exp;  // 1: the range contract of the table exp holds (see kFastPathRadius)
   int g;          // derivative observations per point (general path: rows = (N + U) * (1 + g))
-  int derivs[8];
+  int derivs[CMOE_MAX_DIM];
   double inv_len[CMOE_MAX_DIM];
   double alpha;
   const double* Xt;     // [N][DIM]
@@ -753,9 +754,70 @@ __device__ __forceinline__ void stream_point_weights(const double* aw, double* r
     const double* w = ring + (st & (kRingDepth - 1)) * SR * T;
     const int j1 = min(N, (st + 1) * P);
 #pragma unroll 2
-    for (int j = st * P; j < j1; ++j, w += b1 * T) body(j, w);
+    for (int j = st * P; j < j1; ++j, w += b1 * T) body(j, w, 0);
   }
   cp_async_wait<0>();
+}
+
+// Wide variant (g > 8, up to 32 rows per point): eight stages of whole points no longer fit the kRingRows slots, so the
+// same ring is filled in stages of kWideStageRows rows, not tied to point boundaries; row r of the column lives in slot
+// r % kRingRows, and a point's rows may wrap around the end of the ring.  kWideLookahead stages are in flight; after
+// stage st has landed, every point whose last row it holds is evaluated, then stage st + kWideLookahead is issued into
+// the slots of stage st + kWideLookahead - kWideStages.  No point evaluated later starts in those slots: its first row
+// is past (st + 1) kWideStageRows - 32 (static_assert below).  body(j, ring, base): weight m of point j is in slot
+// (base + m) % kRingRows (ring_weight).
+constexpr int kWideStageRows = 8;
+constexpr int kWideStages = kRingRows / kWideStageRows;
+constexpr int kWideLookahead = 6;
+constexpr int kMaxGWide = 31;  // 1 + g <= 32 rows per point (Q = U (1 + g) <= 32)
+static_assert(kWideStages * kWideStageRows == kRingRows, "the wide stages tile the ring");
+static_assert((kWideStages - kWideLookahead) * kWideStageRows >= kMaxGWide, "a refill never overwrites a live point");
+template <typename F>
+__device__ __forceinline__ void stream_point_weights_wide(const double* aw, double* ring, int N, int b1, F&& body) {
+  constexpr int T = kMcThreads, SR = kWideStageRows, L = kWideLookahead;
+  const int R = N * b1;
+  const int nst = (R + SR - 1) / SR;
+  auto issue = [&](int st) {
+    if (st < nst) {
+      const int r0 = st * SR;
+      const int cnt = min(SR, R - r0);
+      double* dst = ring + (st % kWideStages) * SR * T;
+      const double* src = aw + static_cast<size_t>(r0) * T;
+      for (int k = 0; k < cnt; ++k) cp_async8(dst + k * T, src + static_cast<size_t>(k) * T, true);
+    }
+    cp_async_commit();
+  };
+  for (int st = 0; st < L; ++st) issue(st);
+  int j = 0, base = 0;
+  for (int st = 0; st < nst; ++st) {
+    cp_async_wait<L - 1>();
+    const int ready = min(R, (st + 1) * SR);
+    for (; (j + 1) * b1 <= ready; ++j) {
+      body(j, ring, base);
+      base += b1;
+      if (base >= kRingRows) base -= kRingRows;
+    }
+    issue(st + L);  // after the evaluations above: it refills slots they may have read
+  }
+  cp_async_wait<0>();
+}
+
+// weight m of a point: narrow ring w = the point's first slot (contiguous rows); wide ring w = the ring, rows from base
+template <bool WIDE>
+__device__ __forceinline__ double ring_weight(const double* w, int base, int m) {
+  if (!WIDE) return w[m * kMcThreads];
+  int k = base + m;
+  if (k >= kRingRows) k -= kRingRows;
+  return w[k * kMcThreads];
+}
+
+template <bool WIDE, typename F>
+__device__ __forceinline__ void stream_weights(const double* aw, double* ring, int N, int b1, F&& body) {
+  if constexpr (WIDE) {
+    stream_point_weights_wide(aw, ring, N, b1, body);
+  } else {
+    stream_point_weights(aw, ring, N, b1, body);
+  }
 }
 
 // General evaluation with derivative observations (d-KG): every training point owns 1+g rows
@@ -764,7 +826,10 @@ __device__ __forceinline__ void stream_point_weights(const double* aw, double* r
 //   d/dx~_d   = (X~_jd - x~_d) (a_j0 kb + kc wsum) + kb a~_jm [d == t]
 // The weights a_(j,m) come from this lane's ring slots (aj), the point operands from shared memory when they were
 // parked there (XS) and through the read-only path otherwise.
-template <int KERNEL, int DIM, int QP, bool XS>
+// WIDE (g > 8): the derivative rows are visited in coordinate order d (row prm.drow[d]), so the query coordinate and the
+// point's coordinate of row m are xq[d] and xv[d] with compile-time d and no per-row register arrays are needed; the
+// kb a~_jm terms go straight into s[d] instead of em.
+template <int KERNEL, int DIM, int QP, bool XS, bool WIDE = false>
 __device__ __forceinline__ void eval_posterior_gen(const KgMcParams& prm, const double* __restrict__ Xt,
                                                    const double* __restrict__ Pk, const double* __restrict__ Xu,
                                                    const double (&xq)[DIM], const double* aw, double* ring,
@@ -777,21 +842,23 @@ __device__ __forceinline__ void eval_posterior_gen(const KgMcParams& prm, const 
   const double hq = -0.5 * nq;
   // query coordinates at the derivative indices (compile-time register indexing only)
   double xm[kMaxG];
+  if (!WIDE) {
 #pragma unroll
-  for (int m = 0; m < kMaxG; ++m) {
-    xm[m] = 0.0;
-    em[m] = 0.0;
-    if (m < g) {
+    for (int m = 0; m < kMaxG; ++m) {
+      xm[m] = 0.0;
+      em[m] = 0.0;
+      if (m < g) {
 #pragma unroll
-      for (int d = 0; d < DIM; ++d)
-        if (d == prm.derivs[m]) xm[m] = xq[d];
+        for (int d = 0; d < DIM; ++d)
+          if (d == prm.derivs[m]) xm[m] = xq[d];
+      }
     }
   }
   S0 = 0.0;
   SB = 0.0;
 #pragma unroll
   for (int d = 0; d < DIM; ++d) s[d] = 0.0;
-  stream_point_weights(aw, ring, N, 1 + g, [&](int j, const double* aj) {
+  stream_weights<WIDE>(aw, ring, N, 1 + g, [&](int j, const double* aj, int base) {
     const double* xj = Xt + static_cast<size_t>(j) * DIM;
     const double* pk = Pk + static_cast<size_t>(j) * stride;
     double xv[DIM];
@@ -806,14 +873,26 @@ __device__ __forceinline__ void eval_posterior_gen(const KgMcParams& prm, const 
     for (int d = 0; d < DIM; ++d) dot = fma(xq[d], xv[d], dot);
     double kv, kb, kc;
     kernel_triple<KERNEL>(dot, ld1<XS>(pk), hq, prm.alpha, kv, kb, kc);
-    const double a0 = aj[0];  // this lane's weights of point j (ring slots)
+    const double a0 = ring_weight<WIDE>(aj, base, 0);  // this lane's weights of point j (ring slots)
     double wsum = 0.0;
+    if (WIDE) {
 #pragma unroll
-    for (int m = 0; m < kMaxG; ++m) {
-      if (m < g) {
-        const double am = aj[(m + 1) * kMcThreads];
-        wsum = fma(am, xm[m] - ld1<XS>(xj + prm.derivs[m]), wsum);
-        em[m] = fma(kb, am, em[m]);
+      for (int d = 0; d < DIM; ++d) {
+        const int r = prm.drow[d];
+        if (r > 0) {
+          const double am = ring_weight<WIDE>(aj, base, r);
+          wsum = fma(am, xq[d] - xv[d], wsum);
+          s[d] = fma(kb, am, s[d]);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int m = 0; m < kMaxG; ++m) {
+        if (m < g) {
+          const double am = aj[(m + 1) * kMcThreads];
+          wsum = fma(am, xm[m] - ld1<XS>(xj + prm.derivs[m]), wsum);
+          em[m] = fma(kb, am, em[m]);
+        }
       }
     }
     S0 = fma(a0, kv, S0);
@@ -840,12 +919,24 @@ __device__ __forceinline__ void eval_posterior_gen(const KgMcParams& prm, const 
     kernel_triple<KERNEL>(dot, __ldg(xu + DIM), hq, prm.alpha, kv, kb, kc);
     const double a0 = cl[u * bs];
     double wsum = 0.0;
+    if (WIDE) {
 #pragma unroll
-    for (int m = 0; m < kMaxG; ++m) {
-      if (m < g) {
-        const double am = cl[u * bs + 1 + m] * prm.inv_len[prm.derivs[m]];
-        wsum = fma(am, xm[m] - __ldg(xu + prm.derivs[m]), wsum);
-        em[m] = fma(kb, am, em[m]);
+      for (int d = 0; d < DIM; ++d) {
+        const int r = prm.drow[d];
+        if (r > 0) {
+          const double am = cl[u * bs + r] * prm.inv_len[d];
+          wsum = fma(am, xq[d] - xv[d], wsum);
+          s[d] = fma(kb, am, s[d]);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int m = 0; m < kMaxG; ++m) {
+        if (m < g) {
+          const double am = cl[u * bs + 1 + m] * prm.inv_len[prm.derivs[m]];
+          wsum = fma(am, xm[m] - __ldg(xu + prm.derivs[m]), wsum);
+          em[m] = fma(kb, am, em[m]);
+        }
       }
     }
     S0 = fma(a0, kv, S0);
@@ -862,7 +953,8 @@ __device__ __forceinline__ void eval_posterior_gen(const KgMcParams& prm, const 
 //     u_j = sum_m a~_jm (x~_t - X~_jt),  v_j = sum_m a~_jm g~_t,  k0_j = k(x, X_j),  G_jk = exp(a_k p_j)
 // the trial values are  E_k [ sum_j k0_j G_jk (a_j0 + u_j) + a_k sum_j k0_j G_jk v_j ]:  S[k] and T[k] below.
 // The (1+g) Q weight FMAs per point — the dominant cost of this path — are paid once per step instead of once per trial.
-template <int DIM, int QP, bool XS>
+// WIDE: the derivative rows in coordinate order, as in eval_posterior_gen.
+template <int DIM, int QP, bool XS, bool WIDE = false>
 __device__ __forceinline__ void eval_line_gen(const KgMcParams& prm, const double* __restrict__ Xt,
                                               const double* __restrict__ Pk, const double* __restrict__ Xu,
                                               const double (&xb)[DIM], const double (&gt)[DIM], const double* aw,
@@ -882,23 +974,25 @@ __device__ __forceinline__ void eval_line_gen(const KgMcParams& prm, const doubl
   const double xga = -alpha_min * xg;
   // base coordinates and direction at the derivative indices (compile-time register indexing only)
   double xm[kMaxG], gm[kMaxG];
+  if (!WIDE) {
 #pragma unroll
-  for (int m = 0; m < kMaxG; ++m) {
-    xm[m] = 0.0;
-    gm[m] = 0.0;
-    if (m < g) {
+    for (int m = 0; m < kMaxG; ++m) {
+      xm[m] = 0.0;
+      gm[m] = 0.0;
+      if (m < g) {
 #pragma unroll
-      for (int d = 0; d < DIM; ++d)
-        if (d == prm.derivs[m]) {
-          xm[m] = xb[d];
-          gm[m] = gt[d];
-        }
+        for (int d = 0; d < DIM; ++d)
+          if (d == prm.derivs[m]) {
+            xm[m] = xb[d];
+            gm[m] = gt[d];
+          }
+      }
     }
   }
 #pragma unroll
   for (int k = 0; k < kLineBatch; ++k) S[k] = T[k] = 0.0;
   pmax_hi = 0;
-  stream_point_weights(aw, ring, N, 1 + g, [&](int j, const double* aj) {
+  stream_weights<WIDE>(aw, ring, N, 1 + g, [&](int j, const double* aj, int base) {
     const double* xj = Xt + static_cast<size_t>(j) * DIM;
     const double* pk = Pk + static_cast<size_t>(j) * stride;
     double xv[DIM];
@@ -914,14 +1008,26 @@ __device__ __forceinline__ void eval_line_gen(const KgMcParams& prm, const doubl
       dot = fma(xb[d], xv[d], dot);
       pj = fma(ga[d], xv[d], pj);
     }
-    const double a0 = aj[0];
+    const double a0 = ring_weight<WIDE>(aj, base, 0);
     double us = 0.0, vs = 0.0;
+    if (WIDE) {
 #pragma unroll
-    for (int m = 0; m < kMaxG; ++m) {
-      if (m < g) {
-        const double am = aj[(m + 1) * kMcThreads];
-        us = fma(am, xm[m] - ld1<XS>(xj + prm.derivs[m]), us);
-        vs = fma(am, gm[m], vs);
+      for (int d = 0; d < DIM; ++d) {
+        const int r = prm.drow[d];
+        if (r > 0) {
+          const double am = ring_weight<WIDE>(aj, base, r);
+          us = fma(am, xb[d] - xv[d], us);
+          vs = fma(am, gt[d], vs);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int m = 0; m < kMaxG; ++m) {
+        if (m < g) {
+          const double am = aj[(m + 1) * kMcThreads];
+          us = fma(am, xm[m] - ld1<XS>(xj + prm.derivs[m]), us);
+          vs = fma(am, gm[m], vs);
+        }
       }
     }
     pmax_hi = max(pmax_hi, __double2hiint(pj) & 0x7fffffff);
@@ -953,12 +1059,24 @@ __device__ __forceinline__ void eval_line_gen(const KgMcParams& prm, const doubl
     }
     const double a0 = cl[u * bs];
     double us = 0.0, vs = 0.0;
+    if (WIDE) {
 #pragma unroll
-    for (int m = 0; m < kMaxG; ++m) {
-      if (m < g) {
-        const double am = cl[u * bs + 1 + m] * prm.inv_len[prm.derivs[m]];
-        us = fma(am, xm[m] - __ldg(xu + prm.derivs[m]), us);
-        vs = fma(am, gm[m], vs);
+      for (int d = 0; d < DIM; ++d) {
+        const int r = prm.drow[d];
+        if (r > 0) {
+          const double am = cl[u * bs + r] * prm.inv_len[d];
+          us = fma(am, xb[d] - xv[d], us);
+          vs = fma(am, gt[d], vs);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int m = 0; m < kMaxG; ++m) {
+        if (m < g) {
+          const double am = cl[u * bs + 1 + m] * prm.inv_len[prm.derivs[m]];
+          us = fma(am, xm[m] - __ldg(xu + prm.derivs[m]), us);
+          vs = fma(am, gm[m], vs);
+        }
       }
     }
     pmax_hi = max(pmax_hi, __double2hiint(pj) & 0x7fffffff);
@@ -1078,7 +1196,7 @@ enum : int { ST_FETCH = 0, ST_INIT = 1, ST_TRIAL = 2, ST_LIMIT = 3, ST_DONE = 4,
 // observations a sample's start evaluation comes from the start-point table (start_from_table) when the lane takes the
 // sample, so a new sample's first round is a LINE round, in phase with the lanes that continue; only the general path
 // (GEN) spends a POINT round on it (ST_INIT).
-template <int KERNEL, int DIM, int QP, bool SMEM, bool GEN>
+template <int KERNEL, int DIM, int QP, bool SMEM, bool GEN, bool WIDE = false>
 __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* __restrict__ Xt,
                                            const double* __restrict__ Pk, const double* __restrict__ Xu, int cand,
                                            int s_begin, int s_end, int* next_sample, double* aw = nullptr,
@@ -1209,7 +1327,7 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
         pmax_hi = 0;  // no factor can leave the double range on this path
         eval_line_matern<DIM, QP, SMEM>(Xt, Pk, Xu, N, U, prm.alpha, xt, gt, c, alpha_n, S);
       } else if (GEN) {
-        eval_line_gen<DIM, QP, SMEM>(prm, Xt, Pk, Xu, xt, gt, aw, ring, cl, alpha_n * (1.0 / kTop), S,
+        eval_line_gen<DIM, QP, SMEM, WIDE>(prm, Xt, Pk, Xu, xt, gt, aw, ring, cl, alpha_n * (1.0 / kTop), S,
                                reinterpret_cast<double (&)[kLineBatch]>(T), pmax_hi);
       } else {
         eval_line<DIM, QP, SMEM, TILE>(Xt, Pk, Xu, N, U, xt, gt, c, alpha_n * (1.0 / kTop), S, pmax_hi, xb, gb,
@@ -1267,16 +1385,18 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
       double S0, SB, s[DIM];
       double em[kMaxG];
       if (GEN) {
-        eval_posterior_gen<KERNEL, DIM, QP, SMEM>(prm, Xt, Pk, Xu, xq, aw, ring, cl, S0, SB, s, em);
+        eval_posterior_gen<KERNEL, DIM, QP, SMEM, WIDE>(prm, Xt, Pk, Xu, xq, aw, ring, cl, S0, SB, s, em);
         // kb a~_jm lands on coordinate derivs[m]: fold it into s so that the common gradient formula below holds
-        // (grad_d = inv_len_d (s_d - x~_d SB)), using compile-time register indices only
+        // (grad_d = inv_len_d (s_d - x~_d SB)), using compile-time register indices only (WIDE: already in s)
+        if (!WIDE) {
 #pragma unroll
-        for (int m = 0; m < kMaxG; ++m)
-          if (m < prm.g) {
+          for (int m = 0; m < kMaxG; ++m)
+            if (m < prm.g) {
 #pragma unroll
-            for (int d = 0; d < DIM; ++d)
-              if (d == prm.derivs[m]) s[d] += em[m];
-          }
+              for (int d = 0; d < DIM; ++d)
+                if (d == prm.derivs[m]) s[d] += em[m];
+            }
+        }
       } else {
         eval_posterior<KERNEL, DIM, QP, SMEM, TILE>(Xt, Pk, Xu, N, U, prm.alpha, xq, c, S0, SB, s);
       }
@@ -1450,7 +1570,8 @@ __global__ void __launch_bounds__(kMcThreads, CMOE_MC_MINBLOCKS) kg_mc_kernel(co
 #ifndef CMOE_MC_GEN_MINBLOCKS
 #define CMOE_MC_GEN_MINBLOCKS 2
 #endif
-template <int KERNEL, int DIM, int QP>
+// WIDE: the instantiations for 9 <= g <= 31 (stream_point_weights_wide; derivative rows in coordinate order).
+template <int KERNEL, int DIM, int QP, bool WIDE = false>
 __global__ void __launch_bounds__(kMcThreads, CMOE_MC_GEN_MINBLOCKS)
     kg_mc_gen_kernel(const __grid_constant__ KgMcParams prm) {
   extern __shared__ __align__(16) double gen_ring[];  // [kRingRows][kMcThreads]
@@ -1485,11 +1606,11 @@ __global__ void __launch_bounds__(kMcThreads, CMOE_MC_GEN_MINBLOCKS)
     const double* gXu = prm.Xu + static_cast<size_t>(cand) * prm.U * (DIM + 2);
     const double* gWt = prm.Wt + static_cast<size_t>(cand) * (1 + QP) * R;
     if (prm.stage_ops) {
-      kg_mc_body<KERNEL, DIM, QP, true, true>(prm, sX, sE, gXu, cand, s_begin, s_end, &next_sample, aw, gWt,
-                                              gen_ring + threadIdx.x);
+      kg_mc_body<KERNEL, DIM, QP, true, true, WIDE>(prm, sX, sE, gXu, cand, s_begin, s_end, &next_sample, aw, gWt,
+                                                    gen_ring + threadIdx.x);
     } else {
-      kg_mc_body<KERNEL, DIM, QP, false, true>(prm, prm.Xt, gPk, gXu, cand, s_begin, s_end, &next_sample, aw, gWt,
-                                               gen_ring + threadIdx.x);
+      kg_mc_body<KERNEL, DIM, QP, false, true, WIDE>(prm, prm.Xt, gPk, gXu, cand, s_begin, s_end, &next_sample, aw,
+                                                     gWt, gen_ring + threadIdx.x);
     }
     __syncthreads();  // next_sample / work_item are rewritten by thread 0
   }
@@ -1673,9 +1794,11 @@ struct KgDispatchEntry {
   KgAccLaunch acc;
   KgAccLaunch acc_gen;  // general path; null where mc_gen is
   size_t (*smem_bytes)(int N, int U);
+  bool wide = false;  // general path for 9 <= g <= 31 only (mc and acc are null)
 };
 void register_kg_entries(const KgDispatchEntry* entries, int count);
-const KgDispatchEntry* find_kg_entry(int kernel, int dim, int Q, bool need_gen);
+// g: derivative observations per point; entries with g <= 8 never dispatch to a wide entry, g > 8 only to one
+const KgDispatchEntry* find_kg_entry(int kernel, int dim, int Q, int g);
 
 template <int KERNEL, int DIM, int QP>
 void launch_kg_mc(const KgMcParams& p, dim3 grid, size_t smem, cudaStream_t s) {
@@ -1683,18 +1806,19 @@ void launch_kg_mc(const KgMcParams& p, dim3 grid, size_t smem, cudaStream_t s) {
   cudaFuncSetAttribute(kg_mc_kernel<KERNEL, DIM, QP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   kg_mc_kernel<KERNEL, DIM, QP><<<grid, kMcThreads, smem, s>>>(p);
 }
-template <int KERNEL, int DIM, int QP>
+template <int KERNEL, int DIM, int QP, bool WIDE = false>
 void launch_kg_mc_gen(const KgMcParams& p, dim3, size_t, cudaStream_t s) {
   int dev = 0, sms = 1, per_sm = 1;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const size_t ring_bytes = static_cast<size_t>(kRingRows + kRingDepth) * kMcThreads * sizeof(double) +
                             (p.stage_ops ? static_cast<size_t>(p.N) * (DIM + 2) * sizeof(double) : 0);
-  cudaFuncSetAttribute(kg_mc_gen_kernel<KERNEL, DIM, QP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  cudaFuncSetAttribute(kg_mc_gen_kernel<KERNEL, DIM, QP, WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                        static_cast<int>(ring_bytes));
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kg_mc_gen_kernel<KERNEL, DIM, QP>, kMcThreads, ring_bytes);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kg_mc_gen_kernel<KERNEL, DIM, QP, WIDE>, kMcThreads,
+                                                ring_bytes);
   const int grid = std::max(1, std::min(std::min(p.aw_slots, p.work_total), sms * std::max(1, per_sm)));
-  kg_mc_gen_kernel<KERNEL, DIM, QP><<<grid, kMcThreads, ring_bytes, s>>>(p);
+  kg_mc_gen_kernel<KERNEL, DIM, QP, WIDE><<<grid, kMcThreads, ring_bytes, s>>>(p);
 }
 template <int KERNEL, int DIM, int QP>
 void launch_kg_acc(const KgAccParams& p, dim3 grid, cudaStream_t s) {
@@ -1727,5 +1851,13 @@ size_t kg_smem_bytes(int N, int U) {
       CMOE_KG_ENTRY_GEN(0, D, 24), CMOE_KG_ENTRY_GEN(0, D, 32), CMOE_KG_ENTRY(1, D, 2), CMOE_KG_ENTRY(1, D, 4),  \
       CMOE_KG_ENTRY_GEN(1, D, 8), CMOE_KG_ENTRY_GEN(1, D, 16), CMOE_KG_ENTRY_GEN(1, D, 24),                    \
       CMOE_KG_ENTRY_GEN(1, D, 32)
+
+// Wide general path (9 <= g <= 31, kg_mc_wide_*.cu): only what such a g can reach — dim >= 9 (padded 12, 16, 32) and
+// Q = U (1 + g) >= 10 (widths 16, 24, 32).  The accumulation kernel does not depend on g and is the narrow entry's.
+#define CMOE_KG_ENTRY_WIDE(K, D, Q) \
+  { K, D, Q, nullptr, &launch_kg_mc_gen<K, D, Q, true>, nullptr, &launch_kg_acc_gen<K, D, Q>, &kg_smem_bytes<D, Q>, true }
+#define CMOE_KG_WIDE_ENTRIES_FOR_DIM(D)                                                                    \
+  CMOE_KG_ENTRY_WIDE(0, D, 16), CMOE_KG_ENTRY_WIDE(0, D, 24), CMOE_KG_ENTRY_WIDE(0, D, 32),                 \
+      CMOE_KG_ENTRY_WIDE(1, D, 16), CMOE_KG_ENTRY_WIDE(1, D, 24), CMOE_KG_ENTRY_WIDE(1, D, 32)
 
 }  // namespace cmoe
