@@ -803,9 +803,13 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
                             (spec.g == 0 ? static_cast<size_t>(pl->M) * (1 + QP) * (DIMP + 2) * sizeof(double) : 0);
     pl->batch = static_cast<int>(std::max<size_t>(
         1, std::min<size_t>({static_cast<size_t>(max_candidates), (size_t(3) << 30) / per_cand, kMaxGridY})));
-    // samples per CTA: aim for >= ~8 waves of CTAs over the whole batch, between 2 and 16 samples per lane
+    // samples per CTA: aim for >= ~8 waves of CTAs over the whole batch, between 2 and 16 samples per lane.  A wave is
+    // the fast-path kernel's residency as the occupancy API reports it (2 CTAs per SM for the tile instantiation at the
+    // bench shape); the general path hands its work items to a persistent grid and keeps 3 per SM, the count its
+    // scratch slots are sized for.
     {
-      const long long target_ctas = 8LL * sms * 3;
+      const int per_sm = spec.g == 0 ? std::max(1, pl->entry->mc_ctas_per_sm(pl->use_smem ? smem_need : 0)) : 3;
+      const long long target_ctas = 8LL * sms * per_sm;
       long long chunk = (static_cast<long long>(pl->batch) * num_mc + target_ctas - 1) / target_ctas;
       chunk = std::max<long long>(2 * kMcThreads, std::min<long long>(chunk, 16 * kMcThreads));
       chunk = (chunk + kMcThreads - 1) / kMcThreads * kMcThreads;

@@ -195,8 +195,9 @@ __device__ __forceinline__ double weight_row(const double* __restrict__ pk, doub
 // Tile evaluation of the training rows (shared-memory fast path, DESIGN.md K6).  A round is warp-uniform, so the
 // three small contractions of a round — x~ . X~_j (and a_min g~ . X~_j on LINE rounds), a_j = beta_j - B_j . c and, on
 // POINT rounds, the gradient sums s_d = sum_j w_j X~_jd — are, for one block of 8 training rows, products of shape
-// 32 samples x 8 rows x K.  They run on FP64 DMMA m16n8k4 (M = 16 samples: the warp's lanes in two halves run one after
-// the other, N = 8 rows, K = DIM or QP in steps of 4, K tails zero-filled); only the exps and the trial arithmetic stay
+// 32 samples x 8 rows x K.  They run on FP64 DMMA m16n8k4 (M = 16 samples: the warp's lanes in two halves, both in
+// one row sweep on POINT rounds and one after the other on LINE rounds, N = 8 rows, K = DIM or QP in steps of 4, K
+// tails zero-filled); only the exps and the trial arithmetic stay
 // element-wise, in the accumulator layout.  Fragment layout (PTX ISA, f64, lane = 4 g + t):
 //   A: a0 = A[g][t], a1 = A[g+8][t];   B: b = B[t][g];   C: c0 = C[g][2t], c1 = C[g][2t+1], c2 = C[g+8][2t], c3 = C[g+8][2t+1]
 // A sample's row of every product depends on that sample's operands only, and its partial sums over the 8 columns of a
@@ -205,12 +206,23 @@ __device__ __forceinline__ double weight_row(const double* __restrict__ pk, doub
 // ---------------------------------------------------------------------------------------------------------------
 
 // Which instantiations run the tile path: the ones measured to gain, SquareExponential at DIM = 8, QP = 8.  All the
-// others keep the scalar row loops (DESIGN.md K6 lists both groups).  The LINE tile needs ~240 registers per thread
-// against the 168 that 3 CTAs of 128 threads leave; the spill code grows with DIM and QP, and Matern-5/2's LINE rounds
-// are dominated by the per-trial sqrt and exp.
+// others keep the scalar row loops (DESIGN.md K6 lists both groups).  The tile rounds need ~240 registers per thread
+// (kg_mc_min_blocks); with the 168 that 3 CTAs of 128 threads leave, the spill code grows with DIM and QP, and
+// Matern-5/2's LINE rounds are dominated by the per-trial sqrt and exp.
 template <int KERNEL, int DIM, int QP>
 constexpr bool kg_tile_path() {
   return KERNEL == CMOE_KERNEL_SQUARE_EXPONENTIAL && DIM == 8 && QP == 8;
+}
+
+// CTAs of kMcThreads per SM that kg_mc_kernel's launch bounds ask for.  The tile instantiation takes 2, so that it gets
+// up to 255 registers (it uses 240 and spills nothing; the 168 that 3 CTAs leave spilled its round-level state).  Its
+// operands (72.6 KB at N = 500) leave room for 2 CTAs.  Every other instantiation keeps 3 CTAs (168 registers).
+#ifndef CMOE_MC_TILE_MINBLOCKS
+#define CMOE_MC_TILE_MINBLOCKS 2
+#endif
+template <int KERNEL, int DIM, int QP>
+constexpr int kg_mc_min_blocks() {
+  return kg_tile_path<KERNEL, DIM, QP>() ? CMOE_MC_TILE_MINBLOCKS : CMOE_MC_MINBLOCKS;
 }
 
 // A fragments of the half h (samples 16h .. 16h+15) from the lanes' own rows v[0..W): element k is -v[k] (NEG),
@@ -297,77 +309,100 @@ struct TileRows {
   }
 };
 
-// acc[4] (C layout) += A (K = W, fragments f) x B, B[k][n] = src[(row n) * stride + k] of the lane's row jb
+// B fragments of one block (K = W): b[ks] = B[4 ks + t][g] = row[4 ks + t] of the lane's row jb, zero past W
 template <int W>
-__device__ __forceinline__ void tile_mma(double (&acc)[4], const double (&f)[(W + 3) / 4][2], const double* row) {
+__device__ __forceinline__ void tile_bfrag(const double* row, double (&b)[(W + 3) / 4]) {
   const int t = threadIdx.x & 3;
 #pragma unroll
-  for (int ks = 0; ks < (W + 3) / 4; ++ks) {
-    const double b = (4 * ks + t < W) ? row[4 * ks + t] : 0.0;
-    dmma_m16n8k4(acc[0], acc[1], acc[2], acc[3], f[ks][0], f[ks][1], b);
-  }
+  for (int ks = 0; ks < (W + 3) / 4; ++ks) b[ks] = (4 * ks + t < W) ? row[4 * ks + t] : 0.0;
+}
+
+// acc[4] (C layout) += A (K = W, fragments f) x B (fragments b)
+template <int W>
+__device__ __forceinline__ void tile_mma(double (&acc)[4], const double (&f)[(W + 3) / 4][2],
+                                         const double (&b)[(W + 3) / 4]) {
+#pragma unroll
+  for (int ks = 0; ks < (W + 3) / 4; ++ks) dmma_m16n8k4(acc[0], acc[1], acc[2], acc[3], f[ks][0], f[ks][1], b[ks]);
 }
 
 // POINT round (SquareExponential) over the training rows: S0 = sum_j a_j k_j and s_d = sum_j a_j k_j X~_jd of every
-// lane's query point xq (hq = -|xq|^2 / 2).
+// lane's query point xq (hq = -|xq|^2 / 2).  One sweep over the rows serves both halves: a block's B fragments and
+// (e_j, beta_j) are loaded once and feed the products of samples 0-15 and 16-31.
 template <int DIM, int QP>
 __device__ __forceinline__ void tile_posterior(const double* __restrict__ Xt, const double* __restrict__ Pk, int N,
                                                const double (&xq)[DIM], const double (&c)[QP], double hq, double& S0,
                                                double (&s)[DIM]) {
   constexpr int KD = (DIM + 3) / 4, KQ = (QP + 3) / 4, ND = (DIM + 7) / 8;
   const int lane = threadIdx.x & 31, g = lane >> 2;
-  S0 = 0.0;
+  double xa[2][KD][2], ca[2][KQ][2], hqr[2][2];
 #pragma unroll
-  for (int d = 0; d < DIM; ++d) s[d] = 0.0;
-#pragma unroll 1
   for (int h = 0; h < 2; ++h) {
-    double xa[KD][2], ca[KQ][2];
-    tile_frag<DIM, false>(xq, nullptr, h, xa);
-    tile_frag<QP, true>(c, nullptr, h, ca);  // a = beta + (-c) . B: the negation is exact, each product is the scalar one
-    double hq0, hq1;
-    tile_rows(hq, h, hq0, hq1);
-    double s0[2] = {0.0, 0.0}, sacc[ND][4];
+    tile_frag<DIM, false>(xq, nullptr, h, xa[h]);
+    // a = beta + (-c) . B: the negation is exact, each product is the scalar one
+    tile_frag<QP, true>(c, nullptr, h, ca[h]);
+    tile_rows(hq, h, hqr[h][0], hqr[h][1]);
+  }
+  double s0[2][2], sacc[2][ND][4];
 #pragma unroll
-    for (int n = 0; n < ND; ++n) sacc[n][0] = sacc[n][1] = sacc[n][2] = sacc[n][3] = 0.0;
-    auto block = [&](int j0, auto tail) {
-      constexpr bool TAIL = decltype(tail)::value;
-      const TileRows<QP, TAIL> r(Pk, N, j0);
+  for (int h = 0; h < 2; ++h) {
+    s0[h][0] = s0[h][1] = 0.0;
+#pragma unroll
+    for (int n = 0; n < ND; ++n) sacc[h][n][0] = sacc[h][n][1] = sacc[h][n][2] = sacc[h][n][3] = 0.0;
+  }
+  auto block = [&](int j0, auto tail) {
+    constexpr bool TAIL = decltype(tail)::value;
+    const TileRows<QP, TAIL> r(Pk, N, j0);
+    double bx[KD], bq[KQ], b0[ND], b1[ND];
+    tile_bfrag<DIM>(Xt + r.jb * DIM, bx);
+    tile_bfrag<QP>(Pk + r.jb * (QP + 2) + 2, bq);
+#pragma unroll
+    for (int n = 0; n < ND; ++n) {
+      const int d = 8 * n + g;
+      b0[n] = (d < DIM) ? Xt[r.je0 * DIM + d] : 0.0;
+      b1[n] = (d < DIM) ? Xt[r.je1 * DIM + d] : 0.0;
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
       // the exponent's e_j enters as the accumulator seed
       double dot[4] = {r.h0.x, r.h1.x, r.h0.x, r.h1.x};
       double a[4] = {r.h0.y, r.h1.y, r.h0.y, r.h1.y};
-      tile_mma<DIM>(dot, xa, Xt + r.jb * DIM);
-      tile_mma<QP>(a, ca, Pk + r.jb * (QP + 2) + 2);
+      tile_mma<DIM>(dot, xa[h], bx);
+      tile_mma<QP>(a, ca[h], bq);
       double w[4];
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const double ai = ((i & 1) ? r.v1 : r.v0) ? a[i] : 0.0;
-        const double kv = exp_tab(dot[i] + ((i < 2) ? hq0 : hq1));
-        s0[i >> 1] = fma(ai, kv, s0[i >> 1]);
+        const double kv = exp_tab(dot[i] + hqr[h][i >> 1]);
+        s0[h][i >> 1] = fma(ai, kv, s0[h][i >> 1]);
         w[i] = ai * kv;
       }
       // s += W X~: k-step 0 takes the even columns (rows je0: A = (w0, w2)), k-step 1 the odd ones (rows je1)
 #pragma unroll
       for (int n = 0; n < ND; ++n) {
-        const int d = 8 * n + g;
-        const double b0 = (d < DIM) ? Xt[r.je0 * DIM + d] : 0.0;
-        const double b1 = (d < DIM) ? Xt[r.je1 * DIM + d] : 0.0;
-        dmma_m16n8k4(sacc[n][0], sacc[n][1], sacc[n][2], sacc[n][3], w[0], w[2], b0);
-        dmma_m16n8k4(sacc[n][0], sacc[n][1], sacc[n][2], sacc[n][3], w[1], w[3], b1);
+        dmma_m16n8k4(sacc[h][n][0], sacc[h][n][1], sacc[h][n][2], sacc[h][n][3], w[0], w[2], b0[n]);
+        dmma_m16n8k4(sacc[h][n][0], sacc[h][n][1], sacc[h][n][2], sacc[h][n][3], w[1], w[3], b1[n]);
       }
-    };
-    const int nfull = N & ~7;
-#pragma unroll 1
-    for (int j0 = 0; j0 < nfull; j0 += 8) block(j0, std::false_type());
-    if (nfull < N) block(nfull, std::true_type());
-    S0 = tile_to_owner(quad_sum(s0[0]), quad_sum(s0[1]), h, S0);
-#pragma unroll
-    for (int d = 0; d < DIM; ++d) {
-      // s[row][d] sits in lane 4 (row & 7) + ((d & 7) >> 1) of the row's quad, register (d & 1) (+ 2 for rows 8..15)
-      const int src = 4 * (lane & 7) + ((d & 7) >> 1);
-      const double vl = __shfl_sync(0xffffffffu, sacc[d / 8][d & 1], src);
-      const double vh = __shfl_sync(0xffffffffu, sacc[d / 8][2 + (d & 1)], src);
-      if ((lane >> 4) == h) s[d] = (lane & 8) ? vh : vl;
     }
+  };
+  const int nfull = N & ~7;
+#pragma unroll 1
+  for (int j0 = 0; j0 < nfull; j0 += 8) block(j0, std::false_type());
+  if (nfull < N) block(nfull, std::true_type());
+  S0 = 0.0;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) S0 = tile_to_owner(quad_sum(s0[h][0]), quad_sum(s0[h][1]), h, S0);
+#pragma unroll
+  for (int d = 0; d < DIM; ++d) {
+    // s[row][d] sits in lane 4 (row & 7) + ((d & 7) >> 1) of the row's quad, register (d & 1) (+ 2 for rows 8..15)
+    const int src = 4 * (lane & 7) + ((d & 7) >> 1);
+    double v[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const double vl = __shfl_sync(0xffffffffu, sacc[h][d / 8][d & 1], src);
+      const double vh = __shfl_sync(0xffffffffu, sacc[h][d / 8][2 + (d & 1)], src);
+      v[h] = (lane & 8) ? vh : vl;
+    }
+    s[d] = (lane >> 4) ? v[1] : v[0];
   }
 }
 
@@ -457,7 +492,9 @@ constexpr int kLineBatch = 8;  // trial step sizes per batch (6 measured +1.5 %,
 
 // LINE round (SquareExponential) over the training rows, added to S[k] and pmax_hi as eval_line computes them.  The
 // lanes' operands come from their unscaled state: base point xr, gradient gr (x~ = xr / l, a_min g~ = a_min (gr / l)),
-// with hq = -|x~|^2 / 2 and xga = -a_min x~ . g~.
+// with hq = -|x~|^2 / 2 and xga = -a_min x~ . g~.  Unlike tile_posterior, the halves sweep the rows one after the other:
+// one sweep for both (twice the 16 trial sums and the fragments live) measured slower on the H100, by 1.8 % per bench
+// step even with the lane state parked in shared memory to keep it from spilling (DESIGN.md K6).
 template <int DIM, int QP>
 __device__ __forceinline__ void tile_line(const double* __restrict__ Xt, const double* __restrict__ Pk, int N,
                                           const double (&xr)[DIM], const double (&gr)[DIM], const double* inv_len,
@@ -484,10 +521,12 @@ __device__ __forceinline__ void tile_line(const double* __restrict__ Xt, const d
       double dot[4] = {r.h0.x, r.h1.x, r.h0.x, r.h1.x};
       double p[4] = {xg0, xg0, xg1, xg1};
       double a[4] = {r.h0.y, r.h1.y, r.h0.y, r.h1.y};
-      const double* xj = Xt + r.jb * DIM;
-      tile_mma<DIM>(dot, xa, xj);
-      tile_mma<DIM>(p, gf, xj);
-      tile_mma<QP>(a, ca, Pk + r.jb * (QP + 2) + 2);
+      double bx[KD], bq[KQ];
+      tile_bfrag<DIM>(Xt + r.jb * DIM, bx);
+      tile_bfrag<QP>(Pk + r.jb * (QP + 2) + 2, bq);
+      tile_mma<DIM>(dot, xa, bx);
+      tile_mma<DIM>(p, gf, bx);
+      tile_mma<QP>(a, ca, bq);
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const bool v = (i & 1) ? r.v1 : r.v0;
@@ -1528,7 +1567,8 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
 }
 
 template <int KERNEL, int DIM, int QP>
-__global__ void __launch_bounds__(kMcThreads, CMOE_MC_MINBLOCKS) kg_mc_kernel(const __grid_constant__ KgMcParams prm) {
+__global__ void __launch_bounds__(kMcThreads, (kg_mc_min_blocks<KERNEL, DIM, QP>()))
+    kg_mc_kernel(const __grid_constant__ KgMcParams prm) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ uint64_t mbar;
   __shared__ int next_sample;
@@ -1795,6 +1835,7 @@ struct KgDispatchEntry {
   KgAccLaunch acc_gen;  // general path; null where mc_gen is
   size_t (*smem_bytes)(int N, int U);
   bool wide = false;  // general path for 9 <= g <= 31 only (mc and acc are null)
+  int (*mc_ctas_per_sm)(size_t operands) = nullptr;  // residency of mc (null where mc is)
 };
 void register_kg_entries(const KgDispatchEntry* entries, int count);
 // g: derivative observations per point; entries with g <= 8 never dispatch to a wide entry, g > 8 only to one
@@ -1805,6 +1846,15 @@ void launch_kg_mc(const KgMcParams& p, dim3 grid, size_t smem, cudaStream_t s) {
   // function attributes are per device: set on every launch (cheap), never cached process-wide
   cudaFuncSetAttribute(kg_mc_kernel<KERNEL, DIM, QP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   kg_mc_kernel<KERNEL, DIM, QP><<<grid, kMcThreads, smem, s>>>(p);
+}
+// resident CTAs of kg_mc_kernel per SM on the current device with `smem` bytes of staged operands (0: global memory)
+template <int KERNEL, int DIM, int QP>
+int kg_mc_ctas_per_sm(size_t smem) {
+  CMOE_CUDA(
+      cudaFuncSetAttribute(kg_mc_kernel<KERNEL, DIM, QP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  int per_sm = 0;
+  CMOE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kg_mc_kernel<KERNEL, DIM, QP>, kMcThreads, smem));
+  return per_sm;
 }
 template <int KERNEL, int DIM, int QP, bool WIDE = false>
 void launch_kg_mc_gen(const KgMcParams& p, dim3, size_t, cudaStream_t s) {
@@ -1837,12 +1887,15 @@ size_t kg_smem_bytes(int N, int U) {
   return (static_cast<size_t>(N) * (DIM + QP + 2) + static_cast<size_t>(U) * (DIM + 2)) * sizeof(double);
 }
 
-#define CMOE_KG_ENTRY(K, D, Q) \
-  { K, D, Q, &launch_kg_mc<K, D, Q>, nullptr, &launch_kg_acc<K, D, Q>, nullptr, &kg_smem_bytes<D, Q> }
+#define CMOE_KG_ENTRY(K, D, Q)                                                                                  \
+  {                                                                                                             \
+    K, D, Q, &launch_kg_mc<K, D, Q>, nullptr, &launch_kg_acc<K, D, Q>, nullptr, &kg_smem_bytes<D, Q>, false,     \
+        &kg_mc_ctas_per_sm<K, D, Q>                                                                              \
+  }
 #define CMOE_KG_ENTRY_GEN(K, D, Q)                                                                                \
   {                                                                                                               \
     K, D, Q, &launch_kg_mc<K, D, Q>, &launch_kg_mc_gen<K, D, Q>, &launch_kg_acc<K, D, Q>, &launch_kg_acc_gen<K, D, Q>, \
-        &kg_smem_bytes<D, Q>                                                                                       \
+        &kg_smem_bytes<D, Q>, false, &kg_mc_ctas_per_sm<K, D, Q>                                                   \
   }
 // union-row counts: 2, 4, 8, 16, 24, 32 (24 serves config 4: q = 4 with 4 derivative observations -> 20 rows; the
 // 32-wide instantiation spilled ~1.5 KB per thread there)
