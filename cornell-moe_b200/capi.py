@@ -357,6 +357,23 @@ def log_marginal_likelihood(kernel, alpha, lengths, X, y, noise, derivs=None, de
     return val.value
 
 
+def log_marginal_likelihood_list(kernel, hypers, X, y, derivs=None, device=0):
+    """cmoe_log_marginal_likelihood_list (EvaluateLogLikelihoodAtPointList, gpp_model_selection.hpp:1274-1308): the
+    log marginal likelihood at every row of ``hypers`` [num_sets, 2 + dim + g] = (alpha, lengths..., noise by
+    observation type) in one device call.  Returns a [num_sets] array; a set whose Cholesky fails is -inf."""
+    X = _f64(X)
+    N, dim = X.shape
+    derivs = _i32(derivs)
+    H = _f64(hypers).reshape(-1, 2 + dim + derivs.size)
+    values = np.empty(H.shape[0])
+    info = ctypes.c_int()
+    rc = lib().cmoe_log_marginal_likelihood_list(int(kernel), _d(H), H.shape[0], _d(X), _d(_f64(y).ravel()),
+                                                 _i(derivs), derivs.size, dim, N, int(device), _d(values),
+                                                 ctypes.byref(info))
+    _check(rc, info.value)
+    return values
+
+
 def grad_log_marginal_likelihood(kernel, alpha, lengths, X, y, noise, derivs=None, device=0):
     """cmoe_grad_log_marginal_likelihood: d log p / d (alpha, lengths..., noise by observation type)."""
     X = _f64(X)

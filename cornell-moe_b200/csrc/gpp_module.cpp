@@ -34,6 +34,7 @@
 #include <cmath>
 #include <cstdint>
 #include <cstdlib>
+#include <limits>
 #include <memory>
 #include <random>
 #include <string>
@@ -1099,8 +1100,58 @@ PYBIND11_MODULE(GPP, m) {
                                                   grad.data(), &info), info);
           return to_list(grad);
         });
+  // evaluate_log_likelihood_at_hyperparameter_list(hyperparameter_list, points_sampled, points_sampled_value, dim,
+  //     num_sampled, objective_mode, hyperparameters, noise_variance, derivatives, num_derivatives, num_multistarts,
+  //     max_num_threads, status)                                    gpp_python_model_selection.cpp:281-341, 520-556
+  // One device call for the whole list (cmoe_log_marginal_likelihood_list); `max_num_threads` is accepted and ignored
+  // (the sets run in parallel on the GPU).  Each set is (alpha, lengths..., noise by observation type).
+  m.def("evaluate_log_likelihood_at_hyperparameter_list",
+        [](const py::list& hyperparameter_list, const py::list& points_sampled, const py::list& points_sampled_value,
+           int dim, int num_sampled, LogLikelihoodTypes objective_mode, const py::list& hyperparameters,
+           const py::list& noise_variance, const py::list& derivatives, int num_derivatives, int num_multistarts,
+           int /*max_num_threads*/, py::dict status) -> py::list {
+          // the reference's order: input lists, covariance constructor, list copy, objective mode, then the driver
+          const auto X = to_vec(points_sampled, static_cast<size_t>(dim) * num_sampled);
+          const auto y = to_vec(points_sampled_value, static_cast<size_t>(num_sampled) * (1 + num_derivatives));
+          to_vec(noise_variance, 1 + num_derivatives);
+          const auto derivs = to_ivec(derivatives, num_derivatives);
+          const double alpha = hyperparameters[0].cast<double>();
+          const auto lengths = to_vec(hyperparameters[1].cast<py::list>(), dim);
+          if (!(alpha > 0.0)) {  // MaternNu2p5's constructor (gpp_covariance.cpp:80-91)
+            PyErr_SetString(g_exc_bounds, "Invalid hyperparameter (alpha).");
+            throw py::error_already_set();
+          }
+          for (double l : lengths) {
+            if (!(l > 0.0)) {
+              PyErr_SetString(g_exc_bounds, "Invalid hyperparameter (length).");
+              throw py::error_already_set();
+            }
+          }
+          const size_t nh = static_cast<size_t>(dim) + 2 + num_derivatives;
+          const auto hypers = to_vec(hyperparameter_list, nh * std::max(num_multistarts, 0));
+          if (objective_mode != LogLikelihoodTypes::kLogMarginalLikelihood) {  // leave-one-out is commented out (:323-333)
+            status["evaluate_invalid_log_likelihood_at_hyperparameter_list"] = false;
+            PyErr_SetString(g_exc_base, "ERROR: invalid objective mode choice. Setting all results to -DBL_MAX.");
+            throw py::error_already_set();
+          }
+          if (num_multistarts < 1) {  // gpp_model_selection.hpp:1285-1287
+            PyErr_SetString(g_exc_bounds, "num_multistarts must be > 1");
+            throw py::error_already_set();
+          }
+          std::vector<double> values(num_multistarts);
+          int info = 0;
+          // MaternNu2p5 hard-wired, as the reference's boundary does (:297)
+          check(cmoe_log_marginal_likelihood_list(CMOE_KERNEL_MATERN_NU_2P5, hypers.data(), num_multistarts, X.data(),
+                                                  y.data(), derivs.data(), num_derivatives, dim, num_sampled, 0,
+                                                  values.data(), &info),
+                info);
+          // found_flag of MultistartOptimize: some value beat the initial -inf with a strict < (gpp_optimization.hpp:1511)
+          const bool found = std::any_of(values.begin(), values.end(),
+                                         [](double v) { return -std::numeric_limits<double>::infinity() < v; });
+          status["evaluate_log_marginal_likelihood_at_hyperparameter_list"] = found;
+          return to_list(values);
+        });
   for (const char* name : {"multistart_hyperparameter_optimization", "restarted_hyperparameter_optimization",
-                           "evaluate_log_likelihood_at_hyperparameter_list",
                            "heuristic_expected_improvement_optimization"}) {
     const std::string n(name);
     m.def(name, [n](const py::args&, const py::kwargs&) -> py::object { not_on_path(n.c_str()); });

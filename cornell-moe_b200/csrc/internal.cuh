@@ -184,6 +184,18 @@ void trsm_lower(const double* L, int n, double* X, int ldx, int nrhs, bool trans
 bool trsv_coop(const double* L, int n, double* x, bool trans, cudaStream_t s);
 bool trsv_coop_pair(const double* L, int n, double* x, cudaStream_t s);
 
+// ---- sample.cu: batched blocked Cholesky (DESIGN.md K8) -------------------------------------------------------
+constexpr int kMaxSampleQ = 8192;                          // rows of one set's matrix
+constexpr size_t kSampleWorkspaceBytes = size_t(2) << 30;  // device workspace of one chunk (or of one set, if larger)
+// sets per chunk: one CTA row per set on grid.y / grid.z of the per-set launches (cov_tile, batched Cholesky,
+// sample_rows, lhs, the likelihood list), well inside their 65535.  It does not bound the chunk's points:
+// build_mix_covariance puts those on grid.x.
+constexpr int kMaxChunkSets = 4096;
+// In-place lower Cholesky of nsets Q x Q column-major matrices (only the lower triangle is read); fail[nsets] must be
+// zero on entry and receives 0 or the 1-based leading minor of the first pivot that fails `> 1e-16`.  `stage` holds the
+// diagonal factors until the end (nsets * ceil(Q/64) * 64 * 64 doubles).  Asynchronous on `s`.
+void potrf_batched(double* A, int Q, int nsets, int* fail, DevBuf<double>& stage, cudaStream_t s);
+
 // ---- posterior.cu -------------------------------------------------------------------------------------------
 constexpr int kMaxQ = 96;  // largest (q+p)*(1+num_derivatives) handled by the per-set kernels
 

@@ -13,6 +13,14 @@ constexpr int NB = 64;        // Cholesky block size == K depth of one DMMA tile
 constexpr int LDT = NB + 4;   // smem leading dimension: 68 = 4 (mod 16) makes the DMMA fragment loads conflict-free
 constexpr double kPivotTol = 1.0e-16;  // gpp_linear_algebra.cpp:118
 
+// linear index of a lower-triangular tile grid -> (ti, tj), tj <= ti
+__device__ __forceinline__ void tri_tile(int t, int& ti, int& tj) {
+  ti = static_cast<int>((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+  while (ti * (ti + 1) / 2 > t) --ti;
+  while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
+  tj = t - ti * (ti + 1) / 2;
+}
+
 // --------------------------------------------------------------------------------------------------------------
 // Diagonal-block factorisation + panel solve.  The column recurrence sqrt -> scale -> update is the latency-critical
 // chain of the whole factorisation (n/64 dependent block steps), so it runs out of REGISTERS: a warp factors a 32x32

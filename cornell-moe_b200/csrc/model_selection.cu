@@ -11,11 +11,21 @@
 // its 1 + dim partial sums in a fixed order; the host adds the per-CTA partials in launch order.
 // Quirks kept (pinned by tests/test_oracle_vs_reference.py::test_grad_log_marginal_likelihood): the Matern routine fills
 // only the value-value entry of a block, returns d/d alpha = 1 at coincident points and zero length derivatives there.
+//
+// Log marginal likelihood at a list of hyper-parameter sets (DESIGN.md K10): EvaluateLogLikelihoodAtPointList
+// (gpp_model_selection.hpp:1274-1308), Python boundary evaluate_log_likelihood_at_hyperparameter_list
+// (gpp_python_model_selection.cpp:281-341).  Per chunk of sets, three steps that treat every set independently:
+//   K_s = K(X, X; theta_s) + diag(noise_s + 1e-6)   lml_cov_kernel, lower 64 x 64 tiles, grid (tiles, 1, sets)
+//   L_s L_s^T = K_s                                 potrf_batched (sample.cu), failure flag per set
+//   -1/2 z^T z - sum log L_ii - n/2 log 2 pi,       lml_solve_kernel, one CTA per set, z = L_s^-1 (y - m)
+// so a set's value does not depend on the other sets of the call or on the chunking.
 #include <algorithm>
 #include <cmath>
+#include <limits>
 
 #include "device_math.cuh"
 #include "internal.cuh"
+#include "linalg_dev.cuh"
 
 namespace cmoe {
 namespace {
@@ -116,6 +126,146 @@ __global__ void hyper_grad_diag_kernel(const double* __restrict__ a, const doubl
   if (r < n) out[r] = a[r] * a[r] - Kinv[static_cast<size_t>(r) * n + r];
 }
 
+// ---- log marginal likelihood at a list of hyper-parameter sets ---------------------------------------------------
+constexpr int kLmlCovThreads = 256;
+constexpr int kLmlSolveThreads = 256;
+constexpr double kLog2Pi = 1.8378770664093453;
+static_assert(sizeof(KernelSpec) % sizeof(unsigned long long) == 0, "KernelSpec is staged as 8-byte words");
+
+// K_s = K(X, X; theta_s) + diag(noise_s by observation type), lower 64 x 64 tiles of the column-major n x n matrix of
+// every set; grid (tiles, 1, sets).  The set's KernelSpec is staged in shared memory, the (at most 64) points of the
+// tile's rows and columns beside it; entries are cov_build_generic_kernel's (kernel_parts / weighted_sqdist / cov_entry
+// on the raw points).  Only the lower triangle is written: potrf_batched reads nothing else.
+__global__ void __launch_bounds__(kLmlCovThreads) lml_cov_kernel(const KernelSpec* __restrict__ specs,
+                                                                 const double* __restrict__ noise,
+                                                                 const double* __restrict__ X, int N,
+                                                                 double* __restrict__ K) {
+  extern __shared__ double lml_pts[];  // [NB][dim] row points, then [NB][dim] column points
+  __shared__ KernelSpec spec;
+  const int set = blockIdx.z, tid = threadIdx.x;
+  {
+    const auto* src = reinterpret_cast<const unsigned long long*>(specs + set);
+    auto* dst = reinterpret_cast<unsigned long long*>(&spec);
+    for (int w = tid; w < static_cast<int>(sizeof(KernelSpec) / sizeof(unsigned long long)); w += blockDim.x)
+      dst[w] = src[w];
+  }
+  __syncthreads();
+  const int dim = spec.dim, b = 1 + spec.g, n = N * b;
+  int ti, tj;
+  tri_tile(blockIdx.x, ti, tj);
+  const int row0 = ti * NB, col0 = tj * NB;
+  const int rows = min(NB, n - row0), cols = min(NB, n - col0);
+  const int pr0 = row0 / b, pc0 = col0 / b;
+  const int npr = (row0 + rows - 1) / b - pr0 + 1, npc = (col0 + cols - 1) / b - pc0 + 1;
+  double* Pr = lml_pts;
+  double* Pc = lml_pts + NB * dim;
+  for (int e = tid; e < npr * dim; e += blockDim.x) Pr[e] = X[static_cast<size_t>(pr0) * dim + e];
+  for (int e = tid; e < npc * dim; e += blockDim.x) Pc[e] = X[static_cast<size_t>(pc0) * dim + e];
+  __syncthreads();
+  const double* nz = noise + static_cast<size_t>(set) * b;
+  double* Ks = K + static_cast<size_t>(set) * n * n;
+  for (int e = tid; e < NB * NB; e += blockDim.x) {
+    const int r = e % NB, c = e / NB;  // consecutive threads store consecutive rows of one column
+    const int gr = row0 + r, gc = col0 + c;
+    if (r >= rows || c >= cols || gr < gc) continue;
+    const double* p1 = Pr + (gr / b - pr0) * dim;
+    const double* p2 = Pc + (gc / b - pc0) * dim;
+    const KParts kp = kernel_parts(spec, weighted_sqdist(spec, p1, p2));
+    const int m = gr % b, cn = gc % b;
+    double v = cov_entry(spec, kp, p1, p2, m ? spec.derivs[m - 1] : -1, cn ? spec.derivs[cn - 1] : -1);
+    if (gr == gc) v += nz[m];
+    Ks[static_cast<size_t>(gc) * n + gr] = v;
+  }
+}
+
+// One CTA per set: z = L^-1 r by blocked forward substitution over 64-row blocks (warp 0 solves the diagonal block out
+// of shared memory; then every thread updates its rows below, summing the block's products in ascending column order),
+// then  -1/2 z^T z - sum_i log L_ii - n/2 log 2 pi  with a fixed thread-to-row assignment and block_sum.  A set whose
+// factorisation failed (fail[set] != 0) gets -inf.
+__global__ void __launch_bounds__(kLmlSolveThreads) lml_solve_kernel(const double* __restrict__ L, int n,
+                                                                     const double* __restrict__ r,
+                                                                     const int* __restrict__ fail,
+                                                                     double* __restrict__ out) {
+  extern __shared__ double lml_z[];         // [n] right-hand side -> solution
+  double* D = lml_z + n;                    // [NB][NB + 1] diagonal block, D[c * (NB + 1) + row]
+  __shared__ double scratch[kLmlSolveThreads / 32];
+  const int set = blockIdx.x, tid = threadIdx.x;
+  if (fail[set] != 0) {
+    if (tid == 0) out[set] = -INFINITY;
+    return;
+  }
+  const double* Ls = L + static_cast<size_t>(set) * n * n;
+  for (int i = tid; i < n; i += blockDim.x) lml_z[i] = r[i];
+  for (int k0 = 0; k0 < n; k0 += NB) {
+    const int nb = min(NB, n - k0);
+    __syncthreads();  // the previous block's update of z and its reads of D are done
+    for (int e = tid; e < NB * NB; e += blockDim.x) {
+      const int rr = e % NB, c = e / NB;
+      if (rr < nb && c < nb && rr >= c) D[c * (NB + 1) + rr] = Ls[static_cast<size_t>(k0 + c) * n + k0 + rr];
+    }
+    __syncthreads();
+    if (tid < 32) {  // lane owns rows tid and tid + 32 of the block
+      const int r0 = tid, r1 = tid + 32;
+      double v0 = r0 < nb ? lml_z[k0 + r0] : 0.0, v1 = r1 < nb ? lml_z[k0 + r1] : 0.0;
+      for (int j = 0; j < nb; ++j) {
+        const double xj = __shfl_sync(0xffffffffu, j < 32 ? v0 : v1, j & 31) / D[j * (NB + 1) + j];
+        if (r0 == j) v0 = xj;
+        if (r1 == j) v1 = xj;
+        if (r0 > j && r0 < nb) v0 = fma(-D[j * (NB + 1) + r0], xj, v0);
+        if (r1 > j && r1 < nb) v1 = fma(-D[j * (NB + 1) + r1], xj, v1);
+      }
+      if (r0 < nb) lml_z[k0 + r0] = v0;
+      if (r1 < nb) lml_z[k0 + r1] = v1;
+    }
+    __syncthreads();
+    for (int i = k0 + nb + tid; i < n; i += blockDim.x) {  // z_i -= sum_c L[i, k0 + c] z[k0 + c]
+      const double* Li = Ls + static_cast<size_t>(k0) * n + i;
+      double acc = 0.0;
+      for (int c = 0; c < nb; ++c) acc = fma(Li[static_cast<size_t>(c) * n], lml_z[k0 + c], acc);
+      lml_z[i] -= acc;
+    }
+  }
+  __syncthreads();
+  double zz = 0.0, logdiag = 0.0;
+  for (int i = tid; i < n; i += blockDim.x) {
+    zz = fma(lml_z[i], lml_z[i], zz);
+    logdiag += log(Ls[static_cast<size_t>(i) * n + i]);
+  }
+  zz = block_sum(zz, scratch);
+  logdiag = block_sum(logdiag, scratch);
+  if (tid == 0) out[set] = -0.5 * zz - logdiag - 0.5 * static_cast<double>(n) * kLog2Pi;
+}
+
+// Device workspace of cmoe_log_marginal_likelihood_list, one per host thread, kept for the device of the last call, so
+// that the calls of a sampler loop do not allocate (it grows to at most one chunk: kSampleWorkspaceBytes plus the
+// shared inputs, or one set if that is larger).
+struct LmlWork {
+  int device = -1;
+  cudaStream_t stream = nullptr;
+  DevBuf<double> X, r, noise, K, stage, values;
+  DevBuf<KernelSpec> specs;
+  DevBuf<int> fail;
+  void reset() {
+    X.release(); r.release(); noise.release(); K.release(); stage.release(); values.release();
+    specs.release();
+    fail.release();
+    if (stream) cudaStreamDestroy(stream);
+    stream = nullptr;
+    device = -1;
+  }
+  ~LmlWork() { reset(); }
+};
+
+LmlWork& lml_workspace(int device) {
+  static thread_local LmlWork ws;
+  if (ws.device != device) {
+    ws.reset();
+    CMOE_CUDA(cudaStreamCreateWithFlags(&ws.stream, cudaStreamNonBlocking));
+    ws.device = device;
+  }
+  return ws;
+}
+
 }  // namespace
 }  // namespace cmoe
 
@@ -170,4 +320,103 @@ extern "C" int cmoe_grad_log_marginal_likelihood(int kernel, double alpha, const
   });
   cmoe_gp_destroy(gp);
   return out;
+}
+
+extern "C" int cmoe_log_marginal_likelihood_list(int kernel, const double* hyperparameters, int num_sets,
+                                                 const double* points_sampled, const double* points_sampled_value,
+                                                 const int* derivatives, int num_derivatives, int dim,
+                                                 int num_sampled, int device, double* values, int* info) {
+  return guarded(info, [&] {
+    CMOE_REQUIRE(num_sets >= 1, CMOE_ERR_BOUNDS, "num_sets must be >= 1");
+    CMOE_REQUIRE(hyperparameters != nullptr && points_sampled != nullptr && points_sampled_value != nullptr &&
+                     values != nullptr,
+                 CMOE_ERR_INVALID_VALUE, "NULL argument");
+    CMOE_REQUIRE(kernel == CMOE_KERNEL_SQUARE_EXPONENTIAL || kernel == CMOE_KERNEL_MATERN_NU_2P5,
+                 CMOE_ERR_INVALID_VALUE, "unknown covariance kernel id");
+    CMOE_REQUIRE(dim >= 1 && dim <= CMOE_MAX_DIM, CMOE_ERR_BOUNDS, "dim must be in [1, CMOE_MAX_DIM]");
+    CMOE_REQUIRE(num_sampled >= 1, CMOE_ERR_BOUNDS, "num_sampled must be >= 1");
+    CMOE_REQUIRE(num_derivatives >= 0 && num_derivatives <= dim, CMOE_ERR_BOUNDS, "num_derivatives out of range");
+    CMOE_REQUIRE(num_derivatives == 0 || derivatives != nullptr, CMOE_ERR_INVALID_VALUE, "derivatives is NULL");
+    for (int k = 0; k < num_derivatives; ++k)
+      CMOE_REQUIRE(derivatives[k] >= 0 && derivatives[k] < dim, CMOE_ERR_BOUNDS, "derivative index out of range");
+    const int g = num_derivatives, b = 1 + g, nh = 2 + dim + g, N = num_sampled;
+    CMOE_REQUIRE(static_cast<long long>(N) * b <= kMaxSampleQ, CMOE_ERR_BOUNDS,
+                 "num_sampled * (1 + num_derivatives) must be <= 8192");
+    const int n = N * b;
+    // per set: the covariance hyper-parameters as cmoe_gp_create takes them (InitializeCovariance's checks,
+    // gpp_covariance.cpp:74-98, naming the set), the noise with the single call's 1e-6 added first
+    std::vector<KernelSpec> specs(num_sets);
+    std::vector<double> noise(static_cast<size_t>(num_sets) * b);
+    for (int s = 0; s < num_sets; ++s) {
+      const double* h = hyperparameters + static_cast<size_t>(s) * nh;
+      if (!(h[0] > 0.0))
+        throw Error(CMOE_ERR_BOUNDS, "hyperparameter set " + std::to_string(s) + ": Invalid hyperparameter (alpha).");
+      for (int k = 0; k < dim; ++k)
+        if (!(h[1 + k] > 0.0))
+          throw Error(CMOE_ERR_BOUNDS,
+                      "hyperparameter set " + std::to_string(s) + ": Invalid hyperparameter (length).");
+      KernelSpec& sp = specs[s];
+      sp = KernelSpec{};
+      sp.kernel = kernel;
+      sp.dim = dim;
+      sp.g = g;
+      sp.alpha = h[0];
+      for (int k = 0; k < CMOE_MAX_DIM; ++k) {
+        sp.lsq[k] = 1.0;
+        sp.inv_len[k] = 0.0;
+        sp.derivs[k] = 0;
+      }
+      for (int k = 0; k < dim; ++k) {
+        sp.lsq[k] = h[1 + k] * h[1 + k];
+        sp.inv_len[k] = 1.0 / h[1 + k];
+      }
+      for (int k = 0; k < g; ++k) sp.derivs[k] = derivatives[k];
+      for (int t = 0; t < b; ++t) noise[static_cast<size_t>(s) * b + t] = h[1 + dim + t] + 1.0e-6;
+    }
+    require_device(device);
+    // y - m, m = average of the function values in the reference's order (gpp_model_selection.cpp:556-560); it does
+    // not depend on the set
+    double m = 0.0;
+    for (int i = 0; i < N; ++i) m += points_sampled_value[static_cast<size_t>(i) * b];
+    m /= N;
+    std::vector<double> rc(points_sampled_value, points_sampled_value + n);
+    for (int i = 0; i < N; ++i) rc[static_cast<size_t>(i) * b] -= m;
+
+    LmlWork& w = lml_workspace(device);
+    cudaStream_t s = w.stream;
+    const int nsteps = (n + NB - 1) / NB;
+    const size_t per_set = sizeof(double) * (static_cast<size_t>(n) * n + static_cast<size_t>(nsteps) * NB * NB + b + 1) +
+                           sizeof(KernelSpec) + sizeof(int);
+    const int chunk = static_cast<int>(std::max<size_t>(
+        1, std::min<size_t>({kSampleWorkspaceBytes / per_set, static_cast<size_t>(num_sets),
+                             static_cast<size_t>(kMaxChunkSets)})));
+    w.X.upload(points_sampled, static_cast<size_t>(N) * dim, s);
+    w.r.upload(rc.data(), n, s);
+    w.specs.ensure(chunk);
+    w.noise.ensure(static_cast<size_t>(chunk) * b);
+    w.K.ensure(static_cast<size_t>(chunk) * n * n);
+    w.values.ensure(chunk);
+    w.fail.ensure(chunk);
+    const size_t smem_cov = 2 * static_cast<size_t>(NB) * dim * sizeof(double);
+    const size_t smem_solve = (static_cast<size_t>(n) + NB * (NB + 1)) * sizeof(double);
+    CMOE_CUDA(cudaFuncSetAttribute(lml_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   static_cast<int>(smem_solve)));
+    const int t = nsteps;
+    for (int c0 = 0; c0 < num_sets; c0 += chunk) {
+      const int nc = std::min(chunk, num_sets - c0);
+      w.specs.upload(specs.data() + c0, nc, s);
+      w.noise.upload(noise.data() + static_cast<size_t>(c0) * b, static_cast<size_t>(nc) * b, s);
+      CMOE_CUDA(cudaMemsetAsync(w.fail.p, 0, nc * sizeof(int), s));
+      lml_cov_kernel<<<dim3(t * (t + 1) / 2, 1, nc), kLmlCovThreads, smem_cov, s>>>(w.specs.p, w.noise.p, w.X.p, N,
+                                                                                  w.K.p);
+      count_launch();
+      CMOE_CUDA(cudaGetLastError());
+      potrf_batched(w.K.p, n, nc, w.fail.p, w.stage, s);
+      lml_solve_kernel<<<nc, kLmlSolveThreads, smem_solve, s>>>(w.K.p, n, w.r.p, w.fail.p, w.values.p);
+      count_launch();
+      CMOE_CUDA(cudaGetLastError());
+      w.values.download(values + c0, nc, s);
+      CMOE_CUDA(cudaStreamSynchronize(s));
+    }
+  });
 }

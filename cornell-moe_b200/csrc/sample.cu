@@ -32,24 +32,10 @@ namespace cmoe {
 
 namespace {
 
-constexpr int kMaxSampleQ = 8192;                          // rows of one set's joint draw
-constexpr size_t kSampleWorkspaceBytes = size_t(2) << 30;  // device workspace of one chunk (or of one set, if larger)
-// sets per chunk: one CTA row per set on grid.y / grid.z of the per-set launches (cov_tile, batched Cholesky,
-// sample_rows, lhs), well inside their 65535.  It does not bound the chunk's points: build_mix_covariance puts those on
-// grid.x.
-constexpr int kMaxChunkSets = 4096;
 constexpr int kTileThreads = 128;
 constexpr int kRowThreads = 256;
 
 __device__ __forceinline__ int set_row_type(int local, const int* derivs) { return local ? derivs[local - 1] : -1; }
-
-// linear index of a lower-triangular tile grid -> (ti, tj), tj <= ti
-__device__ __forceinline__ void tri_tile(int t, int& ti, int& tj) {
-  ti = static_cast<int>((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
-  while (ti * (ti + 1) / 2 > t) --ti;
-  while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
-  tj = t - ti * (ti + 1) / 2;
-}
 
 // acc += As^T-tile * Bs-tile over one 64-deep chunk: warp (wm, wn) owns a 32 x 32 sub-tile, 2 x 4 m16n8k4 products per
 // k-step (the fragment layout of dmma_tile_kernel in linalg.cu).  As / Bs: [k][LDT], element (k, row).
@@ -416,8 +402,9 @@ size_t panel_smem_bytes() {
   return (static_cast<size_t>(NB) * LTS + NB + 128 + NB + NB * (NB + 1)) * sizeof(double);
 }
 
-// In-place lower Cholesky of nsets Q x Q column-major matrices; fail[nsets] must be zero on entry.  `stage` holds the
-// diagonal factors until the end (nsets * ceil(Q/64) * 64 * 64 doubles).
+}  // namespace
+
+// declared in internal.cuh; also factors the covariance matrices of cmoe_log_marginal_likelihood_list
 void potrf_batched(double* A, int Q, int nsets, int* fail, DevBuf<double>& stage, cudaStream_t s) {
   const size_t smem_panel = panel_smem_bytes();
   const size_t smem_tile = 2 * NB * LDT * sizeof(double);
@@ -441,6 +428,8 @@ void potrf_batched(double* A, int Q, int nsets, int* fail, DevBuf<double>& stage
   count_launch();
   CMOE_CUDA(cudaGetLastError());
 }
+
+namespace {
 
 // Device workspace of the sampling calls, kept on the GP handle (cmoe_gp::sample_ws) and grown on demand, so repeated
 // calls do not allocate and free up to kSampleWorkspaceBytes each time.  Released with the handle.

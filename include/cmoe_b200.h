@@ -103,6 +103,20 @@ int cmoe_grad_log_marginal_likelihood(int kernel, double alpha, const double* le
                                       const double* points_sampled_value, const double* noise_variance,
                                       const int* derivatives, int num_derivatives, int dim, int num_sampled, int device,
                                       double* grad, int* info);
+/* log p(y | X, theta_s) for num_sets hyper-parameter sets in one device call: EvaluateLogLikelihoodAtPointList
+ * (gpp_model_selection.hpp:1274-1308); Python boundary evaluate_log_likelihood_at_hyperparameter_list
+ * (gpp_python_model_selection.cpp:281-341, 520-556).  hyperparameters[num_sets][2 + dim + g], each set
+ * (alpha, lengths[dim], noise_variance[1 + g]), the reference's problem-size layout (gpp_model_selection.cpp:798-811).
+ * Per set the value is cmoe_log_marginal_likelihood's: 1e-6 added to every noise entry, the prior mean = average of
+ * the function values, -1/2 z^T z - sum_i log L_ii - n/2 log 2 pi with z = L^-1 (y - mean); a set whose Cholesky fails
+ * gets -inf and leaves the others unaffected.  values[num_sets] in list order.  Unlike the reference, every set is
+ * checked (alpha > 0, lengths > 0; CMOE_ERR_BOUNDS naming the set); num_sets >= 1, num_sampled (1 + g) <= 8192.
+ * The sets are processed in chunks of at most 4096 sets and about 2 GiB of device workspace, which is kept per host
+ * thread for the device of the last call.  A set's value does not depend on the rest of the list. */
+int cmoe_log_marginal_likelihood_list(int kernel, const double* hyperparameters, int num_sets,
+                                      const double* points_sampled, const double* points_sampled_value,
+                                      const int* derivatives, int num_derivatives, int dim, int num_sampled, int device,
+                                      double* values, int* info);
 /* Run-time switches between kernel generations (also read once from the environment: CMOE_LEGACY_LINALG, CMOE_COV_TMA):
  *   "legacy_linalg" 1 = round-1 launch-per-step Cholesky / chained trsv for large n (default 0: cooperative kernels);
  *   "cov_tma"       1 = TMA / DMMA covariance build with tensor-map tile stores (default 0: LDGSTS kernel, faster at d ~ 10). */
