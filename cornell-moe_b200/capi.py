@@ -374,6 +374,47 @@ def log_marginal_likelihood_list(kernel, hypers, X, y, derivs=None, device=0):
     return values
 
 
+def grad_log_marginal_likelihood_list(kernel, hypers, X, y, derivs=None, device=0):
+    """cmoe_grad_log_marginal_likelihood_list: (values [num_sets], grads [num_sets, 2 + dim + g]) at every row of
+    ``hypers`` (the layout of log_marginal_likelihood_list) in one device call.  The values equal
+    log_marginal_likelihood_list's bit for bit; a set whose Cholesky fails gets -inf and a zero gradient."""
+    X = _f64(X)
+    N, dim = X.shape
+    derivs = _i32(derivs)
+    H = _f64(hypers).reshape(-1, 2 + dim + derivs.size)
+    values = np.empty(H.shape[0])
+    grads = np.empty(H.shape)
+    info = ctypes.c_int()
+    rc = lib().cmoe_grad_log_marginal_likelihood_list(int(kernel), _d(H), H.shape[0], _d(X), _d(_f64(y).ravel()),
+                                                      _i(derivs), derivs.size, dim, N, int(device), _d(values),
+                                                      _d(grads), ctypes.byref(info))
+    _check(rc, info.value)
+    return values, grads
+
+
+def hyperparameter_gradient_descent(kernel, gd, bounds, starts, X, y, derivs=None, device=0):
+    """cmoe_hyperparameter_gradient_descent: restarted gradient ascent of the log marginal likelihood from every row of
+    ``starts`` [num_starts, 2 + dim + g] on the linear-space box ``bounds`` [2 + dim + g, 2].  Returns
+    (best_point, best_value, found, end_points, end_values)."""
+    X = _f64(X)
+    N, dim = X.shape
+    derivs = _i32(derivs)
+    nh = 2 + dim + derivs.size
+    S = _f64(starts).reshape(-1, nh)
+    B = _f64(bounds).reshape(-1)
+    if B.size < 2 * nh:
+        raise BoundsError(ERR_BOUNDS, f"bounds needs 2 * (2 + dim + g) = {2 * nh} values, got {B.size}")
+    gd = GDParams.from_seq(gd)
+    best, ends, end_v = np.empty(nh), np.empty(S.shape), np.empty(S.shape[0])
+    best_v, found, info = ctypes.c_double(), ctypes.c_int(), ctypes.c_int()
+    rc = lib().cmoe_hyperparameter_gradient_descent(int(kernel), ctypes.byref(gd), _d(B), _d(S), S.shape[0], _d(X),
+                                                    _d(_f64(y).ravel()), _i(derivs), derivs.size, dim, N, int(device),
+                                                    _d(best), ctypes.byref(best_v), ctypes.byref(found), _d(ends),
+                                                    _d(end_v), ctypes.byref(info))
+    _check(rc, info.value)
+    return best, best_v.value, bool(found.value), ends, end_v
+
+
 def grad_log_marginal_likelihood(kernel, alpha, lengths, X, y, noise, derivs=None, device=0):
     """cmoe_grad_log_marginal_likelihood: d log p / d (alpha, lengths..., noise by observation type)."""
     X = _f64(X)

@@ -839,6 +839,129 @@ py::list evaluate_EI_mcmc_at_point_list(const GaussianProcessMCMC& gp, const py:
   throw py::error_already_set();
 }
 
+[[noreturn]] void raise_exc(PyObject* type, const char* msg) {
+  PyErr_SetString(type, msg);
+  throw py::error_already_set();
+}
+
+// ---- hyper-parameter optimisation (gpp_python_model_selection.cpp:150-279, 343-376) ---------------------------------
+// The inputs of both entries in the reference's order: the input lists (PythonInterfaceInputContainer), the MaternNu2p5
+// constructor's checks, then the log10 domain copy.  start = (alpha, lengths..., noise by observation type).
+struct HyperInputs {
+  std::vector<double> X, y, start, log_bounds;
+  std::vector<int> derivs;
+  int nh = 0;
+};
+
+HyperInputs hyper_inputs(const py::list& hyperparameter_domain, const py::list& points_sampled,
+                         const py::list& points_sampled_value, int dim, int num_sampled,
+                         const py::list& hyperparameters, const py::list& noise_variance, const py::list& derivatives,
+                         int num_derivatives) {
+  HyperInputs in;
+  in.X = to_vec(points_sampled, static_cast<size_t>(dim) * num_sampled);
+  in.y = to_vec(points_sampled_value, static_cast<size_t>(num_sampled) * (1 + num_derivatives));
+  const auto noise = to_vec(noise_variance, 1 + num_derivatives);
+  in.derivs = to_ivec(derivatives, num_derivatives);
+  const double alpha = hyperparameters[0].cast<double>();
+  const auto lengths = to_vec(hyperparameters[1].cast<py::list>(), dim);
+  if (!(alpha > 0.0)) raise_exc(g_exc_bounds, "Invalid hyperparameter (alpha).");  // gpp_covariance.cpp:80-91
+  for (double l : lengths)
+    if (!(l > 0.0)) raise_exc(g_exc_bounds, "Invalid hyperparameter (length).");
+  in.nh = dim + 2 + num_derivatives;
+  in.start.push_back(alpha);
+  in.start.insert(in.start.end(), lengths.begin(), lengths.end());
+  in.start.insert(in.start.end(), noise.begin(), noise.end());
+  in.log_bounds = to_vec(hyperparameter_domain, 2 * static_cast<size_t>(in.nh));
+  return in;
+}
+
+std::vector<double> pow10(std::vector<double> v) {
+  for (double& x : v) x = std::pow(10.0, x);
+  return v;
+}
+
+// multistart_hyperparameter_optimization (:219-279): the MaternNu2p5 kernel hard-wired, as in the reference; starts
+// drawn in log10 space from the uniform engine (ConvertFromLogToLinearDomainAndBuildInitialGuesses,
+// gpp_model_selection.hpp:841-858).  `max_num_threads` is accepted and ignored: the starts run in parallel on one GPU.
+py::list multistart_hyperparameter_optimization(const py::object& optimizer_parameters,
+                                                const py::list& hyperparameter_domain, const py::list& points_sampled,
+                                                const py::list& points_sampled_value, int dim, int num_sampled,
+                                                const py::list& hyperparameters, const py::list& noise_variance,
+                                                const py::list& derivatives, int num_derivatives,
+                                                int /*max_num_threads*/, RandomnessSourceContainer& rnd,
+                                                py::dict status) {
+  const HyperInputs in = hyper_inputs(hyperparameter_domain, points_sampled, points_sampled_value, dim, num_sampled,
+                                      hyperparameters, noise_variance, derivatives, num_derivatives);
+  const auto opt_type = optimizer_parameters.attr("optimizer_type").cast<OptimizerTypes>();
+  const auto objective = optimizer_parameters.attr("objective_type").cast<LogLikelihoodTypes>();
+  if (objective != LogLikelihoodTypes::kLogMarginalLikelihood)  // leave-one-out is commented out (:258-267)
+    raise_exc(g_exc_base, "ERROR: invalid objective type choice. Setting all hyperparameters to 1.0.");
+  const int nh = in.nh;
+  std::vector<double> best(nh);
+  int info = 0;
+  if (opt_type == OptimizerTypes::kNull) {
+    // LatinHypercubeSearchHyperparameterOptimization (gpp_model_selection.hpp:1342-1363): the start values and the
+    // strict-`<` arg-max from -inf of EvaluateLogLikelihoodAtPointList
+    const int n = optimizer_parameters.attr("num_random_samples").cast<int>();
+    if (n <= 0) raise_exc(g_exc_bounds, "num_multistarts must be > 1");
+    const auto starts = pow10(lhc_starts(in.log_bounds, nh, 1, n, rnd.uniform_engine));
+    std::vector<double> values(n);
+    check(cmoe_log_marginal_likelihood_list(CMOE_KERNEL_MATERN_NU_2P5, starts.data(), n, in.X.data(), in.y.data(),
+                                            in.derivs.data(), num_derivatives, dim, num_sampled, 0, values.data(),
+                                            &info),
+          info);
+    double bv = -std::numeric_limits<double>::infinity();
+    int bi = 0;
+    bool found = false;
+    for (int i = 0; i < n; ++i)
+      if (bv < values[i]) {
+        bv = values[i];
+        bi = i;
+        found = true;
+      }
+    std::copy(starts.begin() + static_cast<size_t>(bi) * nh, starts.begin() + static_cast<size_t>(bi + 1) * nh,
+              best.begin());
+    status["log_marginal_likelihood_lhc_found_update"] = found;
+  } else if (opt_type == OptimizerTypes::kGradientDescent) {
+    const cmoe_gd_params gd = gd_of(optimizer_parameters);
+    if (gd.num_multistarts <= 0) raise_exc(g_exc_bounds, "num_multistarts must be > 1");
+    const auto starts = pow10(lhc_starts(in.log_bounds, nh, 1, gd.num_multistarts, rnd.uniform_engine));
+    const auto bounds = pow10(in.log_bounds);
+    double bv = 0.0;
+    int found = 0;
+    check(cmoe_hyperparameter_gradient_descent(CMOE_KERNEL_MATERN_NU_2P5, &gd, bounds.data(), starts.data(),
+                                               gd.num_multistarts, in.X.data(), in.y.data(), in.derivs.data(),
+                                               num_derivatives, dim, num_sampled, 0, best.data(), &bv, &found, nullptr,
+                                               nullptr, &info),
+          info);
+    status["log_marginal_likelihood_gradient_descent_found_update"] = found != 0;
+  } else {  // kNewton is commented out at the reference's boundary (:194-206)
+    raise_exc(g_exc_base, "ERROR: invalid optimizer choice. Setting all hyperparameters to 1.0.");
+  }
+  return to_list(best);
+}
+
+// restarted_hyperparameter_optimization (:343-376): one start from (hyperparameters, noise_variance) on the linear-space
+// box; with max_num_restarts <= 0 the reference's driver returns before writing, so the result is its zero vector.
+py::list restarted_hyperparameter_optimization(const py::object& optimizer_parameters,
+                                               const py::list& hyperparameter_domain, const py::list& points_sampled,
+                                               const py::list& points_sampled_value, int dim, int num_sampled,
+                                               const py::list& hyperparameters, const py::list& noise_variance,
+                                               const py::list& derivatives, int num_derivatives, py::dict /*status*/) {
+  const HyperInputs in = hyper_inputs(hyperparameter_domain, points_sampled, points_sampled_value, dim, num_sampled,
+                                      hyperparameters, noise_variance, derivatives, num_derivatives);
+  const cmoe_gd_params gd = gd_of(optimizer_parameters);
+  std::vector<double> out(in.nh, 0.0), best(in.nh);
+  if (gd.max_num_restarts <= 0) return to_list(out);
+  const auto bounds = pow10(in.log_bounds);
+  int info = 0;
+  check(cmoe_hyperparameter_gradient_descent(CMOE_KERNEL_MATERN_NU_2P5, &gd, bounds.data(), in.start.data(), 1,
+                                             in.X.data(), in.y.data(), in.derivs.data(), num_derivatives, dim,
+                                             num_sampled, 0, best.data(), nullptr, nullptr, out.data(), nullptr, &info),
+        info);
+  return to_list(out);
+}
+
 }  // namespace
 
 // ---- ensemble posterior mean (not in the reference module) ------------------------------------------------------------
@@ -1151,11 +1274,25 @@ PYBIND11_MODULE(GPP, m) {
           status["evaluate_log_marginal_likelihood_at_hyperparameter_list"] = found;
           return to_list(values);
         });
-  for (const char* name : {"multistart_hyperparameter_optimization", "restarted_hyperparameter_optimization",
-                           "heuristic_expected_improvement_optimization"}) {
+  // multistart_hyperparameter_optimization(optimizer_parameters, hyperparameter_domain, points_sampled,
+  //     points_sampled_value, dim, num_sampled, hyperparameters, noise_variance, derivatives, num_derivatives,
+  //     max_num_threads, randomness_source, status)                              gpp_python_model_selection.cpp:219-279
+  // restarted_hyperparameter_optimization(optimizer_parameters, hyperparameter_domain, points_sampled,
+  //     points_sampled_value, dim, num_sampled, hyperparameters, noise_variance, derivatives, num_derivatives,
+  //     status)                                                                  gpp_python_model_selection.cpp:343-376
+  // A call that matches neither signature reaches the catch-all overload and raises the library's own exception.
+  m.def("multistart_hyperparameter_optimization", &multistart_hyperparameter_optimization);
+  m.def("restarted_hyperparameter_optimization", &restarted_hyperparameter_optimization);
+  for (const char* name : {"multistart_hyperparameter_optimization", "restarted_hyperparameter_optimization"}) {
     const std::string n(name);
-    m.def(name, [n](const py::args&, const py::kwargs&) -> py::object { not_on_path(n.c_str()); });
+    m.def(name, [n](const py::args&, const py::kwargs&) -> py::object {
+      raise_exc(g_exc_base, (n + ": the arguments match no signature of the reference's function").c_str());
+    });
   }
+  m.def("heuristic_expected_improvement_optimization",
+        [](const py::args&, const py::kwargs&) -> py::object {
+          not_on_path("heuristic_expected_improvement_optimization");
+        });
   m.def("run_cpp_tests", []() -> int { not_on_path("run_cpp_tests"); });
   m.def("device_count", []() { return cmoe_device_count(); });
   m.def("version", []() { return std::string(cmoe_version()); });

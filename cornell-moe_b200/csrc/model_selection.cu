@@ -19,6 +19,10 @@
 //   L_s L_s^T = K_s                                 potrf_batched (sample.cu), failure flag per set
 //   -1/2 z^T z - sum log L_ii - n/2 log 2 pi,       lml_solve_kernel, one CTA per set, z = L_s^-1 (y - m)
 // so a set's value does not depend on the other sets of the call or on the chunking.
+//
+// Value and hyper-parameter gradient at a list of sets (DESIGN.md K11): the same chunks, plus a = K_s^-1 (y - m) from
+// the solve kernel, K_s^-1 = L^-T L^-1 by a blocked triangular inverse on DMMA tiles, the single call's per-pair
+// contraction for every set and a fixed-order reduction per set.
 #include <algorithm>
 #include <cmath>
 #include <limits>
@@ -38,6 +42,70 @@ __global__ void identity_kernel(double* __restrict__ A, int n) {
 
 constexpr int kHgTx = 32, kHgTy = 8;
 
+// The hyper-gradient block of one point pair (row point j at p1, column point i at p2): acc[h], h in [0, dim], zero on
+// entry, receives sum_{m,nn} W[j*bs+m, i*bs+nn] * dK/d theta_h [j*bs+m, i*bs+nn], where Wf(row, col) returns the entry
+// of W = a a^T - K^-1.  Shared by the single-set and the list contraction kernels.
+template <class WF>
+__device__ __forceinline__ void hyper_grad_pair(const KernelSpec& spec, const double* p1, const double* p2, int j, int i,
+                                                const WF& Wf, double (&acc)[CMOE_MAX_DIM + 1]) {
+  const int dim = spec.dim, bs = 1 + spec.g;
+  const double r2 = weighted_sqdist(spec, p1, p2);
+  if (spec.kernel != CMOE_KERNEL_SQUARE_EXPONENTIAL) {
+    // value-value entry only (gpp_covariance.cpp:461-489)
+    const double W = Wf(j * bs, i * bs);
+    if (r2 == 0.0) {
+      acc[0] = W;
+    } else {
+      const double arg = kSqrt5 * sqrt(r2);
+      const double poly = arg + 5.0 / 3.0 * r2;
+      const double e = exp(-arg);
+      acc[0] = W * (1.0 + poly) * e;
+      for (int k = 0; k < dim; ++k) {
+        const double len = sqrt(spec.lsq[k]);
+        const double dl = (p1[k] - p2[k]) / len;
+        const double dr2 = -2.0 * dl * dl / len;
+        const double dr = 0.5 * dr2 / sqrt(r2);
+        acc[k + 1] = W * spec.alpha * e * (5.0 / 3.0 * dr2 - poly * kSqrt5 * dr);
+      }
+    }
+  } else {
+    // every entry is k * P, P in {1, u_a, -u_b, -u_a u_b + [a==b]/l_a^2}, u_a = (p2_a - p1_a)/l_a^2 (:245-317)
+    const double kv = spec.alpha * exp(-0.5 * r2);
+    for (int m = 0; m < bs; ++m) {
+      for (int nn = 0; nn < bs; ++nn) {
+        const int ta = m ? spec.derivs[m - 1] : -1, tb = nn ? spec.derivs[nn - 1] : -1;
+        const double ua = (ta >= 0) ? (p2[ta] - p1[ta]) / spec.lsq[ta] : 0.0;
+        const double ub = (tb >= 0) ? (p2[tb] - p1[tb]) / spec.lsq[tb] : 0.0;
+        double P;
+        if (ta < 0 && tb < 0) {
+          P = 1.0;
+        } else if (tb < 0) {
+          P = ua;
+        } else if (ta < 0) {
+          P = -ub;
+        } else {
+          P = -ua * ub + ((ta == tb) ? 1.0 / spec.lsq[ta] : 0.0);
+        }
+        const double W = Wf(j * bs + m, i * bs + nn);
+        acc[0] = fma(W, kv * P / spec.alpha, acc[0]);
+        for (int k = 0; k < dim; ++k) {
+          const double len = sqrt(spec.lsq[k]);
+          const double D = p1[k] - p2[k];
+          double dP = 0.0;
+          if (ta >= 0 && tb < 0 && ta == k) dP = -2.0 * ua / len;
+          if (ta < 0 && tb >= 0 && tb == k) dP = 2.0 * ub / len;
+          if (ta >= 0 && tb >= 0) {
+            if (ta == k) dP += 2.0 * ua * ub / len;
+            if (tb == k) dP += 2.0 * ua * ub / len;
+            if (ta == tb && ta == k) dP += -2.0 / (spec.lsq[ta] * len);
+          }
+          acc[k + 1] = fma(W, kv * P * (D / len) * (D / len) / len + kv * dP, acc[k + 1]);
+        }
+      }
+    }
+  }
+}
+
 // partial[cta][h], h in [0, dim]: 1/2 sum over this CTA's point pairs (row point j, column point i) of
 //   sum_{m,nn} W[j*bs+m, i*bs+nn] * dK/d theta_h [j*bs+m, i*bs+nn]
 __global__ void __launch_bounds__(kHgTx * kHgTy)
@@ -52,64 +120,8 @@ __global__ void __launch_bounds__(kHgTx * kHgTy)
   double acc[CMOE_MAX_DIM + 1];
   for (int h = 0; h < hd; ++h) acc[h] = 0.0;
   if (i < N && j < N) {
-    const double* p1 = X + static_cast<size_t>(j) * dim;
-    const double* p2 = X + static_cast<size_t>(i) * dim;
-    const double r2 = weighted_sqdist(spec, p1, p2);
-    if (spec.kernel != CMOE_KERNEL_SQUARE_EXPONENTIAL) {
-      // value-value entry only (gpp_covariance.cpp:461-489)
-      const double W = a[j * bs] * a[i * bs] - Kinv[static_cast<size_t>(i * bs) * n + j * bs];
-      if (r2 == 0.0) {
-        acc[0] = W;
-      } else {
-        const double arg = kSqrt5 * sqrt(r2);
-        const double poly = arg + 5.0 / 3.0 * r2;
-        const double e = exp(-arg);
-        acc[0] = W * (1.0 + poly) * e;
-        for (int k = 0; k < dim; ++k) {
-          const double len = sqrt(spec.lsq[k]);
-          const double dl = (p1[k] - p2[k]) / len;
-          const double dr2 = -2.0 * dl * dl / len;
-          const double dr = 0.5 * dr2 / sqrt(r2);
-          acc[k + 1] = W * spec.alpha * e * (5.0 / 3.0 * dr2 - poly * kSqrt5 * dr);
-        }
-      }
-    } else {
-      // every entry is k * P, P in {1, u_a, -u_b, -u_a u_b + [a==b]/l_a^2}, u_a = (p2_a - p1_a)/l_a^2 (:245-317)
-      const double kv = spec.alpha * exp(-0.5 * r2);
-      for (int m = 0; m < bs; ++m) {
-        for (int nn = 0; nn < bs; ++nn) {
-          const int ta = m ? spec.derivs[m - 1] : -1, tb = nn ? spec.derivs[nn - 1] : -1;
-          const double ua = (ta >= 0) ? (p2[ta] - p1[ta]) / spec.lsq[ta] : 0.0;
-          const double ub = (tb >= 0) ? (p2[tb] - p1[tb]) / spec.lsq[tb] : 0.0;
-          double P;
-          if (ta < 0 && tb < 0) {
-            P = 1.0;
-          } else if (tb < 0) {
-            P = ua;
-          } else if (ta < 0) {
-            P = -ub;
-          } else {
-            P = -ua * ub + ((ta == tb) ? 1.0 / spec.lsq[ta] : 0.0);
-          }
-          const int row = j * bs + m, col = i * bs + nn;
-          const double W = a[row] * a[col] - Kinv[static_cast<size_t>(col) * n + row];
-          acc[0] = fma(W, kv * P / spec.alpha, acc[0]);
-          for (int k = 0; k < dim; ++k) {
-            const double len = sqrt(spec.lsq[k]);
-            const double D = p1[k] - p2[k];
-            double dP = 0.0;
-            if (ta >= 0 && tb < 0 && ta == k) dP = -2.0 * ua / len;
-            if (ta < 0 && tb >= 0 && tb == k) dP = 2.0 * ub / len;
-            if (ta >= 0 && tb >= 0) {
-              if (ta == k) dP += 2.0 * ua * ub / len;
-              if (tb == k) dP += 2.0 * ua * ub / len;
-              if (ta == tb && ta == k) dP += -2.0 / (spec.lsq[ta] * len);
-            }
-            acc[k + 1] = fma(W, kv * P * (D / len) * (D / len) / len + kv * dP, acc[k + 1]);
-          }
-        }
-      }
-    }
+    hyper_grad_pair(spec, X + static_cast<size_t>(j) * dim, X + static_cast<size_t>(i) * dim, j, i,
+                    [&](int row, int col) { return a[row] * a[col] - Kinv[static_cast<size_t>(col) * n + row]; }, acc);
   }
   const int cta = blockIdx.y * gridDim.x + blockIdx.x;
   for (int h = 0; h < hd; ++h) {
@@ -181,11 +193,13 @@ __global__ void __launch_bounds__(kLmlCovThreads) lml_cov_kernel(const KernelSpe
 // One CTA per set: z = L^-1 r by blocked forward substitution over 64-row blocks (warp 0 solves the diagonal block out
 // of shared memory; then every thread updates its rows below, summing the block's products in ascending column order),
 // then  -1/2 z^T z - sum_i log L_ii - n/2 log 2 pi  with a fixed thread-to-row assignment and block_sum.  A set whose
-// factorisation failed (fail[set] != 0) gets -inf.
+// factorisation failed (fail[set] != 0) gets -inf.  With a_out, the kernel then goes on to a = L^-T z = K^-1 r by
+// blocked backward substitution (the value is computed before and does not depend on it): a_out[set][n].
 __global__ void __launch_bounds__(kLmlSolveThreads) lml_solve_kernel(const double* __restrict__ L, int n,
                                                                      const double* __restrict__ r,
                                                                      const int* __restrict__ fail,
-                                                                     double* __restrict__ out) {
+                                                                     double* __restrict__ out,
+                                                                     double* __restrict__ a_out) {
   extern __shared__ double lml_z[];         // [n] right-hand side -> solution
   double* D = lml_z + n;                    // [NB][NB + 1] diagonal block, D[c * (NB + 1) + row]
   __shared__ double scratch[kLmlSolveThreads / 32];
@@ -234,19 +248,274 @@ __global__ void __launch_bounds__(kLmlSolveThreads) lml_solve_kernel(const doubl
   zz = block_sum(zz, scratch);
   logdiag = block_sum(logdiag, scratch);
   if (tid == 0) out[set] = -0.5 * zz - logdiag - 0.5 * static_cast<double>(n) * kLog2Pi;
+  if (a_out == nullptr) return;
+  for (int k0 = ((n - 1) / NB) * NB; k0 >= 0; k0 -= NB) {
+    const int nb = min(NB, n - k0);
+    __syncthreads();  // the previous block's update of z and its reads of D are done
+    for (int e = tid; e < NB * NB; e += blockDim.x) {
+      const int rr = e % NB, c = e / NB;
+      if (rr < nb && c < nb && rr >= c) D[c * (NB + 1) + rr] = Ls[static_cast<size_t>(k0 + c) * n + k0 + rr];
+    }
+    __syncthreads();
+    if (tid < 32) {  // L_bb^T x = z_b, last row first; lane owns rows tid and tid + 32 of the block
+      const int r0 = tid, r1 = tid + 32;
+      double v0 = r0 < nb ? lml_z[k0 + r0] : 0.0, v1 = r1 < nb ? lml_z[k0 + r1] : 0.0;
+      for (int j = nb - 1; j >= 0; --j) {
+        const double xj = __shfl_sync(0xffffffffu, j < 32 ? v0 : v1, j & 31) / D[j * (NB + 1) + j];
+        if (r0 == j) v0 = xj;
+        if (r1 == j) v1 = xj;
+        if (r0 < j) v0 = fma(-D[r0 * (NB + 1) + j], xj, v0);
+        if (r1 < j) v1 = fma(-D[r1 * (NB + 1) + j], xj, v1);
+      }
+      if (r0 < nb) lml_z[k0 + r0] = v0;
+      if (r1 < nb) lml_z[k0 + r1] = v1;
+    }
+    __syncthreads();
+    for (int i = tid; i < k0; i += blockDim.x) {  // z_i -= sum_c L[k0 + c, i] z[k0 + c]
+      const double* Li = Ls + static_cast<size_t>(i) * n + k0;
+      double acc = 0.0;
+      for (int c = 0; c < nb; ++c) acc = fma(Li[c], lml_z[k0 + c], acc);
+      lml_z[i] -= acc;
+    }
+  }
+  __syncthreads();
+  for (int i = tid; i < n; i += blockDim.x) a_out[static_cast<size_t>(set) * n + i] = lml_z[i];
 }
 
-// Device workspace of cmoe_log_marginal_likelihood_list, one per host thread, kept for the device of the last call, so
-// that the calls of a sampler loop do not allocate (it grows to at most one chunk: kSampleWorkspaceBytes plus the
-// shared inputs, or one set if that is larger).
+// ---- hyper-parameter gradient at a list of sets (DESIGN.md K11) ----------------------------------------------------
+// K_s^-1 = L^-T L^-1 with L^-1 held row-major in its own n x n buffer per set (Linv[r * n + c] = (L^-1)_rc): its
+// diagonal 64 x 64 blocks by substitution, its off-diagonal blocks one block row at a time and K^-1 in one launch,
+// both as DMMA tile products (tile_mma64).  Only the lower triangle of L^-1 (and the zero upper triangle of its
+// diagonal blocks) is ever read.
+constexpr int kInvThreads = 128;
+
+// (L^-1)_bb = (L_bb)^-1 for every diagonal block b = blockIdx.x of every set: thread c solves column c by forward
+// substitution.  The whole 64 x 64 block is written, zeros above the diagonal.
+__global__ void __launch_bounds__(NB) tri_inv_diag_kernel(const double* __restrict__ L, int n,
+                                                          const int* __restrict__ fail, double* __restrict__ Linv) {
+  extern __shared__ double inv_smem[];
+  double (*S)[NB + 1] = reinterpret_cast<double (*)[NB + 1]>(inv_smem);            // L_bb, S[row][col]
+  double (*Xs)[NB + 1] = reinterpret_cast<double (*)[NB + 1]>(inv_smem + NB * (NB + 1));  // its inverse
+  const int set = blockIdx.z, tid = threadIdx.x;
+  if (fail[set] != 0) return;
+  const int k0 = blockIdx.x * NB, nb = min(NB, n - k0);
+  const double* Ls = L + static_cast<size_t>(set) * n * n;
+  for (int e = tid; e < NB * NB; e += blockDim.x) {
+    const int r = e % NB, c = e / NB;
+    S[r][c] = (r < nb && c < nb && r >= c) ? Ls[static_cast<size_t>(k0 + c) * n + k0 + r] : 0.0;
+  }
+  __syncthreads();
+  const int c = tid;
+  for (int r = 0; r < nb; ++r) {
+    double v = 0.0;
+    if (r == c) {
+      v = 1.0 / S[c][c];
+    } else if (r > c) {
+      double acc = 0.0;
+      for (int k = c; k < r; ++k) acc = fma(S[r][k], Xs[k][c], acc);
+      v = -acc / S[r][r];
+    }
+    Xs[r][c] = v;
+  }
+  __syncthreads();
+  double* Li = Linv + static_cast<size_t>(set) * n * n;
+  for (int e = tid; e < NB * NB; e += blockDim.x) {
+    const int cc = e % NB, r = e / NB;
+    if (r < nb && cc < nb) Li[static_cast<size_t>(k0 + r) * n + k0 + cc] = Xs[r][cc];
+  }
+}
+
+// Block row bi of L^-1 left of the diagonal, for every set: tile (bi, bj = blockIdx.x < bi)
+//   (L^-1)_{bi,bj} = -(L^-1)_{bi,bi} sum_{k=bj}^{bi-1} L_{bi,k} (L^-1)_{k,bj}
+// Block rows above bi are final (earlier launches).  Blocks k < bi are full 64-row blocks.
+__global__ void __launch_bounds__(kInvThreads) tri_inv_offdiag_kernel(const double* __restrict__ L, int n, int bi,
+                                                                      const int* __restrict__ fail,
+                                                                      double* __restrict__ Linv) {
+  extern __shared__ double inv_smem[];
+  const int set = blockIdx.z;
+  if (fail[set] != 0) return;
+  L += static_cast<size_t>(set) * n * n;
+  Linv += static_cast<size_t>(set) * n * n;
+  double* As = inv_smem;
+  double* Bs = inv_smem + NB * LDT;
+  const int row0 = bi * NB, col0 = blockIdx.x * NB, rows = min(NB, n - row0);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wm = (warp & 1) * 32, wn = (warp >> 1) * 32;
+  const int lr = lane >> 2, lc = lane & 3;
+  double acc[4][4][2];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
+  for (int k0 = col0; k0 < row0; k0 += NB) {
+    __syncthreads();  // the previous product's reads of As / Bs are done
+    for (int e = threadIdx.x; e < NB * NB; e += blockDim.x) {
+      const int x = e % NB, y = e / NB;
+      // As[k][r] = L[row0 + r, k0 + k] (column-major L), Bs[k][c] = L^-1[k0 + k, col0 + c] (row-major L^-1)
+      const double* src = L + static_cast<size_t>(k0 + y) * n + row0 + x;
+      cp_async8(As + y * LDT + x, x < rows ? src : L, x < rows);
+      cp_async8(Bs + y * LDT + x, Linv + static_cast<size_t>(k0 + y) * n + col0 + x, true);
+    }
+    cp_async_commit();
+    cp_async_wait<0>();
+    __syncthreads();
+    tile_mma64(As, Bs, acc, wm, wn, lr, lc);
+  }
+  __syncthreads();
+  // T = the sum above -> Bs[k][c]; (L^-1)_{bi,bi} -> As[k][r] = L^-1[row0 + r, row0 + k]
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        Bs[(wm + i * 8 + lr) * LDT + wn + j * 8 + lc * 2 + h] = acc[i][j][h];
+        acc[i][j][h] = 0.0;
+      }
+  for (int e = threadIdx.x; e < NB * NB; e += blockDim.x) {
+    const int k = e % NB, r = e / NB;
+    As[k * LDT + r] = (r < rows && k < rows) ? Linv[static_cast<size_t>(row0 + r) * n + row0 + k] : 0.0;
+  }
+  __syncthreads();
+  tile_mma64(As, Bs, acc, wm, wn, lr, lc);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int r = wm + i * 8 + lr;
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (r < rows) Linv[static_cast<size_t>(row0 + r) * n + col0 + wn + j * 8 + lc * 2 + h] = -acc[i][j][h];
+  }
+}
+
+// K^-1 = L^-T L^-1 on the lower 64 x 64 tiles (ti >= tj) of every set: sum over block rows k >= ti of
+// (L^-1)_{k,ti}^T (L^-1)_{k,tj}, written column-major over the factor (which is no longer needed).
+__global__ void __launch_bounds__(kInvThreads) inv_syrk_kernel(const double* __restrict__ Linv, int n,
+                                                               const int* __restrict__ fail,
+                                                               double* __restrict__ Kinv) {
+  extern __shared__ double inv_smem[];
+  const int set = blockIdx.z;
+  if (fail[set] != 0) return;
+  Linv += static_cast<size_t>(set) * n * n;
+  Kinv += static_cast<size_t>(set) * n * n;
+  double* As = inv_smem;
+  double* Bs = inv_smem + NB * LDT;
+  int ti, tj;
+  tri_tile(blockIdx.x, ti, tj);
+  const int row0 = ti * NB, col0 = tj * NB, rows = min(NB, n - row0), cols = min(NB, n - col0);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wm = (warp & 1) * 32, wn = (warp >> 1) * 32;
+  const int lr = lane >> 2, lc = lane & 3;
+  double acc[4][4][2];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
+  for (int k0 = row0; k0 < n; k0 += NB) {
+    const int kb = min(NB, n - k0);
+    __syncthreads();
+    for (int e = threadIdx.x; e < NB * NB; e += blockDim.x) {
+      const int x = e % NB, k = e / NB;
+      const double* src = Linv + static_cast<size_t>(k0 + k) * n;
+      const bool oka = k < kb && x < rows, okb = k < kb && x < cols;
+      cp_async8(As + k * LDT + x, oka ? src + row0 + x : Linv, oka);
+      cp_async8(Bs + k * LDT + x, okb ? src + col0 + x : Linv, okb);
+    }
+    cp_async_commit();
+    cp_async_wait<0>();
+    __syncthreads();
+    tile_mma64(As, Bs, acc, wm, wn, lr, lc);
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int r = wm + i * 8 + lr;
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int c = wn + j * 8 + lc * 2 + h;
+        if (r < rows && c < cols && row0 + r >= col0 + c) Kinv[static_cast<size_t>(col0 + c) * n + row0 + r] = acc[i][j][h];
+      }
+  }
+}
+
+// partial[set][cta][h], h in [0, dim]: hyper_grad_contract_kernel for every set, grid (point-pair tiles, 1, sets) with
+// CTA (bx, by) = (x % gx, x / gx).  The set's KernelSpec is staged in shared memory; W is read from the lower
+// triangle of K^-1 only.
+__global__ void __launch_bounds__(kHgTx * kHgTy)
+    lml_grad_contract_kernel(const KernelSpec* __restrict__ specs, const double* __restrict__ X, int N, int gx,
+                             const double* __restrict__ a, const double* __restrict__ Kinv,
+                             const int* __restrict__ fail, double* __restrict__ partial) {
+  __shared__ double scratch[kHgTx * kHgTy / 32];
+  __shared__ KernelSpec spec;
+  const int set = blockIdx.z, tid = threadIdx.x;
+  if (fail[set] != 0) return;
+  {
+    const auto* src = reinterpret_cast<const unsigned long long*>(specs + set);
+    auto* dst = reinterpret_cast<unsigned long long*>(&spec);
+    for (int w = tid; w < static_cast<int>(sizeof(KernelSpec) / sizeof(unsigned long long)); w += blockDim.x)
+      dst[w] = src[w];
+  }
+  __syncthreads();
+  const int dim = spec.dim, hd = dim + 1, n = N * (1 + spec.g);
+  const int j = (blockIdx.x % gx) * kHgTx + (tid % kHgTx);  // row point (fast)
+  const int i = (blockIdx.x / gx) * kHgTy + (tid / kHgTx);  // column point
+  const double* as = a + static_cast<size_t>(set) * n;
+  const double* Ks = Kinv + static_cast<size_t>(set) * n * n;
+  double acc[CMOE_MAX_DIM + 1];
+  for (int h = 0; h < hd; ++h) acc[h] = 0.0;
+  if (i < N && j < N) {
+    hyper_grad_pair(spec, X + static_cast<size_t>(j) * dim, X + static_cast<size_t>(i) * dim, j, i,
+                    [&](int row, int col) {
+                      const int lo = min(row, col), hi = max(row, col);
+                      return as[row] * as[col] - Ks[static_cast<size_t>(lo) * n + hi];
+                    },
+                    acc);
+  }
+  for (int h = 0; h < hd; ++h) {
+    const double s = block_sum(acc[h], scratch);
+    if (tid == 0) partial[(static_cast<size_t>(set) * gridDim.x + blockIdx.x) * hd + h] = 0.5 * s;
+    __syncthreads();
+  }
+}
+
+// One CTA per set, one thread per output: out[set][0] = value; out[set][1 + h] = the set's CTA partials in CTA order
+// (h <= dim), or 1/2 sum of a_r^2 - K^-1_rr over the rows r of observation type t in row order (h = dim + 1 + t).  A
+// failed set keeps its -inf value and gets zeros.
+__global__ void lml_grad_reduce_kernel(const double* __restrict__ values, const double* __restrict__ partial,
+                                       int nctas, const double* __restrict__ a, const double* __restrict__ Kinv, int n,
+                                       int hd, int bs, const int* __restrict__ fail, double* __restrict__ out) {
+  const int set = blockIdx.x, h = threadIdx.x, nh = hd + bs;
+  double* o = out + static_cast<size_t>(set) * (1 + nh);
+  if (h == 0) o[0] = values[set];
+  if (h >= nh) return;
+  double s = 0.0;
+  if (fail[set] == 0) {
+    if (h < hd) {
+      for (int c = 0; c < nctas; ++c) s += partial[(static_cast<size_t>(set) * nctas + c) * hd + h];
+    } else {
+      const double* as = a + static_cast<size_t>(set) * n;
+      const double* Ks = Kinv + static_cast<size_t>(set) * n * n;
+      for (int r = h - hd; r < n; r += bs) s += 0.5 * (as[r] * as[r] - Ks[static_cast<size_t>(r) * n + r]);
+    }
+  }
+  o[1 + h] = s;
+}
+
+// Device workspace of cmoe_log_marginal_likelihood_list and cmoe_grad_log_marginal_likelihood_list, one per host
+// thread, kept for the device of the last call, so that the calls of a sampler loop or a descent do not allocate (it
+// grows to at most one chunk: kSampleWorkspaceBytes plus the shared inputs, or one set if that is larger).
 struct LmlWork {
   int device = -1;
   cudaStream_t stream = nullptr;
   DevBuf<double> X, r, noise, K, stage, values;
+  DevBuf<double> Linv, a, partial, gout;  // gradient list only
   DevBuf<KernelSpec> specs;
   DevBuf<int> fail;
   void reset() {
     X.release(); r.release(); noise.release(); K.release(); stage.release(); values.release();
+    Linv.release(); a.release(); partial.release(); gout.release();
     specs.release();
     fail.release();
     if (stream) cudaStreamDestroy(stream);
@@ -322,11 +591,13 @@ extern "C" int cmoe_grad_log_marginal_likelihood(int kernel, double alpha, const
   return out;
 }
 
-extern "C" int cmoe_log_marginal_likelihood_list(int kernel, const double* hyperparameters, int num_sets,
-                                                 const double* points_sampled, const double* points_sampled_value,
-                                                 const int* derivatives, int num_derivatives, int dim,
-                                                 int num_sampled, int device, double* values, int* info) {
-  return guarded(info, [&] {
+namespace {
+
+// The body of both list calls: values[num_sets], and with grads != NULL also grads[num_sets][2 + dim + g].
+void lml_list(int kernel, const double* hyperparameters, int num_sets, const double* points_sampled,
+              const double* points_sampled_value, const int* derivatives, int num_derivatives, int dim,
+              int num_sampled, int device, double* values, double* grads) {
+  {
     CMOE_REQUIRE(num_sets >= 1, CMOE_ERR_BOUNDS, "num_sets must be >= 1");
     CMOE_REQUIRE(hyperparameters != nullptr && points_sampled != nullptr && points_sampled_value != nullptr &&
                      values != nullptr,
@@ -385,8 +656,12 @@ extern "C" int cmoe_log_marginal_likelihood_list(int kernel, const double* hyper
     LmlWork& w = lml_workspace(device);
     cudaStream_t s = w.stream;
     const int nsteps = (n + NB - 1) / NB;
-    const size_t per_set = sizeof(double) * (static_cast<size_t>(n) * n + static_cast<size_t>(nsteps) * NB * NB + b + 1) +
-                           sizeof(KernelSpec) + sizeof(int);
+    // the gradient adds L^-1 (n x n), a, the contraction's CTA partials and the [1 + nh] output row per set
+    const int gx = (N + kHgTx - 1) / kHgTx, nctas = gx * ((N + kHgTy - 1) / kHgTy);
+    size_t per_set = sizeof(double) * (static_cast<size_t>(n) * n + static_cast<size_t>(nsteps) * NB * NB + b + 1) +
+                     sizeof(KernelSpec) + sizeof(int);
+    if (grads)
+      per_set += sizeof(double) * (static_cast<size_t>(n) * n + n + static_cast<size_t>(nctas) * (dim + 1) + 1 + nh);
     const int chunk = static_cast<int>(std::max<size_t>(
         1, std::min<size_t>({kSampleWorkspaceBytes / per_set, static_cast<size_t>(num_sets),
                              static_cast<size_t>(kMaxChunkSets)})));
@@ -399,9 +674,23 @@ extern "C" int cmoe_log_marginal_likelihood_list(int kernel, const double* hyper
     w.fail.ensure(chunk);
     const size_t smem_cov = 2 * static_cast<size_t>(NB) * dim * sizeof(double);
     const size_t smem_solve = (static_cast<size_t>(n) + NB * (NB + 1)) * sizeof(double);
+    const size_t smem_inv = 2 * NB * LDT * sizeof(double), smem_diag = 2 * NB * (NB + 1) * sizeof(double);
     CMOE_CUDA(cudaFuncSetAttribute(lml_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    static_cast<int>(smem_solve)));
+    if (grads) {
+      w.Linv.ensure(static_cast<size_t>(chunk) * n * n);
+      w.a.ensure(static_cast<size_t>(chunk) * n);
+      w.partial.ensure(static_cast<size_t>(chunk) * nctas * (dim + 1));
+      w.gout.ensure(static_cast<size_t>(chunk) * (1 + nh));
+      CMOE_CUDA(cudaFuncSetAttribute(tri_inv_offdiag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     static_cast<int>(smem_inv)));
+      CMOE_CUDA(cudaFuncSetAttribute(inv_syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     static_cast<int>(smem_inv)));
+      CMOE_CUDA(cudaFuncSetAttribute(tri_inv_diag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     static_cast<int>(smem_diag)));
+    }
     const int t = nsteps;
+    std::vector<double> hout(grads ? static_cast<size_t>(chunk) * (1 + nh) : 0);
     for (int c0 = 0; c0 < num_sets; c0 += chunk) {
       const int nc = std::min(chunk, num_sets - c0);
       w.specs.upload(specs.data() + c0, nc, s);
@@ -412,11 +701,56 @@ extern "C" int cmoe_log_marginal_likelihood_list(int kernel, const double* hyper
       count_launch();
       CMOE_CUDA(cudaGetLastError());
       potrf_batched(w.K.p, n, nc, w.fail.p, w.stage, s);
-      lml_solve_kernel<<<nc, kLmlSolveThreads, smem_solve, s>>>(w.K.p, n, w.r.p, w.fail.p, w.values.p);
+      lml_solve_kernel<<<nc, kLmlSolveThreads, smem_solve, s>>>(w.K.p, n, w.r.p, w.fail.p, w.values.p,
+                                                                grads ? w.a.p : nullptr);
       count_launch();
       CMOE_CUDA(cudaGetLastError());
-      w.values.download(values + c0, nc, s);
+      if (!grads) {
+        w.values.download(values + c0, nc, s);
+        CMOE_CUDA(cudaStreamSynchronize(s));
+        continue;
+      }
+      tri_inv_diag_kernel<<<dim3(t, 1, nc), NB, smem_diag, s>>>(w.K.p, n, w.fail.p, w.Linv.p);
+      for (int bi = 1; bi < t; ++bi)
+        tri_inv_offdiag_kernel<<<dim3(bi, 1, nc), kInvThreads, smem_inv, s>>>(w.K.p, n, bi, w.fail.p, w.Linv.p);
+      inv_syrk_kernel<<<dim3(t * (t + 1) / 2, 1, nc), kInvThreads, smem_inv, s>>>(w.Linv.p, n, w.fail.p, w.K.p);
+      lml_grad_contract_kernel<<<dim3(nctas, 1, nc), kHgTx * kHgTy, 0, s>>>(w.specs.p, w.X.p, N, gx, w.a.p, w.K.p,
+                                                                           w.fail.p, w.partial.p);
+      lml_grad_reduce_kernel<<<nc, ((nh + 31) / 32) * 32, 0, s>>>(w.values.p, w.partial.p, nctas, w.a.p, w.K.p, n,
+                                                                  dim + 1, b, w.fail.p, w.gout.p);
+      count_launch(t + 3);
+      CMOE_CUDA(cudaGetLastError());
+      w.gout.download(hout.data(), static_cast<size_t>(nc) * (1 + nh), s);
       CMOE_CUDA(cudaStreamSynchronize(s));
+      for (int k = 0; k < nc; ++k) {
+        const double* o = hout.data() + static_cast<size_t>(k) * (1 + nh);
+        values[c0 + k] = o[0];
+        std::copy(o + 1, o + 1 + nh, grads + static_cast<size_t>(c0 + k) * nh);
+      }
     }
+  }
+}
+
+}  // namespace
+
+extern "C" int cmoe_log_marginal_likelihood_list(int kernel, const double* hyperparameters, int num_sets,
+                                                 const double* points_sampled, const double* points_sampled_value,
+                                                 const int* derivatives, int num_derivatives, int dim,
+                                                 int num_sampled, int device, double* values, int* info) {
+  return guarded(info, [&] {
+    lml_list(kernel, hyperparameters, num_sets, points_sampled, points_sampled_value, derivatives, num_derivatives,
+             dim, num_sampled, device, values, nullptr);
+  });
+}
+
+extern "C" int cmoe_grad_log_marginal_likelihood_list(int kernel, const double* hyperparameters, int num_sets,
+                                                      const double* points_sampled,
+                                                      const double* points_sampled_value, const int* derivatives,
+                                                      int num_derivatives, int dim, int num_sampled, int device,
+                                                      double* values, double* grads, int* info) {
+  return guarded(info, [&] {
+    CMOE_REQUIRE(grads != nullptr, CMOE_ERR_INVALID_VALUE, "NULL argument");
+    lml_list(kernel, hyperparameters, num_sets, points_sampled, points_sampled_value, derivatives, num_derivatives,
+             dim, num_sampled, device, values, grads);
   });
 }

@@ -797,4 +797,60 @@ int cmoe_ei_gradient_descent_mcmc(const cmoe_gp* const* gps, int num_gp, const c
   });
 }
 
+// MultistartGradientDescentHyperparameterOptimization (gpp_model_selection.hpp:1063-1103) with one thread: the best
+// start by InitializeBestKnownPoint (:911-930), then GradientDescentOptimizer::Optimize from EVERY start (no top-20
+// screening), then the arg-max of MultistartOptimize (gpp_optimization.hpp:1504-1545).  The point is the set itself,
+// so the descent runs on one "point" of nh coordinates over the linear-space box.
+int cmoe_hyperparameter_gradient_descent(int kernel, const cmoe_gd_params* gd_params, const double* bounds,
+                                         const double* starts, int num_starts, const double* points_sampled,
+                                         const double* points_sampled_value, const int* derivatives,
+                                         int num_derivatives, int dim, int num_sampled, int device,
+                                         double* best_point, double* best_value, int* found_flag,
+                                         double* end_points, double* end_values, int* info) {
+  return guarded(info, [&] {
+    CMOE_REQUIRE(num_starts >= 1, CMOE_ERR_BOUNDS, "num_multistarts must be > 1");
+    CMOE_REQUIRE(gd_params != nullptr && bounds != nullptr && starts != nullptr && best_point != nullptr,
+                 CMOE_ERR_INVALID_VALUE, "NULL argument");
+    CMOE_REQUIRE(dim >= 1 && dim <= CMOE_MAX_DIM, CMOE_ERR_BOUNDS, "dim must be in [1, CMOE_MAX_DIM]");
+    CMOE_REQUIRE(num_derivatives >= 0 && num_derivatives <= dim, CMOE_ERR_BOUNDS, "num_derivatives out of range");
+    const int nh = 2 + dim + num_derivatives;
+    validate_bounds(bounds, nh);
+    BatchEval eval = [&](const double* pts, int nc, double* values, double* grads) {
+      int linfo = 0;
+      const int rc = grads ? cmoe_grad_log_marginal_likelihood_list(kernel, pts, nc, points_sampled,
+                                                                    points_sampled_value, derivatives, num_derivatives,
+                                                                    dim, num_sampled, device, values, grads, &linfo)
+                           : cmoe_log_marginal_likelihood_list(kernel, pts, nc, points_sampled, points_sampled_value,
+                                                               derivatives, num_derivatives, dim, num_sampled, device,
+                                                               values, &linfo);
+      if (rc != CMOE_OK) throw Error(rc, cmoe_last_error(), linfo);
+    };
+    std::vector<double> start_v(num_starts), fin_v(num_starts), fin_p(static_cast<size_t>(num_starts) * nh);
+    eval(starts, num_starts, start_v.data(), nullptr);
+    // InitializeBestKnownPoint: -inf and the first start, strict `<`
+    double init_best = -std::numeric_limits<double>::infinity();
+    int ib = 0;
+    for (int i = 0; i < num_starts; ++i)
+      if (init_best < start_v[i]) {
+        init_best = start_v[i];
+        ib = i;
+      }
+    gradient_descent_batch(eval, *gd_params, bounds, 1, nh, starts, num_starts, fin_v.data(), fin_p.data());
+    // MultistartOptimize: the running best starts at init_best; an end value replaces it only if strictly larger
+    double best = init_best;
+    int bi = -1;
+    for (int i = 0; i < num_starts; ++i)
+      if (best < fin_v[i]) {
+        best = fin_v[i];
+        bi = i;
+      }
+    const double* bp = (bi >= 0) ? fin_p.data() + static_cast<size_t>(bi) * nh : starts + static_cast<size_t>(ib) * nh;
+    std::copy(bp, bp + nh, best_point);
+    if (best_value) *best_value = best;
+    if (found_flag) *found_flag = bi >= 0 ? 1 : 0;
+    if (end_points) std::copy(fin_p.begin(), fin_p.end(), end_points);
+    if (end_values) std::copy(fin_v.begin(), fin_v.end(), end_values);
+  });
+}
+
 }  // extern "C"

@@ -37,25 +37,6 @@ constexpr int kRowThreads = 256;
 
 __device__ __forceinline__ int set_row_type(int local, const int* derivs) { return local ? derivs[local - 1] : -1; }
 
-// acc += As^T-tile * Bs-tile over one 64-deep chunk: warp (wm, wn) owns a 32 x 32 sub-tile, 2 x 4 m16n8k4 products per
-// k-step (the fragment layout of dmma_tile_kernel in linalg.cu).  As / Bs: [k][LDT], element (k, row).
-__device__ __forceinline__ void tile_mma64(const double* As, const double* Bs, double (&acc)[4][4][2], int wm, int wn,
-                                           int lr, int lc) {
-#pragma unroll 4
-  for (int kk = 0; kk < NB; kk += 4) {
-    double a[4], b[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) a[i] = As[(kk + lc) * LDT + wm + i * 8 + lr];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) b[j] = Bs[(kk + lc) * LDT + wn + j * 8 + lr];
-#pragma unroll
-    for (int i = 0; i < 4; i += 2)
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        dmma_m16n8k4(acc[i][j][0], acc[i][j][1], acc[i + 1][j][0], acc[i + 1][j][1], a[i], a[i + 1], b[j]);
-  }
-}
-
 // --------------------------------------------------------------------------------------------------------------
 // Latin hypercube: one CTA per (dimension, set).  The strata of a dimension are permuted by ranking Philox keys (ties
 // broken by point index); point j lies in stratum rank_j at offset u_j:  x = min + edge rank_j + edge u_j,  clamped to

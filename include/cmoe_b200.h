@@ -117,6 +117,28 @@ int cmoe_log_marginal_likelihood_list(int kernel, const double* hyperparameters,
                                       const double* points_sampled, const double* points_sampled_value,
                                       const int* derivatives, int num_derivatives, int dim, int num_sampled, int device,
                                       double* values, int* info);
+/* Value and hyper-parameter gradient at num_sets sets in one device call (DESIGN.md K11), in the layout and with the
+ * size contract and checks of cmoe_log_marginal_likelihood_list.  values[num_sets] are bit for bit that call's;
+ * grads[num_sets][2 + dim + g] = d log p / d (alpha, lengths..., noise by observation type), defined as
+ * cmoe_grad_log_marginal_likelihood's (1e-6 added to the noise; the Matern-5/2 value-entry-only quirk).  A set whose
+ * Cholesky fails gets value -inf and a zero gradient.  A set's outputs do not depend on the rest of the list. */
+int cmoe_grad_log_marginal_likelihood_list(int kernel, const double* hyperparameters, int num_sets,
+                                           const double* points_sampled, const double* points_sampled_value,
+                                           const int* derivatives, int num_derivatives, int dim, int num_sampled,
+                                           int device, double* values, double* grads, int* info);
+/* Maximum-likelihood fit of the hyper-parameters by restarted gradient ascent from every one of num_starts starts
+ * [num_starts][nh], nh = 2 + dim + g, on the linear-space box bounds[nh][2]: MultistartGradientDescentHyperparameter-
+ * Optimization (gpp_model_selection.hpp:1063-1103) with one thread, every start descending in lock step with one
+ * cmoe_grad_log_marginal_likelihood_list call per step.  best_point[nh] / best_value: the best start (first maximum of
+ * the start values) unless some end value beats it, then the first maximum of the end values; found_flag: whether one
+ * did.  end_points[num_starts][nh] / end_values[num_starts] (each may be NULL): every start's result.  Unlike the
+ * reference, a set whose Cholesky fails mid-descent has a zero gradient, so that start stops where it is. */
+int cmoe_hyperparameter_gradient_descent(int kernel, const cmoe_gd_params* gd_params, const double* bounds,
+                                         const double* starts, int num_starts, const double* points_sampled,
+                                         const double* points_sampled_value, const int* derivatives,
+                                         int num_derivatives, int dim, int num_sampled, int device,
+                                         double* best_point, double* best_value, int* found_flag,
+                                         double* end_points, double* end_values, int* info);
 /* Run-time switches between kernel generations (also read once from the environment: CMOE_LEGACY_LINALG, CMOE_COV_TMA):
  *   "legacy_linalg" 1 = round-1 launch-per-step Cholesky / chained trsv for large n (default 0: cooperative kernels);
  *   "cov_tma"       1 = TMA / DMMA covariance build with tensor-map tile stores (default 0: LDGSTS kernel, faster at d ~ 10). */
