@@ -537,6 +537,7 @@ struct cmoe_kg_plan {
   int Q = 0, stride = 0;  // rows of the union block U*(1+g); doubles per training point in the operand pack
   bool use_smem = true;
   bool smem_fits = true;      // the operand pack fits in shared memory
+  KgMcLaunch mc_big = nullptr;  // the entry's exp_tab2k build, where it runs at the same residency (shared-memory path)
   double rmax_static = 0.0;   // max scaled norm of training / pending / discrete points (see kFastPathRadius)
   int chunk = 0;
   // static device data
@@ -636,6 +637,8 @@ void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
   cudaEventRecord(pl.mc_events[ev_idx].first, s);
   if (gen) {
     pl.entry->mc_gen(prm, dim3(chunks, nb), 0, s);
+  } else if (pl.use_smem && pl.mc_big) {
+    pl.mc_big(prm, dim3(chunks, nb), smem_mc, s);
   } else {
     pl.entry->mc(prm, dim3(chunks, nb), smem_mc, s);
   }
@@ -807,8 +810,14 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     // the fast-path kernel's residency as the occupancy API reports it (2 CTAs per SM for the tile instantiation at the
     // bench shape); the general path hands its work items to a persistent grid and keeps 3 per SM, the count its
     // scratch slots are sized for.
+    // The tile instantiation has a second build whose tile rounds use the 2048-entry exp table (16 KB more shared
+    // memory per CTA); it is taken on the shared-memory path wherever it keeps the residency of the 64-entry build, so
+    // that neither the fast path's N range nor its occupancy shrinks.
     {
       const int per_sm = spec.g == 0 ? std::max(1, pl->entry->mc_ctas_per_sm(pl->use_smem ? smem_need : 0)) : 3;
+      if (pl->smem_fits && pl->entry->mc_big &&
+          pl->entry->mc_big_ctas_per_sm(smem_need) >= std::max(1, pl->entry->mc_ctas_per_sm(smem_need)))
+        pl->mc_big = pl->entry->mc_big;
       const long long target_ctas = 8LL * sms * per_sm;
       long long chunk = (static_cast<long long>(pl->batch) * num_mc + target_ctas - 1) / target_ctas;
       chunk = std::max<long long>(2 * kMcThreads, std::min<long long>(chunk, 16 * kMcThreads));

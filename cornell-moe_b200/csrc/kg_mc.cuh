@@ -131,6 +131,43 @@ __device__ __forceinline__ double exp_tab(double t) {
   const int k = max(n >> 6, -1000);
   return __hiloint2double(__double2hiint(p) + (k << 20), __double2loint(p));
 }
+// exp(t) = 2^k * 2^(i/2048) * e^r with |r| <= ln2/4096: 2048-entry table (16 KB of shared memory) + degree-3 Taylor
+// polynomial (truncation r^4/24 <= 3.4e-17 relative).  8 FP64-pipe instructions.  Same range contract as exp_tab
+// (kFastPathRadius), no per-call guard: n = round(t 2048 / ln2) no longer fits the low word for |t| >= 7.3e5, so the
+// exponent k = n >> 11 is taken from both words of the shifted double with one funnel shift (the shift's bias
+// 2^51 >> 11 = 2^40 vanishes mod 2^32); k is exact for |t| < 2^31 ln2 = 1.5e9 and clamped on the integer side like
+// exp_tab's.  Used by the tile rounds of kg_mc_kernel<SE,8,8> where its operands leave room for the table
+// (KgDispatchEntry::mc_big); measured max relative error 3.0e-16 over [-690, 1] like exp_tab
+// (profiles/exp_accuracy.py), exp(0) = 1 exactly.
+__device__ const double kExp2Table2k[2048] = {
+#include "exp2_table2048.inc"
+};
+__shared__ double g_exp_tab2k[2048];
+__device__ __forceinline__ void exp_table2k_stage() {
+  for (int i = threadIdx.x; i < 2048; i += blockDim.x) g_exp_tab2k[i] = kExp2Table2k[i];
+  __syncthreads();
+}
+__device__ __forceinline__ double exp_tab2k(double t) {
+  const double kShift = 6755399441055744.0;
+  double nf = fma(t, 2048.0 * 1.4426950408889634, kShift);
+  const int lo = __double2loint(nf), hi = __double2hiint(nf);
+  nf -= kShift;
+  double r = fma(nf, -6.93147180369123816490e-01 / 2048.0, t);
+  r = fma(nf, -1.90821492927058770002e-10 / 2048.0, r);
+  double p = 1.6666666666666666e-01;
+  p = fma(p, r, 0.5);
+  p = fma(p, r, 1.0);
+  p = fma(p, r, 1.0);
+  p *= g_exp_tab2k[lo & 2047];
+  const int k = max(static_cast<int>(__funnelshift_r(static_cast<unsigned>(lo), static_cast<unsigned>(hi), 11)), -1000);
+  return __hiloint2double(__double2hiint(p) + (k << 20), __double2loint(p));
+}
+// the exp of the tile rounds: exp_tab2k where the kernel staged the 2048-entry table (BIG), else exp_tab
+template <bool BIG>
+__device__ __forceinline__ double exp_row(double t) {
+  if (BIG) return exp_tab2k(t);
+  return exp_tab(t);
+}
 template <bool TAB>
 __device__ __forceinline__ double exp_sel(double t) {
   if (TAB) return exp_tab(t);
@@ -328,7 +365,7 @@ __device__ __forceinline__ void tile_mma(double (&acc)[4], const double (&f)[(W 
 // POINT round (SquareExponential) over the training rows: S0 = sum_j a_j k_j and s_d = sum_j a_j k_j X~_jd of every
 // lane's query point xq (hq = -|xq|^2 / 2).  One sweep over the rows serves both halves: a block's B fragments and
 // (e_j, beta_j) are loaded once and feed the products of samples 0-15 and 16-31.
-template <int DIM, int QP>
+template <int DIM, int QP, bool BIG>
 __device__ __forceinline__ void tile_posterior(const double* __restrict__ Xt, const double* __restrict__ Pk, int N,
                                                const double (&xq)[DIM], const double (&c)[QP], double hq, double& S0,
                                                double (&s)[DIM]) {
@@ -372,7 +409,7 @@ __device__ __forceinline__ void tile_posterior(const double* __restrict__ Xt, co
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const double ai = ((i & 1) ? r.v1 : r.v0) ? a[i] : 0.0;
-        const double kv = exp_tab(dot[i] + hqr[h][i >> 1]);
+        const double kv = exp_row<BIG>(dot[i] + hqr[h][i >> 1]);
         s0[h][i >> 1] = fma(ai, kv, s0[h][i >> 1]);
         w[i] = ai * kv;
       }
@@ -407,7 +444,7 @@ __device__ __forceinline__ void tile_posterior(const double* __restrict__ Xt, co
 }
 
 // mu+(xq) - m  and  the scaled-gradient accumulators, for one query point (scaled coordinates xq).
-template <int KERNEL, int DIM, int QP, bool SMEM, bool TILE = false>
+template <int KERNEL, int DIM, int QP, bool SMEM, bool TILE = false, bool BIG = false>
 __device__ __forceinline__ void eval_posterior(const double* __restrict__ Xt, const double* __restrict__ Pk,
                                                const double* __restrict__ Xu, int N, int U, double alpha,
                                                const double (&xq)[DIM], const double (&c)[QP], double& S0, double& SB,
@@ -422,7 +459,7 @@ __device__ __forceinline__ void eval_posterior(const double* __restrict__ Xt, co
 #pragma unroll
   for (int d = 0; d < DIM; ++d) s[d] = 0.0;
   static_assert(!TILE || KERNEL == CMOE_KERNEL_SQUARE_EXPONENTIAL, "the tile path is SquareExponential only");
-  if (TILE) tile_posterior<DIM, QP>(Xt, Pk, N, xq, c, hq, S0, s);
+  if (TILE) tile_posterior<DIM, QP, BIG>(Xt, Pk, N, xq, c, hq, S0, s);
 #pragma unroll 2
   for (int j = 0; j < (TILE ? 0 : N); ++j) {
     const double* xj = Xt + j * DIM;
@@ -495,7 +532,7 @@ constexpr int kLineBatch = 8;  // trial step sizes per batch (6 measured +1.5 %,
 // with hq = -|x~|^2 / 2 and xga = -a_min x~ . g~.  Unlike tile_posterior, the halves sweep the rows one after the other:
 // one sweep for both (twice the 16 trial sums and the fragments live) measured slower on the H100, by 1.8 % per bench
 // step even with the lane state parked in shared memory to keep it from spilling (DESIGN.md K6).
-template <int DIM, int QP>
+template <int DIM, int QP, bool BIG>
 __device__ __forceinline__ void tile_line(const double* __restrict__ Xt, const double* __restrict__ Pk, int N,
                                           const double (&xr)[DIM], const double (&gr)[DIM], const double* inv_len,
                                           double alpha_min, const double (&c)[QP], double hq, double xga,
@@ -532,8 +569,8 @@ __device__ __forceinline__ void tile_line(const double* __restrict__ Xt, const d
         const bool v = (i & 1) ? r.v1 : r.v0;
         const double pj = v ? p[i] : 0.0;
         pm[i >> 1] = max(pm[i >> 1], __double2hiint(pj) & 0x7fffffff);
-        const double w = (v ? a[i] : 0.0) * exp_tab(dot[i] + ((i < 2) ? hq0 : hq1));
-        double G = exp_tab(pj);
+        const double w = (v ? a[i] : 0.0) * exp_row<BIG>(dot[i] + ((i < 2) ? hq0 : hq1));
+        double G = exp_row<BIG>(pj);
 #pragma unroll
         for (int k = KB - 1; k >= 0; --k) {
           Sp[i >> 1][k] = fma(w, G, Sp[i >> 1][k]);
@@ -558,7 +595,7 @@ __device__ __forceinline__ void tile_line(const double* __restrict__ Xt, const d
   }
 }
 
-template <int DIM, int QP, bool SMEM, bool TILE = false>
+template <int DIM, int QP, bool SMEM, bool TILE = false, bool BIG = false>
 __device__ __forceinline__ void eval_line(const double* __restrict__ Xt, const double* __restrict__ Pk,
                                           const double* __restrict__ Xu, int N, int U, const double (&xb)[DIM],
                                           const double (&gt)[DIM], const double (&c)[QP], double alpha_min,
@@ -632,7 +669,7 @@ __device__ __forceinline__ void eval_line(const double* __restrict__ Xt, const d
     }
   }
   // tile path: the training rows last, so that the scaled operands above are dead during the row loop
-  if (TILE) tile_line<DIM, QP>(Xt, Pk, N, xr, gr, inv_len, alpha_min, c, hq, xga, S, pmax_hi);
+  if (TILE) tile_line<DIM, QP, BIG>(Xt, Pk, N, xr, gr, inv_len, alpha_min, c, hq, xga, S, pmax_hi);
 }
 
 // Batched backtracking for the Matern-5/2 kernel.  No factorisation along the line here, but the trial points
@@ -1235,7 +1272,7 @@ enum : int { ST_FETCH = 0, ST_INIT = 1, ST_TRIAL = 2, ST_LIMIT = 3, ST_DONE = 4,
 // observations a sample's start evaluation comes from the start-point table (start_from_table) when the lane takes the
 // sample, so a new sample's first round is a LINE round, in phase with the lanes that continue; only the general path
 // (GEN) spends a POINT round on it (ST_INIT).
-template <int KERNEL, int DIM, int QP, bool SMEM, bool GEN, bool WIDE = false>
+template <int KERNEL, int DIM, int QP, bool SMEM, bool GEN, bool WIDE = false, bool BIG = false>
 __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* __restrict__ Xt,
                                            const double* __restrict__ Pk, const double* __restrict__ Xu, int cand,
                                            int s_begin, int s_end, int* next_sample, double* aw = nullptr,
@@ -1369,8 +1406,8 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
         eval_line_gen<DIM, QP, SMEM, WIDE>(prm, Xt, Pk, Xu, xt, gt, aw, ring, cl, alpha_n * (1.0 / kTop), S,
                                reinterpret_cast<double (&)[kLineBatch]>(T), pmax_hi);
       } else {
-        eval_line<DIM, QP, SMEM, TILE>(Xt, Pk, Xu, N, U, xt, gt, c, alpha_n * (1.0 / kTop), S, pmax_hi, xb, gb,
-                                        prm.inv_len);
+        eval_line<DIM, QP, SMEM, TILE, BIG>(Xt, Pk, Xu, N, U, xt, gt, c, alpha_n * (1.0 / kTop), S, pmax_hi, xb,
+                                             gb, prm.inv_len);
       }
       if (state == ST_LINE) {
         n_line += 1;
@@ -1437,7 +1474,7 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
             }
         }
       } else {
-        eval_posterior<KERNEL, DIM, QP, SMEM, TILE>(Xt, Pk, Xu, N, U, prm.alpha, xq, c, S0, SB, s);
+        eval_posterior<KERNEL, DIM, QP, SMEM, TILE, BIG>(Xt, Pk, Xu, N, U, prm.alpha, xq, c, S0, SB, s);
       }
       if (state == ST_INIT || state == ST_TRIAL || state == ST_LIMIT) {
         n_evals += 1;
@@ -1566,9 +1603,13 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
   }
 }
 
-template <int KERNEL, int DIM, int QP>
+// BIG: the tile rounds use exp_tab2k, whose 2048-entry table takes 16 KB of static shared memory next to the operands.
+// Only the tile instantiation has a BIG build.  The host launches it on the shared-memory path only, where it does not
+// lower the residency (cmoe_kg_plan_create), so the BIG build has no global-memory branch.
+template <int KERNEL, int DIM, int QP, bool BIG = false>
 __global__ void __launch_bounds__(kMcThreads, (kg_mc_min_blocks<KERNEL, DIM, QP>()))
     kg_mc_kernel(const __grid_constant__ KgMcParams prm) {
+  static_assert(!BIG || kg_tile_path<KERNEL, DIM, QP>(), "only the tile rounds use the 2048-entry table");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ uint64_t mbar;
   __shared__ int next_sample;
@@ -1581,7 +1622,8 @@ __global__ void __launch_bounds__(kMcThreads, (kg_mc_min_blocks<KERNEL, DIM, QP>
   const double* gXu = prm.Xu + static_cast<size_t>(cand) * U * (DIM + 2);
   if (threadIdx.x == 0) next_sample = s_begin + blockDim.x;
   exp_table_stage();
-  if (prm.use_smem) {
+  if (BIG) exp_table2k_stage();
+  if (BIG || prm.use_smem) {
     // stage the per-candidate operands with TMA bulk copies (UBLKCP) signalled through an mbarrier
     double* sXt = reinterpret_cast<double*>(smem_raw);
     double* sPk = sXt + static_cast<size_t>(N) * DIM;
@@ -1597,7 +1639,7 @@ __global__ void __launch_bounds__(kMcThreads, (kg_mc_min_blocks<KERNEL, DIM, QP>
       tma_bulk_g2s(sXu, gXu, bU, &mbar);
     }
     mbar_wait(&mbar, 0);
-    kg_mc_body<KERNEL, DIM, QP, true, false>(prm, sXt, sPk, sXu, cand, s_begin, s_end, &next_sample);
+    kg_mc_body<KERNEL, DIM, QP, true, false, false, BIG>(prm, sXt, sPk, sXu, cand, s_begin, s_end, &next_sample);
   } else {
     __syncthreads();
     kg_mc_body<KERNEL, DIM, QP, false, false>(prm, gXt, gPk, gXu, cand, s_begin, s_end, &next_sample);
@@ -1827,6 +1869,7 @@ __global__ void __launch_bounds__(128) kg_acc_gen_kernel(const __grid_constant__
 // launchers instantiated per (DIM) translation unit
 using KgMcLaunch = void (*)(const KgMcParams&, dim3 grid, size_t smem, cudaStream_t s);
 using KgAccLaunch = void (*)(const KgAccParams&, dim3 grid, cudaStream_t s);
+using KgCtasPerSm = int (*)(size_t operands);
 struct KgDispatchEntry {
   int kernel, dim, qp;
   KgMcLaunch mc;      // g == 0 fast path (TMA-staged operands)
@@ -1835,26 +1878,41 @@ struct KgDispatchEntry {
   KgAccLaunch acc_gen;  // general path; null where mc_gen is
   size_t (*smem_bytes)(int N, int U);
   bool wide = false;  // general path for 9 <= g <= 31 only (mc and acc are null)
-  int (*mc_ctas_per_sm)(size_t operands) = nullptr;  // residency of mc (null where mc is)
+  KgCtasPerSm mc_ctas_per_sm = nullptr;  // residency of mc (null where mc is)
+  // the build of mc whose tile rounds use exp_tab2k (shared-memory path only) and its residency; null but for the tile
+  // instantiation
+  KgMcLaunch mc_big = nullptr;
+  KgCtasPerSm mc_big_ctas_per_sm = nullptr;
 };
 void register_kg_entries(const KgDispatchEntry* entries, int count);
 // g: derivative observations per point; entries with g <= 8 never dispatch to a wide entry, g > 8 only to one
 const KgDispatchEntry* find_kg_entry(int kernel, int dim, int Q, int g);
 
-template <int KERNEL, int DIM, int QP>
+template <int KERNEL, int DIM, int QP, bool BIG = false>
 void launch_kg_mc(const KgMcParams& p, dim3 grid, size_t smem, cudaStream_t s) {
   // function attributes are per device: set on every launch (cheap), never cached process-wide
-  cudaFuncSetAttribute(kg_mc_kernel<KERNEL, DIM, QP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  kg_mc_kernel<KERNEL, DIM, QP><<<grid, kMcThreads, smem, s>>>(p);
+  cudaFuncSetAttribute(kg_mc_kernel<KERNEL, DIM, QP, BIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  kg_mc_kernel<KERNEL, DIM, QP, BIG><<<grid, kMcThreads, smem, s>>>(p);
 }
 // resident CTAs of kg_mc_kernel per SM on the current device with `smem` bytes of staged operands (0: global memory)
-template <int KERNEL, int DIM, int QP>
+template <int KERNEL, int DIM, int QP, bool BIG = false>
 int kg_mc_ctas_per_sm(size_t smem) {
-  CMOE_CUDA(
-      cudaFuncSetAttribute(kg_mc_kernel<KERNEL, DIM, QP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  CMOE_CUDA(cudaFuncSetAttribute(kg_mc_kernel<KERNEL, DIM, QP, BIG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 200 * 1024));
   int per_sm = 0;
-  CMOE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kg_mc_kernel<KERNEL, DIM, QP>, kMcThreads, smem));
+  CMOE_CUDA(
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kg_mc_kernel<KERNEL, DIM, QP, BIG>, kMcThreads, smem));
   return per_sm;
+}
+template <int KERNEL, int DIM, int QP>
+constexpr KgMcLaunch kg_mc_big_launch() {
+  if constexpr (kg_tile_path<KERNEL, DIM, QP>()) return &launch_kg_mc<KERNEL, DIM, QP, true>;
+  return nullptr;
+}
+template <int KERNEL, int DIM, int QP>
+constexpr KgCtasPerSm kg_mc_big_ctas_per_sm() {
+  if constexpr (kg_tile_path<KERNEL, DIM, QP>()) return &kg_mc_ctas_per_sm<KERNEL, DIM, QP, true>;
+  return nullptr;
 }
 template <int KERNEL, int DIM, int QP, bool WIDE = false>
 void launch_kg_mc_gen(const KgMcParams& p, dim3, size_t, cudaStream_t s) {
@@ -1890,12 +1948,13 @@ size_t kg_smem_bytes(int N, int U) {
 #define CMOE_KG_ENTRY(K, D, Q)                                                                                  \
   {                                                                                                             \
     K, D, Q, &launch_kg_mc<K, D, Q>, nullptr, &launch_kg_acc<K, D, Q>, nullptr, &kg_smem_bytes<D, Q>, false,     \
-        &kg_mc_ctas_per_sm<K, D, Q>                                                                              \
+        &kg_mc_ctas_per_sm<K, D, Q>, kg_mc_big_launch<K, D, Q>(), kg_mc_big_ctas_per_sm<K, D, Q>()                \
   }
 #define CMOE_KG_ENTRY_GEN(K, D, Q)                                                                                \
   {                                                                                                               \
     K, D, Q, &launch_kg_mc<K, D, Q>, &launch_kg_mc_gen<K, D, Q>, &launch_kg_acc<K, D, Q>, &launch_kg_acc_gen<K, D, Q>, \
-        &kg_smem_bytes<D, Q>, false, &kg_mc_ctas_per_sm<K, D, Q>                                                   \
+        &kg_smem_bytes<D, Q>, false, &kg_mc_ctas_per_sm<K, D, Q>, kg_mc_big_launch<K, D, Q>(),                     \
+        kg_mc_big_ctas_per_sm<K, D, Q>()                                                                            \
   }
 // union-row counts: 2, 4, 8, 16, 24, 32 (24 serves config 4: q = 4 with 4 derivative observations -> 20 rows; the
 // 32-wide instantiation spilled ~1.5 KB per thread there)
