@@ -415,6 +415,40 @@ def hyperparameter_gradient_descent(kernel, gd, bounds, starts, X, y, derivs=Non
     return best, best_v.value, bool(found.value), ends, end_v
 
 
+class MCMCTable(ctypes.Structure):
+    """cmoe_mcmc_table: host-supplied random numbers of hyperparameter_mcmc, each [num_steps, num_walkers]."""
+    _fields_ = [("z_uniform", _dp), ("partner", _ip), ("accept_uniform", _dp)]
+
+
+def hyperparameter_mcmc(kernel, p0, X, y, num_steps, derivs=None, noisy=True, default_prior=True, seed=0, first_step=0,
+                        table=None, device=0):
+    """cmoe_hyperparameter_mcmc (DESIGN.md K12): num_steps steps of emcee 2.2.1's stretch-move ensemble sampler on the
+    log-probability of GaussianProcessLogLikelihoodMCMC.compute_log_likelihood, from the walkers ``p0`` [num_walkers,
+    2 + dim + g] (log scale), in one device call.  ``table`` = (z_uniform, partner, accept_uniform), each [num_steps,
+    num_walkers], replaces the Philox draws.  Returns (positions [num_walkers, 2 + dim + g], lnprob [num_walkers])."""
+    X = _f64(X)
+    N, dim = X.shape
+    derivs = _i32(derivs)
+    nh = 2 + dim + derivs.size
+    P = _f64(p0).reshape(-1, nh)
+    W = P.shape[0]
+    pos, lnp = np.empty(P.shape), np.empty(W)
+    tab, keep = None, None
+    if table is not None:
+        keep = (_f64(table[0]).ravel(), _i32(table[1]).ravel(), _f64(table[2]).ravel())
+        need = int(num_steps) * W
+        if any(t.size < need for t in keep):
+            raise BoundsError(ERR_BOUNDS, f"each table needs num_steps * num_walkers = {need} entries")
+        tab = ctypes.byref(MCMCTable(_d(keep[0]), _i(keep[1]), _d(keep[2])))
+    info = ctypes.c_int()
+    rc = lib().cmoe_hyperparameter_mcmc(int(kernel), int(bool(default_prior)), int(bool(noisy)), _d(P), W,
+                                        int(num_steps), ctypes.c_uint64(seed), ctypes.c_uint64(first_step), tab, _d(X),
+                                        _d(_f64(y).ravel()), _i(derivs), derivs.size, dim, N, int(device), _d(pos),
+                                        _d(lnp), ctypes.byref(info))
+    _check(rc, info.value)
+    return pos, lnp
+
+
 def grad_log_marginal_likelihood(kernel, alpha, lengths, X, y, noise, derivs=None, device=0):
     """cmoe_grad_log_marginal_likelihood: d log p / d (alpha, lengths..., noise by observation type)."""
     X = _f64(X)

@@ -17,8 +17,8 @@
 //   evaluate_KG_mcmc_at_point_list                                        gpp_python_knowledge_gradient_mcmc.cpp:49-384
 //   compute_{,grad_}expected_improvement_mcmc, multistart_expected_improvement_mcmc_optimization,
 //   evaluate_EI_mcmc_at_point_list                                        gpp_python_expected_improvement_mcmc.cpp:46-300
-//   compute_posterior_mean_of_points, compute_{,grad_}posterior_mean_mcmc_of_points, posterior_mean_mcmc_optimization
-//                                                                         batched forms, not in the reference module
+//   compute_posterior_mean_of_points, compute_{,grad_}posterior_mean_mcmc_of_points, posterior_mean_mcmc_optimization,
+//   sample_hyperparameters_mcmc                                           batched forms, not in the reference module
 //   GradientDescentParameters, NewtonParameters, RandomnessSourceContainer, OptimizerTypes, DomainTypes,
 //   LogLikelihoodTypes                                                    gpp_python_common.cpp:201-370
 //   OptimalLearningException, BoundsException, InvalidValueException, SingularMatrixException   gpp_python.cpp:189-206
@@ -1289,6 +1289,35 @@ PYBIND11_MODULE(GPP, m) {
       raise_exc(g_exc_base, (n + ": the arguments match no signature of the reference's function").c_str());
     });
   }
+  // sample_hyperparameters_mcmc(points_sampled, points_sampled_value, dim, num_sampled, derivatives, num_derivatives,
+  //     initial_positions, num_walkers, num_steps, noisy, use_default_prior, seed, first_step)
+  // Not in the reference module: the emcee chain of GaussianProcessLogLikelihoodMCMC.train (log_likelihood_mcmc.py:
+  // 170-239) in one device call (cmoe_hyperparameter_mcmc, DESIGN.md K12).  Walkers are log-scale
+  // [log alpha, log lengths..., log noise...]; returns (positions, log_probabilities) as flat lists.
+  m.def("sample_hyperparameters_mcmc",
+        [](const py::list& points_sampled, const py::list& points_sampled_value, int dim, int num_sampled,
+           const py::list& derivatives, int num_derivatives, const py::list& initial_positions, int num_walkers,
+           int num_steps, bool noisy, bool use_default_prior, uint64_t seed, uint64_t first_step) -> py::tuple {
+          const auto X = to_vec(points_sampled, static_cast<size_t>(dim) * num_sampled);
+          const auto y = to_vec(points_sampled_value, static_cast<size_t>(num_sampled) * (1 + num_derivatives));
+          const auto derivs = to_ivec(derivatives, num_derivatives);
+          const size_t nh = static_cast<size_t>(dim) + 2 + num_derivatives;
+          const auto p0 = to_vec(initial_positions, nh * std::max(num_walkers, 0));
+          std::vector<double> pos(p0.size()), lnp(std::max(num_walkers, 0));
+          int info = 0;
+          // MaternNu2p5 hard-wired, as compute_log_likelihood's boundary does
+          check(cmoe_hyperparameter_mcmc(CMOE_KERNEL_MATERN_NU_2P5,
+                                         use_default_prior ? CMOE_HYPER_PRIOR_DEFAULT : CMOE_HYPER_PRIOR_NONE,
+                                         noisy ? 1 : 0, p0.data(), num_walkers, num_steps, seed, first_step, nullptr,
+                                         X.data(), y.data(), derivs.data(), num_derivatives, dim, num_sampled, 0,
+                                         pos.data(), lnp.data(), &info),
+                info);
+          return py::make_tuple(to_list(pos), to_list(lnp));
+        },
+        py::arg("points_sampled"), py::arg("points_sampled_value"), py::arg("dim"), py::arg("num_sampled"),
+        py::arg("derivatives"), py::arg("num_derivatives"), py::arg("initial_positions"), py::arg("num_walkers"),
+        py::arg("num_steps"), py::arg("noisy"), py::arg("use_default_prior"), py::arg("seed"),
+        py::arg("first_step") = 0);
   m.def("heuristic_expected_improvement_optimization",
         [](const py::args&, const py::kwargs&) -> py::object {
           not_on_path("heuristic_expected_improvement_optimization");

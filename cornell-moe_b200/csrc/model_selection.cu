@@ -754,3 +754,308 @@ extern "C" int cmoe_grad_log_marginal_likelihood_list(int kernel, const double* 
              dim, num_sampled, device, values, grads);
   });
 }
+
+// ---- hyper-parameter MCMC (DESIGN.md K12) --------------------------------------------------------------------------
+// emcee 2.2.1's EnsembleSampler.sample with the stretch move (a = 2) on GaussianProcessLogLikelihoodMCMC's
+// log-probability (log_likelihood_mcmc.py:277-312), every half-step on the device:
+//   hmc_propose_kernel   one thread per moving walker: draws, z = ((a - 1) u + 1)^2 / a, q = c - z (c - s) rounded as
+//                        numpy rounds it, the box check, the noise pinning, the prior, and the K10 inputs of q
+//   lml_cov_kernel, potrf_batched, lml_solve_kernel   (K10, unchanged) on the half-ensemble's sets
+//   hmc_accept_kernel    one thread per moving walker: lnpdiff = (nh - 1) log z + lnp(q) - lnp(s) and the accept
+// The initial evaluation runs the same kernels with the move switched off.  One step is captured as a CUDA graph and
+// replayed; the step index lives in a device counter that the second half's accept kernel advances.
+namespace cmoe {
+namespace {
+
+constexpr int kHmcThreads = 128;
+constexpr double kStretchA = 2.0;
+constexpr double kLogNoiseFree = -0x1.26bb1bbb55516p+4;  // numpy.log(1e-8), the pinned noise of a noise-free model
+constexpr double kSqrt2Pi = 2.5066282746310002;           // scipy.stats.norm's _norm_pdf_C = sqrt(2 pi)
+
+struct HmcArgs {
+  int Wh, nh, dim, g, kernel, prior, noisy;
+  int derivs[CMOE_MAX_DIM];
+  uint64_t seed, first_step;
+  const double* tz;  // table (NULL: Philox): [num_steps][W] z uniform, partner, accept uniform
+  const int* tp;
+  const double* tu;
+  double* pos;       // [W][nh] walker positions
+  double* lnp;       // [W] their log-probabilities
+  double* prop;      // [Wh][nh] proposals of the moving half
+  double* lprior;    // [Wh] their prior, -inf when the likelihood is skipped
+  double* zz;        // [Wh] stretch factors
+  double* lu;        // [Wh] log of the acceptance uniforms
+  unsigned long long* step;  // steps done in this call
+  KernelSpec* specs;  // K10 inputs and outputs of the half-ensemble's sets
+  double* noise;
+  int* fail;
+  const double* values;
+};
+
+// Philox draws of walker w at absolute step `step`: counter (step_lo, step_hi, w, 2) gives the z uniform (words 0, 1)
+// and the acceptance uniform (words 2, 3), 53 bits each in [0, 1); counter (step_lo, step_hi, w, 3) gives the partner
+// as the high word of its first 64 bits times Wh.  Word 3 = 0 and 1 are the normals' and the Latin hypercube's streams.
+__device__ __forceinline__ void hmc_draws(uint64_t seed, uint64_t step, int w, int Wh, double& uz, int& partner,
+                                          double& ua) {
+  uint32_t c[4] = {static_cast<uint32_t>(step), static_cast<uint32_t>(step >> 32), static_cast<uint32_t>(w), 2u};
+  philox4x32_10(c, static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
+  uz = static_cast<double>(((static_cast<uint64_t>(c[0]) << 32) | c[1]) >> 11) * 0x1.0p-53;
+  ua = static_cast<double>(((static_cast<uint64_t>(c[2]) << 32) | c[3]) >> 11) * 0x1.0p-53;
+  uint32_t d[4] = {static_cast<uint32_t>(step), static_cast<uint32_t>(step >> 32), static_cast<uint32_t>(w), 3u};
+  philox4x32_10(d, static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
+  partner = static_cast<int>(__umul64hi((static_cast<uint64_t>(d[0]) << 32) | d[1], static_cast<uint64_t>(Wh)));
+}
+
+// Moving walker w = half * Wh + j.  With move == 0 the proposal is the walker itself (the initial evaluation).
+__global__ void __launch_bounds__(kHmcThreads) hmc_propose_kernel(const __grid_constant__ HmcArgs a, int half,
+                                                                  int move) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= a.Wh) return;
+  const int nh = a.nh, dim = a.dim, b = 1 + a.g, w = half * a.Wh + j;
+  const double* s = a.pos + static_cast<size_t>(w) * nh;
+  double* q = a.prop + static_cast<size_t>(j) * nh;
+  if (move) {
+    const unsigned long long step = *a.step;
+    double uz, ua;
+    int p;
+    if (a.tz) {
+      const size_t e = static_cast<size_t>(step) * (2 * a.Wh) + w;
+      uz = a.tz[e];
+      p = a.tp[e];
+      ua = a.tu[e];
+    } else {
+      hmc_draws(a.seed, a.first_step + step, w, a.Wh, uz, p, ua);
+    }
+    // zz = ((a - 1) rand + 1) ** 2 / a; q = c[rint] - zz (c[rint] - s): each operation rounded as numpy rounds it
+    const double t = __dadd_rn(__dmul_rn(kStretchA - 1.0, uz), 1.0);
+    const double z = __ddiv_rn(__dmul_rn(t, t), kStretchA);
+    const double* c = a.pos + static_cast<size_t>((1 - half) * a.Wh + p) * nh;
+    for (int k = 0; k < nh; ++k) q[k] = __dsub_rn(c[k], __dmul_rn(z, __dsub_rn(c[k], s[k])));
+    a.zz[j] = z;
+    a.lu[j] = log(ua);
+  } else {
+    for (int k = 0; k < nh; ++k) q[k] = s[k];
+  }
+  // compute_log_likelihood's order: the box (theta untouched outside it), the pinning, the prior
+  bool inbox = true;
+  for (int k = 0; k < nh; ++k)
+    if (q[k] < -20.0 || q[k] > 20.0) inbox = false;
+  double lp = 1.0;
+  if (inbox) {
+    if (!a.noisy)
+      for (int t = 0; t < b; ++t) q[1 + dim + t] = kLogNoiseFree;
+    if (a.prior == CMOE_HYPER_PRIOR_DEFAULT) {
+      // NormalPrior(0, 1).lnprob returns the pdf (base_prior.py:338-354); TophatPrior(-2, 3) over the lengths
+      // (:104-123); HorseshoePrior(0.1) per noise entry in order (:183-201)
+      lp = exp(-(q[0] * q[0]) / 2.0) / kSqrt2Pi;
+      for (int k = 0; k < dim; ++k)
+        if (q[1 + k] < -2.0 || q[1 + k] > 3.0) lp = -INFINITY;
+      for (int t = 0; t < b; ++t) {
+        const double th = q[1 + dim + t];
+        const double r = 0.1 / th;
+        lp += (th == 0.0) ? INFINITY : log(log(1.0 + 3.0 * (r * r)));
+      }
+    }
+  }
+  const bool skip = !inbox || lp == -INFINITY;
+  a.lprior[j] = skip ? -INFINITY : lp;
+  // the set's KernelSpec and noise as lml_list builds them on the host; a skipped proposal gets the finite placeholder
+  // theta = 0 and a preset failure flag, so the Cholesky skips it and lml_solve_kernel writes -inf
+  KernelSpec& sp = a.specs[j];
+  sp.kernel = a.kernel;
+  sp.dim = dim;
+  sp.g = a.g;
+  sp.alpha = exp(skip ? 0.0 : q[0]);
+  for (int k = 0; k < CMOE_MAX_DIM; ++k) {
+    double lsq = 1.0, il = 0.0;
+    if (k < dim) {
+      const double l = exp(skip ? 0.0 : q[1 + k]);
+      lsq = l * l;
+      il = 1.0 / l;
+    }
+    sp.lsq[k] = lsq;
+    sp.inv_len[k] = il;
+    sp.derivs[k] = a.derivs[k];
+  }
+  for (int t = 0; t < b; ++t) a.noise[static_cast<size_t>(j) * b + t] = exp(skip ? 0.0 : q[1 + dim + t]) + 1.0e-6;
+  a.fail[j] = skip ? -1 : 0;
+}
+
+__global__ void __launch_bounds__(kHmcThreads) hmc_accept_kernel(const __grid_constant__ HmcArgs a, int half,
+                                                                 int move) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= a.Wh) return;
+  const int nh = a.nh, w = half * a.Wh + j;
+  const double lq = a.lprior[j] + a.values[j];  // -inf + -inf for a skipped proposal
+  bool take = true;
+  if (move) {
+    // lnpdiff = (dim - 1.) * np.log(zz) + newlnprob - lnprob0, left to right; accept = lnpdiff > log(rand)
+    const double d = __dsub_rn(__dadd_rn(__dmul_rn(static_cast<double>(nh - 1), log(a.zz[j])), lq), a.lnp[w]);
+    take = d > a.lu[j];
+    if (half == 1 && j == 0) *a.step += 1;
+  }
+  if (take) {
+    const double* q = a.prop + static_cast<size_t>(j) * nh;
+    double* p = a.pos + static_cast<size_t>(w) * nh;
+    for (int k = 0; k < nh; ++k) p[k] = q[k];
+    a.lnp[w] = lq;
+  }
+}
+
+struct GraphGuard {
+  cudaGraph_t graph = nullptr;
+  cudaGraphExec_t exec = nullptr;
+  ~GraphGuard() {
+    if (exec) cudaGraphExecDestroy(exec);
+    if (graph) cudaGraphDestroy(graph);
+  }
+};
+
+void hyper_mcmc(int kernel, int prior, int noisy, const double* initial_positions, int num_walkers, int num_steps,
+                uint64_t seed, uint64_t first_step, const cmoe_mcmc_table* table, const double* points_sampled,
+                const double* points_sampled_value, const int* derivatives, int num_derivatives, int dim,
+                int num_sampled, int device, double* positions, double* log_probabilities) {
+  CMOE_REQUIRE(initial_positions != nullptr && points_sampled != nullptr && points_sampled_value != nullptr &&
+                   positions != nullptr && log_probabilities != nullptr,
+               CMOE_ERR_INVALID_VALUE, "NULL argument");
+  CMOE_REQUIRE(kernel == CMOE_KERNEL_SQUARE_EXPONENTIAL || kernel == CMOE_KERNEL_MATERN_NU_2P5,
+               CMOE_ERR_INVALID_VALUE, "unknown covariance kernel id");
+  CMOE_REQUIRE(prior == CMOE_HYPER_PRIOR_NONE || prior == CMOE_HYPER_PRIOR_DEFAULT, CMOE_ERR_INVALID_VALUE,
+               "prior must be CMOE_HYPER_PRIOR_NONE or CMOE_HYPER_PRIOR_DEFAULT");
+  CMOE_REQUIRE(dim >= 1 && dim <= CMOE_MAX_DIM, CMOE_ERR_BOUNDS, "dim must be in [1, CMOE_MAX_DIM]");
+  CMOE_REQUIRE(num_sampled >= 1, CMOE_ERR_BOUNDS, "num_sampled must be >= 1");
+  CMOE_REQUIRE(num_derivatives >= 0 && num_derivatives <= dim, CMOE_ERR_BOUNDS, "num_derivatives out of range");
+  CMOE_REQUIRE(num_derivatives == 0 || derivatives != nullptr, CMOE_ERR_INVALID_VALUE, "derivatives is NULL");
+  for (int k = 0; k < num_derivatives; ++k)
+    CMOE_REQUIRE(derivatives[k] >= 0 && derivatives[k] < dim, CMOE_ERR_BOUNDS, "derivative index out of range");
+  const int g = num_derivatives, b = 1 + g, nh = 2 + dim + g, N = num_sampled, W = num_walkers, Wh = W / 2;
+  CMOE_REQUIRE(static_cast<long long>(N) * b <= kMaxSampleQ, CMOE_ERR_BOUNDS,
+               "num_sampled * (1 + num_derivatives) must be <= 8192");
+  // EnsembleSampler.__init__'s checks
+  CMOE_REQUIRE(W % 2 == 0, CMOE_ERR_BOUNDS, "num_walkers must be even");
+  CMOE_REQUIRE(W >= 2 * nh, CMOE_ERR_BOUNDS, "num_walkers must be at least twice the number of hyperparameters");
+  CMOE_REQUIRE(num_steps >= 1, CMOE_ERR_BOUNDS, "num_steps must be >= 1");
+  const int n = N * b, nsteps = (n + NB - 1) / NB;
+  // the half-ensemble is one K10 chunk (lml_list's per-set bytes without the gradient)
+  const size_t per_set = sizeof(double) * (static_cast<size_t>(n) * n + static_cast<size_t>(nsteps) * NB * NB + b + 1) +
+                         sizeof(KernelSpec) + sizeof(int);
+  const size_t chunk = std::max<size_t>(1, std::min<size_t>(kSampleWorkspaceBytes / per_set, kMaxChunkSets));
+  CMOE_REQUIRE(static_cast<size_t>(Wh) <= chunk, CMOE_ERR_BOUNDS,
+               "num_walkers / 2 = " + std::to_string(Wh) + " sets exceed one likelihood chunk (" +
+                   std::to_string(chunk) + " sets at n = " + std::to_string(n) + ")");
+  for (size_t e = 0; e < static_cast<size_t>(W) * nh; ++e)
+    CMOE_REQUIRE(std::isfinite(initial_positions[e]), CMOE_ERR_INVALID_VALUE, "initial position is not finite");
+  const size_t tcount = static_cast<size_t>(num_steps) * W;
+  if (table) {
+    CMOE_REQUIRE(table->z_uniform != nullptr && table->partner != nullptr && table->accept_uniform != nullptr,
+                 CMOE_ERR_INVALID_VALUE, "NULL table array");
+    for (size_t e = 0; e < tcount; ++e)
+      CMOE_REQUIRE(table->partner[e] >= 0 && table->partner[e] < Wh, CMOE_ERR_BOUNDS,
+                   "table partner out of range [0, num_walkers / 2)");
+  }
+  require_device(device);
+  // y - m as lml_list centres it (gpp_model_selection.cpp:556-560)
+  double m = 0.0;
+  for (int i = 0; i < N; ++i) m += points_sampled_value[static_cast<size_t>(i) * b];
+  m /= N;
+  std::vector<double> rc(points_sampled_value, points_sampled_value + n);
+  for (int i = 0; i < N; ++i) rc[static_cast<size_t>(i) * b] -= m;
+
+  LmlWork& w = lml_workspace(device);
+  cudaStream_t s = w.stream;
+  // every buffer is sized here, before the capture
+  w.X.upload(points_sampled, static_cast<size_t>(N) * dim, s);
+  w.r.upload(rc.data(), n, s);
+  w.specs.ensure(Wh);
+  w.noise.ensure(static_cast<size_t>(Wh) * b);
+  w.K.ensure(static_cast<size_t>(Wh) * n * n);
+  w.stage.ensure(static_cast<size_t>(Wh) * nsteps * NB * NB);
+  w.values.ensure(Wh);
+  w.fail.ensure(Wh);
+  DevBuf<double> pos, lnp(W), prop(static_cast<size_t>(Wh) * nh), lprior(Wh), zz(Wh), lu(Wh), tz, tu;
+  DevBuf<int> tp;
+  DevBuf<unsigned long long> step(1);
+  pos.upload(initial_positions, static_cast<size_t>(W) * nh, s);
+  if (table) {
+    tz.upload(table->z_uniform, tcount, s);
+    tp.upload(table->partner, tcount, s);
+    tu.upload(table->accept_uniform, tcount, s);
+  }
+  step.zero(s);
+  HmcArgs a{};
+  a.Wh = Wh;
+  a.nh = nh;
+  a.dim = dim;
+  a.g = g;
+  a.kernel = kernel;
+  a.prior = prior;
+  a.noisy = noisy ? 1 : 0;
+  for (int k = 0; k < g; ++k) a.derivs[k] = derivatives[k];
+  a.seed = seed;
+  a.first_step = first_step;
+  a.tz = table ? tz.p : nullptr;
+  a.tp = table ? tp.p : nullptr;
+  a.tu = table ? tu.p : nullptr;
+  a.pos = pos.p;
+  a.lnp = lnp.p;
+  a.prop = prop.p;
+  a.lprior = lprior.p;
+  a.zz = zz.p;
+  a.lu = lu.p;
+  a.step = step.p;
+  a.specs = w.specs.p;
+  a.noise = w.noise.p;
+  a.fail = w.fail.p;
+  a.values = w.values.p;
+  const size_t smem_cov = 2 * static_cast<size_t>(NB) * dim * sizeof(double);
+  const size_t smem_solve = (static_cast<size_t>(n) + NB * (NB + 1)) * sizeof(double);
+  CMOE_CUDA(cudaFuncSetAttribute(lml_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 static_cast<int>(smem_solve)));
+  const unsigned blocks = static_cast<unsigned>((Wh + kHmcThreads - 1) / kHmcThreads);
+  auto half_step = [&](int half, int move) {
+    hmc_propose_kernel<<<blocks, kHmcThreads, 0, s>>>(a, half, move);
+    lml_cov_kernel<<<dim3(nsteps * (nsteps + 1) / 2, 1, Wh), kLmlCovThreads, smem_cov, s>>>(w.specs.p, w.noise.p,
+                                                                                            w.X.p, N, w.K.p);
+    count_launch(2);
+    CMOE_CUDA(cudaGetLastError());
+    potrf_batched(w.K.p, n, Wh, w.fail.p, w.stage, s);
+    lml_solve_kernel<<<Wh, kLmlSolveThreads, smem_solve, s>>>(w.K.p, n, w.r.p, w.fail.p, w.values.p, nullptr);
+    hmc_accept_kernel<<<blocks, kHmcThreads, 0, s>>>(a, half, move);
+    count_launch(2);
+    CMOE_CUDA(cudaGetLastError());
+  };
+  // run_mcmc evaluates the initial positions first (and pins their noise)
+  half_step(0, 0);
+  half_step(1, 0);
+  GraphGuard gg;
+  CMOE_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
+  try {
+    half_step(0, 1);
+    half_step(1, 1);
+  } catch (...) {
+    cudaStreamEndCapture(s, &gg.graph);  // leave the cached stream usable
+    throw;
+  }
+  CMOE_CUDA(cudaStreamEndCapture(s, &gg.graph));
+  CMOE_CUDA(cudaGraphInstantiate(&gg.exec, gg.graph, 0));
+  for (int i = 0; i < num_steps; ++i) CMOE_CUDA(cudaGraphLaunch(gg.exec, s));
+  pos.download(positions, static_cast<size_t>(W) * nh, s);
+  lnp.download(log_probabilities, W, s);
+  CMOE_CUDA(cudaStreamSynchronize(s));
+}
+
+}  // namespace
+}  // namespace cmoe
+
+extern "C" int cmoe_hyperparameter_mcmc(int kernel, int prior, int noisy, const double* initial_positions,
+                                        int num_walkers, int num_steps, uint64_t seed, uint64_t first_step,
+                                        const cmoe_mcmc_table* table, const double* points_sampled,
+                                        const double* points_sampled_value, const int* derivatives,
+                                        int num_derivatives, int dim, int num_sampled, int device, double* positions,
+                                        double* log_probabilities, int* info) {
+  return guarded(info, [&] {
+    hyper_mcmc(kernel, prior, noisy, initial_positions, num_walkers, num_steps, seed, first_step, table,
+               points_sampled, points_sampled_value, derivatives, num_derivatives, dim, num_sampled, device, positions,
+               log_probabilities);
+  });
+}

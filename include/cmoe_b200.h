@@ -139,6 +139,35 @@ int cmoe_hyperparameter_gradient_descent(int kernel, const cmoe_gd_params* gd_pa
                                          int num_derivatives, int dim, int num_sampled, int device,
                                          double* best_point, double* best_value, int* found_flag,
                                          double* end_points, double* end_values, int* info);
+/* Priors of cmoe_hyperparameter_mcmc: the two the reference's GaussianProcessLogLikelihoodMCMC front end uses. */
+#define CMOE_HYPER_PRIOR_NONE 0    /* prior = None: the constant 1 (log_likelihood_mcmc.py:291) */
+#define CMOE_HYPER_PRIOR_DEFAULT 1 /* DefaultPrior(nh, 1 + g) (default_priors.py:27-37) */
+/* Host-supplied random numbers of cmoe_hyperparameter_mcmc, each [num_steps][num_walkers] and indexed by the step of
+ * the call and the walker: the uniform of the stretch factor, the partner (an index into the other half of the
+ * ensemble, in [0, num_walkers / 2)) and the acceptance uniform.  Entries of the half that does not move are unused. */
+typedef struct cmoe_mcmc_table {
+  const double* z_uniform;
+  const int* partner;
+  const double* accept_uniform;
+} cmoe_mcmc_table;
+/* Hyper-parameter MCMC (DESIGN.md K12): num_steps steps of emcee 2.2.1's EnsembleSampler.sample (stretch move, a = 2)
+ * on the log-probability of GaussianProcessLogLikelihoodMCMC.compute_log_likelihood (log_likelihood_mcmc.py:277-312),
+ * the whole chain on the device in one call.  A walker is theta = (log alpha, log l_1..l_dim, log noise_0..noise_g),
+ * nh = 2 + dim + g entries; its log-probability is -inf outside [-20, 20]^nh, else (with noisy == 0 the noise entries
+ * are first set to log(1e-8) in the walker itself, so the pinned values persist in the chain) prior + the value of
+ * cmoe_log_marginal_likelihood_list at exp(theta), -inf if the prior is -inf or the Cholesky fails.
+ * initial_positions[num_walkers][nh]; the initial log-probabilities are evaluated first, as run_mcmc does.  Random
+ * numbers: table == NULL draws them from Philox4x32-10 keyed by seed, a pure function of (seed, first_step + step,
+ * walker), so a chain split over several calls (first_step = steps done so far) is bit-identical to one call; else
+ * from *table.  Outputs: positions[num_walkers][nh] and log_probabilities[num_walkers] after the last step.
+ * Bounds (CMOE_ERR_BOUNDS, before any device work): num_walkers even and >= 2 nh, num_steps >= 1, the K10 size
+ * contract (dim <= CMOE_MAX_DIM, num_sampled (1 + g) <= 8192) and num_walkers / 2 sets within one K10 chunk (4096
+ * sets and about 2 GiB: 3 sets at n = 8192).  Non-finite initial positions are CMOE_ERR_INVALID_VALUE (emcee raises). */
+int cmoe_hyperparameter_mcmc(int kernel, int prior, int noisy, const double* initial_positions, int num_walkers,
+                             int num_steps, uint64_t seed, uint64_t first_step, const cmoe_mcmc_table* table,
+                             const double* points_sampled, const double* points_sampled_value, const int* derivatives,
+                             int num_derivatives, int dim, int num_sampled, int device, double* positions,
+                             double* log_probabilities, int* info);
 /* Run-time switches between kernel generations (also read once from the environment: CMOE_LEGACY_LINALG, CMOE_COV_TMA):
  *   "legacy_linalg" 1 = round-1 launch-per-step Cholesky / chained trsv for large n (default 0: cooperative kernels);
  *   "cov_tma"       1 = TMA / DMMA covariance build with tensor-map tile stores (default 0: LDGSTS kernel, faster at d ~ 10). */
