@@ -672,6 +672,8 @@ void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
       pl.entry->acc_gen(ap, dim3((n + Q + 127) / 128, nb), s);
       kg_g1_kernel<<<nb, 256, 0, s>>>(spec, U, q, QP, DIMP, mc, pb.P.p, pl.dRecC.p, pl.dOutX.p, pl.dG1.p);
       count_launch();
+    } else if (pl.use_smem && pl.entry->acc_tile) {
+      pl.entry->acc_tile(ap, dim3(1, nb), s);
     } else {
       pl.entry->acc(ap, dim3((N + U + 127) / 128, nb), s);
     }

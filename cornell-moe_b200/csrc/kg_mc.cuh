@@ -1704,10 +1704,57 @@ __global__ void __launch_bounds__(kMcThreads, CMOE_MC_GEN_MINBLOCKS)
 //   Gu[u][d]  = sum_i c_iu kb(Xu_u, x*_i) x~*_id ,  GkB[u] = sum_i c_iu kb(Xu_u, x*_i)
 // grid (row blocks, candidates); one thread per row.
 // ---------------------------------------------------------------------------------------------------------------
-constexpr int kAccTile = 64;  // samples per shared-memory tile of kg_acc_kernel
+constexpr int kAccTile = 64;  // samples per shared-memory tile of the accumulation kernels
 
-// One thread per row of [training points; union points]; the samples' records (minimiser, c, -|x*|^2/2) stream through
-// shared memory in double-buffered tiles (LDGSTS, 16-byte chunks) and are read back as warp-broadcast LDS.128.
+// Streams candidate `cand`'s sample records (minimiser, c, -|x*|^2/2) through shared memory in double-buffered tiles
+// of kAccTile samples (LDGSTS, 16-byte chunks) and calls body(sx, sc, sh, cnt) once per tile, in sample order:
+// sx = [kAccTile][DIM], sc = [kAccTile][QP], sh = [kAccTile], cnt = valid samples.  Slots past num_mc are zero-filled.
+// sbuf: 2 * kAccTile * (DIM + QP + 1) doubles.  Every thread of the CTA must call it.
+template <int DIM, int QP, typename F>
+__device__ __forceinline__ void acc_stream_samples(const KgAccParams& prm, int cand, double* __restrict__ sbuf,
+                                                   F&& body) {
+  const double* xs = prm.outX + static_cast<size_t>(cand) * prm.num_mc * DIM;
+  const double* cs = prm.recC + static_cast<size_t>(cand) * prm.num_mc * QP;
+  const double* hs = prm.outH + static_cast<size_t>(cand) * prm.num_mc;
+  constexpr int TS = kAccTile;
+  constexpr int kBuf = TS * (DIM + QP + 1);  // doubles per buffer: [TS][DIM] | [TS][QP] | [TS]
+  const int num_mc = prm.num_mc;
+  const int ntiles = (num_mc + TS - 1) / TS;
+  auto load_tile = [&](int tile, int buf) {
+    double* sx = sbuf + buf * kBuf;
+    double* sc = sx + TS * DIM;
+    double* sh = sc + TS * QP;
+    const int i0 = tile * TS;
+    for (int e = threadIdx.x; e < TS * DIM / 2; e += blockDim.x) {
+      const bool ok = i0 + (2 * e) / DIM < num_mc;
+      cp_async16(sx + 2 * e, ok ? xs + static_cast<size_t>(i0) * DIM + 2 * e : xs, ok);
+    }
+    for (int e = threadIdx.x; e < TS * QP / 2; e += blockDim.x) {
+      const bool ok = i0 + (2 * e) / QP < num_mc;
+      cp_async16(sc + 2 * e, ok ? cs + static_cast<size_t>(i0) * QP + 2 * e : cs, ok);
+    }
+    for (int e = threadIdx.x; e < TS; e += blockDim.x) {
+      const bool ok = i0 + e < num_mc;
+      cp_async8(sh + e, ok ? hs + i0 + e : hs, ok);
+    }
+  };
+  load_tile(0, 0);
+  cp_async_commit();
+  for (int tile = 0; tile < ntiles; ++tile) {
+    const int buf = tile & 1;
+    if (tile + 1 < ntiles) load_tile(tile + 1, buf ^ 1);
+    cp_async_commit();
+    cp_async_wait<1>();
+    __syncthreads();
+    const double* sx = sbuf + buf * kBuf;
+    const double* sc = sx + TS * DIM;
+    body(sx, sc, sc + TS * QP, min(TS, num_mc - tile * TS));
+    __syncthreads();  // the buffer is refilled two tiles later
+  }
+}
+
+// One thread per row of [training points; union points]; the samples' records stream through shared memory
+// (acc_stream_samples) and are read back as warp-broadcast LDS.128.
 // TAB selects the table exp under the fast path's range contract (kFastPathRadius).
 // GEN (derivative observations): the rows are (point, m), m = 0..g, training rows first; row (p, m > 0) is the
 // derivative of k(p, x*) with respect to coordinate t = derivs[m-1] of p:  kb (x~*_t - p~_t) / l_t.  The union rows'
@@ -1753,9 +1800,6 @@ __device__ __forceinline__ void kg_acc_body(const KgAccParams& prm, double* __re
   double gu[DIM], gkb = 0.0;
 #pragma unroll
   for (int d = 0; d < DIM; ++d) gu[d] = 0.0;
-  const double* xs = prm.outX + static_cast<size_t>(cand) * prm.num_mc * DIM;
-  const double* cs = prm.recC + static_cast<size_t>(cand) * prm.num_mc * QP;
-  const double* hs = prm.outH + static_cast<size_t>(cand) * prm.num_mc;
   const int uu = is_u ? (row - N) : 0;
   double xrt = 0.0;  // own coordinate along the derivative direction
   if (GEN) {
@@ -1763,40 +1807,7 @@ __device__ __forceinline__ void kg_acc_body(const KgAccParams& prm, double* __re
     for (int d = 0; d < DIM; ++d)
       if (d == tcoord) xrt = xr[d];
   }
-  constexpr int TS = kAccTile;
-  constexpr int kBuf = TS * (DIM + QP + 1);  // doubles per buffer: [TS][DIM] | [TS][QP] | [TS]
-  const int num_mc = prm.num_mc;
-  const int ntiles = (num_mc + TS - 1) / TS;
-  auto load_tile = [&](int tile, int buf) {
-    double* sx = sbuf + buf * kBuf;
-    double* sc = sx + TS * DIM;
-    double* sh = sc + TS * QP;
-    const int i0 = tile * TS;
-    for (int e = threadIdx.x; e < TS * DIM / 2; e += blockDim.x) {
-      const bool ok = i0 + (2 * e) / DIM < num_mc;
-      cp_async16(sx + 2 * e, ok ? xs + static_cast<size_t>(i0) * DIM + 2 * e : xs, ok);
-    }
-    for (int e = threadIdx.x; e < TS * QP / 2; e += blockDim.x) {
-      const bool ok = i0 + (2 * e) / QP < num_mc;
-      cp_async16(sc + 2 * e, ok ? cs + static_cast<size_t>(i0) * QP + 2 * e : cs, ok);
-    }
-    for (int e = threadIdx.x; e < TS; e += blockDim.x) {
-      const bool ok = i0 + e < num_mc;
-      cp_async8(sh + e, ok ? hs + i0 + e : hs, ok);
-    }
-  };
-  load_tile(0, 0);
-  cp_async_commit();
-  for (int tile = 0; tile < ntiles; ++tile) {
-    const int buf = tile & 1;
-    if (tile + 1 < ntiles) load_tile(tile + 1, buf ^ 1);
-    cp_async_commit();
-    cp_async_wait<1>();
-    __syncthreads();
-    const double* sx = sbuf + buf * kBuf;
-    const double* sc = sx + TS * DIM;
-    const double* sh = sc + TS * QP;
-    const int cnt = min(TS, num_mc - tile * TS);
+  acc_stream_samples<DIM, QP>(prm, cand, sbuf, [&](const double* sx, const double* sc, const double* sh, int cnt) {
 #pragma unroll 2
     for (int i = 0; i < cnt; ++i) {
       double xi[DIM], ci[QP];
@@ -1831,8 +1842,7 @@ __device__ __forceinline__ void kg_acc_body(const KgAccParams& prm, double* __re
         for (int d = 0; d < DIM; ++d) gu[d] = fma(w, xi[d], gu[d]);
       }
     }
-    __syncthreads();  // the buffer is refilled two tiles later
-  }
+  });
   if (!active) return;
   double* R = prm.R + static_cast<size_t>(cand) * QP * nrows;
 #pragma unroll
@@ -1866,6 +1876,162 @@ __global__ void __launch_bounds__(128) kg_acc_gen_kernel(const __grid_constant__
   kg_acc_body<KERNEL, DIM, QP, false, true>(prm, acc_smem);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Tile accumulation of the training rows (kg_tile_path instantiation, shared-memory fast path; DESIGN.md K6).
+//   R^T[row][a] = sum_i exp(X~_row . x~*_i + e_row + h_i) c_ia ,   e_row = ln(alpha) - |X~_row|^2 / 2,  h_i = -|x~*_i|^2/2
+// is two FP64 DMMA m16n8k4 products per 16 rows x 8 samples: the exponents (M = 16 rows, N = 8 samples, K = DIM,
+// accumulator seeded with e_row + h_i) and, after the element-wise exp, R^T += KV C (K = the 8 samples, N = QP).  The
+// second product takes KV's accumulator layout as its A operand, k-step 0 = the even columns, k-step 1 = the odd ones.
+// Column n of a sample group s0 is sample s0 + (n >> 1) + 4 (n & 1), so that lane (g, t) holds samples s0 + t and
+// s0 + t + 4, and its C operands c[s0 + t][g], c[s0 + t + 4][g] are two conflict-free LDS.  The K order of the exponent
+// product is coordinate 2t + ks in k-step ks, so that a lane's x* operands of both k-steps are one LDS.128.
+// A warp owns kAccRowTiles tiles of 16 rows: the row operands (A fragments, e_row) and the accumulators stay in
+// registers over all samples, and each group's sample operands feed 4 kAccRowTiles DMMAs.  Every lane walks the samples
+// in ascending groups, so a candidate's R does not depend on its batch or the launch.  Rows past N read row N - 1 and
+// are not stored; samples past num_mc are zero-filled (c = 0, finite exponent): exact zeros.
+// The last CTA of each candidate (blockIdx.x = gridDim.x - 1) does the U <= QP union rows instead: their R rows and the
+// own-point sums Gu, GkB (kg_acc_body's formulas) with kAccUnionSplit threads per union row, each taking every
+// kAccUnionSplit-th sample of a tile, combined by a fixed butterfly.
+// ---------------------------------------------------------------------------------------------------------------
+#ifndef CMOE_ACC_ROW_TILES
+#define CMOE_ACC_ROW_TILES 4
+#endif
+constexpr int kAccRowTiles = CMOE_ACC_ROW_TILES;   // 16-row tiles per warp
+constexpr int kAccTileThreads = 128;
+constexpr int kAccTileRowsPerCta = kAccTileThreads / 32 * 16 * kAccRowTiles;
+constexpr int kAccUnionSplit = 16;
+static_assert(kAccTileThreads / kAccUnionSplit >= 8, "one thread group per union row (U <= QP = 8)");
+
+template <int DIM, int QP>
+__device__ __forceinline__ void kg_acc_tile_rows(const KgAccParams& prm, double* __restrict__ sbuf) {
+  static_assert(DIM == 8 && QP == 8, "one k-step pair of coordinates and of samples, one n-block of union columns");
+  constexpr int T = kAccRowTiles;
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const int cand = blockIdx.y, N = prm.N, nrows = N + prm.U;
+  const int r0 = (blockIdx.x * (kAccTileThreads / 32) + (threadIdx.x >> 5)) * 16 * T;
+  const double lna = log(prm.alpha);
+  double xa[T][2][2], e[T][2], acc[T][4];  // xa[tile][ks][h] = X~[row g + 8h][2t + ks], e[tile][h] = e_row of row g + 8h
+#pragma unroll
+  for (int k = 0; k < T; ++k) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const double* x = prm.Xt + static_cast<size_t>(min(r0 + 16 * k + g + 8 * h, N - 1)) * DIM;
+      double nrm = 0.0;
+#pragma unroll
+      for (int d = 0; d < DIM; ++d) nrm = fma(x[d], x[d], nrm);
+      e[k][h] = lna - 0.5 * nrm;
+      xa[k][0][h] = x[2 * t];
+      xa[k][1][h] = x[2 * t + 1];
+    }
+    acc[k][0] = acc[k][1] = acc[k][2] = acc[k][3] = 0.0;
+  }
+  acc_stream_samples<DIM, QP>(prm, cand, sbuf, [&](const double* sx, const double* sc, const double* sh, int cnt) {
+#pragma unroll 1
+    for (int s0 = 0; s0 < cnt; s0 += 8) {
+      const double2 xb = *reinterpret_cast<const double2*>(sx + (s0 + (g >> 1) + 4 * (g & 1)) * DIM + 2 * t);
+      const double h0 = sh[s0 + t], h1 = sh[s0 + t + 4];
+      const double c0 = sc[(s0 + t) * QP + g], c1 = sc[(s0 + t + 4) * QP + g];
+#pragma unroll
+      for (int k = 0; k < T; ++k) {
+        double kv[4] = {e[k][0] + h0, e[k][0] + h1, e[k][1] + h0, e[k][1] + h1};
+        dmma_m16n8k4(kv[0], kv[1], kv[2], kv[3], xa[k][0][0], xa[k][0][1], xb.x);
+        dmma_m16n8k4(kv[0], kv[1], kv[2], kv[3], xa[k][1][0], xa[k][1][1], xb.y);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) kv[i] = exp_tab2k(kv[i]);
+        dmma_m16n8k4(acc[k][0], acc[k][1], acc[k][2], acc[k][3], kv[0], kv[2], c0);
+        dmma_m16n8k4(acc[k][0], acc[k][1], acc[k][2], acc[k][3], kv[1], kv[3], c1);
+      }
+    }
+  });
+  double* R = prm.R + static_cast<size_t>(cand) * QP * nrows;
+#pragma unroll
+  for (int k = 0; k < T; ++k) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r0 + 16 * k + g + 8 * h;
+      if (row < N) {
+        R[static_cast<size_t>(2 * t) * nrows + row] = acc[k][2 * h];
+        R[static_cast<size_t>(2 * t + 1) * nrows + row] = acc[k][2 * h + 1];
+      }
+    }
+  }
+}
+
+template <int DIM, int QP>
+__device__ __forceinline__ void kg_acc_tile_union(const KgAccParams& prm, double* __restrict__ sbuf) {
+  const int cand = blockIdx.y, N = prm.N, U = prm.U, nrows = N + U;
+  const int u = threadIdx.x / kAccUnionSplit, part = threadIdx.x % kAccUnionSplit;
+  const int uc = min(u, U - 1);  // groups past U read a valid union row and store nothing
+  const double* src = prm.Xu + (static_cast<size_t>(cand) * U + uc) * (DIM + 2);
+  double xr[DIM];
+#pragma unroll
+  for (int d = 0; d < DIM; ++d) xr[d] = src[d];
+  const double pk0 = src[DIM];
+  double acc[QP], gu[DIM], gkb = 0.0;
+#pragma unroll
+  for (int a = 0; a < QP; ++a) acc[a] = 0.0;
+#pragma unroll
+  for (int d = 0; d < DIM; ++d) gu[d] = 0.0;
+  acc_stream_samples<DIM, QP>(prm, cand, sbuf, [&](const double* sx, const double* sc, const double* sh, int cnt) {
+#pragma unroll 2
+    for (int i = part; i < cnt; i += kAccUnionSplit) {
+      double xi[DIM], ci[QP];
+#pragma unroll
+      for (int d = 0; d < DIM; d += 2) {
+        const double2 v = *reinterpret_cast<const double2*>(sx + i * DIM + d);
+        xi[d] = v.x;
+        xi[d + 1] = v.y;
+      }
+#pragma unroll
+      for (int a = 0; a < QP; a += 2) {
+        const double2 v = *reinterpret_cast<const double2*>(sc + i * QP + a);
+        ci[a] = v.x;
+        ci[a + 1] = v.y;
+      }
+      const double kv = exp_tab2k(dot_dim<DIM>(xi, xr, 0.0) + (pk0 + sh[i]));
+      double cu = 0.0;
+#pragma unroll
+      for (int a = 0; a < QP; ++a) {
+        acc[a] = fma(ci[a], kv, acc[a]);
+        if (a == uc) cu = ci[a];
+      }
+      const double w = cu * kv;
+      gkb += w;
+#pragma unroll
+      for (int d = 0; d < DIM; ++d) gu[d] = fma(w, xi[d], gu[d]);
+    }
+  });
+  // fixed butterfly over the group's kAccUnionSplit lanes (the same bits on all of them)
+#pragma unroll
+  for (int m = 1; m < kAccUnionSplit; m <<= 1) {
+#pragma unroll
+    for (int a = 0; a < QP; ++a) acc[a] += __shfl_xor_sync(0xffffffffu, acc[a], m);
+#pragma unroll
+    for (int d = 0; d < DIM; ++d) gu[d] += __shfl_xor_sync(0xffffffffu, gu[d], m);
+    gkb += __shfl_xor_sync(0xffffffffu, gkb, m);
+  }
+  if (part != 0 || u >= U) return;
+  double* R = prm.R + static_cast<size_t>(cand) * QP * nrows;
+#pragma unroll
+  for (int a = 0; a < QP; ++a) R[static_cast<size_t>(a) * nrows + N + u] = acc[a];
+  prm.GkB[static_cast<size_t>(cand) * U + u] = gkb;
+#pragma unroll
+  for (int d = 0; d < DIM; ++d) prm.Gu[(static_cast<size_t>(cand) * U + u) * DIM + d] = gu[d];
+}
+
+// grid (row CTAs of kAccTileRowsPerCta training rows + 1 union CTA, candidates); only under the fast path's range
+// contract (exp_tab2k)
+template <int DIM, int QP>
+__global__ void __launch_bounds__(kAccTileThreads) kg_acc_tile_kernel(const __grid_constant__ KgAccParams prm) {
+  extern __shared__ __align__(16) double acc_smem[];
+  exp_table2k_stage();
+  if (blockIdx.x == gridDim.x - 1) {
+    kg_acc_tile_union<DIM, QP>(prm, acc_smem);
+  } else {
+    kg_acc_tile_rows<DIM, QP>(prm, acc_smem);
+  }
+}
+
 // launchers instantiated per (DIM) translation unit
 using KgMcLaunch = void (*)(const KgMcParams&, dim3 grid, size_t smem, cudaStream_t s);
 using KgAccLaunch = void (*)(const KgAccParams&, dim3 grid, cudaStream_t s);
@@ -1883,6 +2049,9 @@ struct KgDispatchEntry {
   // instantiation
   KgMcLaunch mc_big = nullptr;
   KgCtasPerSm mc_big_ctas_per_sm = nullptr;
+  // the tile accumulation kernel (shared-memory path only; the launcher sizes grid.x); null but for the tile
+  // instantiation
+  KgAccLaunch acc_tile = nullptr;
 };
 void register_kg_entries(const KgDispatchEntry* entries, int count);
 // g: derivative observations per point; entries with g <= 8 never dispatch to a wide entry, g > 8 only to one
@@ -1934,6 +2103,18 @@ void launch_kg_acc(const KgAccParams& p, dim3 grid, cudaStream_t s) {
   cudaFuncSetAttribute(kg_acc_kernel<KERNEL, DIM, QP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
   kg_acc_kernel<KERNEL, DIM, QP><<<grid, 128, smem, s>>>(p);
 }
+// grid.y = candidates; grid.x is the kernel's own (row CTAs + the union CTA)
+template <int DIM, int QP>
+void launch_kg_acc_tile(const KgAccParams& p, dim3 grid, cudaStream_t s) {
+  const size_t smem = 2 * static_cast<size_t>(kAccTile) * (DIM + QP + 1) * sizeof(double);
+  grid.x = (p.N + kAccTileRowsPerCta - 1) / kAccTileRowsPerCta + 1;
+  kg_acc_tile_kernel<DIM, QP><<<grid, kAccTileThreads, smem, s>>>(p);
+}
+template <int KERNEL, int DIM, int QP>
+constexpr KgAccLaunch kg_acc_tile_launch() {
+  if constexpr (kg_tile_path<KERNEL, DIM, QP>()) return &launch_kg_acc_tile<DIM, QP>;
+  return nullptr;
+}
 template <int KERNEL, int DIM, int QP>
 void launch_kg_acc_gen(const KgAccParams& p, dim3 grid, cudaStream_t s) {
   const size_t smem = 2 * static_cast<size_t>(kAccTile) * (DIM + QP + 1) * sizeof(double);
@@ -1948,13 +2129,14 @@ size_t kg_smem_bytes(int N, int U) {
 #define CMOE_KG_ENTRY(K, D, Q)                                                                                  \
   {                                                                                                             \
     K, D, Q, &launch_kg_mc<K, D, Q>, nullptr, &launch_kg_acc<K, D, Q>, nullptr, &kg_smem_bytes<D, Q>, false,     \
-        &kg_mc_ctas_per_sm<K, D, Q>, kg_mc_big_launch<K, D, Q>(), kg_mc_big_ctas_per_sm<K, D, Q>()                \
+        &kg_mc_ctas_per_sm<K, D, Q>, kg_mc_big_launch<K, D, Q>(), kg_mc_big_ctas_per_sm<K, D, Q>(),               \
+        kg_acc_tile_launch<K, D, Q>()                                                                           \
   }
 #define CMOE_KG_ENTRY_GEN(K, D, Q)                                                                                \
   {                                                                                                               \
     K, D, Q, &launch_kg_mc<K, D, Q>, &launch_kg_mc_gen<K, D, Q>, &launch_kg_acc<K, D, Q>, &launch_kg_acc_gen<K, D, Q>, \
         &kg_smem_bytes<D, Q>, false, &kg_mc_ctas_per_sm<K, D, Q>, kg_mc_big_launch<K, D, Q>(),                     \
-        kg_mc_big_ctas_per_sm<K, D, Q>()                                                                            \
+        kg_mc_big_ctas_per_sm<K, D, Q>(), kg_acc_tile_launch<K, D, Q>()                                             \
   }
 // union-row counts: 2, 4, 8, 16, 24, 32 (24 serves config 4: q = 4 with 4 derivative observations -> 20 rows; the
 // 32-wide instantiation spilled ~1.5 KB per thread there)
