@@ -500,8 +500,9 @@ void drop_cached_plan(const cmoe_gp* gp) {
   }
 }
 
-void register_kg_entries(const KgDispatchEntry* entries, int count) {
-  for (int i = 0; i < count; ++i) kg_table().push_back(entries[i]);
+bool register_kg_entries(std::initializer_list<KgDispatchEntry> entries) {
+  kg_table().insert(kg_table().end(), entries);
+  return true;
 }
 
 const KgDispatchEntry* find_kg_entry(int kernel, int dim, int Q, int g) {
@@ -510,7 +511,7 @@ const KgDispatchEntry* find_kg_entry(int kernel, int dim, int Q, int g) {
   for (const auto& e : kg_table()) {
     if (e.kernel != kernel || e.dim < dim || e.qp < Q) continue;
     if (e.wide != wide) continue;
-    if (need_gen && e.mc_gen == nullptr) continue;
+    if (need_gen && !e.gen) continue;
     if (!best || e.dim < best->dim || (e.dim == best->dim && e.qp < best->qp)) best = &e;
   }
   return best;
@@ -532,12 +533,10 @@ struct cmoe_kg_plan {
   uint64_t seed = 0;
   cmoe_gd_params inner{};
   std::vector<double> h_inner_bounds, h_discrete, h_Xp;  // host copies (cache key of cmoe_kg_eval)
-  const KgDispatchEntry* entry = nullptr;
+  KgSelect select = nullptr;  // the instantiation's kg_select
+  KgPath path{};              // its builds for this shape, re-selected per upload (the candidates' radius)
   int DIMP = 0, QP = 0, batch = 0, nc = 0;
   int Q = 0, stride = 0;  // rows of the union block U*(1+g); doubles per training point in the operand pack
-  bool use_smem = true;
-  bool smem_fits = true;      // the operand pack fits in shared memory
-  KgMcLaunch mc_big = nullptr;  // the entry's exp_tab2k build, where it runs at the same residency (shared-memory path)
   double rmax_static = 0.0;   // max scaled norm of training / pending / discrete points (see kFastPathRadius)
   int chunk = 0;
   // static device data
@@ -591,7 +590,7 @@ void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
                                     pl.dStale.count ? pl.dStale.p : nullptr, q, gen ? pl.dWt.p : nullptr);
   count_launch();
   if (!gen) {
-    kg_start_kernel<<<dim3(M, nb), kStartThreads, 0, s>>>(spec, N, U, M, DIMP, QP, pl.use_smem ? 1 : 0, pl.dXt.p,
+    kg_start_kernel<<<dim3(M, nb), kStartThreads, 0, s>>>(spec, N, U, M, DIMP, QP, pl.path.use_smem ? 1 : 0, pl.dXt.p,
                                                          pl.dPk.p, pl.dXu.p, pl.dA.p, pl.dStart.p);
     count_launch();
   }
@@ -624,7 +623,6 @@ void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
   prm.outH = pl.dOutH.p;
   prm.stats = pl.dStats.p;
   const int chunks = (mc + pl.chunk - 1) / pl.chunk;
-  const size_t smem_mc = (!gen && pl.use_smem) ? pl.entry->smem_bytes(N, U) : 0;
   if (gen) {
     prm.Wt = pl.dWt.p;
     prm.aw = pl.dAw.p;
@@ -635,13 +633,7 @@ void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
     CMOE_CUDA(cudaMemsetAsync(pl.dWork.p, 0, sizeof(int), s));
   }
   cudaEventRecord(pl.mc_events[ev_idx].first, s);
-  if (gen) {
-    pl.entry->mc_gen(prm, dim3(chunks, nb), 0, s);
-  } else if (pl.use_smem && pl.mc_big) {
-    pl.mc_big(prm, dim3(chunks, nb), smem_mc, s);
-  } else {
-    pl.entry->mc(prm, dim3(chunks, nb), smem_mc, s);
-  }
+  pl.path.mc(prm, chunks, nb, s);
   cudaEventRecord(pl.mc_events[ev_idx].second, s);
   count_launch();
   kg_value_kernel<<<nb, 256, 0, s>>>(mc, pl.dOutVal.p, pl.dBestPost.p, pb.fail.p, pl.dKG.p + c0);
@@ -659,23 +651,18 @@ void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
     ap.recC = pl.dRecC.p;
     ap.outX = pl.dOutX.p;
     ap.outH = pl.dOutH.p;
-    ap.fast_exp = pl.use_smem ? 1 : 0;
+    ap.fast_exp = pl.path.use_smem ? 1 : 0;
+    ap.g = spec.g;
+    for (int k = 0; k < CMOE_MAX_DIM; ++k) ap.derivs[k] = (k < spec.g) ? spec.derivs[k] : 0;
+    for (int d = 0; d < CMOE_MAX_DIM; ++d) ap.inv_len[d] = (d < dim) ? spec.inv_len[d] : 0.0;
     ap.R = pl.dR.p;
     ap.Gu = pl.dGu.p;
     ap.GkB = pl.dGkB.p;
     CMOE_CUDA(cudaMemsetAsync(pl.dR.p, 0, static_cast<size_t>(nb) * QP * (n + Q) * sizeof(double), s));
+    pl.path.acc(ap, nb, s);
     if (gen) {
-      ap.g = spec.g;
-      for (int k = 0; k < CMOE_MAX_DIM; ++k) ap.derivs[k] = (k < spec.g) ? spec.derivs[k] : 0;
-      for (int d = 0; d < CMOE_MAX_DIM; ++d) ap.inv_len[d] = (d < dim) ? spec.inv_len[d] : 0.0;
-      ap.fast_exp = 0;
-      pl.entry->acc_gen(ap, dim3((n + Q + 127) / 128, nb), s);
       kg_g1_kernel<<<nb, 256, 0, s>>>(spec, U, q, QP, DIMP, mc, pb.P.p, pl.dRecC.p, pl.dOutX.p, pl.dG1.p);
       count_launch();
-    } else if (pl.use_smem && pl.entry->acc_tile) {
-      pl.entry->acc_tile(ap, dim3(1, nb), s);
-    } else {
-      pl.entry->acc(ap, dim3((N + U + 127) / 128, nb), s);
     }
     kg_tprime_kernel<<<nb, 256, 0, s>>>(n, Q, QP, pl.dR.p, pb.B.p, pl.dTp.p);
     count_launch(2);
@@ -740,11 +727,12 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     for (int d = 0; d < ps; ++d)
       CMOE_REQUIRE(inner_bounds[2 * d] <= inner_bounds[2 * d + 1], CMOE_ERR_BOUNDS, "Tensor product region is EMPTY.");
     pl->Q = pl->U * (1 + spec.g);
-    pl->entry = find_kg_entry(spec.kernel, dim, pl->Q, spec.g);
-    CMOE_REQUIRE(pl->entry != nullptr, CMOE_ERR_BOUNDS,
+    const KgDispatchEntry* entry = find_kg_entry(spec.kernel, dim, pl->Q, spec.g);
+    CMOE_REQUIRE(entry != nullptr, CMOE_ERR_BOUNDS,
                  "(q+p)*(1+num_derivatives) or dim exceeds the largest compiled q-KG kernel (32 rows, 32 dims)");
-    pl->DIMP = pl->entry->dim;
-    pl->QP = pl->entry->qp;
+    pl->select = entry->select;
+    pl->DIMP = entry->dim;
+    pl->QP = entry->qp;
     const int DIMP = pl->DIMP, QP = pl->QP, Q = pl->Q;
     pl->stride = spec.g > 0 ? 2 : QP + 2;
     cudaStream_t s = gp->stream;
@@ -777,8 +765,6 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const size_t smem_need = pl->entry->smem_bytes(N, U);
-    pl->smem_fits = spec.g == 0 && smem_need <= 200 * 1024;
     {
       // The shared-memory fast path evaluates exp without per-call range guards; that is valid while every scaled
       // coordinate vector it can meet lies within kFastPathRadius length scales of the origin (kg_mc.cuh).
@@ -800,7 +786,7 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
         pl->rmax_static = std::max(pl->rmax_static, c * std::sqrt(static_cast<double>(dim)));
       }
     }
-    pl->use_smem = pl->smem_fits && pl->rmax_static < kFastPathRadius;
+    pl->path = pl->select(N, U, spec.g, pl->rmax_static < kFastPathRadius);
     // candidates per batch bounded by ~3 GiB of per-sample records and start-point tables, and by grid.y of the
     // per-candidate launches (kg_start_kernel, kg_prep_kernel, the MC and accumulation kernels)
     const size_t per_cand = static_cast<size_t>(num_mc) * (QP + DIMP + 2) * sizeof(double) +
@@ -809,18 +795,9 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     pl->batch = static_cast<int>(std::max<size_t>(
         1, std::min<size_t>({static_cast<size_t>(max_candidates), (size_t(3) << 30) / per_cand, kMaxGridY})));
     // samples per CTA: aim for >= ~8 waves of CTAs over the whole batch, between 2 and 16 samples per lane.  A wave is
-    // the fast-path kernel's residency as the occupancy API reports it (2 CTAs per SM for the tile instantiation at the
-    // bench shape); the general path hands its work items to a persistent grid and keeps 3 per SM, the count its
-    // scratch slots are sized for.
-    // The tile instantiation has a second build whose tile rounds use the 2048-entry exp table (16 KB more shared
-    // memory per CTA); it is taken on the shared-memory path wherever it keeps the residency of the 64-entry build, so
-    // that neither the fast path's N range nor its occupancy shrinks.
+    // the selected path's residency (kg_select; 2 CTAs per SM for the tile instantiation at the bench shape).
     {
-      const int per_sm = spec.g == 0 ? std::max(1, pl->entry->mc_ctas_per_sm(pl->use_smem ? smem_need : 0)) : 3;
-      if (pl->smem_fits && pl->entry->mc_big &&
-          pl->entry->mc_big_ctas_per_sm(smem_need) >= std::max(1, pl->entry->mc_ctas_per_sm(smem_need)))
-        pl->mc_big = pl->entry->mc_big;
-      const long long target_ctas = 8LL * sms * per_sm;
+      const long long target_ctas = 8LL * sms * pl->path.ctas_per_sm;
       long long chunk = (static_cast<long long>(pl->batch) * num_mc + target_ctas - 1) / target_ctas;
       chunk = std::max<long long>(2 * kMcThreads, std::min<long long>(chunk, 16 * kMcThreads));
       chunk = (chunk + kMcThreads - 1) / kMcThreads * kMcThreads;
@@ -878,7 +855,7 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     m.M = pl->M;
     m.num_mc = num_mc;
     m.chunk = pl->chunk;
-    m.use_smem = pl->use_smem ? 1 : 0;
+    m.use_smem = pl->path.use_smem ? 1 : 0;
     m.g = spec.g;
     m.Q = Q;
     m.pk_stride = pl->stride;
@@ -962,8 +939,9 @@ int cmoe_kg_plan_upload(cmoe_kg_plan* plan, const double* candidates, int num_ca
         }
         rmax = std::max(rmax, std::sqrt(r2));
       }
-      plan->use_smem = plan->smem_fits && rmax < kFastPathRadius;  // NaN-safe: a NaN norm fails the comparison
-      plan->mcp.use_smem = plan->use_smem ? 1 : 0;
+      // NaN-safe: a NaN norm fails the comparison
+      plan->path = plan->select(plan->gp->N, plan->U, spec.g, rmax < kFastPathRadius);
+      plan->mcp.use_smem = plan->path.use_smem ? 1 : 0;
     }
     plan->dCand.upload(candidates, static_cast<size_t>(num_candidates) * plan->q * plan->gp->spec.dim,
                        plan->gp->stream);

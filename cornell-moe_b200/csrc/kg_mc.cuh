@@ -19,6 +19,7 @@
 #pragma once
 
 #include <algorithm>
+#include <initializer_list>
 #include <type_traits>
 
 #include "device_math.cuh"
@@ -1854,26 +1855,15 @@ __device__ __forceinline__ void kg_acc_body(const KgAccParams& prm, double* __re
   }
 }
 
-template <int KERNEL, int DIM, int QP>
+template <int KERNEL, int DIM, int QP, bool GEN>
 __global__ void __launch_bounds__(128) kg_acc_kernel(const __grid_constant__ KgAccParams prm) {
   extern __shared__ __align__(16) double acc_smem[];
   if (prm.fast_exp) {
     exp_table_stage();
-    kg_acc_body<KERNEL, DIM, QP, true>(prm, acc_smem);
+    kg_acc_body<KERNEL, DIM, QP, true, GEN>(prm, acc_smem);
     return;
   }
-  kg_acc_body<KERNEL, DIM, QP, false>(prm, acc_smem);
-}
-
-template <int KERNEL, int DIM, int QP>
-__global__ void __launch_bounds__(128) kg_acc_gen_kernel(const __grid_constant__ KgAccParams prm) {
-  extern __shared__ __align__(16) double acc_smem[];
-  if (prm.fast_exp) {
-    exp_table_stage();
-    kg_acc_body<KERNEL, DIM, QP, true, true>(prm, acc_smem);
-    return;
-  }
-  kg_acc_body<KERNEL, DIM, QP, false, true>(prm, acc_smem);
+  kg_acc_body<KERNEL, DIM, QP, false, GEN>(prm, acc_smem);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -2032,36 +2022,30 @@ __global__ void __launch_bounds__(kAccTileThreads) kg_acc_tile_kernel(const __gr
   }
 }
 
-// launchers instantiated per (DIM) translation unit
-using KgMcLaunch = void (*)(const KgMcParams&, dim3 grid, size_t smem, cudaStream_t s);
-using KgAccLaunch = void (*)(const KgAccParams&, dim3 grid, cudaStream_t s);
-using KgCtasPerSm = int (*)(size_t operands);
-struct KgDispatchEntry {
-  int kernel, dim, qp;
-  KgMcLaunch mc;      // g == 0 fast path (TMA-staged operands)
-  KgMcLaunch mc_gen;  // general path (derivative observations); may be null
-  KgAccLaunch acc;
-  KgAccLaunch acc_gen;  // general path; null where mc_gen is
-  size_t (*smem_bytes)(int N, int U);
-  bool wide = false;  // general path for 9 <= g <= 31 only (mc and acc are null)
-  KgCtasPerSm mc_ctas_per_sm = nullptr;  // residency of mc (null where mc is)
-  // the build of mc whose tile rounds use exp_tab2k (shared-memory path only) and its residency; null but for the tile
-  // instantiation
-  KgMcLaunch mc_big = nullptr;
-  KgCtasPerSm mc_big_ctas_per_sm = nullptr;
-  // the tile accumulation kernel (shared-memory path only; the launcher sizes grid.x); null but for the tile
-  // instantiation
-  KgAccLaunch acc_tile = nullptr;
-};
-void register_kg_entries(const KgDispatchEntry* entries, int count);
-// g: derivative observations per point; entries with g <= 8 never dispatch to a wide entry, g > 8 only to one
-const KgDispatchEntry* find_kg_entry(int kernel, int dim, int Q, int g);
+// ---------------------------------------------------------------------------------------------------------------
+// Host dispatch.  Every launcher works out its own grid and dynamic shared memory from its parameters, the sample
+// chunks per candidate (MC launchers) and the candidates of the batch.  kg_select picks an instantiation's launchers
+// for a plan's shape; the compiled set is the entry lists at the end of this file.
+// ---------------------------------------------------------------------------------------------------------------
+using KgMcLaunch = void (*)(const KgMcParams&, int chunks, int nb, cudaStream_t s);
+using KgAccLaunch = void (*)(const KgAccParams&, int nb, cudaStream_t s);
 
+// kg_mc_kernel's operands staged in shared memory (the g == 0 fast path)
+template <int DIM, int QP>
+size_t kg_smem_bytes(int N, int U) {
+  return (static_cast<size_t>(N) * (DIM + QP + 2) + static_cast<size_t>(U) * (DIM + 2)) * sizeof(double);
+}
+// the accumulation kernels' two sample tiles (acc_stream_samples)
+template <int DIM, int QP>
+constexpr size_t kAccSmemBytes = 2 * static_cast<size_t>(kAccTile) * (DIM + QP + 1) * sizeof(double);
+
+// grid (sample chunks, candidates); the operands go to shared memory when p.use_smem is set
 template <int KERNEL, int DIM, int QP, bool BIG = false>
-void launch_kg_mc(const KgMcParams& p, dim3 grid, size_t smem, cudaStream_t s) {
+void launch_kg_mc(const KgMcParams& p, int chunks, int nb, cudaStream_t s) {
+  const size_t smem = p.use_smem ? kg_smem_bytes<DIM, QP>(p.N, p.U) : 0;
   // function attributes are per device: set on every launch (cheap), never cached process-wide
   cudaFuncSetAttribute(kg_mc_kernel<KERNEL, DIM, QP, BIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  kg_mc_kernel<KERNEL, DIM, QP, BIG><<<grid, kMcThreads, smem, s>>>(p);
+  kg_mc_kernel<KERNEL, DIM, QP, BIG><<<dim3(chunks, nb), kMcThreads, smem, s>>>(p);
 }
 // resident CTAs of kg_mc_kernel per SM on the current device with `smem` bytes of staged operands (0: global memory)
 template <int KERNEL, int DIM, int QP, bool BIG = false>
@@ -2073,18 +2057,9 @@ int kg_mc_ctas_per_sm(size_t smem) {
       cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kg_mc_kernel<KERNEL, DIM, QP, BIG>, kMcThreads, smem));
   return per_sm;
 }
-template <int KERNEL, int DIM, int QP>
-constexpr KgMcLaunch kg_mc_big_launch() {
-  if constexpr (kg_tile_path<KERNEL, DIM, QP>()) return &launch_kg_mc<KERNEL, DIM, QP, true>;
-  return nullptr;
-}
-template <int KERNEL, int DIM, int QP>
-constexpr KgCtasPerSm kg_mc_big_ctas_per_sm() {
-  if constexpr (kg_tile_path<KERNEL, DIM, QP>()) return &kg_mc_ctas_per_sm<KERNEL, DIM, QP, true>;
-  return nullptr;
-}
+// persistent grid over the p.work_total = chunks * candidates work items
 template <int KERNEL, int DIM, int QP, bool WIDE = false>
-void launch_kg_mc_gen(const KgMcParams& p, dim3, size_t, cudaStream_t s) {
+void launch_kg_mc_gen(const KgMcParams& p, int, int, cudaStream_t s) {
   int dev = 0, sms = 1, per_sm = 1;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -2097,61 +2072,97 @@ void launch_kg_mc_gen(const KgMcParams& p, dim3, size_t, cudaStream_t s) {
   const int grid = std::max(1, std::min(std::min(p.aw_slots, p.work_total), sms * std::max(1, per_sm)));
   kg_mc_gen_kernel<KERNEL, DIM, QP, WIDE><<<grid, kMcThreads, ring_bytes, s>>>(p);
 }
-template <int KERNEL, int DIM, int QP>
-void launch_kg_acc(const KgAccParams& p, dim3 grid, cudaStream_t s) {
-  const size_t smem = 2 * static_cast<size_t>(kAccTile) * (DIM + QP + 1) * sizeof(double);
-  cudaFuncSetAttribute(kg_acc_kernel<KERNEL, DIM, QP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-  kg_acc_kernel<KERNEL, DIM, QP><<<grid, 128, smem, s>>>(p);
+// grid (128-row CTAs, candidates) over the (N + U) (1 + g) rows
+template <int KERNEL, int DIM, int QP, bool GEN>
+void launch_kg_acc(const KgAccParams& p, int nb, cudaStream_t s) {
+  const int nrows = (p.N + p.U) * (GEN ? 1 + p.g : 1);
+  cudaFuncSetAttribute(kg_acc_kernel<KERNEL, DIM, QP, GEN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
+  kg_acc_kernel<KERNEL, DIM, QP, GEN><<<dim3((nrows + 127) / 128, nb), 128, kAccSmemBytes<DIM, QP>, s>>>(p);
 }
-// grid.y = candidates; grid.x is the kernel's own (row CTAs + the union CTA)
+// grid (row CTAs + the union CTA, candidates)
 template <int DIM, int QP>
-void launch_kg_acc_tile(const KgAccParams& p, dim3 grid, cudaStream_t s) {
-  const size_t smem = 2 * static_cast<size_t>(kAccTile) * (DIM + QP + 1) * sizeof(double);
-  grid.x = (p.N + kAccTileRowsPerCta - 1) / kAccTileRowsPerCta + 1;
-  kg_acc_tile_kernel<DIM, QP><<<grid, kAccTileThreads, smem, s>>>(p);
-}
-template <int KERNEL, int DIM, int QP>
-constexpr KgAccLaunch kg_acc_tile_launch() {
-  if constexpr (kg_tile_path<KERNEL, DIM, QP>()) return &launch_kg_acc_tile<DIM, QP>;
-  return nullptr;
-}
-template <int KERNEL, int DIM, int QP>
-void launch_kg_acc_gen(const KgAccParams& p, dim3 grid, cudaStream_t s) {
-  const size_t smem = 2 * static_cast<size_t>(kAccTile) * (DIM + QP + 1) * sizeof(double);
-  cudaFuncSetAttribute(kg_acc_gen_kernel<KERNEL, DIM, QP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-  kg_acc_gen_kernel<KERNEL, DIM, QP><<<grid, 128, smem, s>>>(p);
-}
-template <int DIM, int QP>
-size_t kg_smem_bytes(int N, int U) {
-  return (static_cast<size_t>(N) * (DIM + QP + 2) + static_cast<size_t>(U) * (DIM + 2)) * sizeof(double);
+void launch_kg_acc_tile(const KgAccParams& p, int nb, cudaStream_t s) {
+  const dim3 grid((p.N + kAccTileRowsPerCta - 1) / kAccTileRowsPerCta + 1, nb);
+  kg_acc_tile_kernel<DIM, QP><<<grid, kAccTileThreads, kAccSmemBytes<DIM, QP>, s>>>(p);
 }
 
-#define CMOE_KG_ENTRY(K, D, Q)                                                                                  \
-  {                                                                                                             \
-    K, D, Q, &launch_kg_mc<K, D, Q>, nullptr, &launch_kg_acc<K, D, Q>, nullptr, &kg_smem_bytes<D, Q>, false,     \
-        &kg_mc_ctas_per_sm<K, D, Q>, kg_mc_big_launch<K, D, Q>(), kg_mc_big_ctas_per_sm<K, D, Q>(),               \
-        kg_acc_tile_launch<K, D, Q>()                                                                           \
+// A plan's builds for its shape: the MC and accumulation launchers, whether the operands are staged in shared memory
+// (the fast path, whose exps rely on kFastPathRadius's range contract) and the resident CTAs per SM that the sample
+// chunks are sized for.
+struct KgPath {
+  KgMcLaunch mc;
+  KgAccLaunch acc;
+  bool use_smem;
+  int ctas_per_sm;
+};
+using KgSelect = KgPath (*)(int N, int U, int g, bool fast);
+
+// The builds an entry compiles.
+enum KgBuilds {
+  kKgFast,     // the g == 0 path only
+  kKgFastGen,  // that and the general path for derivative observations (g <= 8)
+  kKgWide,     // the wide general path only (9 <= g <= 31)
+};
+
+// An instantiation's builds for N training points, U union points, g derivative observations per point and whether the
+// fast path's range contract holds.  find_kg_entry hands g > 0 only to entries with a general path, g > 8 only to wide
+// ones.
+//  * The general path hands its work items to a persistent grid and keeps 3 CTAs per SM, the count its scratch slots
+//    are sized for; its exps are the guarded ones.
+//  * g == 0 stages the operands in shared memory where they fit in 200 KiB and the range contract holds, and sizes the
+//    chunks for kg_mc_kernel's residency as the occupancy API reports it.  There the tile instantiation takes its tile
+//    accumulation kernel, and the build of kg_mc_kernel whose tile rounds use the 2048-entry exp table (16 KB more
+//    shared memory per CTA) wherever that build keeps the residency of the 64-entry one, so that neither the fast
+//    path's N range nor its occupancy shrinks.
+template <int KERNEL, int DIM, int QP, KgBuilds B>
+KgPath kg_select(int N, int U, int g, bool fast) {
+  if constexpr (B == kKgWide) {
+    return {&launch_kg_mc_gen<KERNEL, DIM, QP, true>, &launch_kg_acc<KERNEL, DIM, QP, true>, false, 3};
+  } else {
+    if constexpr (B == kKgFastGen) {
+      if (g > 0) return {&launch_kg_mc_gen<KERNEL, DIM, QP>, &launch_kg_acc<KERNEL, DIM, QP, true>, false, 3};
+    }
+    const size_t smem = kg_smem_bytes<DIM, QP>(N, U);
+    const bool use_smem = smem <= 200 * 1024 && fast;
+    const int per_sm = std::max(1, kg_mc_ctas_per_sm<KERNEL, DIM, QP>(use_smem ? smem : 0));
+    if constexpr (kg_tile_path<KERNEL, DIM, QP>()) {
+      if (use_smem) {
+        const bool big = kg_mc_ctas_per_sm<KERNEL, DIM, QP, true>(smem) >= per_sm;
+        return {big ? &launch_kg_mc<KERNEL, DIM, QP, true> : &launch_kg_mc<KERNEL, DIM, QP>,
+                &launch_kg_acc_tile<DIM, QP>, true, per_sm};
+      }
+    }
+    return {&launch_kg_mc<KERNEL, DIM, QP>, &launch_kg_acc<KERNEL, DIM, QP, false>, use_smem, per_sm};
   }
-#define CMOE_KG_ENTRY_GEN(K, D, Q)                                                                                \
-  {                                                                                                               \
-    K, D, Q, &launch_kg_mc<K, D, Q>, &launch_kg_mc_gen<K, D, Q>, &launch_kg_acc<K, D, Q>, &launch_kg_acc_gen<K, D, Q>, \
-        &kg_smem_bytes<D, Q>, false, &kg_mc_ctas_per_sm<K, D, Q>, kg_mc_big_launch<K, D, Q>(),                     \
-        kg_mc_big_ctas_per_sm<K, D, Q>(), kg_acc_tile_launch<K, D, Q>()                                             \
-  }
-// union-row counts: 2, 4, 8, 16, 24, 32 (24 serves config 4: q = 4 with 4 derivative observations -> 20 rows; the
-// 32-wide instantiation spilled ~1.5 KB per thread there)
-#define CMOE_KG_ENTRIES_FOR_DIM(D)                                                                              \
-  CMOE_KG_ENTRY(0, D, 2), CMOE_KG_ENTRY(0, D, 4), CMOE_KG_ENTRY_GEN(0, D, 8), CMOE_KG_ENTRY_GEN(0, D, 16),       \
-      CMOE_KG_ENTRY_GEN(0, D, 24), CMOE_KG_ENTRY_GEN(0, D, 32), CMOE_KG_ENTRY(1, D, 2), CMOE_KG_ENTRY(1, D, 4),  \
-      CMOE_KG_ENTRY_GEN(1, D, 8), CMOE_KG_ENTRY_GEN(1, D, 16), CMOE_KG_ENTRY_GEN(1, D, 24),                    \
-      CMOE_KG_ENTRY_GEN(1, D, 32)
+}
+
+// One compiled instantiation in the run-time dispatch table of kg.cu.
+struct KgDispatchEntry {
+  int kernel, dim, qp;
+  bool gen;   // has the general path (derivative observations)
+  bool wide;  // the general path for 9 <= g <= 31 only
+  KgSelect select;
+};
+template <int KERNEL, int DIM, int QP, KgBuilds B>
+constexpr KgDispatchEntry kg_entry() {
+  return {KERNEL, DIM, QP, B != kKgFast, B == kKgWide, &kg_select<KERNEL, DIM, QP, B>};
+}
+bool register_kg_entries(std::initializer_list<KgDispatchEntry> entries);
+// g: derivative observations per point; entries with g <= 8 never dispatch to a wide entry, g > 8 only to one
+const KgDispatchEntry* find_kg_entry(int kernel, int dim, int Q, int g);
+
+// The compiled set, per padded dimension D (kg_mc_inst_*.cu).  Union-row counts: 2, 4, 8, 16, 24, 32 (24 serves
+// config 4: q = 4 with 4 derivative observations -> 20 rows; the 32-wide instantiation spilled ~1.5 KB per thread there)
+#define CMOE_KG_ENTRIES_FOR_DIM(D)                                                                                    \
+  kg_entry<0, D, 2, kKgFast>(), kg_entry<0, D, 4, kKgFast>(), kg_entry<0, D, 8, kKgFastGen>(),                        \
+      kg_entry<0, D, 16, kKgFastGen>(), kg_entry<0, D, 24, kKgFastGen>(), kg_entry<0, D, 32, kKgFastGen>(),           \
+      kg_entry<1, D, 2, kKgFast>(), kg_entry<1, D, 4, kKgFast>(), kg_entry<1, D, 8, kKgFastGen>(),                    \
+      kg_entry<1, D, 16, kKgFastGen>(), kg_entry<1, D, 24, kKgFastGen>(), kg_entry<1, D, 32, kKgFastGen>()
 
 // Wide general path (9 <= g <= 31, kg_mc_wide_*.cu): only what such a g can reach — dim >= 9 (padded 12, 16, 32) and
 // Q = U (1 + g) >= 10 (widths 16, 24, 32).  The accumulation kernel does not depend on g and is the narrow entry's.
-#define CMOE_KG_ENTRY_WIDE(K, D, Q) \
-  { K, D, Q, nullptr, &launch_kg_mc_gen<K, D, Q, true>, nullptr, &launch_kg_acc_gen<K, D, Q>, &kg_smem_bytes<D, Q>, true }
 #define CMOE_KG_WIDE_ENTRIES_FOR_DIM(D)                                                                    \
-  CMOE_KG_ENTRY_WIDE(0, D, 16), CMOE_KG_ENTRY_WIDE(0, D, 24), CMOE_KG_ENTRY_WIDE(0, D, 32),                 \
-      CMOE_KG_ENTRY_WIDE(1, D, 16), CMOE_KG_ENTRY_WIDE(1, D, 24), CMOE_KG_ENTRY_WIDE(1, D, 32)
+  kg_entry<0, D, 16, kKgWide>(), kg_entry<0, D, 24, kKgWide>(), kg_entry<0, D, 32, kKgWide>(),             \
+      kg_entry<1, D, 16, kKgWide>(), kg_entry<1, D, 24, kKgWide>(), kg_entry<1, D, 32, kKgWide>()
 
 }  // namespace cmoe

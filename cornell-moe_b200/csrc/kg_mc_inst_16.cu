@@ -4,9 +4,6 @@
 
 namespace cmoe {
 namespace {
-const KgDispatchEntry kEntries[] = {CMOE_KG_ENTRIES_FOR_DIM(16)};
-struct Registrar {
-  Registrar() { register_kg_entries(kEntries, static_cast<int>(sizeof(kEntries) / sizeof(kEntries[0]))); }
-} registrar;
+const bool registered = register_kg_entries({CMOE_KG_ENTRIES_FOR_DIM(16)});
 }  // namespace
 }  // namespace cmoe

@@ -57,7 +57,7 @@ def _compiled_wide_entries():
         src = f.read()
     m = re.search(r"#define CMOE_KG_WIDE_ENTRIES_FOR_DIM\(D\)((?:.*\\\n)*.*)", src)
     assert m, "CMOE_KG_WIDE_ENTRIES_FOR_DIM not found in kg_mc.cuh"
-    per_dim = [(int(k), int(qp)) for k, qp in re.findall(r"CMOE_KG_ENTRY_WIDE\((\d+),\s*D,\s*(\d+)\)", m.group(1))]
+    per_dim = [(int(k), int(qp)) for k, qp in re.findall(r"kg_entry<(\d+),\s*D,\s*(\d+),\s*kKgWide>\(\)", m.group(1))]
     dims = []
     for name in sorted(os.listdir(CSRC)):
         if re.fullmatch(r"kg_mc_wide_\d+\.cu", name):

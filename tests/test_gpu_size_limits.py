@@ -293,13 +293,13 @@ def _compiled_kg_entries():
         src = f.read()
     m = re.search(r"#define CMOE_KG_ENTRIES_FOR_DIM\(D\)((?:.*\\\n)*.*)", src)
     assert m, "CMOE_KG_ENTRIES_FOR_DIM not found in kg_mc.cuh"
-    per_dim = [(bool(gen), int(kern), int(qp)) for gen, kern, qp in
-               re.findall(r"CMOE_KG_ENTRY(_GEN)?\((\d+),\s*D,\s*(\d+)\)", m.group(1))]
+    per_dim = [(builds == "kKgFastGen", int(kern), int(qp)) for kern, qp, builds in
+               re.findall(r"kg_entry<(\d+),\s*D,\s*(\d+),\s*(kKgFast|kKgFastGen)>\(\)", m.group(1))]
     dims = []
     for path in glob.glob(os.path.join(CSRC, "kg_mc_inst_*.cu")):
         with open(path) as f:
             dims += [int(v) for v in re.findall(r"CMOE_KG_ENTRIES_FOR_DIM\((\d+)\)", f.read())]
-    # every entry has kg_mc_kernel; the _GEN ones add kg_mc_gen_kernel
+    # every entry has kg_mc_kernel; the kKgFastGen ones add kg_mc_gen_kernel
     return ({(kern, dim, qp, False) for dim in dims for _, kern, qp in per_dim} |
             {(kern, dim, qp, True) for dim in dims for gen, kern, qp in per_dim if gen})
 
