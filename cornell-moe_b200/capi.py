@@ -316,6 +316,19 @@ class GaussianProcess:
         _check(rc, info.value)
         return out
 
+    def lower_confidence_bound(self, candidates, num_to_sample):
+        """cmoe_lcb_select: the reference's LCB batch selection over ``candidates`` [C, dim].  Returns (indices [q] into
+        candidates, mean [C], sd [C]); mean and sd are the round-0 screen.  The GP is not modified."""
+        cand = _f64(candidates).reshape(-1, self.dim)
+        idx = np.empty(max(int(num_to_sample), 0), dtype=np.int32)
+        mean = np.empty(cand.shape[0])
+        sd = np.empty(cand.shape[0])
+        info = ctypes.c_int(0)
+        rc = lib().cmoe_lcb_select(self.h, _d(cand), cand.shape[0], int(num_to_sample), _i(idx), _d(mean), _d(sd),
+                                   None, ctypes.byref(info))
+        _check(rc, info.value)
+        return idx, mean, sd
+
 
 def latin_hypercube(num_sets, num_pts, domain_bounds, seed=0, first_draw=0, device=0):
     """cmoe_latin_hypercube: [num_sets, num_pts, dim] points; set b is a pure function of (seed, first_draw + b).

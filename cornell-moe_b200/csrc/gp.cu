@@ -212,6 +212,13 @@ void append_points(cmoe_gp* gp, const double* new_points, const double* new_valu
 }
 
 
+void scale_points(const cmoe_gp& gp, const double* P, int m, DevBuf<double>& Ps, cudaStream_t s) {
+  const int dim = gp.spec.dim;
+  ensure_scaled_points(Ps, m, dim, s);
+  scale_points_kernel<<<(m * dim + 255) / 256, 256, 0, s>>>(gp.spec, centre_of(gp.hX, gp.N, dim), P, m, Ps.p);
+  count_launch();
+}
+
 cmoe_gp* clone_gp_to_device(const cmoe_gp* src, int device) {
   require_device(device);
   std::unique_ptr<cmoe_gp> gp(new cmoe_gp());

@@ -1318,6 +1318,31 @@ PYBIND11_MODULE(GPP, m) {
         py::arg("derivatives"), py::arg("num_derivatives"), py::arg("initial_positions"), py::arg("num_walkers"),
         py::arg("num_steps"), py::arg("noisy"), py::arg("use_default_prior"), py::arg("seed"),
         py::arg("first_step") = 0);
+  // lower_confidence_bound_optimization(gaussian_process, candidate_pts, num_candidates, num_to_sample)
+  // Not in the reference module: the body of lower_confidence_bound.py:52-80 in one device call (cmoe_lcb_select,
+  // DESIGN.md K13).  `gaussian_process` is a GaussianProcess or a wrapper holding one as `_gaussian_process`;
+  // candidate_pts is the flat [num_candidates][dim] list.  Returns the num_to_sample * dim coordinates as a flat list.
+  // The GP is left unchanged (the reference leaves its fantasy points in it).
+  m.def("lower_confidence_bound_optimization",
+        [](const py::object& gaussian_process, const py::list& candidate_pts, int num_candidates,
+           int num_to_sample) -> py::list {
+          py::object o = gaussian_process;
+          if (!py::isinstance<GaussianProcess>(o) && py::hasattr(o, "_gaussian_process")) o = o.attr("_gaussian_process");
+          const GaussianProcess& gp = o.cast<const GaussianProcess&>();
+          const int dim = gp.dim();
+          const auto P = to_vec(candidate_pts, static_cast<size_t>(std::max(num_candidates, 0)) * dim);
+          std::vector<int> sel(std::max(num_to_sample, 0));
+          int info = 0;
+          check(cmoe_lcb_select(gp.h, P.data(), num_candidates, num_to_sample, sel.data(), nullptr, nullptr, nullptr,
+                                &info),
+                info);
+          std::vector<double> out(sel.size() * dim);
+          for (size_t i = 0; i < sel.size(); ++i)
+            std::copy(P.begin() + static_cast<size_t>(sel[i]) * dim, P.begin() + static_cast<size_t>(sel[i] + 1) * dim,
+                      out.begin() + i * dim);
+          return to_list(out);
+        },
+        py::arg("gaussian_process"), py::arg("candidate_pts"), py::arg("num_candidates"), py::arg("num_to_sample"));
   m.def("heuristic_expected_improvement_optimization",
         [](const py::args&, const py::kwargs&) -> py::object {
           not_on_path("heuristic_expected_improvement_optimization");

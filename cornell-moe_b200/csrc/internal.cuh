@@ -165,6 +165,9 @@ constexpr size_t kMaxGridY = 65535;
 void fit_gp(cmoe_gp* gp, bool mean_change);
 // bit-identical copy of a fitted GP on another device (peer copies of the factor; no refit)
 cmoe_gp* clone_gp_to_device(const cmoe_gp* gp, int device);
+// Ps <- the m points P (device) in the length-scaled, centred coordinates of gp's covariance build (the Xs argument of
+// build_covariance), exactly as append_points scales the points it adds; Ps is padded as build_covariance needs.
+void scale_points(const cmoe_gp& gp, const double* P, int m, DevBuf<double>& Ps, cudaStream_t s);
 // ---- kg.cu ----
 void drop_cached_plan(const cmoe_gp* gp);
 
@@ -195,6 +198,19 @@ constexpr int kMaxChunkSets = 4096;
 // zero on entry and receives 0 or the 1-based leading minor of the first pivot that fails `> 1e-16`.  `stage` holds the
 // diagonal factors until the end (nsets * ceil(Q/64) * 64 * 64 doubles).  Asynchronous on `s`.
 void potrf_batched(double* A, int Q, int nsets, int* fail, DevBuf<double>& stage, cudaStream_t s);
+// Device workspace of the sampling calls and of the LCB screen (lcb.cu), kept on the GP handle (cmoe_gp::sample_ws) and
+// grown on demand, so repeated calls do not allocate and free up to kSampleWorkspaceBytes each time.  Released with the
+// handle.
+struct SampleWork {
+  DevBuf<double> P, V, A, mu, y, part_v, opt, stage, table;
+  DevBuf<int> dPs, fail, part_i, amin;
+};
+
+// ---- lcb.cu: LCB batch selection (DESIGN.md K13) ----------------------------------------------------------------
+// rows of the selected-set block, (q - 1)(1 + g): its bordered factor is built by one CTA, round by round
+constexpr int kMaxLcbSelectedRows = 1024;
+// the rounds' per-candidate vectors w(x), C' (q - 1)(1 + g) doubles, are held in one workspace-sized buffer
+constexpr size_t kMaxLcbRoundDoubles = kSampleWorkspaceBytes / sizeof(double);
 
 // ---- posterior.cu -------------------------------------------------------------------------------------------
 constexpr int kMaxQ = 96;  // largest (q+p)*(1+num_derivatives) handled by the per-set kernels

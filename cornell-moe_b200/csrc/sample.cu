@@ -412,13 +412,6 @@ void potrf_batched(double* A, int Q, int nsets, int* fail, DevBuf<double>& stage
 
 namespace {
 
-// Device workspace of the sampling calls, kept on the GP handle (cmoe_gp::sample_ws) and grown on demand, so repeated
-// calls do not allocate and free up to kSampleWorkspaceBytes each time.  Released with the handle.
-struct SampleWork {
-  DevBuf<double> P, V, A, mu, y, part_v, opt, stage, table;
-  DevBuf<int> dPs, fail, part_i, amin;
-};
-
 // One chunk of nc sets whose points are in w.P: fills w.mu, w.A (factor), w.y, w.amin and w.fail.
 void sample_chunk(const cmoe_gp& gp, SampleWork& w, int nc, int num, int gs, uint64_t seed, uint64_t draw0,
                   const double* dtable, double jitter, cudaStream_t s) {

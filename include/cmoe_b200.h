@@ -228,6 +228,26 @@ int cmoe_latin_hypercube(uint64_t seed, uint64_t first_draw, int num_sets, int n
 int cmoe_gp_sample_global_optima(const cmoe_gp* gp, int num_optima, int inner_number, const double* domain_bounds,
                                  uint64_t seed, uint64_t first_draw, double jitter, double* points_optima, int* info);
 
+/* ---- lower-confidence-bound batch selection ----------------------------------------------------------------------
+ * lower_confidence_bound_optimization (moe/optimal_learning/python/cpp_wrappers/lower_confidence_bound.py:52-80) in one
+ * call.  candidates [num_candidates][dim].  mu(x) is the value mean, sigma(x) the square root of the value variance.
+ *   selected[0] = argmin(mu - sigma) (first occurrence); the satisfied set is {x : mu - sigma <= min(mu + sigma)} in
+ *   candidate order; selected[i], i = 1 .. num_to_sample - 1, = argmax over the satisfied set (first occurrence) of
+ *   sigma on the GP to which selected[0 .. i-1] have been added as noisy observations with the GP's own derivative rows
+ *   and per-type noise (the reference's refit; here a bordered update, the handle is not modified).  A point may be
+ *   selected again.  selected[num_to_sample] holds indices into `candidates`.
+ * mean[num_candidates], sd[num_candidates] (the round-0 mu and sigma) and *num_satisfied may be NULL.
+ * Candidates are screened in chunks of max(1, floor(2^31 / (8 n))) (n = num_sampled (1 + num_derivatives)) in the
+ * handle's sampling workspace; a candidate's mu and sigma do not depend on the chunking.
+ * Errors: a candidate variance that is not > 1e-16 (round 0, or on a surviving candidate in a later round) ->
+ * CMOE_ERR_SINGULAR, *info = 1, the lowest such candidate index in cmoe_last_error(); a pivot of the enlarged matrix
+ * that is not > 1e-16 -> CMOE_ERR_SINGULAR, *info = its leading minor counted from the GP's n rows, as
+ * cmoe_gp_add_sampled_points counts it.  Limits (CMOE_ERR_BOUNDS): (num_to_sample - 1)(1 + num_derivatives) <= 1024,
+ * and num_satisfied (num_to_sample - 1)(1 + num_derivatives) <= 2^28 (checked after the screen).  Non-finite
+ * candidates -> CMOE_ERR_INVALID_VALUE. */
+int cmoe_lcb_select(const cmoe_gp* gp, const double* candidates, int num_candidates, int num_to_sample, int* selected,
+                    double* mean, double* sd, int* num_satisfied, int* info);
+
 /* ---- q-EI Monte Carlo, batched over candidates ----------------------------------------------------------------
  * Replaces ExpectedImprovementEvaluator::ComputeExpectedImprovement / ComputeGradExpectedImprovement
  * (gpp_math.cpp:1991-2126); Python boundary compute_expected_improvement / compute_grad_expected_improvement /
