@@ -67,6 +67,11 @@ class KGStats(ctypes.Structure):
                 ("line_batches", ctypes.c_uint64)]
 
 
+class RffTable(ctypes.Structure):
+    """cmoe_rff_table: the numbers that replace Philox in cmoe_gp_sample_rff_optima."""
+    _fields_ = [("omega", _dp), ("b", _dp), ("z", _dp), ("eps", _dp)]
+
+
 _lib = None
 
 
@@ -315,6 +320,46 @@ class GaussianProcess:
                                                 ctypes.c_double(jitter), _d(out), ctypes.byref(info))
         _check(rc, info.value)
         return out
+
+    def sample_rff_optima(self, num_features, num_points, domain_bounds, grid, seed=0, first_draw=0, table=None,
+                          return_functions=False):
+        """cmoe_gp_sample_rff_optima: minimisers of num_points random-Fourier-feature draws of the GP, each found on
+        ``grid`` [G, dim] and refined inside ``domain_bounds`` ([dim, 2] or flat).  Sample s uses Philox draw
+        first_draw + s, or row s of ``table`` (a dict with omega [P, F, dim], b [P, F], z [P, F] and, when
+        num_sampled (1 + g) < F, eps [P, num_sampled (1 + g)]).  Returns (points [P, dim], values [P]); with
+        return_functions, also a dict of each sample function f(x) = sqrt(2 alpha / F) theta . cos(omega x + b):
+        omega [P, F, dim] (the frequencies, Omega / lengths), b [P, F], theta [P, F]."""
+        F, P = int(num_features), int(num_points)
+        bounds = _f64(domain_bounds).ravel()
+        if bounds.size != 2 * self.dim:
+            raise BoundsError(ERR_BOUNDS, f"domain_bounds needs 2*dim = {2 * self.dim} values, got {bounds.size}")
+        grid = _f64(grid).reshape(-1, self.dim)
+        tab = None
+        keep = []
+        if table is not None:
+            M = self.n
+            need = {"omega": P * F * self.dim, "b": P * F, "z": P * F, "eps": P * M if M < F else None}
+            tab = RffTable()
+            for name in ("omega", "b", "z", "eps"):
+                a = table.get(name)
+                if a is not None:
+                    a = _f64(a).ravel()
+                    keep.append(a)
+                if need[name] is not None and (a is None or a.size != need[name]):
+                    got = "none" if a is None else a.size
+                    raise BoundsError(ERR_BOUNDS, f"table[{name!r}] needs {need[name]} values, got {got}")
+                setattr(tab, name, _d(a))
+        pts = np.empty((max(P, 0), self.dim))
+        vals = np.empty(max(P, 0))
+        fun = ({"omega": np.empty((P, F, self.dim)), "b": np.empty((P, F)), "theta": np.empty((P, F))}
+               if return_functions and P >= 1 and F >= 1 else None)
+        info = ctypes.c_int(0)
+        rc = lib().cmoe_gp_sample_rff_optima(self.h, F, P, _d(bounds), _d(grid), grid.shape[0], ctypes.c_uint64(seed),
+                                             ctypes.c_uint64(first_draw), None if tab is None else ctypes.byref(tab),
+                                             _d(pts), _d(vals), _d(fun and fun["omega"]), _d(fun and fun["b"]),
+                                             _d(fun and fun["theta"]), ctypes.byref(info))
+        _check(rc, info.value)
+        return (pts, vals, fun) if return_functions else (pts, vals)
 
     def lower_confidence_bound(self, candidates, num_to_sample):
         """cmoe_lcb_select: the reference's LCB batch selection over ``candidates`` [C, dim].  Returns (indices [q] into

@@ -1343,6 +1343,32 @@ PYBIND11_MODULE(GPP, m) {
           return to_list(out);
         },
         py::arg("gaussian_process"), py::arg("candidate_pts"), py::arg("num_candidates"), py::arg("num_to_sample"));
+  // sample_from_global_optima(gaussian_process, num_features, domain_bounds, grid, num_grid, num_points)
+  // Not in the reference module: random_features.sample_from_global_optima (random_features.py:171-175) in one device
+  // call (cmoe_gp_sample_rff_optima, DESIGN.md K14).  `gaussian_process` is a GaussianProcess or a wrapper holding one
+  // as `_gaussian_process`; domain_bounds is the flat [dim][2] list, grid the flat [num_grid][dim] list.  Uses the GP's
+  // (seed, next draw), one draw per point, as sample_global_optima does.  Returns the num_points * dim coordinates as
+  // a flat list.  The GP is not modified.
+  m.def("sample_from_global_optima",
+        [](const py::object& gaussian_process, int num_features, const py::list& domain_bounds, const py::list& grid,
+           int num_grid, int num_points) -> py::list {
+          py::object o = gaussian_process;
+          if (!py::isinstance<GaussianProcess>(o) && py::hasattr(o, "_gaussian_process")) o = o.attr("_gaussian_process");
+          GaussianProcess& gp = o.cast<GaussianProcess&>();
+          const int dim = gp.dim();
+          const auto B = to_vec(domain_bounds, 2 * static_cast<size_t>(dim));
+          const auto Gr = to_vec(grid, static_cast<size_t>(std::max(num_grid, 0)) * dim);
+          std::vector<double> out(static_cast<size_t>(std::max(num_points, 0)) * dim), vals(std::max(num_points, 0));
+          int info = 0;
+          check(cmoe_gp_sample_rff_optima(gp.h, num_features, num_points, B.data(), Gr.data(), num_grid, gp.seed_,
+                                          gp.next_draw_, nullptr, out.data(), vals.data(), nullptr, nullptr, nullptr,
+                                          &info),
+                info);
+          gp.next_draw_ += static_cast<uint64_t>(num_points);
+          return to_list(out);
+        },
+        py::arg("gaussian_process"), py::arg("num_features"), py::arg("domain_bounds"), py::arg("grid"),
+        py::arg("num_grid"), py::arg("num_points"));
   m.def("heuristic_expected_improvement_optimization",
         [](const py::args&, const py::kwargs&) -> py::object {
           not_on_path("heuristic_expected_improvement_optimization");

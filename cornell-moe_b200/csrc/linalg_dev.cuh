@@ -367,5 +367,100 @@ __device__ __forceinline__ void tile_mma64(const double* As, const double* Bs, d
   }
 }
 
+// acc += Vr^T Vc for one 64 x 64 Gram tile: Vr / Vc are the tile's first row / column operand, column-major with
+// leading dimension (and depth) n; rows / cols of them are valid.  The operands are streamed through As / Bs
+// ([NB][LDT] each) in 64-deep cp.async chunks; the CTA has kTileThreads-style 4 warps, (wm, wn, lr, lc) as tile_mma64.
+__device__ __forceinline__ void gram_tile_accumulate(const double* Vr, const double* Vc, int n, int rows, int cols,
+                                                     double* As, double* Bs, double (&acc)[4][4][2], int wm, int wn,
+                                                     int lr, int lc) {
+  const int tid = threadIdx.x;
+  for (int kc = 0; kc < n; kc += NB) {
+    if (kc > 0) __syncthreads();  // everybody is done with the previous chunk
+    for (int e = tid; e < NB * NB; e += blockDim.x) {
+      const int k = e % NB, r = e / NB;  // consecutive threads read consecutive k of one V column
+      const bool okk = kc + k < n;
+      const bool oka = okk && r < rows, okb = okk && r < cols;
+      cp_async8(As + k * LDT + r, oka ? Vr + static_cast<size_t>(r) * n + kc + k : Vr, oka);
+      cp_async8(Bs + k * LDT + r, okb ? Vc + static_cast<size_t>(r) * n + kc + k : Vc, okb);
+    }
+    cp_async_commit();
+    cp_async_wait<0>();
+    __syncthreads();
+    tile_mma64(As, Bs, acc, wm, wn, lr, lc);
+  }
+}
+
+// One CTA solves L x = z (cta_forward_subst) or L^T x = z (cta_backward_subst) in place in shared memory, L the n x n
+// column-major lower factor in global memory, by blocked substitution over 64-row blocks: warp 0 solves the diagonal
+// block out of shared memory (D: [NB][NB + 1]), then every thread updates its rows, summing the block's products in
+// ascending column order.  Every operation has a fixed order, so the result does not depend on the launch.
+__device__ __forceinline__ void cta_forward_subst(const double* Ls, int n, double* z, double* D) {
+  const int tid = threadIdx.x;
+  for (int k0 = 0; k0 < n; k0 += NB) {
+    const int nb = min(NB, n - k0);
+    __syncthreads();  // the previous block's update of z and its reads of D are done
+    for (int e = tid; e < NB * NB; e += blockDim.x) {
+      const int rr = e % NB, c = e / NB;
+      if (rr < nb && c < nb && rr >= c) D[c * (NB + 1) + rr] = Ls[static_cast<size_t>(k0 + c) * n + k0 + rr];
+    }
+    __syncthreads();
+    if (tid < 32) {  // lane owns rows tid and tid + 32 of the block
+      const int r0 = tid, r1 = tid + 32;
+      double v0 = r0 < nb ? z[k0 + r0] : 0.0, v1 = r1 < nb ? z[k0 + r1] : 0.0;
+      for (int j = 0; j < nb; ++j) {
+        const double xj = __shfl_sync(0xffffffffu, j < 32 ? v0 : v1, j & 31) / D[j * (NB + 1) + j];
+        if (r0 == j) v0 = xj;
+        if (r1 == j) v1 = xj;
+        if (r0 > j && r0 < nb) v0 = fma(-D[j * (NB + 1) + r0], xj, v0);
+        if (r1 > j && r1 < nb) v1 = fma(-D[j * (NB + 1) + r1], xj, v1);
+      }
+      if (r0 < nb) z[k0 + r0] = v0;
+      if (r1 < nb) z[k0 + r1] = v1;
+    }
+    __syncthreads();
+    for (int i = k0 + nb + tid; i < n; i += blockDim.x) {  // z_i -= sum_c L[i, k0 + c] z[k0 + c]
+      const double* Li = Ls + static_cast<size_t>(k0) * n + i;
+      double acc = 0.0;
+      for (int c = 0; c < nb; ++c) acc = fma(Li[static_cast<size_t>(c) * n], z[k0 + c], acc);
+      z[i] -= acc;
+    }
+  }
+  __syncthreads();
+}
+
+__device__ __forceinline__ void cta_backward_subst(const double* Ls, int n, double* z, double* D) {
+  const int tid = threadIdx.x;
+  for (int k0 = ((n - 1) / NB) * NB; k0 >= 0; k0 -= NB) {
+    const int nb = min(NB, n - k0);
+    __syncthreads();  // the previous block's update of z and its reads of D are done
+    for (int e = tid; e < NB * NB; e += blockDim.x) {
+      const int rr = e % NB, c = e / NB;
+      if (rr < nb && c < nb && rr >= c) D[c * (NB + 1) + rr] = Ls[static_cast<size_t>(k0 + c) * n + k0 + rr];
+    }
+    __syncthreads();
+    if (tid < 32) {  // L_bb^T x = z_b, last row first; lane owns rows tid and tid + 32 of the block
+      const int r0 = tid, r1 = tid + 32;
+      double v0 = r0 < nb ? z[k0 + r0] : 0.0, v1 = r1 < nb ? z[k0 + r1] : 0.0;
+      for (int j = nb - 1; j >= 0; --j) {
+        const double xj = __shfl_sync(0xffffffffu, j < 32 ? v0 : v1, j & 31) / D[j * (NB + 1) + j];
+        if (r0 == j) v0 = xj;
+        if (r1 == j) v1 = xj;
+        if (r0 < j) v0 = fma(-D[r0 * (NB + 1) + j], xj, v0);
+        if (r1 < j) v1 = fma(-D[r1 * (NB + 1) + j], xj, v1);
+      }
+      if (r0 < nb) z[k0 + r0] = v0;
+      if (r1 < nb) z[k0 + r1] = v1;
+    }
+    __syncthreads();
+    for (int i = tid; i < k0; i += blockDim.x) {  // z_i -= sum_c L[k0 + c, i] z[k0 + c]
+      const double* Li = Ls + static_cast<size_t>(i) * n + k0;
+      double acc = 0.0;
+      for (int c = 0; c < nb; ++c) acc = fma(Li[c], z[k0 + c], acc);
+      z[i] -= acc;
+    }
+  }
+  __syncthreads();
+}
+
 }  // namespace
 }  // namespace cmoe

@@ -210,36 +210,7 @@ __global__ void __launch_bounds__(kLmlSolveThreads) lml_solve_kernel(const doubl
   }
   const double* Ls = L + static_cast<size_t>(set) * n * n;
   for (int i = tid; i < n; i += blockDim.x) lml_z[i] = r[i];
-  for (int k0 = 0; k0 < n; k0 += NB) {
-    const int nb = min(NB, n - k0);
-    __syncthreads();  // the previous block's update of z and its reads of D are done
-    for (int e = tid; e < NB * NB; e += blockDim.x) {
-      const int rr = e % NB, c = e / NB;
-      if (rr < nb && c < nb && rr >= c) D[c * (NB + 1) + rr] = Ls[static_cast<size_t>(k0 + c) * n + k0 + rr];
-    }
-    __syncthreads();
-    if (tid < 32) {  // lane owns rows tid and tid + 32 of the block
-      const int r0 = tid, r1 = tid + 32;
-      double v0 = r0 < nb ? lml_z[k0 + r0] : 0.0, v1 = r1 < nb ? lml_z[k0 + r1] : 0.0;
-      for (int j = 0; j < nb; ++j) {
-        const double xj = __shfl_sync(0xffffffffu, j < 32 ? v0 : v1, j & 31) / D[j * (NB + 1) + j];
-        if (r0 == j) v0 = xj;
-        if (r1 == j) v1 = xj;
-        if (r0 > j && r0 < nb) v0 = fma(-D[j * (NB + 1) + r0], xj, v0);
-        if (r1 > j && r1 < nb) v1 = fma(-D[j * (NB + 1) + r1], xj, v1);
-      }
-      if (r0 < nb) lml_z[k0 + r0] = v0;
-      if (r1 < nb) lml_z[k0 + r1] = v1;
-    }
-    __syncthreads();
-    for (int i = k0 + nb + tid; i < n; i += blockDim.x) {  // z_i -= sum_c L[i, k0 + c] z[k0 + c]
-      const double* Li = Ls + static_cast<size_t>(k0) * n + i;
-      double acc = 0.0;
-      for (int c = 0; c < nb; ++c) acc = fma(Li[static_cast<size_t>(c) * n], lml_z[k0 + c], acc);
-      lml_z[i] -= acc;
-    }
-  }
-  __syncthreads();
+  cta_forward_subst(Ls, n, lml_z, D);
   double zz = 0.0, logdiag = 0.0;
   for (int i = tid; i < n; i += blockDim.x) {
     zz = fma(lml_z[i], lml_z[i], zz);
@@ -249,36 +220,7 @@ __global__ void __launch_bounds__(kLmlSolveThreads) lml_solve_kernel(const doubl
   logdiag = block_sum(logdiag, scratch);
   if (tid == 0) out[set] = -0.5 * zz - logdiag - 0.5 * static_cast<double>(n) * kLog2Pi;
   if (a_out == nullptr) return;
-  for (int k0 = ((n - 1) / NB) * NB; k0 >= 0; k0 -= NB) {
-    const int nb = min(NB, n - k0);
-    __syncthreads();  // the previous block's update of z and its reads of D are done
-    for (int e = tid; e < NB * NB; e += blockDim.x) {
-      const int rr = e % NB, c = e / NB;
-      if (rr < nb && c < nb && rr >= c) D[c * (NB + 1) + rr] = Ls[static_cast<size_t>(k0 + c) * n + k0 + rr];
-    }
-    __syncthreads();
-    if (tid < 32) {  // L_bb^T x = z_b, last row first; lane owns rows tid and tid + 32 of the block
-      const int r0 = tid, r1 = tid + 32;
-      double v0 = r0 < nb ? lml_z[k0 + r0] : 0.0, v1 = r1 < nb ? lml_z[k0 + r1] : 0.0;
-      for (int j = nb - 1; j >= 0; --j) {
-        const double xj = __shfl_sync(0xffffffffu, j < 32 ? v0 : v1, j & 31) / D[j * (NB + 1) + j];
-        if (r0 == j) v0 = xj;
-        if (r1 == j) v1 = xj;
-        if (r0 < j) v0 = fma(-D[r0 * (NB + 1) + j], xj, v0);
-        if (r1 < j) v1 = fma(-D[r1 * (NB + 1) + j], xj, v1);
-      }
-      if (r0 < nb) lml_z[k0 + r0] = v0;
-      if (r1 < nb) lml_z[k0 + r1] = v1;
-    }
-    __syncthreads();
-    for (int i = tid; i < k0; i += blockDim.x) {  // z_i -= sum_c L[k0 + c, i] z[k0 + c]
-      const double* Li = Ls + static_cast<size_t>(i) * n + k0;
-      double acc = 0.0;
-      for (int c = 0; c < nb; ++c) acc = fma(Li[c], lml_z[k0 + c], acc);
-      lml_z[i] -= acc;
-    }
-  }
-  __syncthreads();
+  cta_backward_subst(Ls, n, lml_z, D);
   for (int i = tid; i < n; i += blockDim.x) a_out[static_cast<size_t>(set) * n + i] = lml_z[i];
 }
 

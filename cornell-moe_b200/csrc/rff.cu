@@ -1,0 +1,693 @@
+// Random-feature Thompson sampling of the global minimum (DESIGN.md K14), batched over samples.
+//
+// Replaces (reference, moe/optimal_learning/python/random_features.py):
+//   sample_gp_with_random_features            :29-133  (features, design matrix, posterior of the weights)
+//   global_optimization_of_GP_approximation   :144-168 (grid argmin + local optimisation)
+//   sample_from_global_optima                 :171-175 (one sample at a time)
+//
+// Per chunk of samples (the contract is in cmoe_b200.h, next to cmoe_gp_sample_rff_optima):
+//   W = Omega / l, b = 2 pi u                         rff_features_kernel
+//   Phi (M < F) or the column-reversed Phi^T (M >= F) rff_design_kernel
+//   I + Phi^T Phi  or  reversed I + Phi Phi^T         rff_gram_kernel: DMMA m16n8k4 (gram_tile_accumulate)
+//   L L^T = Gram                                      potrf_batched
+//   theta                                             rff_theta_kernel: one CTA per sample, fixed-order GEMVs and
+//                                                     blocked substitutions (cta_forward_subst / cta_backward_subst)
+//   f on the grid, per-CTA argmin partials           rff_grid_kernel, rff_argmin_kernel
+//   projected Newton from the grid argmin            rff_opt_kernel: one warp per sample
+// Every kernel treats the samples of a chunk independently and every reduction has a fixed order, so a sample's result
+// is a pure function of its randomness, not of num_points or the chunking.
+//
+// The M >= F branch factors the order-reversed B = I_F + Phi Phi^T: with J the reversal, J B J = L L^T gives the upper
+// factor U = J L J of B = U U^T.  The design kernel stores the columns of Phi^T in reversed feature order, so the Gram
+// kernel's ordinary product is J B J.  In the reversed coordinates theta_rev = L^-T (L^-1 (J Phi y') + J z).
+#include <algorithm>
+#include <climits>
+#include <cmath>
+
+#include "device_math.cuh"
+#include "internal.cuh"
+#include "linalg_dev.cuh"
+
+namespace cmoe {
+
+namespace {
+
+constexpr int kRffThreads = 256;      // design, theta, grid kernels
+constexpr int kRffTileThreads = 128;  // rff_gram_kernel: 4 warps over a 64 x 64 tile (tile_mma64)
+constexpr int kRffGridTile = 128;     // features staged in shared memory per round of rff_grid_kernel
+constexpr int kRffGridCtas = 1024;    // grid-kernel CTAs per sample at most (the rest is a grid-stride loop)
+constexpr int kRffOptWarps = 2;       // samples per CTA of rff_opt_kernel
+constexpr int kRffMaxIter = 100;      // SLSQP's default iteration limit
+constexpr int kRffMaxHalvings = 60;
+constexpr double kRffKktTol = 1e-9;   // stop: ||x - P(x - grad)||_inf <= kRffKktTol (1 + |f|)
+constexpr double kRffArmijo = 1e-4;
+constexpr double kRffSlack = 1e-13;   // Armijo rounding slack, relative to 1 + |f|
+constexpr double kRffEpsActive = 1e-3;  // epsilon-active set margin, relative to the box's width
+constexpr double kTwoPi = 6.283185307179586476925286766559;
+
+struct RffBox {
+  double lo[CMOE_MAX_DIM];
+  double hi[CMOE_MAX_DIM];
+};
+
+struct RffShape {
+  int F, M, N, d, g, woodbury;  // woodbury = M < F
+  double c;                     // sqrt(2 alpha / F)
+  double len[CMOE_MAX_DIM];
+  double sqrt_nu[CMOE_MAX_DIM + 1];  // sqrt(nu_t): the design divides by it, as the reference does
+  int derivs[CMOE_MAX_DIM];
+};
+
+// sin and cos of a for the sample functions, without the library's slow-path argument reduction (and its local-memory
+// frame): a three-part Cody-Waite reduction by pi/2 with FMA, exact to rounding for |a| < 2^30, then the fdlibm kernel
+// polynomials on [-pi/4, pi/4].  The argument W x + b itself carries a rounding error of order ulp(a), which dominates.
+__device__ __forceinline__ void rff_sincos(double a, double& sn, double& cs) {
+  const double k = rint(a * 0.63661977236758134308);
+  double r = fma(-k, 1.5707963267948965580e+00, a);
+  r = fma(-k, 6.1232339957367658e-17, r);
+  r = fma(-k, -1.4973849048591698e-33, r);
+  const int q = static_cast<int>(__double2ll_rn(k) & 3);
+  const double z = r * r;
+  const double ps = fma(z, fma(z, fma(z, fma(z, 1.58969099521155010221e-10, -2.50507602534068634195e-08),
+                                      2.75573137070700676789e-06),
+                               -1.98412698298579493134e-04),
+                        8.33333333332248946124e-03);
+  const double sr = fma(z * r, fma(z, ps, -1.66666666666666324348e-01), r);
+  const double pc = z * fma(z, fma(z, fma(z, fma(z, fma(z, -1.13596475577881948265e-11, 2.08757232129817482790e-09),
+                                              -2.75573143513906633035e-07),
+                                       2.48015872894767294178e-05),
+                                -1.38888888888741095749e-03),
+                            4.16666666666666019037e-02);
+  const double hz = 0.5 * z, w = 1.0 - hz;
+  const double cr = w + (((1.0 - w) - hz) + z * pc);
+  sn = (q == 0) ? sr : (q == 1) ? cr : (q == 2) ? -sr : -cr;
+  cs = (q == 0) ? cr : (q == 1) ? -sr : (q == 2) ? -cr : sr;
+}
+
+__device__ __forceinline__ double rff_cos(double a) {
+  double sn, cs;
+  rff_sincos(a, sn, cs);
+  return cs;
+}
+
+__device__ __forceinline__ double rff_sin(double a) {
+  double sn, cs;
+  rff_sincos(a, sn, cs);
+  return sn;
+}
+
+__device__ __forceinline__ double philox_normal_at(uint64_t seed, uint64_t draw, size_t k) {
+  double a, b;
+  philox_normal_pair(seed, draw, static_cast<uint32_t>(k >> 1), a, b);
+  return (k & 1) ? b : a;
+}
+
+__device__ __forceinline__ double philox_uniform_at(uint64_t seed, uint64_t draw, int f) {
+  uint32_t c[4] = {static_cast<uint32_t>(draw), static_cast<uint32_t>(draw >> 32), static_cast<uint32_t>(f >> 1), 2u};
+  philox4x32_10(c, static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
+  const uint64_t w = (f & 1) ? ((static_cast<uint64_t>(c[2]) << 32) | c[3]) : ((static_cast<uint64_t>(c[0]) << 32) | c[1]);
+  return __dmul_rn(__dadd_rn(static_cast<double>(w >> 11), 0.5), 0x1.0p-53);
+}
+
+// W[s][f][k] = Omega / l_k and b[s][f]; grid (ceil(max(F, M) / 256), samples).  Omega and b come from row s of the
+// table, or from Philox draw draw0 + s; in Philox mode the kernel also writes z[s][F] and, when M < F, eps[s][M] (the
+// table mode uploads them).  The Box-Muller step is philox_normal_pair's, so the numbers are cmoe_philox_normals'.
+__global__ void __launch_bounds__(kRffThreads) rff_features_kernel(const __grid_constant__ RffShape sh, uint64_t seed,
+                                                                   uint64_t draw0, const double* __restrict__ t_omega,
+                                                                   const double* __restrict__ t_b,
+                                                                   double* __restrict__ W, double* __restrict__ b,
+                                                                   double* __restrict__ z, double* __restrict__ eps) {
+  const int s = blockIdx.y, f = blockIdx.x * blockDim.x + threadIdx.x, F = sh.F, d = sh.d;
+  const uint64_t draw = draw0 + s;
+  const size_t zoff = static_cast<size_t>(F) * d;
+  if (!t_omega && sh.woodbury && f < sh.M)
+    eps[static_cast<size_t>(s) * sh.M + f] = philox_normal_at(seed, draw, zoff + F + f);
+  if (f >= F) return;
+  const size_t row = (static_cast<size_t>(s) * F + f) * d;
+  double n0 = 0.0, n1 = 0.0;  // the Philox pair holding normal f d + k (one Philox call per pair)
+  for (int k = 0; k < d; ++k) {
+    const size_t i = static_cast<size_t>(f) * d + k;
+    if (!t_omega && (k == 0 || (i & 1) == 0)) philox_normal_pair(seed, draw, static_cast<uint32_t>(i >> 1), n0, n1);
+    const double om = t_omega ? t_omega[row + k] : ((i & 1) ? n1 : n0);
+    W[row + k] = __ddiv_rn(om, sh.len[k]);
+  }
+  if (t_omega) {
+    b[static_cast<size_t>(s) * F + f] = t_b[static_cast<size_t>(s) * F + f];
+  } else {
+    b[static_cast<size_t>(s) * F + f] = __dmul_rn(kTwoPi, philox_uniform_at(seed, draw, f));
+    z[static_cast<size_t>(s) * F + f] = philox_normal_at(seed, draw, zoff + f);
+  }
+}
+
+// The design matrix of every sample, one element per thread: grid (fast blocks, samples, slow splits); the thread's
+// fast index is fixed and it steps over the slow index.  M < F: Phi column-major (fast = feature f, slow = column).
+// M >= F: Phi^T with reversed features (fast = column, slow = F - 1 - f).  Consecutive threads write consecutive
+// addresses in both layouts.
+__global__ void __launch_bounds__(kRffThreads) rff_design_kernel(const __grid_constant__ RffShape sh,
+                                                                 const double* __restrict__ X,
+                                                                 const double* __restrict__ W,
+                                                                 const double* __restrict__ b,
+                                                                 double* __restrict__ Phi) {
+  const int s = blockIdx.y, F = sh.F, M = sh.M, N = sh.N, d = sh.d;
+  const int nfast = sh.woodbury ? F : M, nslow = sh.woodbury ? M : F;
+  const int fast = blockIdx.x * blockDim.x + threadIdx.x;
+  if (fast >= nfast) return;
+  const double* Ws = W + static_cast<size_t>(s) * F * d;
+  const double* bs = b + static_cast<size_t>(s) * F;
+  double* Ps = Phi + static_cast<size_t>(s) * F * M;
+  for (int slow = blockIdx.z; slow < nslow; slow += gridDim.z) {
+    const int f = sh.woodbury ? fast : F - 1 - slow, col = sh.woodbury ? slow : fast;
+    const int t = col / N, i = col % N;
+    const double* w = Ws + static_cast<size_t>(f) * d;
+    const double* x = X + static_cast<size_t>(i) * d;
+    double a = 0.0;
+    for (int k = 0; k < d; ++k) a = fma(w[k], x[k], a);
+    a += bs[f];
+    const double v = (t == 0) ? sh.c * rff_cos(a) / sh.sqrt_nu[0] : -sh.c * w[sh.derivs[t - 1]] * rff_sin(a) / sh.sqrt_nu[t];
+    Ps[static_cast<size_t>(slow) * nfast + fast] = v;
+  }
+}
+
+// Gram_s = I + V_s^T V_s on the lower 64 x 64 tiles; V_s is K x Q column-major (Phi for M < F: K = F, Q = M; the
+// reversed Phi^T for M >= F: K = M, Q = F).  grid (tiles, 1, samples).  Only the lower triangle is written.
+__global__ void __launch_bounds__(kRffTileThreads) rff_gram_kernel(const double* __restrict__ V, int K, int Q,
+                                                                   double* __restrict__ A) {
+  extern __shared__ double smem[];
+  double* As = smem;           // [NB][LDT]
+  double* Bs = As + NB * LDT;  // [NB][LDT]
+  const int s = blockIdx.z, tid = threadIdx.x;
+  int ti, tj;
+  tri_tile(blockIdx.x, ti, tj);
+  const int row0 = ti * NB, col0 = tj * NB;
+  const int rows = min(NB, Q - row0), cols = min(NB, Q - col0);
+  const double* Vs = V + static_cast<size_t>(s) * K * Q;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int wm = (warp & 1) * 32, wn = (warp >> 1) * 32;
+  const int lr = lane >> 2, lc = lane & 3;
+  double acc[4][4][2];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
+  gram_tile_accumulate(Vs + static_cast<size_t>(row0) * K, Vs + static_cast<size_t>(col0) * K, K, rows, cols, As, Bs,
+                       acc, wm, wn, lr, lc);
+  double* Ab = A + static_cast<size_t>(s) * Q * Q;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int r = wm + i * 8 + lr, gr = row0 + r;
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int c = wn + j * 8 + lc * 2 + h, gc = col0 + c;
+        if (r < rows && c < cols && gr >= gc) Ab[static_cast<size_t>(gc) * Q + gr] = acc[i][j][h] + (gr == gc ? 1.0 : 0.0);
+      }
+  }
+}
+
+// theta of one sample per CTA (the header's two branches), z[s][F] and eps[s][M] as rff_features_kernel or the table
+// left them.  A sample whose factorisation failed is skipped (the host reports it).  Dot products
+// over F are lane-strided in one warp and combined by the warp_sum butterfly; those over M run serially in ascending
+// order; theta doubles as the F-vector r of the Woodbury branch.
+__global__ void __launch_bounds__(kRffThreads) rff_theta_kernel(const __grid_constant__ RffShape sh,
+                                                                const double* __restrict__ Phi,
+                                                                const double* __restrict__ yp,
+                                                                const double* __restrict__ L,
+                                                                const int* __restrict__ fail,
+                                                                const double* __restrict__ z,
+                                                                const double* __restrict__ eps, double* theta) {
+  extern __shared__ double rff_v[];  // [Q] right-hand side -> solution
+  const int s = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, nw = blockDim.x >> 5;
+  if (fail[s] != 0) return;
+  const int F = sh.F, M = sh.M, Q = sh.woodbury ? M : F;
+  double* D = rff_v + Q;  // [NB][NB + 1]
+  const double* Ps = Phi + static_cast<size_t>(s) * F * M;
+  const double* Ls = L + static_cast<size_t>(s) * Q * Q;
+  double* th = theta + static_cast<size_t>(s) * F;
+  const double* zs = z + static_cast<size_t>(s) * F;
+  if (sh.woodbury) {
+    for (int f = tid; f < F; f += blockDim.x) {  // r = Phi y' + z
+      double acc = 0.0;
+      for (int i = 0; i < M; ++i) acc = fma(Ps[static_cast<size_t>(i) * F + f], yp[i], acc);
+      th[f] = acc + zs[f];
+    }
+    __syncthreads();
+    for (int i = warp; i < M; i += nw) {  // v = Phi^T r + eps
+      const double* col = Ps + static_cast<size_t>(i) * F;
+      double acc = 0.0;
+      for (int f = lane; f < F; f += 32) acc = fma(col[f], th[f], acc);
+      acc = warp_sum(acc);
+      if (lane == 0) rff_v[i] = acc + eps[static_cast<size_t>(s) * M + i];
+    }
+  } else {
+    for (int c = warp; c < F; c += nw) {  // v = J Phi y'
+      const double* col = Ps + static_cast<size_t>(c) * M;
+      double acc = 0.0;
+      for (int i = lane; i < M; i += 32) acc = fma(col[i], yp[i], acc);
+      acc = warp_sum(acc);
+      if (lane == 0) rff_v[c] = acc;
+    }
+  }
+  cta_forward_subst(Ls, Q, rff_v, D);
+  if (!sh.woodbury)
+    for (int c = tid; c < F; c += blockDim.x) rff_v[c] += zs[F - 1 - c];
+  cta_backward_subst(Ls, Q, rff_v, D);
+  if (sh.woodbury) {
+    for (int f = tid; f < F; f += blockDim.x) {  // theta = r - Phi A^-1 v
+      double acc = 0.0;
+      for (int i = 0; i < M; ++i) acc = fma(Ps[static_cast<size_t>(i) * F + f], rff_v[i], acc);
+      th[f] -= acc;
+    }
+  } else {
+    for (int f = tid; f < F; f += blockDim.x) th[f] = rff_v[F - 1 - f];
+  }
+}
+
+// f at the grid points of one sample (grid.y), a grid-stride loop over the points; features staged kRffGridTile at a
+// time in shared memory.  Each thread keeps the first minimum of its points (ascending), each CTA the first minimum of
+// its threads: (part_v, part_i)[s][blockIdx.x].
+__global__ void __launch_bounds__(kRffThreads) rff_grid_kernel(const __grid_constant__ RffShape sh,
+                                                               const double* __restrict__ grid, int G,
+                                                               const double* __restrict__ W,
+                                                               const double* __restrict__ b,
+                                                               const double* __restrict__ theta,
+                                                               double* __restrict__ part_v, int* __restrict__ part_i) {
+  extern __shared__ double gs[];  // [kRffGridTile][d] W, [kRffGridTile] b, [kRffGridTile] theta
+  __shared__ double bv[kRffThreads];
+  __shared__ int bi[kRffThreads];
+  const int s = blockIdx.y, tid = threadIdx.x, F = sh.F, d = sh.d;
+  double* Wt = gs;
+  double* bt = Wt + kRffGridTile * d;
+  double* tt = bt + kRffGridTile;
+  const double* Ws = W + static_cast<size_t>(s) * F * d;
+  const double* bs = b + static_cast<size_t>(s) * F;
+  const double* ts = theta + static_cast<size_t>(s) * F;
+  double best = INFINITY;
+  int bidx = INT_MAX;
+  for (int base = blockIdx.x * blockDim.x; base < G; base += gridDim.x * blockDim.x) {  // uniform over the CTA
+    const int j = base + tid;
+    const bool valid = j < G;
+    double x[CMOE_MAX_DIM];
+#pragma unroll
+    for (int k = 0; k < CMOE_MAX_DIM; ++k) x[k] = (valid && k < d) ? grid[static_cast<size_t>(j) * d + k] : 0.0;
+    double acc = 0.0;
+    for (int f0 = 0; f0 < F; f0 += kRffGridTile) {
+      const int nf = min(kRffGridTile, F - f0);
+      __syncthreads();
+      for (int e = tid; e < nf * d; e += blockDim.x) Wt[e] = Ws[static_cast<size_t>(f0) * d + e];
+      for (int e = tid; e < nf; e += blockDim.x) {
+        bt[e] = bs[f0 + e];
+        tt[e] = ts[f0 + e];
+      }
+      __syncthreads();
+      if (valid) {
+        for (int f = 0; f < nf; ++f) {
+          const double* w = Wt + f * d;
+          double a = 0.0;
+#pragma unroll
+          for (int k = 0; k < CMOE_MAX_DIM; ++k)
+            if (k < d) a = fma(w[k], x[k], a);
+          acc = fma(tt[f], rff_cos(a + bt[f]), acc);
+        }
+      }
+    }
+    const double v = sh.c * acc;
+    if (valid && v < best) {
+      best = v;
+      bidx = j;
+    }
+  }
+  bv[tid] = best;
+  bi[tid] = bidx;
+  __syncthreads();
+  if (tid == 0) {
+    for (int t = 1; t < kRffThreads; ++t)
+      if (bv[t] < best || (bv[t] == best && bi[t] < bidx)) {
+        best = bv[t];
+        bidx = bi[t];
+      }
+    part_v[static_cast<size_t>(s) * gridDim.x + blockIdx.x] = best;
+    part_i[static_cast<size_t>(s) * gridDim.x + blockIdx.x] = bidx;
+  }
+}
+
+// first minimum over the grid kernel's CTAs of each sample, in CTA order (no finite value: index 0, value +inf)
+__global__ void rff_argmin_kernel(int ns, int nparts, const double* __restrict__ part_v,
+                                  const int* __restrict__ part_i, int* __restrict__ amin, double* __restrict__ vmin) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= ns) return;
+  double best = INFINITY;
+  int bidx = INT_MAX;
+  for (int p = 0; p < nparts; ++p) {
+    const double v = part_v[static_cast<size_t>(s) * nparts + p];
+    const int k = part_i[static_cast<size_t>(s) * nparts + p];
+    if (v < best || (v == best && k < bidx)) {
+      best = v;
+      bidx = k;
+    }
+  }
+  amin[s] = (bidx == INT_MAX) ? 0 : bidx;
+  vmin[s] = best;
+}
+
+// f (and with G, the gradient, into gout: shared, d values) of one sample at x (shared, d values), lanes striding over the features and combined by
+// the warp_sum butterfly, so every lane holds the same bits.  With wc, wc[f] = c theta_f cos(W_f x + b_f) is stored
+// for the Hessian.
+template <bool G>
+__device__ __forceinline__ double rff_eval(const RffShape& sh, const double* Ws, const double* bs, const double* ts,
+                                           const double* x, int lane, double* gout, double* wc) {
+  const int F = sh.F, d = sh.d;
+  double fv = 0.0;
+  double g[CMOE_MAX_DIM];
+  if (G) {
+#pragma unroll
+    for (int k = 0; k < CMOE_MAX_DIM; ++k) g[k] = 0.0;
+  }
+  for (int f = lane; f < F; f += 32) {
+    const double* w = Ws + static_cast<size_t>(f) * d;
+    double a = 0.0;
+#pragma unroll
+    for (int k = 0; k < CMOE_MAX_DIM; ++k)
+      if (k < d) a = fma(w[k], x[k], a);
+    a += bs[f];
+    if (G) {
+      double sn, cs;
+      rff_sincos(a, sn, cs);
+      fv = fma(ts[f], cs, fv);
+      const double ws = ts[f] * sn;
+#pragma unroll
+      for (int k = 0; k < CMOE_MAX_DIM; ++k)
+        if (k < d) g[k] = fma(ws, w[k], g[k]);
+      wc[f] = sh.c * ts[f] * cs;
+    } else {
+      fv = fma(ts[f], rff_cos(a), fv);
+    }
+  }
+  if (G) {
+#pragma unroll
+    for (int k = 0; k < CMOE_MAX_DIM; ++k)
+      if (k < d) {
+        const double v = -sh.c * warp_sum(g[k]);
+        if (lane == k) gout[k] = v;
+      }
+  }
+  const double fsum = sh.c * warp_sum(fv);
+  __syncwarp();
+  return fsum;
+}
+
+// Projected Newton (the header's local step) for one sample per warp, from the clamped grid argmin.  Each warp keeps
+// its iterate, trial point, step and Hessian in shared memory; every scalar decision is warp-uniform.
+__global__ void __launch_bounds__(kRffOptWarps * 32) rff_opt_kernel(const __grid_constant__ RffShape sh, int ns,
+                                                                    const __grid_constant__ RffBox box,
+                                                                    const double* __restrict__ grid,
+                                                                    const int* __restrict__ amin,
+                                                                    const double* __restrict__ vmin,
+                                                                    const double* __restrict__ W,
+                                                                    const double* __restrict__ b,
+                                                                    const double* __restrict__ theta,
+                                                                    double* __restrict__ wc_all,
+                                                                    double* __restrict__ pts,
+                                                                    double* __restrict__ vals) {
+  __shared__ double sx[kRffOptWarps][CMOE_MAX_DIM], st[kRffOptWarps][CMOE_MAX_DIM], sp[kRffOptWarps][CMOE_MAX_DIM];
+  __shared__ double sH[kRffOptWarps][CMOE_MAX_DIM][CMOE_MAX_DIM + 1];
+  __shared__ double sL[kRffOptWarps][CMOE_MAX_DIM][CMOE_MAX_DIM + 1];
+  __shared__ double sg[kRffOptWarps][CMOE_MAX_DIM];
+  __shared__ int sfree[kRffOptWarps][CMOE_MAX_DIM];
+  const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int s = blockIdx.x * kRffOptWarps + wid;
+  if (s >= ns) return;
+  const int F = sh.F, d = sh.d;
+  const double* Ws = W + static_cast<size_t>(s) * F * d;
+  const double* bs = b + static_cast<size_t>(s) * F;
+  const double* ts = theta + static_cast<size_t>(s) * F;
+  double* wc = wc_all + static_cast<size_t>(s) * F;
+  double* x = sx[wid];
+  double* xt = st[wid];
+  double* p = sp[wid];
+  double* g = sg[wid];
+  double (*H)[CMOE_MAX_DIM + 1] = sH[wid];
+  double (*Lc)[CMOE_MAX_DIM + 1] = sL[wid];
+  int* fr = sfree[wid];
+  const double* x0 = grid + static_cast<size_t>(amin[s]) * d;
+  if (lane < d) x[lane] = fmin(fmax(x0[lane], box.lo[lane]), box.hi[lane]);
+  __syncwarp();
+  double fx;
+  for (int it = 0;; ++it) {  // one gradient evaluation site: at most kRffMaxIter steps
+    fx = rff_eval<true>(sh, Ws, bs, ts, x, lane, g, wc);
+    if (it == kRffMaxIter) break;
+    // projected-gradient residual, then Bertsekas' epsilon-active set: variable k is held when it lies within
+    // eps_k = min(1e-3 (hi_k - lo_k), residual) of a bound and its gradient points out of the box
+    double res = 0.0;
+#pragma unroll
+    for (int k = 0; k < CMOE_MAX_DIM; ++k)
+      if (k < d) res = fmax(res, fabs(x[k] - fmin(fmax(x[k] - g[k], box.lo[k]), box.hi[k])));
+    if (res <= kRffKktTol * (1.0 + fabs(fx))) break;
+    int nf = 0;
+#pragma unroll
+    for (int k = 0; k < CMOE_MAX_DIM; ++k) {
+      if (k < d) {
+        const double xk = x[k], ek = fmin(kRffEpsActive * (box.hi[k] - box.lo[k]), res);
+        const bool held = (xk <= box.lo[k] + ek && g[k] > 0.0) || (xk >= box.hi[k] - ek && g[k] < 0.0);
+        if (!held) {
+          if (lane == 0) fr[nf] = k;
+          ++nf;
+        }
+      }
+    }
+    __syncwarp();
+    // Hessian rows of the free variables: H[j][k] = -sum_f wc_f W_fj W_fk, row j over k
+    for (int a = 0; a < nf; ++a) {
+      const int j = fr[a];
+      double h[CMOE_MAX_DIM];
+#pragma unroll
+      for (int k = 0; k < CMOE_MAX_DIM; ++k) h[k] = 0.0;
+      for (int f = lane; f < F; f += 32) {
+        const double* w = Ws + static_cast<size_t>(f) * d;
+        const double t = wc[f] * w[j];
+#pragma unroll
+        for (int k = 0; k < CMOE_MAX_DIM; ++k)
+          if (k < d) h[k] = fma(t, w[k], h[k]);
+      }
+#pragma unroll
+      for (int k = 0; k < CMOE_MAX_DIM; ++k)
+        if (k < d) {
+          const double v = -warp_sum(h[k]);
+          if (lane == k) H[j][k] = v;
+        }
+    }
+    __syncwarp();
+    // shifted Cholesky of the free block (lower triangle from rows a >= b: H[fr[a]][fr[b]])
+    double hmax = 0.0, hmin = INFINITY;
+    for (int a = 0; a < nf; ++a) {
+      hmax = fmax(hmax, fabs(H[fr[a]][fr[a]]));
+      hmin = fmin(hmin, H[fr[a]][fr[a]]);
+    }
+    const double beta = 1e-3 * fmax(hmax, 1e-12);
+    double tau = hmin > 0.0 ? 0.0 : beta - hmin;
+    bool ok = false;
+    for (int tries = 0; tries < 64 && !ok; ++tries) {
+      ok = true;
+      for (int c = 0; c < nf; ++c) {
+        double dg = H[fr[c]][fr[c]] + tau;
+        for (int k = 0; k < c; ++k) dg = fma(-Lc[c][k], Lc[c][k], dg);
+        if (!(dg > 0.0)) {
+          ok = false;
+          break;
+        }
+        const double ri = rsqrt(dg);  // the diagonal slot holds 1 / L_cc: no division in the loop
+        if (lane > c && lane < nf) {
+          double v = H[fr[lane]][fr[c]];
+          for (int k = 0; k < c; ++k) v = fma(-Lc[lane][k], Lc[c][k], v);
+          Lc[lane][c] = v * ri;
+        }
+        if (lane == c) Lc[c][c] = ri;
+        __syncwarp();
+      }
+      if (!ok) tau = fmax(2.0 * tau, beta);
+      __syncwarp();
+    }
+    if (!ok) break;
+    // p_free = -(H_ff + tau I)^-1 g_free (lane 0, then shared; xt holds the intermediate vector)
+    if (lane == 0) {
+      double* y = xt;
+      for (int a = 0; a < nf; ++a) {
+        double v = -g[fr[a]];
+        for (int k = 0; k < a; ++k) v = fma(-Lc[a][k], y[k], v);
+        y[a] = v * Lc[a][a];
+      }
+      for (int a = nf - 1; a >= 0; --a) {
+        double v = y[a];
+        for (int k = a + 1; k < nf; ++k) v = fma(-Lc[k][a], y[k], v);
+        y[a] = v * Lc[a][a];
+      }
+      // held variables step along -g (onto their bound); a free variable at a bound drops an outward Newton
+      // component, so every component of the projected step is a descent direction for small steps
+      for (int k = 0; k < d; ++k) p[k] = -g[k];
+      for (int a = 0; a < nf; ++a) {
+        const int k = fr[a];
+        const bool out = (x[k] <= box.lo[k] && y[a] < 0.0) || (x[k] >= box.hi[k] && y[a] > 0.0);
+        p[k] = out ? 0.0 : y[a];
+      }
+    }
+    __syncwarp();
+    // Armijo backtracking along the projected arc
+    double alpha = 1.0, ft = 0.0;
+    bool acc = false;
+    for (int h = 0; h < kRffMaxHalvings; ++h) {
+      if (lane < d) xt[lane] = fmin(fmax(x[lane] + alpha * p[lane], box.lo[lane]), box.hi[lane]);
+      __syncwarp();
+      double dec = 0.0;
+#pragma unroll
+      for (int k = 0; k < CMOE_MAX_DIM; ++k)
+        if (k < d) dec = fma(g[k], xt[k] - x[k], dec);
+      ft = rff_eval<false>(sh, Ws, bs, ts, xt, lane, nullptr, nullptr);
+      if (ft <= fx + kRffArmijo * dec + kRffSlack * (1.0 + fabs(fx))) {
+        acc = true;
+        break;
+      }
+      alpha *= 0.5;
+      __syncwarp();
+    }
+    if (!acc) break;
+    if (lane < d) x[lane] = xt[lane];
+    __syncwarp();
+  }
+  const double gmin = vmin[s];
+  const bool keep = fx < gmin;
+  if (lane < d) pts[static_cast<size_t>(s) * d + lane] = keep ? x[lane] : x0[lane];
+  if (lane == 0) vals[s] = keep ? fx : gmin;
+}
+
+}  // namespace
+
+}  // namespace cmoe
+
+using namespace cmoe;  // NOLINT
+
+extern "C" int cmoe_gp_sample_rff_optima(const cmoe_gp* gp, int num_features, int num_points,
+                                         const double* domain_bounds, const double* grid, int num_grid,
+                                         uint64_t seed, uint64_t first_draw, const cmoe_rff_table* table,
+                                         double* points, double* values, double* omega, double* b, double* theta,
+                                         int* info) {
+  return guarded(info, [&] {
+    CMOE_REQUIRE(num_features >= 1 && num_points >= 1 && num_grid >= 1, CMOE_ERR_BOUNDS,
+                 "num_features, num_points and num_grid must be >= 1");
+    CMOE_REQUIRE(gp != nullptr, CMOE_ERR_INVALID_VALUE, "gp is NULL");
+    const int F = num_features, P = num_points, G = num_grid, d = gp->spec.dim, g = gp->spec.g, N = gp->N;
+    const int M = gp->n;
+    const int Q = std::min(F, M);
+    CMOE_REQUIRE(d >= 1 && d <= CMOE_MAX_DIM, CMOE_ERR_BOUNDS, "dim must be in [1, 32]");
+    CMOE_REQUIRE(Q <= kMaxSampleQ, CMOE_ERR_BOUNDS, "min(num_features, num_sampled (1 + num_derivatives)) must be <= 8192");
+    const size_t phi = static_cast<size_t>(F) * M, gram = static_cast<size_t>(Q) * Q;
+    CMOE_REQUIRE(phi <= kSampleWorkspaceBytes / sizeof(double) - gram, CMOE_ERR_BOUNDS,
+                 "one sample's design matrix and Gram matrix must fit in the 2 GiB sampling workspace");
+    CMOE_REQUIRE(domain_bounds != nullptr && grid != nullptr && points != nullptr && values != nullptr,
+                 CMOE_ERR_INVALID_VALUE, "domain_bounds, grid, points or values is NULL");
+    const bool woodbury = M < F;
+    if (table)
+      CMOE_REQUIRE(table->omega && table->b && table->z && (table->eps || !woodbury), CMOE_ERR_INVALID_VALUE,
+                   "table field is NULL");
+    RffBox box{};
+    for (int k = 0; k < d; ++k) {
+      box.lo[k] = domain_bounds[2 * k];
+      box.hi[k] = domain_bounds[2 * k + 1];
+      CMOE_REQUIRE(std::isfinite(box.lo[k]) && std::isfinite(box.hi[k]) && box.lo[k] <= box.hi[k],
+                   CMOE_ERR_INVALID_VALUE, "domain bounds must be finite with min <= max");
+    }
+    for (size_t e = 0; e < static_cast<size_t>(G) * d; ++e)
+      CMOE_REQUIRE(std::isfinite(grid[e]), CMOE_ERR_INVALID_VALUE, "grid points must be finite");
+    for (int t = 0; t <= g; ++t)
+      CMOE_REQUIRE(gp->hnoise[t] > 0.0, CMOE_ERR_INVALID_VALUE, "noise variances must be > 0");
+    require_device(gp->device);
+
+    RffShape sh{};
+    sh.F = F;
+    sh.M = M;
+    sh.N = N;
+    sh.d = d;
+    sh.g = g;
+    sh.woodbury = woodbury ? 1 : 0;
+    sh.c = std::sqrt(2.0 * gp->spec.alpha / F);
+    for (int k = 0; k < d; ++k) sh.len[k] = gp->hlengths[k];
+    for (int t = 0; t <= g; ++t) sh.sqrt_nu[t] = std::sqrt(gp->hnoise[t]);
+    for (int k = 0; k < g; ++k) sh.derivs[k] = gp->spec.derivs[k];
+    // y' = y[:, t] / sqrt(nu_t), type-major (the reference's flatten('F'))
+    std::vector<double> hyp(M);
+    for (int t = 0; t <= g; ++t)
+      for (int i = 0; i < N; ++i) hyp[static_cast<size_t>(t) * N + i] = gp->hy[static_cast<size_t>(i) * (1 + g) + t] / sh.sqrt_nu[t];
+
+    cudaStream_t s = gp->stream;
+    const int nsteps = (Q + NB - 1) / NB;
+    const int gx = static_cast<int>(std::min<size_t>(kRffGridCtas, (static_cast<size_t>(G) + kRffThreads - 1) / kRffThreads));
+    const size_t per = sizeof(double) * (phi + gram + static_cast<size_t>(nsteps) * NB * NB +
+                                         static_cast<size_t>(F) * (d + 4) + M + static_cast<size_t>(gx) + 2 * d + 1 +
+                                         (table ? static_cast<size_t>(F) * (d + 2) + M : 0)) +
+                       sizeof(int) * (static_cast<size_t>(gx) + 2);
+    const int chunk = static_cast<int>(std::max<size_t>(
+        1, std::min<size_t>({kSampleWorkspaceBytes / per, static_cast<size_t>(P), static_cast<size_t>(kMaxChunkSets)})));
+    if (!gp->sample_ws) gp->sample_ws = std::make_shared<SampleWork>();
+    SampleWork& w = *static_cast<SampleWork*>(gp->sample_ws.get());
+    w.V.ensure(static_cast<size_t>(chunk) * phi);
+    w.A.ensure(static_cast<size_t>(chunk) * gram);
+    w.fail.ensure(chunk);
+    w.part_v.ensure(static_cast<size_t>(chunk) * gx);
+    w.part_i.ensure(static_cast<size_t>(chunk) * gx);
+    w.amin.ensure(chunk);
+    DevBuf<double> dX, dyp, dgrid, dW(static_cast<size_t>(chunk) * F * d), db(static_cast<size_t>(chunk) * F),
+        dth(static_cast<size_t>(chunk) * F), dwc(static_cast<size_t>(chunk) * F), dvmin(chunk),
+        dpts(static_cast<size_t>(chunk) * d), dvals(chunk), dz(static_cast<size_t>(chunk) * F),
+        deps(woodbury ? static_cast<size_t>(chunk) * M : 1), tom, tb;
+    dX.upload(gp->hX.data(), static_cast<size_t>(N) * d, s);
+    dyp.upload(hyp.data(), M, s);
+    dgrid.upload(grid, static_cast<size_t>(G) * d, s);
+    const size_t smem_gram = 2 * static_cast<size_t>(NB) * LDT * sizeof(double);
+    const size_t smem_theta = (static_cast<size_t>(Q) + NB * (NB + 1)) * sizeof(double);
+    const size_t smem_grid = static_cast<size_t>(kRffGridTile) * (d + 2) * sizeof(double);
+    CMOE_CUDA(cudaFuncSetAttribute(rff_gram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   static_cast<int>(smem_gram)));
+    CMOE_CUDA(cudaFuncSetAttribute(rff_theta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   static_cast<int>(smem_theta)));
+    std::vector<int> hfail(chunk);
+    for (int c0 = 0; c0 < P; c0 += chunk) {
+      const int nc = std::min(chunk, P - c0);
+      const uint64_t draw0 = first_draw + c0;
+      if (table) {
+        tom.upload(table->omega + static_cast<size_t>(c0) * F * d, static_cast<size_t>(nc) * F * d, s);
+        tb.upload(table->b + static_cast<size_t>(c0) * F, static_cast<size_t>(nc) * F, s);
+        dz.upload(table->z + static_cast<size_t>(c0) * F, static_cast<size_t>(nc) * F, s);
+        if (woodbury) deps.upload(table->eps + static_cast<size_t>(c0) * M, static_cast<size_t>(nc) * M, s);
+      }
+      rff_features_kernel<<<dim3((std::max(F, M) + kRffThreads - 1) / kRffThreads, nc), kRffThreads, 0, s>>>(
+          sh, seed, draw0, table ? tom.p : nullptr, table ? tb.p : nullptr, dW.p, db.p, dz.p, deps.p);
+      const int nfast = woodbury ? F : M, nslow = woodbury ? M : F, fx = (nfast + kRffThreads - 1) / kRffThreads;
+      const int zs = std::max(1, std::min(nslow, 4096 / std::max(1, fx * nc)));
+      rff_design_kernel<<<dim3(fx, nc, zs), kRffThreads, 0, s>>>(sh, dX.p, dW.p, db.p, w.V.p);
+      const int t = (Q + NB - 1) / NB;
+      rff_gram_kernel<<<dim3(t * (t + 1) / 2, 1, nc), kRffTileThreads, smem_gram, s>>>(w.V.p, woodbury ? F : M, Q,
+                                                                                       w.A.p);
+      count_launch(3);
+      CMOE_CUDA(cudaGetLastError());
+      CMOE_CUDA(cudaMemsetAsync(w.fail.p, 0, nc * sizeof(int), s));
+      potrf_batched(w.A.p, Q, nc, w.fail.p, w.stage, s);
+      rff_theta_kernel<<<nc, kRffThreads, smem_theta, s>>>(sh, w.V.p, dyp.p, w.A.p, w.fail.p, dz.p, deps.p, dth.p);
+      rff_grid_kernel<<<dim3(gx, nc), kRffThreads, smem_grid, s>>>(sh, dgrid.p, G, dW.p, db.p, dth.p, w.part_v.p,
+                                                                   w.part_i.p);
+      rff_argmin_kernel<<<(nc + 127) / 128, 128, 0, s>>>(nc, gx, w.part_v.p, w.part_i.p, w.amin.p, dvmin.p);
+      rff_opt_kernel<<<(nc + kRffOptWarps - 1) / kRffOptWarps, kRffOptWarps * 32, 0, s>>>(
+          sh, nc, box, dgrid.p, w.amin.p, dvmin.p, dW.p, db.p, dth.p, dwc.p, dpts.p, dvals.p);
+      count_launch(4);
+      CMOE_CUDA(cudaGetLastError());
+      w.fail.download(hfail.data(), nc, s);
+      dpts.download(points + static_cast<size_t>(c0) * d, static_cast<size_t>(nc) * d, s);
+      dvals.download(values + c0, nc, s);
+      if (omega) dW.download(omega + static_cast<size_t>(c0) * F * d, static_cast<size_t>(nc) * F * d, s);
+      if (b) db.download(b + static_cast<size_t>(c0) * F, static_cast<size_t>(nc) * F, s);
+      if (theta) dth.download(theta + static_cast<size_t>(c0) * F, static_cast<size_t>(nc) * F, s);
+      CMOE_CUDA(cudaStreamSynchronize(s));
+      for (int c = 0; c < nc; ++c)
+        if (hfail[c] != 0)
+          throw Error(CMOE_ERR_SINGULAR, "random-feature Gram matrix singular (non-finite data?)", hfail[c]);
+    }
+  });
+}

@@ -121,20 +121,7 @@ __global__ void __launch_bounds__(kTileThreads) cov_tile_kernel(const __grid_con
   for (int i = 0; i < 4; ++i)
 #pragma unroll
     for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
-  for (int kc = 0; kc < n; kc += NB) {
-    if (kc > 0) __syncthreads();  // everybody is done with the previous chunk
-    for (int e = tid; e < NB * NB; e += blockDim.x) {
-      const int k = e % NB, r = e / NB;  // consecutive threads read consecutive k of one V column
-      const bool okk = kc + k < n;
-      const bool oka = okk && r < rows, okb = okk && r < cols;
-      cp_async8(As + k * LDT + r, oka ? Vr + static_cast<size_t>(r) * n + kc + k : Vr, oka);
-      cp_async8(Bs + k * LDT + r, okb ? Vc + static_cast<size_t>(r) * n + kc + k : Vc, okb);
-    }
-    cp_async_commit();
-    cp_async_wait<0>();
-    __syncthreads();
-    tile_mma64(As, Bs, acc, wm, wn, lr, lc);
-  }
+  gram_tile_accumulate(Vr, Vc, n, rows, cols, As, Bs, acc, wm, wn, lr, lc);
   double* Ab = A + static_cast<size_t>(set) * Q * Q;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {

@@ -228,6 +228,57 @@ int cmoe_latin_hypercube(uint64_t seed, uint64_t first_draw, int num_sets, int n
 int cmoe_gp_sample_global_optima(const cmoe_gp* gp, int num_optima, int inner_number, const double* domain_bounds,
                                  uint64_t seed, uint64_t first_draw, double jitter, double* points_optima, int* info);
 
+/* ---- random-feature Thompson sampling of the global minimum ------------------------------------------------------
+ * sample_from_global_optima (moe/optimal_learning/python/random_features.py:29-175) in one call: num_points samples of
+ * the GP drawn as random-Fourier-feature functions, each minimised over the grid and then locally inside the domain.
+ * The handle holds n points X (raw coordinates), values y[n][1+g], partials derivs[g], per-type noise nu[1+g] and
+ * alpha = sigma^2, lengths l[d].  M = n (1 + g), F = num_features, c = sqrt(2 sigma^2 / F).  For sample s:
+ *   features    W = Omega / l (Omega F x d standard normals), b = 2 pi u (u F uniforms); always the spectral density of
+ *               SquareExponential, whatever the handle's kernel;
+ *   design      Phi (F x M), value columns first: column i = c cos(W x_i + b) / sqrt(nu_0), then one block per derivative
+ *               type k (partial j = derivs[k]): -c W[:, j] sin(W x_i + b) / sqrt(nu_{k+1}); y' = y[:, t] / sqrt(nu_t)
+ *               flattened type-major.  The raw values are used with a zero prior mean (the GP's mean is not subtracted);
+ *   posterior   theta ~ N(m, (I + Phi Phi^T)^-1), m = (I + Phi Phi^T)^-1 Phi y'.  Branch by size, as the reference:
+ *               M < F  (Woodbury): A = I_M + Phi^T Phi = L L^T, theta = r - Phi A^-1 (Phi^T r + eps), r = Phi y' + z,
+ *                      z in R^F and eps in R^M standard normals.  This pathwise update has exactly the target
+ *                      distribution; the reference applies the symmetric square root of A from an eigensolver instead, so
+ *                      this branch matches it in distribution, not draw for draw;
+ *               M >= F: B = I_F + Phi Phi^T = U U^T (U upper, the lower factor of the order-reversed B), m = B^-1 Phi y',
+ *                      theta = m + U^-T z: the reference's z^T cholesky(B^-1, upper), draw for draw given (Omega, u, z);
+ *   function    f(x) = c sum_f theta_f cos(W_f x + b_f);
+ *   grid        argmin of f over grid[num_grid][d] (shared by all samples), ties to the lowest index;
+ *   local       projected Newton inside domain_bounds from the grid argmin (clamped into the box), one warp per sample:
+ *               exact d x d Hessian; a variable within eps_k = min(1e-3 (hi_k - lo_k), ||x - P(x - grad f)||_inf) of a
+ *               bound whose gradient points outward is held and steps along -grad f (Bertsekas' epsilon-active set); a
+ *               free variable at a bound drops an outward Newton component; the free block is shifted to positive definite (H + tau I, tau doubled from 1e-3 max|H_ii| until its Cholesky succeeds);
+ *               Armijo backtracking along the projected arc (sufficient decrease 1e-4, up to 60 halvings, rounding slack
+ *               1e-13 (1 + |f|)); at most 100 iterations; stops when ||x - P(x - grad f(x))||_inf <= 1e-9 (1 + |f(x)|).
+ *               The end point is kept only if f there is strictly below the grid minimum, else the grid point is
+ *               returned (random_features.py:164).  The reference uses SLSQP here.
+ * points[num_points][d], values[num_points] (f at the returned point).  omega[num_points][F][d] (the frequencies W =
+ * Omega / l), b[num_points][F] and theta[num_points][F] may be NULL; they return each sample function.
+ * Randomness: sample s is a pure function of (seed, first_draw + s): Omega (row-major), then z, then eps (M < F only) are
+ * the normals 0 .. F d + F + M - 1 of Philox draw first_draw + s (cmoe_philox_normals), and u_f comes from the Philox
+ * call (draw, f / 2) with counter word 3 = 2 (words 0, 1 for even f, 2, 3 for odd f, as 53-bit uniforms).  With a table,
+ * the table's numbers replace Philox: omega[P][F][d] (Omega), b[P][F] (b itself), z[P][F], eps[P][M] (read only when
+ * M < F).  Samples run in chunks that fit the handle's 2 GiB sampling workspace; a sample's result does not depend on
+ * num_points or the chunking.  The caller's GP is not modified.
+ * Errors (before any device work, the first two before gp is read): CMOE_ERR_BOUNDS unless num_features, num_points,
+ * num_grid >= 1; CMOE_ERR_INVALID_VALUE for a NULL gp; CMOE_ERR_BOUNDS unless min(F, M) <= 8192 and
+ * (F M + min(F, M)^2) doubles fit in 2 GiB; CMOE_ERR_INVALID_VALUE for NULL arguments, non-finite grid points or bounds,
+ * min > max, or a noise variance that is not > 0.  A failed factorisation (non-finite data) -> CMOE_ERR_SINGULAR. */
+typedef struct cmoe_rff_table {
+  const double* omega; /* [P][F][d] standard normals */
+  const double* b;     /* [P][F] phases */
+  const double* z;     /* [P][F] */
+  const double* eps;   /* [P][M], read only when M < F */
+} cmoe_rff_table;
+
+int cmoe_gp_sample_rff_optima(const cmoe_gp* gp, int num_features, int num_points, const double* domain_bounds,
+                              const double* grid, int num_grid, uint64_t seed, uint64_t first_draw,
+                              const cmoe_rff_table* table, double* points, double* values, double* omega, double* b,
+                              double* theta, int* info);
+
 /* ---- lower-confidence-bound batch selection ----------------------------------------------------------------------
  * lower_confidence_bound_optimization (moe/optimal_learning/python/cpp_wrappers/lower_confidence_bound.py:52-80) in one
  * call.  candidates [num_candidates][dim].  mu(x) is the value mean, sigma(x) the square root of the value variance.
