@@ -4,6 +4,7 @@ This is the thinnest possible host layer: numpy arrays in, numpy arrays out, eve
 libcornell_moe_b200.so (hand-written sm_90a kernels).  If the library is missing or no CUDA device is visible the
 calls raise — there is deliberately no fallback.
 """
+import collections
 import ctypes
 import os
 
@@ -937,6 +938,38 @@ class GaussianProcessEnsemble:
         initial = pts[int(np.argmin(test))]
         point, value, _, _ = self.posterior_mean_optimization(initial[None], params, domain_bounds, num_fidelity)
         return initial.copy() if -value > np.min(test) else point
+
+    def posterior_mean_optima(self, points, params, domain_bounds, num_fidelity=0, include_sampled=True,
+                              shared_discrete=None):
+        """cmoe_posterior_mean_optima_mcmc: per member, screen `points` (and the member's own sampled points if
+        include_sampled) by posterior mean, descend from the argmin with the reference's line search, keep the start if
+        the descent ended higher, and take the least mean over [shared_discrete ; optimum].  points is [P, ps] (shared by
+        the members) or [M, P, ps] (one list per member), ps = dim - num_fidelity; `params` as in
+        posterior_mean_optimization.  Returns a PosteriorMeanOptima; its discrete_pts [M, num_shared + 1, ps] and
+        best_so_far [M] are what kg / multistart_kg take."""
+        ps, M = self.dim - num_fidelity, len(self.members)
+        pts = _f64(points)
+        per_member = pts.ndim == 3
+        pts = pts.reshape((M, -1, ps) if per_member else (-1, ps))
+        P = pts.shape[-2]
+        shared = _f64(shared_discrete).reshape(-1, ps) if shared_discrete is not None else np.zeros((0, ps))
+        ns = shared.shape[0]
+        params = _gd_params_any(params)
+        db = _f64(domain_bounds).ravel()
+        out = PosteriorMeanOptima(np.empty((M, ps)), np.empty(M), np.empty(M, dtype=np.int32),
+                                  np.empty(M, dtype=np.int32), np.empty(M), np.empty((M, ns + 1, ps)), np.empty(M))
+        _ip = ctypes.POINTER(ctypes.c_int)
+        info = ctypes.c_int()
+        _check(lib().cmoe_posterior_mean_optima_mcmc(
+            self._handles(), M, int(num_fidelity), ctypes.byref(params), _d(db), _d(pts), P, int(per_member),
+            int(bool(include_sampled)), _d(shared) if ns else None, ns, _d(out.optima), _d(out.means),
+            out.start_index.ctypes.data_as(_ip), out.kept_start.ctypes.data_as(_ip), _d(out.screen_min),
+            _d(out.discrete_pts), _d(out.best_so_far), ctypes.byref(info)), info.value)
+        return out
+
+
+PosteriorMeanOptima = collections.namedtuple(
+    "PosteriorMeanOptima", "optima means start_index kept_start screen_min discrete_pts best_so_far")
 
 
 def _gd_params_any(p):

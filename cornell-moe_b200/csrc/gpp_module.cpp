@@ -18,6 +18,7 @@
 //   compute_{,grad_}expected_improvement_mcmc, multistart_expected_improvement_mcmc_optimization,
 //   evaluate_EI_mcmc_at_point_list                                        gpp_python_expected_improvement_mcmc.cpp:46-300
 //   compute_posterior_mean_of_points, compute_{,grad_}posterior_mean_mcmc_of_points, posterior_mean_mcmc_optimization,
+//   posterior_mean_optima_mcmc,
 //   sample_hyperparameters_mcmc                                           batched forms, not in the reference module
 //   GradientDescentParameters, NewtonParameters, RandomnessSourceContainer, OptimizerTypes, DomainTypes,
 //   LogLikelihoodTypes                                                    gpp_python_common.cpp:201-370
@@ -1039,6 +1040,29 @@ py::tuple posterior_mean_mcmc_optimization(const py::object& gps, int num_fideli
   return py::make_tuple(to_list(best), to_list(vals));
 }
 
+// The discretisation step of examples/main.py:172-197 for every member at once (not in the reference module):
+// screen `points` (flat [num_points][dim-nf], shared by the members) and, if include_sampled, each member's own sampled
+// points by posterior mean, descend from the argmin with posterior_mean_optimization's line search, keep the start if
+// the descent ended higher.  Returns (discrete_pts flat [M][num_shared + 1][dim-nf] = shared_discrete_pts followed by
+// the member's optimum, best_so_far [M] as KnowledgeGradientMCMC computes it, optima flat [M][dim-nf]).
+py::tuple posterior_mean_optima_mcmc(const py::object& gps, int num_fidelity, const py::object& optimizer_parameters,
+                                     const py::list& domain_bounds, const py::list& points, int num_points,
+                                     const py::list& shared_discrete_pts, int num_shared, bool include_sampled) {
+  const auto h = ensemble_handles(gps);
+  const size_t ps = std::max(ensemble_dim(h) - num_fidelity, 0), n = std::max(num_points, 0), ns = std::max(num_shared, 0);
+  const auto bounds = to_vec(domain_bounds, 2 * ps);
+  const auto pts = to_vec(points, n * ps);
+  const auto shared = to_vec(shared_discrete_pts, ns * ps);
+  const cmoe_gd_params gd = gd_by_attr(optimizer_parameters);
+  std::vector<double> optima(h.size() * ps), disc(h.size() * (ns + 1) * ps), best(h.size());
+  int info = 0;
+  check(cmoe_posterior_mean_optima_mcmc(h.data(), static_cast<int>(h.size()), num_fidelity, &gd, bounds.data(),
+                                        pts.data(), num_points, 0, include_sampled ? 1 : 0,
+                                        ns ? shared.data() : nullptr, num_shared, optima.data(), nullptr, nullptr,
+                                        nullptr, nullptr, disc.data(), best.data(), &info), info);
+  return py::make_tuple(to_list(disc), to_list(best), to_list(optima));
+}
+
 PYBIND11_MODULE(GPP, m) {
   m.doc() = "H100-native drop-in for moe.build.GPP (GP posterior + MC acquisition hot path)";
   g_exc_base = PyErr_NewExceptionWithDoc("GPP.OptimalLearningException",
@@ -1175,6 +1199,9 @@ PYBIND11_MODULE(GPP, m) {
         py::arg("num_fidelity"), py::arg("points"), py::arg("num_points"));
   m.def("posterior_mean_mcmc_optimization", &posterior_mean_mcmc_optimization, py::arg("gps"), py::arg("num_fidelity"),
         py::arg("optimizer_parameters"), py::arg("domain_bounds"), py::arg("starting_points"), py::arg("num_starts"));
+  m.def("posterior_mean_optima_mcmc", &posterior_mean_optima_mcmc, py::arg("gps"), py::arg("num_fidelity"),
+        py::arg("optimizer_parameters"), py::arg("domain_bounds"), py::arg("points"), py::arg("num_points"),
+        py::arg("shared_discrete_pts"), py::arg("num_shared"), py::arg("include_sampled") = true);
   // names of the reference module that are outside the hot path (model selection, heuristic EI): present, so that an
   // unmodified front end fails with the library's own exception class and a clear message rather than AttributeError
   // compute_log_likelihood(points_sampled, points_sampled_value, dim, num_sampled, objective_type, hyperparameters,

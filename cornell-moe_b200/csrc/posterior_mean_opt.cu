@@ -12,6 +12,9 @@
 // The ensemble forms (cmoe_posterior_mean_mcmc, cmoe_posterior_mean_mcmc_optimization) serve the recommendation step
 // of the MCMC loop: screening many points, then the Python fixed-step gradient descent on the averaged mean from many
 // starts at once (one CTA per start); they share the row arithmetic (pm_rows) with pm_opt_kernel.
+//
+// cmoe_posterior_mean_optima_mcmc is the discretisation step of the MCMC q-KG loop: the same line search
+// (pm_descend) for every member of an ensemble at once, one CTA per member, after a screen over (member, point).
 #include <algorithm>
 #include <cmath>
 #include <limits>
@@ -22,9 +25,10 @@
 namespace cmoe {
 namespace {
 
-struct PmOptParams {
-  int N, ps, max_steps, max_restarts;
-  double mean, mrc, tol;
+// the line-search gradient descent's parameters (cmoe_gd_params) and box; coordinates >= ps (fidelity) do not move
+struct PmDescent {
+  int ps, max_steps, max_restarts;
+  double mrc, tol;
   double lo[CMOE_MAX_DIM], hi[CMOE_MAX_DIM];
 };
 
@@ -63,28 +67,28 @@ __device__ __forceinline__ void pm_rows(const KernelSpec& spec, int N, int ps, c
 }
 
 // f(x) = -mu(x), grad f = -dmu/dx on the free coordinates; all lanes return the same values
-__device__ double pm_eval(const KernelSpec& spec, const PmOptParams& prm, const double* __restrict__ X,
+__device__ double pm_eval(const KernelSpec& spec, int N, int ps, double mean, const double* __restrict__ X,
                           const double* __restrict__ beta, const double* xq, double* grad /* [dim] or null */) {
   const int dim = spec.dim, lane = threadIdx.x & 31;
   double val = 0.0;
   double g[CMOE_MAX_DIM];
   for (int d = 0; d < dim; ++d) g[d] = 0.0;
-  pm_rows(spec, prm.N, prm.ps, X, beta, xq, lane, 32, val, grad ? g : nullptr);
+  pm_rows(spec, N, ps, X, beta, xq, lane, 32, val, grad ? g : nullptr);
   val = warp_sum(val);
   if (grad)
-    for (int d = 0; d < dim; ++d) grad[d] = (d < prm.ps) ? -warp_sum(g[d]) : 0.0;
-  return -(prm.mean + val);
+    for (int d = 0; d < dim; ++d) grad[d] = (d < ps) ? -warp_sum(g[d]) : 0.0;
+  return -(mean + val);
 }
 
-__global__ void __launch_bounds__(32) pm_opt_kernel(const __grid_constant__ KernelSpec spec,
-                                                    const __grid_constant__ PmOptParams prm,
-                                                    const double* __restrict__ X, const double* __restrict__ beta,
-                                                    const double* __restrict__ alpha0, const double* __restrict__ x0,
-                                                    double* __restrict__ out) {
-  const int dim = spec.dim, ps = prm.ps;
-  double x[CMOE_MAX_DIM], gb[CMOE_MAX_DIM], xt[CMOE_MAX_DIM], step[CMOE_MAX_DIM], run0[CMOE_MAX_DIM];
-  for (int d = 0; d < dim; ++d) x[d] = x0[d];
-  double fb = pm_eval(spec, prm, X, beta, x, gb);
+// The reference's restarted line-search gradient descent on f from x [dim] (moved in place); returns f at the end
+// point.  eval(xq, grad or null) = f(xq) must return the same bits in every thread that calls this, so that every
+// decision below is uniform over those threads and each of them carries the same optimiser state.
+template <class Eval>
+__device__ __forceinline__ double pm_descend(const PmDescent& prm, int dim, const double* __restrict__ alpha0, double* x,
+                                             Eval&& eval) {
+  const int ps = prm.ps;
+  double gb[CMOE_MAX_DIM], xt[CMOE_MAX_DIM], step[CMOE_MAX_DIM], run0[CMOE_MAX_DIM];
+  double fb = eval(x, gb);
   if (prm.max_restarts > 0) {
     const double step_tol = prm.max_steps > 0 ? prm.tol / static_cast<double>(prm.max_steps) : 0.0;
     for (int r = 0; r < prm.max_restarts; ++r) {
@@ -97,7 +101,7 @@ __global__ void __launch_bounds__(32) pm_opt_kernel(const __grid_constant__ Kern
         double obj = 0.0;
         while (search < 30) {
           for (int d = 0; d < dim; ++d) xt[d] = x[d] + ((d < ps) ? alpha * gb[d] : 0.0);
-          obj = pm_eval(spec, prm, X, beta, xt, nullptr);
+          obj = eval(xt, nullptr);
           if (obj - fb > 0.5 * alpha * nrm) break;
           alpha *= 0.5;
           search += 1;
@@ -105,14 +109,14 @@ __global__ void __launch_bounds__(32) pm_opt_kernel(const __grid_constant__ Kern
         for (int d = 0; d < dim; ++d)
           step[d] = (d < ps) ? limit_step_pm(alpha * gb[d], x[d], prm.lo[d], prm.hi[d], prm.mrc) : 0.0;
         for (int d = 0; d < dim; ++d) xt[d] = x[d] + step[d];
-        obj = pm_eval(spec, prm, X, beta, xt, nullptr);
+        obj = eval(xt, nullptr);
         if (obj <= fb || search == 30) break;
         double ns = 0.0;
         for (int d = 0; d < dim; ++d) {
           x[d] += step[d];
           ns += step[d] * step[d];
         }
-        fb = pm_eval(spec, prm, X, beta, x, gb);
+        fb = eval(x, gb);
         if (sqrt(ns) < step_tol) break;
       }
       double nd = 0.0;
@@ -120,6 +124,20 @@ __global__ void __launch_bounds__(32) pm_opt_kernel(const __grid_constant__ Kern
       if (sqrt(nd) <= prm.tol) break;
     }
   }
+  return fb;
+}
+
+__global__ void __launch_bounds__(32) pm_opt_kernel(const __grid_constant__ KernelSpec spec,
+                                                    const __grid_constant__ PmDescent prm, int N, double mean,
+                                                    const double* __restrict__ X, const double* __restrict__ beta,
+                                                    const double* __restrict__ alpha0, const double* __restrict__ x0,
+                                                    double* __restrict__ out) {
+  const int dim = spec.dim, ps = prm.ps;
+  double x[CMOE_MAX_DIM];
+  for (int d = 0; d < dim; ++d) x[d] = x0[d];
+  const double fb = pm_descend(prm, dim, alpha0, x, [&](const double* xq, double* grad) {
+    return pm_eval(spec, N, ps, mean, X, beta, xq, grad);
+  });
   if (threadIdx.x == 0) {
     for (int d = 0; d < ps; ++d) out[d] = x[d];
     out[ps] = fb;
@@ -254,6 +272,220 @@ __global__ void __launch_bounds__(256) pm_mcmc_combine_kernel(int M, size_t P, i
   }
 }
 
+// --------------------------------------------------------------------------------------------------------------
+// Per-member posterior-mean optima (cmoe_posterior_mean_optima_mcmc): for every member on its own, screen a list of
+// points by mu_m, descend from the argmin with the line search above, fall back to the start if the descent ended
+// higher, and take the least mu_m over the member's discretisation set [shared points ; optimum]
+// (examples/main.py:172-197, knowledge_gradient_mcmc.py:386-393).
+//   pm_members_screen_kernel   one CTA per (member, screen index) of a chunk
+//   pm_members_argmin_kernel   one CTA per member: the chunk's least value and lowest index, merged into the running one
+//   pm_members_opt_kernel      one CTA per member: descent, fallback, baseline
+// Per member the three kernels share one row of `state`, kPmStateHead + 2 ps doubles:
+//   [0] least screened mu  [1] its index in the member's screen list  [2] mu at the optimum  [3] best_so_far
+//   [4] 1 if the start was kept  [5, 5 + ps) the start x0  [5 + ps, 5 + 2 ps) the optimum
+// --------------------------------------------------------------------------------------------------------------
+constexpr int kPmScreenParts = 128;    // partial sums per screened value: post_mean_only_kernel's thread count
+constexpr int kPmOptimaThreads = 256;  // pm_members_argmin_kernel, pm_members_opt_kernel
+constexpr int kPmMaxSlices = kPmOptimaThreads / 32;
+constexpr int kPmStateHead = 5;
+constexpr size_t kPmOptimaWorkspaceBytes = size_t(64) << 20;  // one screen chunk: its points and its values
+
+// row slices (warps) of a member's descent: a function of its rows n = N (1 + g) only, none shorter than two rows a lane
+__device__ __forceinline__ int pm_member_slices(int n) { return max(1, min(kPmMaxSlices, n / 64)); }
+
+__device__ __forceinline__ void load_member(PmMember* dst, const PmMember* __restrict__ src) {
+  const unsigned long long* in = reinterpret_cast<const unsigned long long*>(src);
+  unsigned long long* out = reinterpret_cast<unsigned long long*>(dst);
+  for (int i = threadIdx.x; i < static_cast<int>(sizeof(PmMember) / sizeof(unsigned long long)); i += blockDim.x)
+    out[i] = in[i];
+}
+
+// mu(x) of one member with the arithmetic of posterior_mean_points (post_mean_only_kernel, value only), so that a value
+// screened here and one returned by cmoe_posterior_mean_mcmc or cmoe_gp_posterior are the same bits: thread
+// p < kPmScreenParts adds the sampled points p, p + kPmScreenParts, ... in ascending order, thread 0 adds the partial
+// sums in ascending order.  Called by the whole CTA (>= kPmScreenParts threads); x [dim] and red [kPmScreenParts] are
+// shared memory; the result is valid in thread 0.
+__device__ __forceinline__ double pm_screen_mean(const PmMember& mb, const double* x, double* red) {
+  const int tid = threadIdx.x, dim = mb.spec.dim, b1 = 1 + mb.spec.g;
+  if (tid < kPmScreenParts) {
+    double acc = 0.0;
+    for (int j = tid; j < mb.N; j += kPmScreenParts) {
+      const double* xj = mb.X + static_cast<size_t>(j) * dim;
+      const KParts kp = kernel_parts(mb.spec, weighted_sqdist(mb.spec, x, xj));
+      for (int cc = 0; cc < b1; ++cc) {
+        const int a2 = cc ? mb.spec.derivs[cc - 1] : -1;
+        acc = fma(cov_entry(mb.spec, kp, x, xj, -1, a2), mb.beta[static_cast<size_t>(j) * b1 + cc], acc);
+      }
+    }
+    red[tid] = acc;
+  }
+  __syncthreads();
+  double t = 0.0;
+  if (tid == 0)
+    for (int q = 0; q < kPmScreenParts; ++q) t += red[q];
+  __syncthreads();
+  return mb.mean + t;
+}
+
+// Screen indices [i0, i0 + len) of every member's list: the given points (shared by the members, or one list per
+// member), then the member's own sampled points, read from its X.  grid.x = num_gp * len; V [num_gp][len].  pts holds
+// the given points of this chunk only, [1 or num_gp][num_given][ps], num_given = those of the chunk's indices below
+// num_points.
+__global__ void __launch_bounds__(kPmScreenParts) pm_members_screen_kernel(const PmMember* __restrict__ members, int ps,
+                                                                           const double* __restrict__ pts,
+                                                                           int per_member, int num_points,
+                                                                           int include_sampled, int i0, int len,
+                                                                           int num_given, double* __restrict__ V) {
+  __shared__ PmMember mb;
+  __shared__ double x[CMOE_MAX_DIM];
+  __shared__ double red[kPmScreenParts];
+  const int m = blockIdx.x / len, i = blockIdx.x % len, gi = i0 + i;
+  load_member(&mb, members + m);
+  __syncthreads();
+  if (gi >= num_points + (include_sampled ? mb.N : 0)) return;
+  const double* src = (gi < num_points) ? pts + (static_cast<size_t>(per_member ? m : 0) * num_given + i) * ps
+                                        : mb.X + static_cast<size_t>(gi - num_points) * mb.spec.dim;
+  for (int d = threadIdx.x; d < mb.spec.dim; d += blockDim.x) x[d] = (d < ps) ? src[d] : 1.0;  // fidelity = 1
+  __syncthreads();
+  const double mu = pm_screen_mean(mb, x, red);
+  if (threadIdx.x == 0) V[static_cast<size_t>(m) * len + i] = mu;
+}
+
+// (value, index) order of the argmin: the smaller value, and among equal values the lower index
+__device__ __forceinline__ bool pm_less(double v, int i, double w, int j) { return v < w || (v == w && i < j); }
+
+// grid.x = num_gp.  Each thread scans its indices of the chunk in ascending order, then a fixed tree combines the
+// threads; the chunk's winner replaces the running one only if it is strictly smaller, so the result is np.argmin's
+// (first occurrence) however the screen is chunked.  The winner's coordinates become the member's start.
+__global__ void __launch_bounds__(kPmOptimaThreads) pm_members_argmin_kernel(const PmMember* __restrict__ members,
+                                                                             int ps, const double* __restrict__ pts,
+                                                                             int per_member, int num_points,
+                                                                             int include_sampled, int i0, int len,
+                                                                             int num_given,
+                                                                             const double* __restrict__ V,
+                                                                             double* __restrict__ state) {
+  __shared__ double sv[kPmOptimaThreads];
+  __shared__ int si[kPmOptimaThreads];
+  const int m = blockIdx.x, tid = threadIdx.x;
+  const PmMember& mb = members[m];
+  const int cnt = min(len, num_points + (include_sampled ? mb.N : 0) - i0);
+  if (cnt <= 0) return;
+  const double* Vm = V + static_cast<size_t>(m) * len;
+  double bv = Vm[0];  // a chunk whose values are all NaN still names a point
+  int bi = 0;
+  for (int i = tid; i < cnt; i += kPmOptimaThreads)
+    if (pm_less(Vm[i], i, bv, bi)) {
+      bv = Vm[i];
+      bi = i;
+    }
+  sv[tid] = bv;
+  si[tid] = bi;
+  __syncthreads();
+  for (int h = kPmOptimaThreads / 2; h > 0; h >>= 1) {
+    if (tid < h && pm_less(sv[tid + h], si[tid + h], sv[tid], si[tid])) {
+      sv[tid] = sv[tid + h];
+      si[tid] = si[tid + h];
+    }
+    __syncthreads();
+  }
+  double* row = state + static_cast<size_t>(m) * (kPmStateHead + 2 * ps);
+  const bool take = i0 == 0 || sv[0] < row[0];
+  __syncthreads();  // every thread has read the running minimum before thread 0 replaces it
+  if (!take) return;
+  const int gi = i0 + si[0];
+  const double* src = (gi < num_points) ? pts + (static_cast<size_t>(per_member ? m : 0) * num_given + si[0]) * ps
+                                        : mb.X + static_cast<size_t>(gi - num_points) * mb.spec.dim;
+  if (tid < ps) row[kPmStateHead + tid] = src[tid];
+  if (tid == 0) {
+    row[0] = sv[0];
+    row[1] = static_cast<double>(gi);
+  }
+}
+
+// f(x) = -mu_m(x) and its gradient for the whole CTA: warp s < S takes the rows s * 32 + lane, stride 32 S (pm_rows),
+// lanes combined by the xor butterfly, slices added in ascending order.  Every thread returns the same bits; with S = 1
+// they are pm_eval's.  red [kPmMaxSlices][1 + ps] is shared memory.  Not inlined: the line search calls it from four
+// places, and one copy of the row loop keeps the kernel's code small and its registers unspilled.
+__device__ __noinline__ double pm_member_eval(const PmMember& mb, int ps, int S, const double* xq, double* grad,
+                                                 double* red) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, dim = mb.spec.dim, w1 = 1 + ps;
+  if (warp < S) {
+    double val = 0.0;
+    double g[CMOE_MAX_DIM];
+    for (int d = 0; d < ps; ++d) g[d] = 0.0;
+    pm_rows(mb.spec, mb.N, ps, mb.X, mb.beta, xq, warp * 32 + lane, S * 32, val, grad ? g : nullptr);
+    val = warp_sum(val);
+    if (lane == 0) red[warp * w1] = val;
+    if (grad)
+      for (int d = 0; d < ps; ++d) {
+        const double t = warp_sum(g[d]);
+        if (lane == 0) red[warp * w1 + 1 + d] = t;
+      }
+  }
+  __syncthreads();
+  double val = red[0];
+  for (int s = 1; s < S; ++s) val = __dadd_rn(val, red[s * w1]);
+  if (grad)
+    for (int d = 0; d < dim; ++d) {
+      double t = 0.0;
+      if (d < ps) {
+        t = red[1 + d];
+        for (int s = 1; s < S; ++s) t = __dadd_rn(t, red[s * w1 + 1 + d]);
+      }
+      grad[d] = (d < ps) ? -t : 0.0;
+    }
+  __syncthreads();
+  return -(mb.mean + val);
+}
+
+// grid.x = num_gp.  Descent from the member's start with every thread carrying the optimiser state (pm_descend), the
+// fallback of main.py:191-193, then mu_m over [shared_pts ; optimum] in the screen's arithmetic, which is what
+// cmoe_gp_posterior returns at those points.
+__global__ void __launch_bounds__(kPmOptimaThreads) pm_members_opt_kernel(const __grid_constant__ PmDescent prm,
+                                                                          const PmMember* __restrict__ members,
+                                                                          const double* __restrict__ alpha0,
+                                                                          const double* __restrict__ shared_pts,
+                                                                          int num_shared, double* __restrict__ state) {
+  __shared__ PmMember mb;
+  __shared__ double red[kPmMaxSlices * (1 + CMOE_MAX_DIM)];
+  __shared__ double sred[kPmScreenParts];
+  __shared__ double xs[CMOE_MAX_DIM];
+  const int tid = threadIdx.x, ps = prm.ps;
+  load_member(&mb, members + blockIdx.x);
+  __syncthreads();
+  const int dim = mb.spec.dim;
+  double* row = state + static_cast<size_t>(blockIdx.x) * (kPmStateHead + 2 * ps);
+  const double screen_min = row[0];
+  double x[CMOE_MAX_DIM];
+  for (int d = 0; d < dim; ++d) x[d] = (d < ps) ? row[kPmStateHead + d] : 1.0;  // fidelity = 1
+  bool kept = true;  // max_num_restarts <= 0: the reference's descent returns without moving
+  double mu_opt = screen_min;
+  if (prm.max_restarts > 0) {
+    const int S = pm_member_slices(mb.N * (1 + mb.spec.g));
+    const double fb = pm_descend(prm, dim, alpha0, x, [&](const double* xq, double* grad) {
+      return pm_member_eval(mb, ps, S, xq, grad, red);
+    });
+    kept = -fb > screen_min;
+    if (!kept) mu_opt = -fb;
+  }
+  if (kept)
+    for (int d = 0; d < ps; ++d) x[d] = row[kPmStateHead + d];
+  double best = 0.0;
+  for (int j = 0; j <= num_shared; ++j) {
+    for (int d = 0; d < dim; ++d)
+      if (tid == d) xs[d] = (d >= ps) ? 1.0 : (j < num_shared) ? shared_pts[static_cast<size_t>(j) * ps + d] : x[d];
+    __syncthreads();
+    const double mu = pm_screen_mean(mb, xs, sred);
+    best = (j == 0 || mu < best) ? mu : best;
+  }
+  if (tid == 0) {
+    row[2] = mu_opt;
+    row[3] = best;
+    row[4] = kept ? 1.0 : 0.0;
+    for (int d = 0; d < ps; ++d) row[kPmStateHead + ps + d] = x[d];
+  }
+}
+
 // the members' fits ran on their own streams; the ensemble calls work on member 0's
 void join_member_streams(const cmoe_gp* const* gps, int num_gp) {
   for (int m = 1; m < num_gp; ++m)
@@ -279,12 +511,10 @@ extern "C" int cmoe_posterior_mean_optimization(const cmoe_gp* gp, int num_fidel
     if (found_flag) *found_flag = 0;
     if (params->max_num_restarts <= 0) return;  // the reference returns without touching its outputs (:424-426)
     cudaStream_t s = gp->stream;
-    PmOptParams prm{};
-    prm.N = gp->N;
+    PmDescent prm{};
     prm.ps = ps;
     prm.max_steps = params->max_num_steps;
     prm.max_restarts = params->max_num_restarts;
-    prm.mean = gp->mean;
     prm.mrc = params->max_relative_change;
     prm.tol = params->tolerance;
     for (int d = 0; d < CMOE_MAX_DIM; ++d) {
@@ -298,7 +528,7 @@ extern "C" int cmoe_posterior_mean_optimization(const cmoe_gp* gp, int num_fidel
     DevBuf<double> dA0, dX0, dOut(ps + 1);
     dA0.upload(a0.data(), a0.size(), s);
     dX0.upload(x0.data(), x0.size(), s);
-    pm_opt_kernel<<<1, 32, 0, s>>>(spec, prm, gp->dX.p, gp->dKinvY.p, dA0.p, dX0.p, dOut.p);
+    pm_opt_kernel<<<1, 32, 0, s>>>(spec, prm, gp->N, gp->mean, gp->dX.p, gp->dKinvY.p, dA0.p, dX0.p, dOut.p);
     count_launch();
     CMOE_CUDA(cudaGetLastError());
     dOut.download(res.data(), ps + 1, s);
@@ -435,5 +665,110 @@ extern "C" int cmoe_posterior_mean_mcmc_optimization(const cmoe_gp* const* gps, 
     }
     if (best_point) std::copy(bp, bp + ps, best_point);
     if (best_value) *best_value = bv;
+  });
+}
+
+extern "C" int cmoe_posterior_mean_optima_mcmc(const cmoe_gp* const* gps, int num_gp, int num_fidelity,
+                                               const cmoe_gd_params* params, const double* domain_bounds,
+                                               const double* points, int num_points, int points_per_member,
+                                               int include_sampled, const double* shared_discrete, int num_shared,
+                                               double* optima, double* optimum_means, int* start_index,
+                                               int* kept_start, double* screen_min, double* discrete_pts,
+                                               double* best_so_far, int* info) {
+  return guarded(info, [&] {
+    // every check comes before any device work; those that need no GP handle come first
+    CMOE_REQUIRE(params != nullptr && domain_bounds != nullptr && points != nullptr && optima != nullptr,
+                 CMOE_ERR_INVALID_VALUE, "params, domain_bounds, points and optima must not be NULL");
+    CMOE_REQUIRE(shared_discrete != nullptr || num_shared <= 0, CMOE_ERR_INVALID_VALUE,
+                 "shared_discrete must not be NULL when num_shared > 0");
+    CMOE_REQUIRE(num_points >= 1, CMOE_ERR_BOUNDS, "num_points must be >= 1");
+    CMOE_REQUIRE(num_shared >= 0, CMOE_ERR_BOUNDS, "num_shared must be >= 0");
+    CMOE_REQUIRE(params->max_num_steps <= 1 << 20, CMOE_ERR_BOUNDS, "max_num_steps too large");
+    CMOE_REQUIRE(num_fidelity >= 0, CMOE_ERR_BOUNDS, "num_fidelity out of range");
+    check_ensemble(gps, num_gp);
+    const int dim = gps[0]->spec.dim, ps = dim - num_fidelity;
+    CMOE_REQUIRE(ps >= 1, CMOE_ERR_BOUNDS, "num_fidelity out of range");
+    for (int d = 0; d < ps; ++d)
+      CMOE_REQUIRE(domain_bounds[2 * d] <= domain_bounds[2 * d + 1], CMOE_ERR_BOUNDS, "Tensor product region is EMPTY.");
+    const size_t M = num_gp, P = num_points, lists = points_per_member ? M : 1, steps = std::max(0, params->max_num_steps);
+    for (size_t k = 0; k < lists * P * ps; ++k)
+      CMOE_REQUIRE(std::isfinite(points[k]), CMOE_ERR_INVALID_VALUE, "screen points must be finite");
+    for (size_t k = 0; k < static_cast<size_t>(num_shared) * ps; ++k)
+      CMOE_REQUIRE(std::isfinite(shared_discrete[k]), CMOE_ERR_INVALID_VALUE, "shared_discrete must be finite");
+    int max_N = 0;
+    for (int m = 0; m < num_gp; ++m) max_N = std::max(max_N, gps[m]->N);
+    const size_t total = P + (include_sampled ? max_N : 0);  // the longest member's screen list
+    CMOE_REQUIRE(total <= static_cast<size_t>(std::numeric_limits<int>::max()), CMOE_ERR_BOUNDS,
+                 "num_points + num_sampled must fit an int");
+    require_device(gps[0]->device);
+    join_member_streams(gps, num_gp);
+    cudaStream_t s = gps[0]->stream;
+
+    PmDescent prm{};
+    prm.ps = ps;
+    prm.max_steps = params->max_num_steps;
+    prm.max_restarts = params->max_num_restarts;
+    prm.mrc = params->max_relative_change;
+    prm.tol = params->tolerance;
+    for (int d = 0; d < CMOE_MAX_DIM; ++d) {
+      prm.lo[d] = (d < ps) ? domain_bounds[2 * d] : -1e300;
+      prm.hi[d] = (d < ps) ? domain_bounds[2 * d + 1] : 1e300;
+    }
+    // screen indices per chunk: the chunk's given points and its values fit kPmOptimaWorkspaceBytes
+    const size_t chunk =
+        std::max<size_t>(1, std::min(total, kPmOptimaWorkspaceBytes / (sizeof(double) * (M + lists * ps))));
+    // one staging buffer, one upload: member table | step sizes | shared discrete points | the chunk's given points
+    const size_t o_alpha = M * sizeof(PmMember) / sizeof(double), o_shared = o_alpha + steps,
+                 o_pts = o_shared + static_cast<size_t>(num_shared) * ps, given_max = std::min(chunk, P);
+    std::vector<double> stage(o_pts + lists * given_max * ps);
+    static_assert(sizeof(PmMember) % sizeof(double) == 0, "the member table is staged as doubles");
+    for (int m = 0; m < num_gp; ++m) {
+      const PmMember mb{gps[m]->spec, gps[m]->dX.p, gps[m]->dKinvY.p, gps[m]->mean, gps[m]->N};
+      std::memcpy(stage.data() + m * (sizeof(PmMember) / sizeof(double)), &mb, sizeof(PmMember));
+    }
+    for (size_t i = 0; i < steps; ++i)
+      stage[o_alpha + i] = params->pre_mult * std::pow(static_cast<double>(i + 1), -params->gamma);
+    std::copy(shared_discrete, shared_discrete + static_cast<size_t>(num_shared) * ps, stage.begin() + o_shared);
+    const size_t W = kPmStateHead + 2 * ps;
+    DevBuf<double> dIn(stage.size()), dV(M * chunk), dState(M * W);
+    const PmMember* dMem = reinterpret_cast<const PmMember*>(dIn.p);
+    for (size_t i0 = 0; i0 < total; i0 += chunk) {
+      const size_t len = std::min(chunk, total - i0), given = i0 < P ? std::min(len, P - i0) : 0;
+      for (size_t l = 0; l < lists; ++l)
+        std::copy(points + (l * P + i0) * ps, points + (l * P + i0 + given) * ps, stage.begin() + o_pts + l * given * ps);
+      const size_t first = i0 == 0 ? 0 : o_pts, count = o_pts + lists * given * ps - first;
+      if (count) CMOE_CUDA(cudaMemcpyAsync(dIn.p + first, stage.data() + first, count * sizeof(double),
+                                           cudaMemcpyHostToDevice, s));
+      pm_members_screen_kernel<<<static_cast<unsigned>(M * len), kPmScreenParts, 0, s>>>(
+          dMem, ps, dIn.p + o_pts, points_per_member != 0, num_points, include_sampled != 0, static_cast<int>(i0),
+          static_cast<int>(len), static_cast<int>(given), dV.p);
+      pm_members_argmin_kernel<<<num_gp, kPmOptimaThreads, 0, s>>>(
+          dMem, ps, dIn.p + o_pts, points_per_member != 0, num_points, include_sampled != 0, static_cast<int>(i0),
+          static_cast<int>(len), static_cast<int>(given), dV.p, dState.p);
+      count_launch(2);
+      CMOE_CUDA(cudaGetLastError());
+    }
+    pm_members_opt_kernel<<<num_gp, kPmOptimaThreads, 0, s>>>(prm, dMem, dIn.p + o_alpha, dIn.p + o_shared, num_shared,
+                                                              dState.p);
+    count_launch();
+    CMOE_CUDA(cudaGetLastError());
+    std::vector<double> res(M * W);
+    dState.download(res.data(), res.size(), s);
+    CMOE_CUDA(cudaStreamSynchronize(s));
+    for (size_t m = 0; m < M; ++m) {
+      const double* r = res.data() + m * W;
+      const double* opt = r + kPmStateHead + ps;
+      std::copy(opt, opt + ps, optima + m * ps);
+      if (screen_min) screen_min[m] = r[0];
+      if (start_index) start_index[m] = static_cast<int>(r[1]);
+      if (optimum_means) optimum_means[m] = r[2];
+      if (best_so_far) best_so_far[m] = r[3];
+      if (kept_start) kept_start[m] = static_cast<int>(r[4]);
+      if (discrete_pts) {
+        double* dp = discrete_pts + m * (static_cast<size_t>(num_shared) + 1) * ps;
+        std::copy(stage.begin() + o_shared, stage.begin() + o_pts, dp);
+        std::copy(opt, opt + ps, dp + static_cast<size_t>(num_shared) * ps);
+      }
+    }
   });
 }

@@ -528,6 +528,44 @@ int cmoe_posterior_mean_mcmc_optimization(const cmoe_gp* const* gps, int num_gp,
                                           const double* starts, int num_starts, double* points_out,
                                           double* values_out, double* best_point, double* best_value, int* info);
 
+/* ---- per-member posterior-mean optima: the discretisation step of the MCMC q-KG loop ---------------------------------
+ * examples/main.py:172-197 and KnowledgeGradientMCMC's best_so_far (cpp_wrappers/knowledge_gradient_mcmc.py:386-393) for
+ * every member of an ensemble (gps[num_gp], same rules as cmoe_posterior_mean_mcmc: members may have different numbers
+ * of sampled points, fidelity coordinates are pinned to 1.0, ps = dim - num_fidelity free coordinates) in one call.
+ * For every member m, independently:
+ *   1. screen   mu_m at points[num_points][ps] (shared by the members) or, with points_per_member != 0, at the member's
+ *               own list points[num_gp][num_points][ps]; with include_sampled != 0 also at the first ps coordinates of
+ *               the member's N_m sampled points, which follow the given points in the member's screen list.
+ *   2. argmin   the least value and its first index (numpy.argmin): screen_min[m], start_index[m], start x0_m.  The
+ *               screened values are bit for bit -member_values of cmoe_posterior_mean_mcmc on the same points.
+ *   3. descent  ComputeOptimalPosteriorMean from x0_m: what cmoe_posterior_mean_optimization computes, with the same
+ *               params and domain_bounds[ps][2].  A member with N_m (1 + g) >= 128 rows spreads them over up to 8 warps
+ *               (the count depends on the member's rows only) and adds the warps' sums in ascending order, so its end
+ *               point agrees with the single-GP call to rounding; a smaller member returns that call's bits.
+ *   4. fallback if mu_m at the end point is greater than screen_min[m] the optimum is x0_m and kept_start[m] = 1.
+ *               max_num_restarts <= 0: the reference's descent returns without moving, so the optimum is x0_m and
+ *               kept_start[m] = 1 (the single-GP call writes nothing then; here the screen always gives an answer).
+ *   5. baseline discrete_pts[m] = [shared_discrete[num_shared][ps] ; optimum_m] and best_so_far[m] = the least mu_m over
+ *               it (values as cmoe_gp_posterior returns them): the discrete_pts (num_pts = num_shared + 1) and
+ *               best_so_far arguments of cmoe_kg_eval_mcmc / cmoe_multistart_kg_mcmc.  shared_discrete may be NULL with
+ *               num_shared = 0.
+ * A member's result depends on that member, its screen points, params and the bounds only: not on num_gp, on the other
+ * members, or on how the screen is split into chunks.  The screen runs in chunks whose given points and values fit a
+ * 64 MiB workspace (at least one screen index per chunk); num_gp (num_points + N) is not bounded by a grid dimension,
+ * num_points + N must fit an int.  A screen point outside the box is allowed (the reference does not check).
+ * Outputs (all but optima may be NULL): optima[num_gp][ps]; optimum_means[num_gp] = mu_m at the returned point;
+ * start_index[num_gp]; kept_start[num_gp]; screen_min[num_gp]; discrete_pts[num_gp][num_shared + 1][ps];
+ * best_so_far[num_gp].
+ * Errors, all before any device work: NULL params / domain_bounds / points / optima (or shared_discrete with
+ * num_shared > 0) and non-finite points are CMOE_ERR_INVALID_VALUE; num_points < 1, num_shared < 0, num_fidelity outside
+ * [0, dim), max_num_steps > 2^20 and an empty box are CMOE_ERR_BOUNDS; ensemble mismatches as in the other *_mcmc calls. */
+int cmoe_posterior_mean_optima_mcmc(const cmoe_gp* const* gps, int num_gp, int num_fidelity,
+                                    const cmoe_gd_params* params, const double* domain_bounds, const double* points,
+                                    int num_points, int points_per_member, int include_sampled,
+                                    const double* shared_discrete, int num_shared, double* optima,
+                                    double* optimum_means, int* start_index, int* kept_start, double* screen_min,
+                                    double* discrete_pts, double* best_so_far, int* info);
+
 /* ---- building blocks exposed for parity tests and micro-benchmarks ------------------------------------------------ */
 /* Covariance build alone on device-resident inputs: returns device time (usec) of `repeats` builds of the n*n matrix. */
 int cmoe_bench_cov_build(const cmoe_gp* gp, int repeats, double* usec_per_build);
