@@ -23,9 +23,8 @@ __global__ void center_values_kernel(const double* __restrict__ y, int N, int b,
 // x.y - |x|^2/2 - |y|^2/2, whose absolute error grows with |x|^2 + |y|^2 in length-scale units — a domain far from the
 // origin ([1000, 1010] with l = 1) would otherwise lose ~1e-10 relative on every entry.  The kernels are translation
 // invariant, so any common shift is exact in exact arithmetic; coincident points still map to identical coordinates.
-struct Centre {
-  double c[CMOE_MAX_DIM];
-};
+// The centre is kept on the handle (cmoe_gp::centre): the q-KG operands (kg.cu) use the same expanded form and are put
+// in the same frame, so a fit and a q-KG plan always share one origin.
 __global__ void scale_points_kernel(const __grid_constant__ KernelSpec spec, const __grid_constant__ Centre centre,
                                     const double* __restrict__ X, int N, double* __restrict__ Xs) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
@@ -41,6 +40,13 @@ Centre centre_of(const std::vector<double>& hX, int N, int dim) {
     for (int i = 0; i < N; ++i) m += hX[static_cast<size_t>(i) * dim + d];
     c.c[d] = N > 0 ? m / N : 0.0;
   }
+  return c;
+}
+
+// the handle's centre from its training points (every (re)fit and append)
+Centre update_centre(cmoe_gp* gp) {
+  const Centre c = centre_of(gp->hX, gp->N, gp->spec.dim);
+  std::copy(c.c, c.c + CMOE_MAX_DIM, gp->centre);
   return c;
 }
 
@@ -109,8 +115,7 @@ void fit_gp(cmoe_gp* gp, bool mean_change) {
   ensure_scaled_points(gp->dXs, N, spec.dim, s);
   if (gp->dFlag.count == 0) gp->dFlag.alloc(1);
 
-  scale_points_kernel<<<(N * spec.dim + 255) / 256, 256, 0, s>>>(spec, centre_of(gp->hX, N, spec.dim), gp->dX.p, N,
-                                                                 gp->dXs.p);
+  scale_points_kernel<<<(N * spec.dim + 255) / 256, 256, 0, s>>>(spec, update_centre(gp), gp->dX.p, N, gp->dXs.p);
   count_launch();
   EventTimer t0, t1, t2;
   t0.start(s);
@@ -199,8 +204,7 @@ void append_points(cmoe_gp* gp, const double* new_points, const double* new_valu
   gp->dy.upload(gp->hy.data(), gp->hy.size(), s);
   ensure_scaled_points(gp->dXs, gp->N, dim, s);
   gp->dKinvY.ensure(n1);
-  scale_points_kernel<<<(gp->N * dim + 255) / 256, 256, 0, s>>>(spec, centre_of(gp->hX, gp->N, dim), gp->dX.p, gp->N,
-                                                                gp->dXs.p);
+  scale_points_kernel<<<(gp->N * dim + 255) / 256, 256, 0, s>>>(spec, update_centre(gp), gp->dX.p, gp->N, gp->dXs.p);
   double mu = 0.0;  // mean_ = average of the function values (gpp_math.cpp:498-504), same summation order
   for (int i = 0; i < gp->N; ++i) mu += gp->hy[static_cast<size_t>(i) * b];
   gp->mean = mu / gp->N;
@@ -215,7 +219,7 @@ void append_points(cmoe_gp* gp, const double* new_points, const double* new_valu
 void scale_points(const cmoe_gp& gp, const double* P, int m, DevBuf<double>& Ps, cudaStream_t s) {
   const int dim = gp.spec.dim;
   ensure_scaled_points(Ps, m, dim, s);
-  scale_points_kernel<<<(m * dim + 255) / 256, 256, 0, s>>>(gp.spec, centre_of(gp.hX, gp.N, dim), P, m, Ps.p);
+  scale_points_kernel<<<(m * dim + 255) / 256, 256, 0, s>>>(gp.spec, centre_of(gp), P, m, Ps.p);
   count_launch();
 }
 
@@ -231,6 +235,7 @@ cmoe_gp* clone_gp_to_device(const cmoe_gp* src, int device) {
   gp->hy = src->hy;
   gp->hnoise = src->hnoise;
   gp->hlengths = src->hlengths;
+  std::copy(src->centre, src->centre + CMOE_MAX_DIM, gp->centre);
   gp->generation = src->generation;
   CMOE_CUDA(cudaStreamCreateWithFlags(&gp->stream, cudaStreamNonBlocking));
   cudaStream_t s = gp->stream;

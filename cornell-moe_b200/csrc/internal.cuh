@@ -134,9 +134,11 @@ struct cmoe_gp {
   int n = 0;  // rows = N * (1 + g)
   double mean = 0.0;
   std::vector<double> hX, hy, hnoise, hlengths;
+  // mean of the training points: the origin of dXs and of every q-KG operand (scaled coordinates are (x - centre) / l)
+  double centre[CMOE_MAX_DIM] = {};
   cudaStream_t stream = nullptr;
   cmoe::DevBuf<double> dX;        // [N][dim]
-  cmoe::DevBuf<double> dXs;       // [N][dim] scaled by 1/l (for the MC kernels)
+  cmoe::DevBuf<double> dXs;       // [N][dim] (x - centre) / l (the fast covariance build)
   cmoe::DevBuf<double> dy;        // [n]
   cmoe::DevBuf<double> dnoise;    // [1+g]
   cmoe::DevBuf<double> dK;        // [n*n] column-major Cholesky factor (lower)
@@ -162,6 +164,15 @@ constexpr int kTrsmNB = 32;
 constexpr size_t kMaxGridY = 65535;
 
 // ---- gp.cu ----
+// the origin of the covariance-build frame (cmoe_gp::centre) as a kernel argument
+struct Centre {
+  double c[CMOE_MAX_DIM];
+};
+inline Centre centre_of(const cmoe_gp& gp) {
+  Centre c{};
+  for (int d = 0; d < CMOE_MAX_DIM; ++d) c.c[d] = gp.centre[d];
+  return c;
+}
 void fit_gp(cmoe_gp* gp, bool mean_change);
 // bit-identical copy of a fitted GP on another device (peer copies of the factor; no refit)
 cmoe_gp* clone_gp_to_device(const cmoe_gp* gp, int device);

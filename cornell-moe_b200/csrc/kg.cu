@@ -40,20 +40,30 @@ __global__ void build_union_kernel(const double* __restrict__ cand, const double
   P[e] = (r < static_cast<size_t>(q) * dim) ? cand[c * q * dim + r] : Xp[r - static_cast<size_t>(q) * dim];
 }
 
+// Frame of the MC and accumulation kernels' operands.  They form -r^2/2 as x.y - |x|^2/2 - |y|^2/2 (e_j, e_u, outH),
+// whose absolute error grows with |x|^2 + |y|^2 in length-scale units, so every operand they read is taken relative to
+// the GP's centre (cmoe_gp::centre, the frame of the fit's covariance build): the training points (Xt), the union points
+// (Xu), the start points (A, fidelity coordinates too), the inner bounds (KgMcParams::lo/hi) and, through them, the
+// minimisers (outX, outH).  The kernels are translation invariant.  The difference-form consumers (build_mix_covariance,
+// kg_discrete_kernel, the posterior batch, kg_grad_kernel's dK* terms) keep raw coordinates: D, Afull and pb.P stay raw,
+// and kg_g1_kernel moves outX back before differencing.
+//
 // scaled + zero-padded training points [N][DIMP]
-__global__ void pack_xt_kernel(const __grid_constant__ KernelSpec spec, const double* __restrict__ X, int N, int DIMP,
-                               double* __restrict__ Xt) {
+__global__ void pack_xt_kernel(const __grid_constant__ KernelSpec spec, const __grid_constant__ Centre ctr,
+                               const double* __restrict__ X, int N, int DIMP, double* __restrict__ Xt) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= N * DIMP) return;
   const int j = e / DIMP, d = e % DIMP;
-  Xt[e] = (d < spec.dim) ? X[static_cast<size_t>(j) * spec.dim + d] * spec.inv_len[d] : 0.0;
+  Xt[e] = (d < spec.dim) ? (X[static_cast<size_t>(j) * spec.dim + d] - ctr.c[d]) * spec.inv_len[d] : 0.0;
 }
 
 // per-candidate operand packs for the MC kernel.  g == 0: the pack row of training point j is [ e_j | beta_j, B_j,0..QP-1 ]
 // (stride QP + 2).  g > 0: training point j owns rows r = (j, m), m = 0..g; the pack row is [ e_j | 0 ] and the weights go
 // to the table Wt[1+QP][N(1+g)]: Wt[0][r] = beta~_r, Wt[1+u][r] = B~_(r,u)  (~ = divided by l_t, t = derivs[m-1], so
 // that derivative rows multiply plain scaled coordinate differences in the kernel).
-__global__ void __launch_bounds__(256) kg_pack_kernel(const __grid_constant__ KernelSpec spec, int N, int U, int ps,
+// Xu and A are in the centred frame; Afull keeps raw coordinates.
+__global__ void __launch_bounds__(256) kg_pack_kernel(const __grid_constant__ KernelSpec spec,
+                                                      const __grid_constant__ Centre ctr, int N, int U, int ps,
                                                       int num_pts, int DIMP, int QP, int stride,
                                                       const double* __restrict__ Xt, const double* __restrict__ beta,
                                                       const double* __restrict__ B, const double* __restrict__ P,
@@ -91,7 +101,7 @@ __global__ void __launch_bounds__(256) kg_pack_kernel(const __grid_constant__ Ke
   for (int u = tid; u < U; u += blockDim.x) {
     double nrm = 0.0;
     for (int d = 0; d < DIMP; ++d) {
-      const double v = (d < dim) ? Pc[u * dim + d] * spec.inv_len[d] : 0.0;
+      const double v = (d < dim) ? (Pc[u * dim + d] - ctr.c[d]) * spec.inv_len[d] : 0.0;
       xu[u * (DIMP + 2) + d] = v;
       nrm = fma(v, v, nrm);
     }
@@ -114,7 +124,7 @@ __global__ void __launch_bounds__(256) kg_pack_kernel(const __grid_constant__ Ke
     } else if (d < dim) {
       v = 1.0;
     }
-    Ac[e] = v;
+    Ac[e] = (d < dim) ? v - ctr.c[d] : 0.0;
     if (j < U && d < dim) Af[j * dim + d] = v;
   }
 }
@@ -350,6 +360,21 @@ __global__ void __launch_bounds__(256) kg_prep_kernel(int Q, int M, int QP, int 
   for (int a = 0; a < QP; ++a) out[a] = (a < Q) ? z[a] : 0.0;
 }
 
+// Inner max_num_restarts = 0: the MC kernel leaves every sample's minimiser at the reference's fill value, 1.0 in each
+// coordinate, but writes it without the centre; put that point in the operands' frame.
+__global__ void kg_fill_point_kernel(const __grid_constant__ KernelSpec spec, const __grid_constant__ Centre ctr,
+                                     int samples, int DIMP, double* __restrict__ outX, double* __restrict__ outH) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= samples) return;
+  double nx = 0.0;
+  for (int d = 0; d < DIMP; ++d) {
+    const double x = (d < spec.dim) ? (1.0 - ctr.c[d]) * spec.inv_len[d] : 0.0;
+    outX[static_cast<size_t>(i) * DIMP + d] = x;
+    nx = fma(x, x, nx);
+  }
+  outH[i] = -0.5 * nx;
+}
+
 // KG[c] = best_posterior + mean_i best_function_value_i ; fixed-order reduction
 __global__ void __launch_bounds__(256) kg_value_kernel(int num_mc, const double* __restrict__ outVal,
                                                        const double* __restrict__ best_post,
@@ -387,7 +412,9 @@ __global__ void __launch_bounds__(256) kg_tprime_kernel(int n, int Q, int QP, co
 // kG1Split threads over the samples i = t, t + kG1Split, ... and the partial sums are combined in a fixed order, so the
 // result does not depend on scheduling.
 constexpr int kG1Split = 16;
-__global__ void __launch_bounds__(256) kg_g1_kernel(const __grid_constant__ KernelSpec spec, int U, int q, int QP,
+// P is raw, outX centred and scaled: x*_i is moved back to raw coordinates before the difference.
+__global__ void __launch_bounds__(256) kg_g1_kernel(const __grid_constant__ KernelSpec spec,
+                                                    const __grid_constant__ Centre ctr, int U, int q, int QP,
                                                     int DIMP, int num_mc, const double* __restrict__ P,
                                                     const double* __restrict__ recC, const double* __restrict__ outX,
                                                     double* __restrict__ G1) {
@@ -406,7 +433,7 @@ __global__ void __launch_bounds__(256) kg_g1_kernel(const __grid_constant__ Kern
       const double* pp = P + (static_cast<size_t>(cand) * U + p) * dim;
       for (int i = t; i < num_mc; i += kG1Split) {
         double xi[CMOE_MAX_DIM];
-        for (int e = 0; e < dim; ++e) xi[e] = xs[static_cast<size_t>(i) * DIMP + e] * len[e];
+        for (int e = 0; e < dim; ++e) xi[e] = fma(xs[static_cast<size_t>(i) * DIMP + e], len[e], ctr.c[e]);
         const KParts kp = kernel_parts(spec, weighted_sqdist(spec, pp, xi));
         const double* ci = cs + static_cast<size_t>(i) * QP;
         for (int m = 0; m < bs; ++m)
@@ -567,6 +594,16 @@ struct cmoe_kg_plan {
 
 namespace {
 
+// |(x - centre) / l|: a point's distance from the origin of the MC kernels' frame, in length scales
+double centred_radius(const cmoe_gp& gp, const double* x, int nd) {
+  double r2 = 0.0;
+  for (int d = 0; d < nd; ++d) {
+    const double v = (x[d] - gp.centre[d]) * gp.spec.inv_len[d];
+    r2 += v * v;
+  }
+  return std::sqrt(r2);
+}
+
 void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
   const cmoe_gp& gp = *pl.gp;
   const KernelSpec& spec = gp.spec;
@@ -574,6 +611,7 @@ void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
   const int N = gp.N, n = gp.n, dim = spec.dim, U = pl.U, q = pl.q, p = pl.p, M = pl.M, QP = pl.QP, DIMP = pl.DIMP;
   const int mc = pl.num_mc, Q = pl.Q;
   const bool gen = spec.g > 0;
+  const Centre ctr = centre_of(gp);
   PosteriorBatch& pb = pl.pb;
   pb.configure(gp, nb, U, spec.derivs, spec.g, pl.want_grad ? q : 0, s);
   {
@@ -585,7 +623,7 @@ void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
   pb.run(gp, /*diag_mode=*/2, /*want_chol=*/true, pl.want_grad, s);
   CMOE_CUDA(cudaMemcpyAsync(pl.dFailAll.p + c0, pb.fail.p, nb * sizeof(int), cudaMemcpyDeviceToDevice, s));
 
-  kg_pack_kernel<<<nb, 256, 0, s>>>(spec, N, U, pl.ps, pl.num_pts, DIMP, QP, pl.stride, pl.dXt.p, gp.dKinvY.p, pb.B.p, pb.P.p,
+  kg_pack_kernel<<<nb, 256, 0, s>>>(spec, ctr, N, U, pl.ps, pl.num_pts, DIMP, QP, pl.stride, pl.dXt.p, gp.dKinvY.p, pb.B.p, pb.P.p,
                                     pl.dD.p, pl.dPk.p, pl.dXu.p, pl.dA.p, pl.dAfull.p,
                                     pl.dStale.count ? pl.dStale.p : nullptr, q, gen ? pl.dWt.p : nullptr);
   count_launch();
@@ -636,6 +674,10 @@ void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
   pl.path.mc(prm, chunks, nb, s);
   cudaEventRecord(pl.mc_events[ev_idx].second, s);
   count_launch();
+  if (pl.inner.max_num_restarts <= 0) {
+    kg_fill_point_kernel<<<(nb * mc + 255) / 256, 256, 0, s>>>(spec, ctr, nb * mc, DIMP, pl.dOutX.p, pl.dOutH.p);
+    count_launch();
+  }
   kg_value_kernel<<<nb, 256, 0, s>>>(mc, pl.dOutVal.p, pl.dBestPost.p, pb.fail.p, pl.dKG.p + c0);
   count_launch();
 
@@ -661,7 +703,7 @@ void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
     CMOE_CUDA(cudaMemsetAsync(pl.dR.p, 0, static_cast<size_t>(nb) * QP * (n + Q) * sizeof(double), s));
     pl.path.acc(ap, nb, s);
     if (gen) {
-      kg_g1_kernel<<<nb, 256, 0, s>>>(spec, U, q, QP, DIMP, mc, pb.P.p, pl.dRecC.p, pl.dOutX.p, pl.dG1.p);
+      kg_g1_kernel<<<nb, 256, 0, s>>>(spec, ctr, U, q, QP, DIMP, mc, pb.P.p, pl.dRecC.p, pl.dOutX.p, pl.dG1.p);
       count_launch();
     }
     kg_tprime_kernel<<<nb, 256, 0, s>>>(n, Q, QP, pl.dR.p, pb.B.p, pl.dTp.p);
@@ -739,7 +781,8 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
 
     // static data: scaled training points, discrete set (full dim, fidelity coords = 1), K(X, D), mu_n(D)
     pl->dXt.alloc(static_cast<size_t>(N) * DIMP);
-    pack_xt_kernel<<<(N * DIMP + 255) / 256, 256, 0, s>>>(spec, gp->dX.p, N, DIMP, pl->dXt.p);
+    const Centre ctr = centre_of(*gp);
+    pack_xt_kernel<<<(N * DIMP + 255) / 256, 256, 0, s>>>(spec, ctr, gp->dX.p, N, DIMP, pl->dXt.p);
     std::vector<double> hD(static_cast<size_t>(std::max(1, num_pts)) * dim, 1.0);
     for (int j = 0; j < num_pts; ++j)
       for (int d = 0; d < ps; ++d) hD[static_cast<size_t>(j) * dim + d] = discrete_pts[static_cast<size_t>(j) * ps + d];
@@ -767,24 +810,23 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     {
       // The shared-memory fast path evaluates exp without per-call range guards; that is valid while every scaled
-      // coordinate vector it can meet lies within kFastPathRadius length scales of the origin (kg_mc.cuh).
+      // coordinate vector it can meet lies within kFastPathRadius length scales of the origin of the kernels' frame,
+      // the GP's centre (kg_mc.cuh).
       auto upd = [&](const double* pts, size_t count, int stride, int nd) {
-        for (size_t i = 0; i < count; ++i) {
-          double r2 = 0.0;
-          for (int d = 0; d < nd; ++d) {
-            const double v = pts[i * stride + d] * spec.inv_len[d];
-            r2 += v * v;
-          }
-          pl->rmax_static = std::max(pl->rmax_static, std::sqrt(r2));
-        }
+        for (size_t i = 0; i < count; ++i)
+          pl->rmax_static = std::max(pl->rmax_static, centred_radius(*gp, pts + i * stride, nd));
       };
       upd(gp->hX.data(), N, dim, dim);
       upd(hD.data(), num_pts, dim, dim);
       if (p) upd(hXp.data(), p, dim, dim);
-      for (int d = 0; d < ps; ++d) {  // the inner optimiser keeps its iterates inside the inner domain
-        const double c = std::max(std::fabs(inner_bounds[2 * d]), std::fabs(inner_bounds[2 * d + 1])) * spec.inv_len[d];
-        pl->rmax_static = std::max(pl->rmax_static, c * std::sqrt(static_cast<double>(dim)));
+      // the inner optimiser keeps its iterates inside the inner domain; their fidelity coordinates stay at 1.0
+      double r2 = 0.0;
+      for (int d = 0; d < dim; ++d) {
+        const double lo = d < ps ? inner_bounds[2 * d] : 1.0, hi = d < ps ? inner_bounds[2 * d + 1] : 1.0;
+        const double c = std::max(std::fabs(lo - gp->centre[d]), std::fabs(hi - gp->centre[d])) * spec.inv_len[d];
+        r2 += c * c;
       }
+      pl->rmax_static = std::max(pl->rmax_static, std::sqrt(r2));
     }
     pl->path = pl->select(N, U, spec.g, pl->rmax_static < kFastPathRadius);
     // candidates per batch bounded by ~3 GiB of per-sample records and start-point tables, and by grid.y of the
@@ -883,9 +925,9 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
       m.inv_len[d] = (d < dim) ? spec.inv_len[d] : 0.0;
       m.len[d] = (d < dim) ? 1.0 / spec.inv_len[d] : 0.0;
     }
-    for (int d = 0; d < ps; ++d) {
-      m.lo[d] = inner_bounds[2 * d];
-      m.hi[d] = inner_bounds[2 * d + 1];
+    for (int d = 0; d < ps; ++d) {  // the frame of A (kg_pack_kernel)
+      m.lo[d] = inner_bounds[2 * d] - gp->centre[d];
+      m.hi[d] = inner_bounds[2 * d + 1] - gp->centre[d];
     }
     *plan_out = pl.release();
   });
@@ -931,14 +973,8 @@ int cmoe_kg_plan_upload(cmoe_kg_plan* plan, const double* candidates, int num_ca
       const KernelSpec& spec = plan->gp->spec;
       double rmax = plan->rmax_static;
       const size_t pts = static_cast<size_t>(num_candidates) * plan->q;
-      for (size_t i = 0; i < pts && rmax < kFastPathRadius; ++i) {
-        double r2 = 0.0;
-        for (int d = 0; d < spec.dim; ++d) {
-          const double v = candidates[i * spec.dim + d] * spec.inv_len[d];
-          r2 += v * v;
-        }
-        rmax = std::max(rmax, std::sqrt(r2));
-      }
+      for (size_t i = 0; i < pts && rmax < kFastPathRadius; ++i)
+        rmax = std::max(rmax, centred_radius(*plan->gp, candidates + i * spec.dim, spec.dim));
       // NaN-safe: a NaN norm fails the comparison
       plan->path = plan->select(plan->gp->N, plan->U, spec.g, rmax < kFastPathRadius);
       plan->mcp.use_smem = plan->path.use_smem ? 1 : 0;

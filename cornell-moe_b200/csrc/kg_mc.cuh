@@ -31,10 +31,13 @@
 namespace cmoe {
 
 // Range contract of the shared-memory fast path.  Its exp (exp_tab, no per-call guard) needs |t| < 2^31 ln2 / 64 =
-// 2.3e7, t = -|x~ - X~_j|^2 / 2 + ln(alpha).  The host only selects the fast path while every scaled operand (training,
-// union, discrete points, inner-domain corners) lies within kFastPathRadius of the origin; a query point farther than
-// kFarRadius is then at least kFarRadius - kFastPathRadius = 2000 length scales from every operand, so all its kernel
-// values are exactly 0 and the evaluation is short-circuited; any other query point has |t| <= 6000^2 / 2 = 1.8e7.
+// 2.3e7, t = -|x~ - X~_j|^2 / 2 + ln(alpha).  All operands of these kernels (training, union, start points, inner
+// bounds, minimisers) share the centred frame of the GP's covariance build, x~ = (x - centre) / l (kg.cu), because the
+// expanded form x~.X~ - |x~|^2/2 - |X~|^2/2 loses ~eps |x~|^2 absolute; the radii below are measured in that frame.  The
+// host only selects the fast path while every scaled operand (training, union, discrete points, inner-domain corners)
+// lies within kFastPathRadius of the origin; a query point farther than kFarRadius is then at least kFarRadius -
+// kFastPathRadius = 2000 length scales from every operand, so all its kernel values are exactly 0 and the evaluation is
+// short-circuited; any other query point has |t| <= 6000^2 / 2 = 1.8e7.
 #ifndef CMOE_MC_THREADS
 #define CMOE_MC_THREADS 128
 #endif
@@ -65,7 +68,7 @@ struct KgMcParams {
   const double* Xt;      // [N][DIM] scaled training points (zero padded)
   const double* Pk;      // [nc][N][QP+2]  (e_j, beta_j, B_j[0..QP))
   const double* Xu;      // [nc][U][DIM+2] (scaled union point, e_u, pad)
-  const double* A;       // [nc][M][DIM]   unscaled start points (fidelity coords = 1, padding = 0)
+  const double* A;       // [nc][M][DIM]   unscaled start points minus the centre (fidelity coords = 1, padding = 0)
   const double* recC;    // [nc][num_mc][QP]
   const int* recStart;   // [nc][num_mc]
   const double* Start;   // g == 0: [nc][M][1+QP][DIM+2] start-point table (kg_start_kernel)
@@ -82,7 +85,7 @@ struct KgMcParams {
   int chunks;        // work items per candidate
   int work_total;    // chunks * candidates of this launch
   int stage_ops;     // general path: scaled training points and e_j fit next to the ring in shared memory
-  double lo[CMOE_MAX_DIM], hi[CMOE_MAX_DIM], inv_len[CMOE_MAX_DIM], len[CMOE_MAX_DIM];
+  double lo[CMOE_MAX_DIM], hi[CMOE_MAX_DIM], inv_len[CMOE_MAX_DIM], len[CMOE_MAX_DIM];  // lo, hi: minus the centre
 };
 
 struct KgAccParams {
