@@ -73,6 +73,14 @@ class RffTable(ctypes.Structure):
     _fields_ = [("omega", _dp), ("b", _dp), ("z", _dp), ("eps", _dp)]
 
 
+RFF_SPECTRAL_REFERENCE, RFF_SPECTRAL_KERNEL = 0, 1
+
+
+class RffOpts(ctypes.Structure):
+    """cmoe_rff_opts: the frequencies' distribution (RFF_SPECTRAL_*) and the chi^2_5 table of the Matern draw."""
+    _fields_ = [("spectral", ctypes.c_int), ("chi2", _dp)]
+
+
 _lib = None
 
 
@@ -152,6 +160,34 @@ def philox_normals(seed, first_draw, num_draws, per_draw, device=0):
     return out.reshape(num_draws, per_draw)
 
 
+def _rff_args(dim, n, F, P, table, spectral):
+    """(table struct or None, opts struct or None, keep-alive list) of the random-feature calls on a GP of dimension
+    dim with n = num_sampled (1 + g) rows."""
+    tab, opts, keep = None, None, []
+    if table is not None:
+        M = n
+        need = {"omega": P * F * dim, "b": P * F, "z": P * F, "eps": P * M if M < F else None}
+        tab = RffTable()
+        for name in ("omega", "b", "z", "eps"):
+            a = table.get(name)
+            if a is not None:
+                a = _f64(a).ravel()
+                keep.append(a)
+            if need[name] is not None and (a is None or a.size != need[name]):
+                got = "none" if a is None else a.size
+                raise BoundsError(ERR_BOUNDS, f"table[{name!r}] needs {need[name]} values, got {got}")
+            setattr(tab, name, _d(a))
+    chi2 = None if table is None else table.get("chi2")
+    if chi2 is not None:
+        chi2 = _f64(chi2).ravel()
+        if chi2.size != P * F:
+            raise BoundsError(ERR_BOUNDS, f"table['chi2'] needs {P * F} values, got {chi2.size}")
+        keep.append(chi2)
+    if spectral != RFF_SPECTRAL_REFERENCE or chi2 is not None:
+        opts = RffOpts(int(spectral), _d(chi2))
+    return tab, opts, keep
+
+
 class GaussianProcess:
     """Device-resident GP (reference: optimal_learning::GaussianProcess, gpp_math.hpp:275)."""
 
@@ -166,6 +202,7 @@ class GaussianProcess:
         lengths = _f64(lengths).ravel()
         assert y.size == self.n and noise.size == 1 + self.g and lengths.size == self.dim
         self.kernel = kernel
+        self.alpha = float(alpha)
         self.device = device
         h = ctypes.c_void_p()
         info = ctypes.c_int(0)
@@ -323,44 +360,53 @@ class GaussianProcess:
         return out
 
     def sample_rff_optima(self, num_features, num_points, domain_bounds, grid, seed=0, first_draw=0, table=None,
-                          return_functions=False):
-        """cmoe_gp_sample_rff_optima: minimisers of num_points random-Fourier-feature draws of the GP, each found on
+                          return_functions=False, spectral=RFF_SPECTRAL_REFERENCE):
+        """cmoe_gp_sample_rff_optima_ex: minimisers of num_points random-Fourier-feature draws of the GP, each found on
         ``grid`` [G, dim] and refined inside ``domain_bounds`` ([dim, 2] or flat).  Sample s uses Philox draw
         first_draw + s, or row s of ``table`` (a dict with omega [P, F, dim], b [P, F], z [P, F] and, when
-        num_sampled (1 + g) < F, eps [P, num_sampled (1 + g)]).  Returns (points [P, dim], values [P]); with
-        return_functions, also a dict of each sample function f(x) = sqrt(2 alpha / F) theta . cos(omega x + b):
-        omega [P, F, dim] (the frequencies, Omega / lengths), b [P, F], theta [P, F]."""
+        num_sampled (1 + g) < F, eps [P, num_sampled (1 + g)]; with the Matern draw also chi2 [P, F]).  ``spectral``:
+        RFF_SPECTRAL_REFERENCE (SquareExponential frequencies whatever the kernel, as the reference) or
+        RFF_SPECTRAL_KERNEL (the GP's own kernel).  Returns (points [P, dim], values [P]); with return_functions, also
+        a dict of each sample function f(x) = sqrt(2 alpha / F) theta . cos(omega x + b): omega [P, F, dim] (the
+        frequencies), b [P, F], theta [P, F]."""
         F, P = int(num_features), int(num_points)
         bounds = _f64(domain_bounds).ravel()
         if bounds.size != 2 * self.dim:
             raise BoundsError(ERR_BOUNDS, f"domain_bounds needs 2*dim = {2 * self.dim} values, got {bounds.size}")
         grid = _f64(grid).reshape(-1, self.dim)
-        tab = None
-        keep = []
-        if table is not None:
-            M = self.n
-            need = {"omega": P * F * self.dim, "b": P * F, "z": P * F, "eps": P * M if M < F else None}
-            tab = RffTable()
-            for name in ("omega", "b", "z", "eps"):
-                a = table.get(name)
-                if a is not None:
-                    a = _f64(a).ravel()
-                    keep.append(a)
-                if need[name] is not None and (a is None or a.size != need[name]):
-                    got = "none" if a is None else a.size
-                    raise BoundsError(ERR_BOUNDS, f"table[{name!r}] needs {need[name]} values, got {got}")
-                setattr(tab, name, _d(a))
+        tab, opts, keep = _rff_args(self.dim, self.n, F, P, table, spectral)
         pts = np.empty((max(P, 0), self.dim))
         vals = np.empty(max(P, 0))
         fun = ({"omega": np.empty((P, F, self.dim)), "b": np.empty((P, F)), "theta": np.empty((P, F))}
                if return_functions and P >= 1 and F >= 1 else None)
         info = ctypes.c_int(0)
-        rc = lib().cmoe_gp_sample_rff_optima(self.h, F, P, _d(bounds), _d(grid), grid.shape[0], ctypes.c_uint64(seed),
-                                             ctypes.c_uint64(first_draw), None if tab is None else ctypes.byref(tab),
-                                             _d(pts), _d(vals), _d(fun and fun["omega"]), _d(fun and fun["b"]),
-                                             _d(fun and fun["theta"]), ctypes.byref(info))
+        rc = lib().cmoe_gp_sample_rff_optima_ex(self.h, F, P, _d(bounds), _d(grid), grid.shape[0],
+                                                ctypes.c_uint64(seed), ctypes.c_uint64(first_draw),
+                                                None if tab is None else ctypes.byref(tab),
+                                                None if opts is None else ctypes.byref(opts), _d(pts), _d(vals),
+                                                _d(fun and fun["omega"]), _d(fun and fun["b"]),
+                                                _d(fun and fun["theta"]), ctypes.byref(info))
+        del keep
         _check(rc, info.value)
         return (pts, vals, fun) if return_functions else (pts, vals)
+
+    def sample_rff_functions(self, num_features, num_points, seed=0, first_draw=0, table=None,
+                             spectral=RFF_SPECTRAL_REFERENCE):
+        """cmoe_gp_sample_rff_functions (sample_gp_with_random_features): the sample functions of num_points draws,
+        without the grid and the optimiser; arguments as sample_rff_optima.  Returns an RffFunctions whose omega, b and
+        theta are those sample_rff_optima returns for the same arguments, bit for bit."""
+        F, P = int(num_features), int(num_points)
+        tab, opts, keep = _rff_args(self.dim, self.n, F, P, table, spectral)
+        omega, b, theta = np.empty((max(P, 0), max(F, 0), self.dim)), np.empty((max(P, 0), max(F, 0))), \
+            np.empty((max(P, 0), max(F, 0)))
+        info = ctypes.c_int(0)
+        rc = lib().cmoe_gp_sample_rff_functions(self.h, F, P, ctypes.c_uint64(seed), ctypes.c_uint64(first_draw),
+                                                None if tab is None else ctypes.byref(tab),
+                                                None if opts is None else ctypes.byref(opts), _d(omega), _d(b),
+                                                _d(theta), ctypes.byref(info))
+        del keep
+        _check(rc, info.value)
+        return RffFunctions(omega, b, theta, float(np.sqrt(2.0 * self.alpha / F)), self.device)
 
     def lower_confidence_bound(self, candidates, num_to_sample):
         """cmoe_lcb_select: the reference's LCB batch selection over ``candidates`` [C, dim].  Returns (indices [q] into
@@ -374,6 +420,53 @@ class GaussianProcess:
                                    None, ctypes.byref(info))
         _check(rc, info.value)
         return idx, mean, sd
+
+
+class RffFunctions:
+    """P random-Fourier-feature sample functions f_p(x) = c sum_f theta[p, f] cos(omega[p, f] . x + b[p, f]):
+    omega [P, F, dim], b [P, F], theta [P, F], c = sqrt(2 alpha / F).  Calling it evaluates them on the device
+    (cmoe_rff_evaluate)."""
+
+    def __init__(self, omega, b, theta, c, device=0):
+        self.omega, self.b, self.theta, self.c, self.device = omega, b, theta, float(c), device
+
+    def __len__(self):
+        return self.theta.shape[0]
+
+    def __call__(self, x, gradient=False):
+        """x: [dim] or [X, dim] (shared by the functions) or [P, X, dim] (per function).  Returns values [P, X]; with
+        gradient, (values [P, X], grads [P, X, dim])."""
+        return rff_evaluate(self.omega, self.b, self.theta, self.c, x, grads=gradient, device=self.device)
+
+
+def rff_evaluate(omega, b, theta, c, points, values=True, grads=False, device=0):
+    """cmoe_rff_evaluate: values [P, X] and/or grads [P, X, dim] of the sample functions (omega [P, F, dim], b [P, F],
+    theta [P, F], c) at points [X, dim] (shared; [dim] is one point) or [P, X, dim] (per function).  Returns values,
+    grads or (values, grads)."""
+    omega = _f64(omega)
+    P, F, dim = omega.shape
+    b, theta = _f64(b).reshape(P, F), _f64(theta).reshape(P, F)
+    pts = _f64(points)
+    per_function = pts.ndim == 3
+    pts = pts.reshape((P, -1, dim) if per_function else (-1, dim))
+    X = pts.shape[-2]
+    v = np.empty((P, X)) if values else None
+    g = np.empty((P, X, dim)) if grads else None
+    info = ctypes.c_int(0)
+    _check(lib().cmoe_rff_evaluate(int(dim), int(F), int(P), _d(omega), _d(b), _d(theta), ctypes.c_double(c), _d(pts),
+                                   int(X), int(per_function), _d(v), _d(g), int(device), ctypes.byref(info)),
+           info.value)
+    if values and grads:
+        return v, g
+    return v if values else g
+
+
+def rff_chi2_draws(seed, first_draw, num_draws, num_features, device=0):
+    """cmoe_rff_chi2_draws: the chi^2_5 numbers g [num_draws, num_features] of the Matern random-feature draw."""
+    out = np.empty((int(num_draws), int(num_features)))
+    _check(lib().cmoe_rff_chi2_draws(ctypes.c_uint64(seed), ctypes.c_uint64(first_draw), int(num_draws),
+                                     int(num_features), _d(out), int(device)))
+    return out
 
 
 def latin_hypercube(num_sets, num_pts, domain_bounds, seed=0, first_draw=0, device=0):

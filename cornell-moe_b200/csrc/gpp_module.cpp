@@ -28,6 +28,7 @@
 //   * normals come from Philox4x32-10 keyed by the RandomnessSourceContainer's seed (not boost mt19937);
 //   * `max_num_threads` is accepted and validated against the container but the parallel axis is the GPU;
 //   * `use_gpu` / `which_gpu` (dead arguments in the reference) select the device.
+#include <pybind11/numpy.h>
 #include <pybind11/pybind11.h>
 #include <pybind11/stl.h>
 
@@ -88,6 +89,21 @@ py::list to_list(const std::vector<double>& v) {
   for (double x : v) out.append(x);
   return out;
 }
+
+// One random-feature sample function of sample_gp_with_random_features, callable as the reference's wrapper(x, gradient):
+// x is one point [dim] or points [X][dim] (a numpy array); gradient = False returns f at the points (a float for one
+// point), gradient = True only the gradient ([dim] for one point, else [X][dim]), as random_features.py:113-131.
+struct RandomFeatureSample {
+  int dim = 0, F = 0, device = 0;
+  double c = 0.0;
+  std::vector<double> omega, b, theta;
+  py::array_t<double> array(const std::vector<double>& v, std::vector<py::ssize_t> shape) const {
+    py::array_t<double> a(shape);
+    std::copy(v.begin(), v.end(), a.mutable_data());
+    return a;
+  }
+  py::object call(const py::object& x, bool gradient) const;
+};
 
 // ---- parameter structs (gpp_optimizer_parameters.hpp:46-200) -------------------------------------------------------
 struct GradientDescentParameters {
@@ -158,11 +174,13 @@ void require_threads(int max_num_threads, const RandomnessSourceContainer& r) {
 struct GaussianProcess {
   cmoe_gp* h = nullptr;
   int dim_ = 0, num_derivatives_ = 0;
+  double alpha_ = 0.0;  // the kernel amplitude sigma^2 (the random features' c = sqrt(2 alpha / F))
   std::vector<int> derivatives_;
   GaussianProcess(const py::list& hyperparameters, const py::list& points_sampled, const py::list& points_sampled_value,
                   const py::list& noise_variance, const py::list& derivatives, int num_derivatives, int dim,
                   int num_sampled, const std::string& kernel, int which_gpu) {
     const double alpha = hyperparameters[0].cast<double>();
+    alpha_ = alpha;
     const std::vector<double> lengths = to_vec(hyperparameters[1].cast<py::list>(), dim);
     const std::vector<double> X = to_vec(points_sampled, static_cast<size_t>(dim) * num_sampled);
     const std::vector<double> y = to_vec(points_sampled_value, static_cast<size_t>(num_sampled) * (1 + num_derivatives));
@@ -270,6 +288,30 @@ struct GaussianProcess {
 
 cmoe_gd_params gd_of(const py::object& optimizer_parameters) {
   return optimizer_parameters.attr("optimizer_parameters").cast<const GradientDescentParameters&>().p;
+}
+
+// a GaussianProcess, or a wrapper holding one as `_gaussian_process` (the reference's python_version objects)
+GaussianProcess& unwrap_gp(const py::object& gaussian_process) {
+  py::object o = gaussian_process;
+  if (!py::isinstance<GaussianProcess>(o) && py::hasattr(o, "_gaussian_process")) o = o.attr("_gaussian_process");
+  return o.cast<GaussianProcess&>();
+}
+
+py::object RandomFeatureSample::call(const py::object& x, bool gradient) const {
+  const auto xa = py::array_t<double, py::array::c_style | py::array::forcecast>::ensure(x);
+  if (!xa || (xa.ndim() != 1 && xa.ndim() != 2) || xa.shape(xa.ndim() - 1) != dim) {
+    PyErr_SetString(g_exc_bounds, "x must be a point [dim] or points [num_points][dim]");
+    throw py::error_already_set();
+  }
+  const int X = xa.ndim() == 1 ? 1 : static_cast<int>(xa.shape(0));
+  std::vector<double> out(static_cast<size_t>(std::max(X, 0)) * (gradient ? dim : 1));
+  int info = 0;
+  check(cmoe_rff_evaluate(dim, F, 1, omega.data(), b.data(), theta.data(), c, xa.data(), X, 0,
+                          gradient ? nullptr : out.data(), gradient ? out.data() : nullptr, device, &info),
+        info);
+  if (gradient) return xa.ndim() == 1 ? array(out, {dim}) : array(out, {X, dim});
+  if (X == 1) return py::float_(out[0]);
+  return array(out, {X});
 }
 
 std::vector<double> full_bounds(const py::list& domain_bounds, int dim) { return to_vec(domain_bounds, 2 * static_cast<size_t>(dim)); }
@@ -1396,6 +1438,59 @@ PYBIND11_MODULE(GPP, m) {
         },
         py::arg("gaussian_process"), py::arg("num_features"), py::arg("domain_bounds"), py::arg("grid"),
         py::arg("num_grid"), py::arg("num_points"));
+  // sample_from_global_optima_kernel_matched: as sample_from_global_optima, with frequencies drawn from the GP's own
+  // kernel (CMOE_RFF_SPECTRAL_KERNEL: the Student-t mixture for Matern-5/2; a SquareExponential GP gives the same
+  // points as sample_from_global_optima).
+  m.def("sample_from_global_optima_kernel_matched",
+        [](const py::object& gaussian_process, int num_features, const py::list& domain_bounds, const py::list& grid,
+           int num_grid, int num_points) -> py::list {
+          GaussianProcess& gp = unwrap_gp(gaussian_process);
+          const int dim = gp.dim();
+          const auto B = to_vec(domain_bounds, 2 * static_cast<size_t>(dim));
+          const auto Gr = to_vec(grid, static_cast<size_t>(std::max(num_grid, 0)) * dim);
+          std::vector<double> out(static_cast<size_t>(std::max(num_points, 0)) * dim), vals(std::max(num_points, 0));
+          const cmoe_rff_opts opts{CMOE_RFF_SPECTRAL_KERNEL, nullptr};
+          int info = 0;
+          check(cmoe_gp_sample_rff_optima_ex(gp.h, num_features, num_points, B.data(), Gr.data(), num_grid, gp.seed_,
+                                             gp.next_draw_, nullptr, &opts, out.data(), vals.data(), nullptr, nullptr,
+                                             nullptr, &info),
+                info);
+          gp.next_draw_ += static_cast<uint64_t>(num_points);
+          return to_list(out);
+        },
+        py::arg("gaussian_process"), py::arg("num_features"), py::arg("domain_bounds"), py::arg("grid"),
+        py::arg("num_grid"), py::arg("num_points"));
+  // sample_gp_with_random_features(gaussian_process, num_features, kernel_matched=False)
+  // random_features.sample_gp_with_random_features (random_features.py:29-133) through cmoe_gp_sample_rff_functions:
+  // one draw of the GP's (seed, next draw).  Returns a RandomFeatureSample, callable as the reference's
+  // wrapper(x, gradient) and evaluated on the device (cmoe_rff_evaluate).
+  py::class_<RandomFeatureSample>(m, "RandomFeatureSample")
+      .def("__call__", &RandomFeatureSample::call, py::arg("x"), py::arg("gradient") = false)
+      .def_property_readonly("omega", [](const RandomFeatureSample& s) { return s.array(s.omega, {s.F, s.dim}); })
+      .def_property_readonly("b", [](const RandomFeatureSample& s) { return s.array(s.b, {s.F}); })
+      .def_property_readonly("theta", [](const RandomFeatureSample& s) { return s.array(s.theta, {s.F}); })
+      .def_readonly("c", &RandomFeatureSample::c);
+  m.def("sample_gp_with_random_features",
+        [](const py::object& gaussian_process, int num_features, bool kernel_matched) {
+          GaussianProcess& gp = unwrap_gp(gaussian_process);
+          RandomFeatureSample r;
+          r.dim = gp.dim();
+          r.F = num_features;
+          r.device = cmoe_gp_device(gp.h);
+          const size_t F = static_cast<size_t>(std::max(num_features, 0));
+          r.omega.resize(F * r.dim);
+          r.b.resize(F);
+          r.theta.resize(F);
+          const cmoe_rff_opts opts{kernel_matched ? CMOE_RFF_SPECTRAL_KERNEL : CMOE_RFF_SPECTRAL_REFERENCE, nullptr};
+          int info = 0;
+          check(cmoe_gp_sample_rff_functions(gp.h, num_features, 1, gp.seed_, gp.next_draw_, nullptr, &opts,
+                                             r.omega.data(), r.b.data(), r.theta.data(), &info),
+                info);
+          gp.next_draw_ += 1;
+          r.c = std::sqrt(2.0 * gp.alpha_ / num_features);
+          return r;
+        },
+        py::arg("gaussian_process"), py::arg("num_features"), py::arg("kernel_matched") = false);
   m.def("heuristic_expected_improvement_optimization",
         [](const py::args&, const py::kwargs&) -> py::object {
           not_on_path("heuristic_expected_improvement_optimization");

@@ -279,6 +279,62 @@ int cmoe_gp_sample_rff_optima(const cmoe_gp* gp, int num_features, int num_point
                               const cmoe_rff_table* table, double* points, double* values, double* omega, double* b,
                               double* theta, int* info);
 
+/* ---- kernel-matched random features, the sample functions alone, and their evaluation -----------------------------
+ * opts->spectral selects the frequencies' distribution:
+ *   CMOE_RFF_SPECTRAL_REFERENCE (the default, and opts == NULL): W = Omega / l whatever the kernel, the reference's draw;
+ *   CMOE_RFF_SPECTRAL_KERNEL: the handle's own kernel.  For Matern-5/2, k = alpha (1 + sqrt5 r + 5 r^2 / 3) e^(-sqrt5 r)
+ *     with r = ||(x - x') / l||, whose spectral measure is a multivariate Student-t with 5 degrees of freedom:
+ *     W_f = (Omega_f / l) sqrt(5 / g_f), g_f ~ chi^2_5, computed as __dmul_rn(Omega / l, sqrt(5 / g)) (each operation
+ *     rounded once).  g_f = -2 ln u0 - 2 ln u1 + (-2 ln u2) cos^2(2 pi v2), the sum of squares of five Box-Muller normals
+ *     (a pair's squares sum to -2 ln u), from the Philox calls (draw, 2f) -> (u0, u1) and (draw, 2f + 1) -> (u2, v2)
+ *     with counter word 3 = 3 (53-bit uniforms as for b).  Omega, b, z and eps are the reference mode's numbers, so a
+ *     matched sample differs from the reference-mode sample of the same (seed, draw) only by the per-row factor.  For a
+ *     SquareExponential handle the matched draw is the reference draw.
+ * opts->chi2[P][F] replaces g in table mode; it is read only when a table is given and the draw is the Matern one, and
+ * then each entry must be finite and > 0.  The design matrix, both posterior branches, the grid stage and the local
+ * optimiser are those of cmoe_gp_sample_rff_optima. */
+#define CMOE_RFF_SPECTRAL_REFERENCE 0
+#define CMOE_RFF_SPECTRAL_KERNEL 1
+typedef struct cmoe_rff_opts {
+  int spectral;        /* CMOE_RFF_SPECTRAL_* */
+  const double* chi2;  /* [P][F], table mode with the Matern draw only */
+} cmoe_rff_opts;
+
+/* cmoe_gp_sample_rff_optima with options; opts == NULL gives cmoe_gp_sample_rff_optima's results bit for bit.  An
+ * unknown opts->spectral -> CMOE_ERR_INVALID_VALUE (after the size checks). */
+int cmoe_gp_sample_rff_optima_ex(const cmoe_gp* gp, int num_features, int num_points, const double* domain_bounds,
+                                 const double* grid, int num_grid, uint64_t seed, uint64_t first_draw,
+                                 const cmoe_rff_table* table, const cmoe_rff_opts* opts, double* points, double* values,
+                                 double* omega, double* b, double* theta, int* info);
+
+/* sample_gp_with_random_features (random_features.py:29-133): the sample functions of num_points draws without the grid
+ * and the local optimiser.  omega[P][F][d], b[P][F] and theta[P][F] (none may be NULL) are bit for bit those
+ * cmoe_gp_sample_rff_optima_ex returns for the same (gp, F, P, seed, first_draw, table, opts).  Errors as for
+ * cmoe_gp_sample_rff_optima_ex, without those of the grid and the bounds. */
+int cmoe_gp_sample_rff_functions(const cmoe_gp* gp, int num_features, int num_points, uint64_t seed,
+                                 uint64_t first_draw, const cmoe_rff_table* table, const cmoe_rff_opts* opts,
+                                 double* omega, double* b, double* theta, int* info);
+
+/* The g[num_draws][num_features] of the Matern draw for Philox draws first_draw .. first_draw + num_draws - 1, as
+ * rff_features_kernel forms them (so that a table can replay a Philox run, as cmoe_philox_normals does for the normals).
+ * num_draws <= 65535. */
+int cmoe_rff_chi2_draws(uint64_t seed, uint64_t first_draw, int num_draws, int num_features, double* out, int device);
+
+/* The sample functions' values and gradients (the reference's wrapper(x, gradient)):
+ *   values[p][j]   = c sum_f theta[p][f] cos(omega[p][f] . x_pj + b[p][f]),
+ *   grads[p][j][k] = -c sum_f theta[p][f] sin(omega[p][f] . x_pj + b[p][f]) omega[p][f][k],
+ * with c = sqrt(2 alpha / F) as the sampler uses it.  points are [num_points][dim], shared by all functions
+ * (per_function = 0), or [num_functions][num_points][dim] (per_function != 0).  values or grads may be NULL, not both.
+ * Each sum runs over the features in ascending order, one point per thread, so a result depends only on its function
+ * and its point, not on num_functions, num_points, the chunking or whether the other output is requested; the values
+ * are the sampler's grid-stage arithmetic, bit for bit.  Runs in chunks of (functions x points) that fit 2 GiB.
+ * Errors (before any device work): CMOE_ERR_BOUNDS unless dim in [1, 32], num_features, num_functions, num_points >= 1
+ * and one function's features and one point fit in 2 GiB; CMOE_ERR_INVALID_VALUE for NULL inputs, both outputs NULL,
+ * or non-finite omega, b, theta, c or points. */
+int cmoe_rff_evaluate(int dim, int num_features, int num_functions, const double* omega, const double* b,
+                      const double* theta, double c, const double* points, int num_points, int per_function,
+                      double* values, double* grads, int device, int* info);
+
 /* ---- lower-confidence-bound batch selection ----------------------------------------------------------------------
  * lower_confidence_bound_optimization (moe/optimal_learning/python/cpp_wrappers/lower_confidence_bound.py:52-80) in one
  * call.  candidates [num_candidates][dim].  mu(x) is the value mean, sigma(x) the square root of the value variance.
