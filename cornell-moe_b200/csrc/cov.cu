@@ -28,28 +28,10 @@ constexpr int WR = TR / (8 * RB);      // warps along the rows (a warp covers 8*
 constexpr int WC = 8 / WR;             // warps along the columns
 constexpr int TC = WC * 16;            // columns per pass over the staged slabs
 
-// 2^(i/64), the table of the reduced-range exp (see exp_tab in kg_mc.cuh: 10 FP64-pipe instructions instead of 15)
+// 2^(i/64), the table of the reduced-range exp exp_tab_cov (device_math.cuh)
 __device__ const double kCovExp2Table[64] = {
 #include "exp2_table64.inc"
 };
-__device__ __forceinline__ double exp_tab_cov(double t, const double* __restrict__ tab) {
-  t = exp_guard_in(t);
-  const double kShift = 6755399441055744.0;
-  double nf = fma(t, 64.0 * 1.4426950408889634, kShift);
-  const int n = __double2loint(nf);
-  nf -= kShift;
-  double r = fma(nf, -6.93147180369123816490e-01 / 64.0, t);
-  r = fma(nf, -1.90821492927058770002e-10 / 64.0, r);
-  double p = 8.3333333333333332e-03;
-  p = fma(p, r, 4.1666666666666664e-02);
-  p = fma(p, r, 1.6666666666666666e-01);
-  p = fma(p, r, 0.5);
-  p = fma(p, r, 1.0);
-  p = fma(p, r, 1.0);
-  p *= tab[n & 63];
-  const int k = max(n >> 6, -1000);
-  return __hiloint2double(__double2hiint(p) + (k << 20), __double2loint(p));
-}
 
 // g == 0 fast path: K[i + j*n] for i >= j (tile granularity), noise[0] on the diagonal.
 // Works on length-scaled coordinates Xs = X / l with the expanded distance

@@ -108,8 +108,11 @@ struct KgAccParams {
 // exp(t) = 2^k * 2^(i/64) * e^r with |r| <= ln2/128: 64-entry table in shared memory + degree-5 Taylor polynomial
 // (truncation r^6/720 <= 3.5e-17 relative).  10 FP64-pipe instructions instead of 15 for exp_fast; same integer-side
 // clamp of the exponent, NO guard for |t| >= 2.3e7 (see kFastPathRadius).  Used by the shared-memory fast path of the
-// fused q-KG kernel (+11 % throughput on the north-star shape); measured max relative error 3.0e-16 over [-690, 1]
-// (profiles/exp_accuracy.py), exp(0) = 1 exactly.
+// fused q-KG kernel (+11 % throughput on the north-star shape).  Arguments: t <= 700 down to -(2 kFastPathRadius)^2 / 2
+// and on to -2.3e7.  Max relative error 4.0e-16 over [-1000 ln2, 700], below that a result in [0, 2^-999]; exp(0) = 1
+// exactly.  An empirical bound ~20 % above the 3.30e-16 measured on the device (tests/test_gpu_fast_math.py): the table
+// entry (0.5 u, u = 2^-53), the polynomial (~1.2 u, as exp_fast's) and the product p * 2^(i/64) (0.5 u) add up to ~2.5 u,
+// the truncation r^6/720 adds 0.3 u.
 __device__ const double kExp2Table[64] = {
 #include "exp2_table64.inc"
 };
@@ -141,8 +144,8 @@ __device__ __forceinline__ double exp_tab(double t) {
 // exponent k = n >> 11 is taken from both words of the shifted double with one funnel shift (the shift's bias
 // 2^51 >> 11 = 2^40 vanishes mod 2^32); k is exact for |t| < 2^31 ln2 = 1.5e9 and clamped on the integer side like
 // exp_tab's.  Used by the tile rounds of kg_mc_kernel<SE,8,8> where its operands leave room for the table
-// (KgDispatchEntry::mc_big); measured max relative error 3.0e-16 over [-690, 1] like exp_tab
-// (profiles/exp_accuracy.py), exp(0) = 1 exactly.
+// (KgDispatchEntry::mc_big).  Arguments and error as exp_tab's: max relative error 4.0e-16 over [-1000 ln2, 700]
+// (tests/test_gpu_fast_math.py), exp(0) = 1 exactly.
 __device__ const double kExp2Table2k[2048] = {
 #include "exp2_table2048.inc"
 };
@@ -688,19 +691,6 @@ __device__ __forceinline__ void eval_line(const double* __restrict__ Xt, const d
 constexpr int kLineBatchM = CMOE_LINE_BATCH_M;
 static_assert(kLineBatchM <= kLineBatch, "S is sized for the SquareExponential batch");
 
-// sqrt(p) for a normal p > 0: MUFU.RSQ64H seed + two coupled Goldschmidt steps (seven FP64 operations, no special-case
-// branch; within ~1 ulp)
-__device__ __forceinline__ double sqrt_seeded(double p) {
-  double y0;
-  asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y0) : "d"(p));
-  double g = p * y0, h = 0.5 * y0;
-  double r = fma(-g, h, 0.5);
-  g = fma(g, r, g);
-  h = fma(h, r, h);
-  r = fma(-g, h, 0.5);
-  return fma(g, r, g);
-}
-
 template <int DIM, int QP, bool SMEM>
 __device__ __forceinline__ void eval_line_matern(const double* __restrict__ Xt, const double* __restrict__ Pk,
                                                  const double* __restrict__ Xu, int N, int U, double alpha,
@@ -732,7 +722,9 @@ __device__ __forceinline__ void eval_line_matern(const double* __restrict__ Xt, 
       // clamped away from 0 for the seed (Matern-5/2 is flat at r = 0: the value is unchanged to the last bit) and,
       // on the table-exp path, from above so that the argument stays inside the table exp's range contract
       const double r2 = fmax(1.0e-280, fma(m2a[k], pj, r2b) + aag[k]);
-      double ar = kSqrt5 * sqrt_seeded(r2);
+      double sr, rsr;  // sqrt_rsqrt (device_math.cuh); the unused 1/sqrt(r2) is dead code
+      sqrt_rsqrt(r2, sr, rsr);
+      double ar = kSqrt5 * sr;
       if (SMEM) ar = fmin(ar, 1.0e6);
       const double we = w * exp_sel<SMEM>(-ar);
       S[k] = fma(we, fma(5.0 / 3.0, r2, 1.0 + ar), S[k]);

@@ -4,6 +4,7 @@
 // substitution, the FP64 tensor-pipe instruction.
 #pragma once
 
+#include "device_math.cuh"
 #include "internal.cuh"
 
 namespace cmoe {
@@ -44,6 +45,26 @@ constexpr int PT = 128;  // threads of the panel kernel: one panel row per threa
 // the last bit in all but rare halfway cases (and exactly when the true results are representable) at a third of the
 // dependent latency; small systems (known-answer cases) keep IEEE sqrt / divide.
 constexpr int LTS = NB + 2;  // row stride of the transposed factor (even: 16-byte aligned rows)
+
+// The FAST pivot step of chol32_warp, in two parts so that the kernels keep their instruction order around the column
+// store: l = sqrt(p) and the multiplier q = a / l from the library rsqrt with one correction step each
+// (chol_pivot_fast), then r = 1/l from rsqrt and one Newton step (chol_pivot_recip: no divide on the per-column critical
+// path).  l and q equal the IEEE sqrt and divide except when the exact value lies within 32 u^2 (relative, u = 2^-53)
+// of a rounding midpoint, and exactly when the true result is representable; r is within 0.55 ulp of 1/l (measured 0.50,
+// tests/test_gpu_fast_math.py).  Arguments: pivots p > kPivotTol (smaller ones fail the factorisation and their results
+// are discarded) and any finite a.
+__device__ __forceinline__ void chol_pivot_fast(double p, double a, double& l, double& q) {
+  const double y = rsqrt(p);
+  l = p * y;
+  l = fma(0.5 * y, fma(-l, l, p), l);
+  q = a * y;
+  q = fma(fma(-q, l, a), y, q);
+}
+__device__ __forceinline__ double chol_pivot_recip(double p, double l) {
+  const double r = rsqrt(p);  // ~ 1/l
+  return fma(fma(-l, r, 1.0), r, r);
+}
+
 template <bool FAST>
 __device__ __forceinline__ int chol32_warp(double (&a)[32], int lane, double* colbuf /* [2][64], [32..63] = 0 */,
                                            double* LT, double* rd, int col0) {
@@ -54,11 +75,7 @@ __device__ __forceinline__ int chol32_warp(double (&a)[32], int lane, double* co
     fail = (fail == 0 && !(piv > kPivotTol)) ? j + 1 : fail;
     double l, q;
     if (FAST) {
-      const double y = rsqrt(piv);
-      l = piv * y;
-      l = fma(0.5 * y, fma(-l, l, piv), l);
-      q = a[0] * y;
-      q = fma(fma(-q, l, a[0]), y, q);
+      chol_pivot_fast(piv, a[0], l, q);
     } else {
       l = sqrt(piv);
       q = a[0] / l;
@@ -66,8 +83,7 @@ __device__ __forceinline__ int chol32_warp(double (&a)[32], int lane, double* co
     const double lj = (lane == j) ? l : q;
     if (lane >= j) LT[(col0 + j) * LTS + col0 + lane] = lj;
     if (FAST) {
-      double r = rsqrt(piv);            // ~ 1/l
-      r = fma(fma(-l, r, 1.0), r, r);   // one Newton step on 1/l: no divide on the per-column critical path
+      const double r = chol_pivot_recip(piv, l);
       if (lane == j) rd[col0 + j] = r;
     } else {
       if (lane == j) rd[col0 + j] = l;
@@ -81,21 +97,6 @@ __device__ __forceinline__ int chol32_warp(double (&a)[32], int lane, double* co
     a[31] = 0.0;
   }
   return fail;
-}
-
-// sqrt(p) and 1/sqrt(p) for a normal p > 0: hardware seed (MUFU.RSQ64H) + two coupled Goldschmidt steps: one MUFU and
-// five dependent FP64 operations instead of the library rsqrt plus a Newton correction on the pivot chain.  Results
-// within ~1 ulp.
-__device__ __forceinline__ void sqrt_rsqrt(double p, double& l, double& y) {
-  double y0;
-  asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y0) : "d"(p));
-  double g = p * y0, h = 0.5 * y0;
-  double r = fma(-g, h, 0.5);
-  g = fma(g, r, g);
-  h = fma(h, r, h);
-  r = fma(-g, h, 0.5);
-  l = fma(g, r, g);
-  y = 2.0 * fma(h, r, h);
 }
 
 // Same factorisation, two columns per round: the 2 x 2 pivot block [l11 0; l21 l22] is formed from three shuffles, both

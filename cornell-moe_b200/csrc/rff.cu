@@ -61,32 +61,7 @@ struct RffShape {
   int matern;  // kernel-matched Matern-5/2 draw: W = (Omega / l) sqrt(5 / g), g ~ chi^2_5 per feature
 };
 
-// sin and cos of a for the sample functions, without the library's slow-path argument reduction (and its local-memory
-// frame): a three-part Cody-Waite reduction by pi/2 with FMA, exact to rounding for |a| < 2^30, then the fdlibm kernel
-// polynomials on [-pi/4, pi/4].  The argument W x + b itself carries a rounding error of order ulp(a), which dominates.
-__device__ __forceinline__ void rff_sincos(double a, double& sn, double& cs) {
-  const double k = rint(a * 0.63661977236758134308);
-  double r = fma(-k, 1.5707963267948965580e+00, a);
-  r = fma(-k, 6.1232339957367658e-17, r);
-  r = fma(-k, -1.4973849048591698e-33, r);
-  const int q = static_cast<int>(__double2ll_rn(k) & 3);
-  const double z = r * r;
-  const double ps = fma(z, fma(z, fma(z, fma(z, 1.58969099521155010221e-10, -2.50507602534068634195e-08),
-                                      2.75573137070700676789e-06),
-                               -1.98412698298579493134e-04),
-                        8.33333333332248946124e-03);
-  const double sr = fma(z * r, fma(z, ps, -1.66666666666666324348e-01), r);
-  const double pc = z * fma(z, fma(z, fma(z, fma(z, fma(z, -1.13596475577881948265e-11, 2.08757232129817482790e-09),
-                                              -2.75573143513906633035e-07),
-                                       2.48015872894767294178e-05),
-                                -1.38888888888741095749e-03),
-                            4.16666666666666019037e-02);
-  const double hz = 0.5 * z, w = 1.0 - hz;
-  const double cr = w + (((1.0 - w) - hz) + z * pc);
-  sn = (q == 0) ? sr : (q == 1) ? cr : (q == 2) ? -sr : -cr;
-  cs = (q == 0) ? cr : (q == 1) ? -sr : (q == 2) ? -cr : sr;
-}
-
+// sin and cos of the sample functions' arguments: rff_sincos (device_math.cuh)
 __device__ __forceinline__ double rff_cos(double a) {
   double sn, cs;
   rff_sincos(a, sn, cs);
