@@ -361,12 +361,16 @@ __device__ __forceinline__ void tile_bfrag(const double* row, double (&b)[(W + 3
   for (int ks = 0; ks < (W + 3) / 4; ++ks) b[ks] = (4 * ks + t < W) ? row[4 * ks + t] : 0.0;
 }
 
-// acc[4] (C layout) += A (K = W, fragments f) x B (fragments b)
+// acc[4] (C layout) += A (K = W, fragments f) x B (fragments b): pairs of k-steps as one m16n8k8 product (half the
+// DMMA instructions, which is what they cost when interleaved with the element-wise FP64 work, DESIGN.md K6)
 template <int W>
 __device__ __forceinline__ void tile_mma(double (&acc)[4], const double (&f)[(W + 3) / 4][2],
                                          const double (&b)[(W + 3) / 4]) {
+  constexpr int KS = (W + 3) / 4;
 #pragma unroll
-  for (int ks = 0; ks < (W + 3) / 4; ++ks) dmma_m16n8k4(acc[0], acc[1], acc[2], acc[3], f[ks][0], f[ks][1], b[ks]);
+  for (int ks = 0; ks + 1 < KS; ks += 2)
+    dmma_m16n8k8(acc[0], acc[1], acc[2], acc[3], f[ks][0], f[ks][1], f[ks + 1][0], f[ks + 1][1], b[ks], b[ks + 1]);
+  if (KS % 2) dmma_m16n8k4(acc[0], acc[1], acc[2], acc[3], f[KS - 1][0], f[KS - 1][1], b[KS - 1]);
 }
 
 // POINT round (SquareExponential) over the training rows: S0 = sum_j a_j k_j and s_d = sum_j a_j k_j X~_jd of every
@@ -422,10 +426,8 @@ __device__ __forceinline__ void tile_posterior(const double* __restrict__ Xt, co
       }
       // s += W X~: k-step 0 takes the even columns (rows je0: A = (w0, w2)), k-step 1 the odd ones (rows je1)
 #pragma unroll
-      for (int n = 0; n < ND; ++n) {
-        dmma_m16n8k4(sacc[h][n][0], sacc[h][n][1], sacc[h][n][2], sacc[h][n][3], w[0], w[2], b0[n]);
-        dmma_m16n8k4(sacc[h][n][0], sacc[h][n][1], sacc[h][n][2], sacc[h][n][3], w[1], w[3], b1[n]);
-      }
+      for (int n = 0; n < ND; ++n)
+        dmma_m16n8k8(sacc[h][n][0], sacc[h][n][1], sacc[h][n][2], sacc[h][n][3], w[0], w[2], w[1], w[3], b0[n], b1[n]);
     }
   };
   const int nfull = N & ~7;
@@ -1919,12 +1921,10 @@ __device__ __forceinline__ void kg_acc_tile_rows(const KgAccParams& prm, double*
 #pragma unroll
       for (int k = 0; k < T; ++k) {
         double kv[4] = {e[k][0] + h0, e[k][0] + h1, e[k][1] + h0, e[k][1] + h1};
-        dmma_m16n8k4(kv[0], kv[1], kv[2], kv[3], xa[k][0][0], xa[k][0][1], xb.x);
-        dmma_m16n8k4(kv[0], kv[1], kv[2], kv[3], xa[k][1][0], xa[k][1][1], xb.y);
+        dmma_m16n8k8(kv[0], kv[1], kv[2], kv[3], xa[k][0][0], xa[k][0][1], xa[k][1][0], xa[k][1][1], xb.x, xb.y);
 #pragma unroll
         for (int i = 0; i < 4; ++i) kv[i] = exp_tab2k(kv[i]);
-        dmma_m16n8k4(acc[k][0], acc[k][1], acc[k][2], acc[k][3], kv[0], kv[2], c0);
-        dmma_m16n8k4(acc[k][0], acc[k][1], acc[k][2], acc[k][3], kv[1], kv[3], c1);
+        dmma_m16n8k8(acc[k][0], acc[k][1], acc[k][2], acc[k][3], kv[0], kv[2], kv[1], kv[3], c0, c1);
       }
     }
   });

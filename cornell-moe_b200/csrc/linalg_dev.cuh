@@ -348,6 +348,16 @@ __device__ __forceinline__ void dmma_m16n8k4(double& d0, double& d1, double& d2,
                : "d"(a0), "d"(a1), "d"(b));
 }
 
+// Two chained m16n8k4 products in one instruction (DMMA.16x8x8 on sm_90): (a0, a1; b0) is the first k-step in the
+// fragment layout of dmma_m16n8k4, (a2, a3; b1) the second.
+__device__ __forceinline__ void dmma_m16n8k8(double& d0, double& d1, double& d2, double& d3, double a0, double a1,
+                                             double a2, double a3, double b0, double b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
+               "{%0,%1,%2,%3};\n"
+               : "+d"(d0), "+d"(d1), "+d"(d2), "+d"(d3)
+               : "d"(a0), "d"(a1), "d"(a2), "d"(a3), "d"(b0), "d"(b1));
+}
+
 // acc += As^T-tile * Bs-tile over one 64-deep chunk: warp (wm, wn) owns a 32 x 32 sub-tile, 2 x 4 m16n8k4 products per
 // k-step (the fragment layout of dmma_tile_kernel in linalg.cu).  As / Bs: [k][LDT], element (k, row).  Accumulator
 // acc[i][j][h] is element (wm + 8 i + lr, wn + 8 j + 2 lc + h) of the 64 x 64 tile.
