@@ -168,8 +168,7 @@ void ei_eval_batch(const cmoe_gp& gp, const double* candidates, int nc, int q, c
                    double best_so_far, uint64_t seed, const double* dtable, double* ei_host, double* grad_host) {
   const int U = q + p, dim = gp.spec.dim;
   const size_t per_cand = static_cast<size_t>(num_mc) * (U + 2) * sizeof(double);
-  const int batch = static_cast<int>(
-      std::max<size_t>(1, std::min<size_t>({static_cast<size_t>(nc), (size_t(2) << 30) / per_cand, kMaxGridY})));
+  const int batch = static_cast<int>(chunk_items(nc, size_t(2) << 30, per_cand, kMaxGridY));
   for (int c0 = 0; c0 < nc; c0 += batch) {
     const int nb = std::min(batch, nc - c0);
     ei_eval_chunk(gp, candidates + static_cast<size_t>(c0) * q * dim, nb, q, Xp, p, num_mc, best_so_far, seed, dtable,

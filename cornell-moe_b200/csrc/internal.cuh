@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <memory>
@@ -192,8 +194,11 @@ bool potrf_lower_coop(double* A, int n, int* flag, cudaStream_t s);
 // X <- (L L^T)^-1 X for nrhs right-hand sides; X is n*nrhs column-major with leading dimension ldx.
 void potrs_lower(const double* L, int n, double* X, int ldx, int nrhs, cudaStream_t s);
 // X <- L^-1 X (trans = false) or L^-T X (trans = true).  nrhs <= 4 with n >= 1024 takes the single-launch chained
-// solver (which synchronises `s`); everything else is the blocked multi-RHS kernel, asynchronous on `s`.
+// solver (which synchronises `s`); everything else is trsm_lower_blocked.
 void trsm_lower(const double* L, int n, double* X, int ldx, int nrhs, bool trans, cudaStream_t s);
+// The blocked multi-RHS kernel for any nrhs, asynchronous on `s`: one CTA per 32 columns, and each column's result
+// depends only on that column, so a column comes out the same however many columns share the call.
+void trsm_lower_blocked(const double* L, int n, double* X, int ldx, int nrhs, bool trans, cudaStream_t s);
 // trsv_coop.cu: one cooperative launch, owner + helper CTAs per 128-unknown block row; false = not applicable / gave up
 bool trsv_coop(const double* L, int n, double* x, bool trans, cudaStream_t s);
 bool trsv_coop_pair(const double* L, int n, double* x, cudaStream_t s);
@@ -216,6 +221,22 @@ struct SampleWork {
   DevBuf<double> P, V, A, mu, y, part_v, opt, stage, table;
   DevBuf<int> dPs, fail, part_i, amin;
 };
+// the handle's SampleWork, created on first use
+inline SampleWork& sample_work(const cmoe_gp& gp) {
+  if (!gp.sample_ws) gp.sample_ws = std::make_shared<SampleWork>();
+  return *static_cast<SampleWork*>(gp.sample_ws.get());
+}
+
+// Items per chunk of a batched call: as many as fit in `budget` bytes at `bytes_per_item` each, at most `total` and
+// `cap` (a grid-dimension or set-count limit), and at least one.
+inline size_t chunk_items(size_t total, size_t budget, size_t bytes_per_item, size_t cap = SIZE_MAX) {
+  return std::max<size_t>(1, std::min<size_t>({total, budget / bytes_per_item, cap}));
+}
+
+// Step size of gradient-descent iteration i (from 0): pre_mult (i + 1)^-gamma, gpp_optimization.hpp:736
+inline double gd_step_size(double pre_mult, double gamma, int i) {
+  return pre_mult * std::pow(static_cast<double>(i + 1), -gamma);
+}
 
 // ---- lcb.cu: LCB batch selection (DESIGN.md K13) ----------------------------------------------------------------
 // rows of the selected-set block, (q - 1)(1 + g): its bordered factor is built by one CTA, round by round

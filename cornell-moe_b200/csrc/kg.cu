@@ -796,7 +796,7 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     }
     std::vector<double> a0(std::max(1, inner->max_num_steps));
     for (int i = 0; i < inner->max_num_steps; ++i)
-      a0[i] = inner->pre_mult * std::pow(static_cast<double>(i + 1), -inner->gamma);  // gpp_optimization.hpp:736
+      a0[i] = gd_step_size(inner->pre_mult, inner->gamma, i);
     pl->dAlpha0.upload(a0.data(), a0.size(), s);
     std::vector<double> hXp(static_cast<size_t>(std::max(1, p)) * dim, 0.0);
     if (p) std::copy(points_being_sampled, points_being_sampled + static_cast<size_t>(p) * dim, hXp.begin());
@@ -834,8 +834,7 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     const size_t per_cand = static_cast<size_t>(num_mc) * (QP + DIMP + 2) * sizeof(double) +
                             static_cast<size_t>(n) * Q * 4 * sizeof(double) +
                             (spec.g == 0 ? static_cast<size_t>(pl->M) * (1 + QP) * (DIMP + 2) * sizeof(double) : 0);
-    pl->batch = static_cast<int>(std::max<size_t>(
-        1, std::min<size_t>({static_cast<size_t>(max_candidates), (size_t(3) << 30) / per_cand, kMaxGridY})));
+    pl->batch = static_cast<int>(chunk_items(max_candidates, size_t(3) << 30, per_cand, kMaxGridY));
     // samples per CTA: aim for >= ~8 waves of CTAs over the whole batch, between 2 and 16 samples per lane.  A wave is
     // the selected path's residency (kg_select; 2 CTAs per SM for the tile instantiation at the bench shape).
     {

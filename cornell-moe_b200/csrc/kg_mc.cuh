@@ -1166,22 +1166,6 @@ __device__ __forceinline__ void eval_line_gen(const KgMcParams& prm, const doubl
   }
 }
 
-// TensorProductDomain::LimitUpdate, gpp_domain.cpp:64-104, for one coordinate
-__device__ __forceinline__ double limit_step(double step, double x, double lo, double hi, double mrc) {
-  double dist = fmin(x - lo, hi - x);
-  if (fabs(step) > mrc * dist) step = copysign(mrc * dist, step);
-  const double next = x + step;
-  if (next < lo || next > hi) {
-    if (next < lo) {
-      dist = lo - x;
-      step = (x + step * 0.5 < lo) ? dist * 0.5 : step * 0.5;
-    } else {
-      dist = hi - x;
-      step = (x + step * 0.5 > hi) ? dist * 0.5 : step * 0.5;
-    }
-  }
-  return step;
-}
 
 // General path: the weights a = beta~ - B~ c depend on the sample only, not on the query point, so they are formed once
 // when a lane takes a new sample and parked in that lane's column of the CTA's scratch (global memory, streamed back

@@ -79,8 +79,8 @@ __global__ void __launch_bounds__(kWarps * 32) lcb_screen_kernel(const __grid_co
 __global__ void __launch_bounds__(kSelThreads) lcb_select_kernel(const double* __restrict__ mu,
                                                                  const double* __restrict__ sd, int C, LcbStatus* st,
                                                                  int* __restrict__ sel, int* __restrict__ sat) {
-  __shared__ double sv[kSelThreads], su[kSelThreads];
-  __shared__ int si[kSelThreads];
+  __shared__ double sv[kSelThreads / 32], su[kSelThreads / 32];
+  __shared__ int si[kSelThreads / 32];
   __shared__ int wcount[kSelThreads / 32];
   __shared__ int base;
   if (st->failed) return;
@@ -95,25 +95,14 @@ __global__ void __launch_bounds__(kSelThreads) lcb_select_kernel(const double* _
     }
     ub = fmin(ub, u);
   }
-  sv[tid] = best;
-  si[tid] = bidx;
-  su[tid] = ub;
+  block_best<false>(best, bidx, sv, si);
+  for (int o = 16; o > 0; o >>= 1) ub = fmin(ub, __shfl_xor_sync(0xffffffffu, ub, o));
+  if (lane == 0) su[warp] = ub;
   __syncthreads();
-  for (int h = kSelThreads / 2; h > 0; h >>= 1) {
-    if (tid < h) {
-      const double v = sv[tid + h];
-      const int k = si[tid + h];
-      if (v < sv[tid] || (v == sv[tid] && k < si[tid])) {
-        sv[tid] = v;
-        si[tid] = k;
-      }
-      su[tid] = fmin(su[tid], su[tid + h]);
-    }
-    __syncthreads();
-  }
-  const double upper = su[0];
+  double upper = INFINITY;
+  for (int w = 0; w < kSelThreads / 32; ++w) upper = fmin(upper, su[w]);
   if (tid == 0) {
-    sel[0] = (si[0] == INT_MAX) ? 0 : si[0];
+    sel[0] = (bidx == INT_MAX) ? 0 : bidx;
     base = 0;
   }
   __syncthreads();
@@ -144,14 +133,14 @@ __global__ void lcb_gather_kernel(const double* __restrict__ cand, int dim, cons
 }
 
 // G[r][c] = T_k[:, r] . T[:, c] for the b rows of the newest point (block k) and the (k+1) b columns of blocks 0..k
-// (T_l = L^-1 K(X, s_l rows), ldb columns per block); one CTA per entry, fixed-order block sum.
-__global__ void __launch_bounds__(256) lcb_cross_kernel(const double* __restrict__ T, int n, int ldb, int b, int k,
+// (T_l = L^-1 K(X, s_l rows), b columns per block); one CTA per entry, fixed-order block sum.
+__global__ void __launch_bounds__(256) lcb_cross_kernel(const double* __restrict__ T, int n, int b, int k,
                                                         double* __restrict__ G, const LcbStatus* st) {
   __shared__ double scratch[8];
   if (st->failed) return;
   const int e = blockIdx.x, r = e % b, c = e / b, lb = c / b, t = c % b;
-  const double* tr = T + (static_cast<size_t>(k) * ldb + r) * n;
-  const double* tc = T + (static_cast<size_t>(lb) * ldb + t) * n;
+  const double* tr = T + (static_cast<size_t>(k) * b + r) * n;
+  const double* tc = T + (static_cast<size_t>(lb) * b + t) * n;
   double acc = 0.0;
   for (int i = threadIdx.x; i < n; i += blockDim.x) acc = fma(tr[i], tc[i], acc);
   acc = block_sum(acc, scratch);
@@ -219,7 +208,7 @@ __global__ void __launch_bounds__(256) lcb_border_kernel(const double* __restric
 }
 
 // One round for the satisfied candidates, one warp each (position p, candidate sat[p]):
-//   c0(s_k row t, x) = k(s_k row t, x) - sum_rows k(x, X_row) B[row][t]     (B = K^-1 K(X, s_k rows), n x ldb)
+//   c0(s_k row t, x) = k(s_k row t, x) - sum_rows k(x, X_row) B[row][t]     (B = K^-1 K(X, s_k rows), n x b)
 //   w = L_kk^-1 (c0 - R_k w_<k(x)),  sigma^2 -= |w|^2
 // Lanes stride over the training points (ascending) and are combined by a fixed butterfly; the triangular steps run on
 // lane 0 in ascending order.  Each CTA leaves max sigma (ties: lowest position) in part_v / part_i.
@@ -297,17 +286,8 @@ __global__ void __launch_bounds__(kWarps * 32) lcb_round_kernel(
       }
     }
   }
-  if (lane == 0) {
-    bv[warp] = best;
-    bi[warp] = bidx;
-  }
-  __syncthreads();
+  block_best<true>(best, bidx, bv, bi);
   if (tid == 0) {
-    for (int w = 1; w < kWarps; ++w)
-      if (bv[w] > best) {  // warps hold ascending positions: the first maximum wins
-        best = bv[w];
-        bidx = bi[w];
-      }
     part_v[blockIdx.x] = best;
     part_i[blockIdx.x] = bidx;
   }
@@ -320,22 +300,12 @@ __global__ void lcb_argmax_kernel(const double* __restrict__ part_v, const int* 
   const int lane = threadIdx.x;
   double best = -INFINITY;
   int bidx = INT_MAX;
-  for (int q = lane; q < nparts; q += 32) {
-    const double v = part_v[q];
-    const int i = part_i[q];
-    if (v > best || (v == best && i < bidx)) {
-      best = v;
-      bidx = i;
+  for (int q = lane; q < nparts; q += 32)
+    if (beats<true>(part_v[q], part_i[q], best, bidx)) {
+      best = part_v[q];
+      bidx = part_i[q];
     }
-  }
-  for (int o = 16; o > 0; o >>= 1) {
-    const double v = __shfl_xor_sync(0xffffffffu, best, o);
-    const int i = __shfl_xor_sync(0xffffffffu, bidx, o);
-    if (v > best || (v == best && i < bidx)) {
-      best = v;
-      bidx = i;
-    }
-  }
+  warp_best<true>(best, bidx);
   if (lane == 0) *sel_out = sat[bidx == INT_MAX ? 0 : bidx];
 }
 
@@ -374,21 +344,15 @@ extern "C" int cmoe_lcb_select(const cmoe_gp* gp, const double* candidates, int 
     CMOE_CUDA(cudaMemsetAsync(dSel.p, 0, q * sizeof(int), s));
 
     // screen, in chunks of the sampling workspace (one column of V per candidate)
-    if (!gp->sample_ws) gp->sample_ws = std::make_shared<SampleWork>();
-    SampleWork& w = *static_cast<SampleWork*>(gp->sample_ws.get());
-    const int chunk = static_cast<int>(
-        std::max<size_t>(1, std::min<size_t>(static_cast<size_t>(C), kSampleWorkspaceBytes / (sizeof(double) * n))));
-    // at least 5 right-hand sides: trsm_lower sends up to 4 columns of a large factor to a different solver, and a
-    // candidate must be solved by the same kernel whatever chunk it lands in
-    w.V.ensure(static_cast<size_t>(std::max(chunk, 5)) * n);
+    SampleWork& w = sample_work(*gp);
+    const int chunk = static_cast<int>(chunk_items(C, kSampleWorkspaceBytes, sizeof(double) * n));
+    w.V.ensure(static_cast<size_t>(chunk) * n);
     for (int c0 = 0; c0 < C; c0 += chunk) {
-      const int nc = std::min(chunk, C - c0), nrhs = std::max(nc, 5);
+      const int nc = std::min(chunk, C - c0);
       const double* Pc = dCand.p + static_cast<size_t>(c0) * dim;
-      if (nrhs > nc)
-        CMOE_CUDA(cudaMemsetAsync(w.V.p + static_cast<size_t>(nc) * n, 0,
-                                  static_cast<size_t>(nrhs - nc) * n * sizeof(double), s));
       build_mix_covariance(spec, gp->dX.p, N, Pc, nc, dDer.p, 0, w.V.p, s);
-      trsm_lower(gp->dK.p, n, w.V.p, n, nrhs, false, s);
+      // the blocked kernel whatever the column count: a candidate's solve does not depend on the chunk it lands in
+      trsm_lower_blocked(gp->dK.p, n, w.V.p, n, nc, false, s);
       posterior_mean_points(*gp, Pc, nc, dDer.p, 0, dMu.p + c0, nullptr, s);
       lcb_screen_kernel<<<(nc + kWarps - 1) / kWarps, kWarps * 32, 0, s>>>(spec, w.V.p, n, Pc, nc, c0, dSd.p, dS2.p,
                                                                           dSt.p);
@@ -412,30 +376,29 @@ extern "C" int cmoe_lcb_select(const cmoe_gp* gp, const double* candidates, int 
                  "num_satisfied * (num_to_sample - 1) * (1 + num_derivatives) must be <= 2^28");
 
     if (q > 1) {
-      // T_k and B_k carry max(1 + g, 5) columns (zero beyond 1 + g): with <= 4 columns on n >= 1024, trsm_lower takes the
-      // cooperative single-vector solver, which synchronises the host, and the rounds must run without a synchronise.
-      // The blocked kernel this selects is one CTA per 32 columns, so at large n it sets a round's time (DESIGN.md K13).
-      const int ldb = std::max(b, 5), nparts = (nsat + kWarps - 1) / kWarps;
-      DevBuf<double> Psel(static_cast<size_t>(q) * dim), Pss, T(static_cast<size_t>(q - 1) * ldb * n),
-          B(static_cast<size_t>(ldb) * n), Kp(static_cast<size_t>(rows) * rows), G(static_cast<size_t>(b) * rows),
+      // The rounds' solves take the blocked kernel: trsm_lower sends few columns of a large factor to the cooperative
+      // single-vector solver, which synchronises the host, and the rounds run without a synchronise.  The blocked
+      // kernel is one CTA per 32 columns, so at large n it sets a round's time (DESIGN.md K13).
+      const int nparts = (nsat + kWarps - 1) / kWarps;
+      DevBuf<double> Psel(static_cast<size_t>(q) * dim), Pss, T(static_cast<size_t>(q - 1) * b * n),
+          B(static_cast<size_t>(b) * n), Kp(static_cast<size_t>(rows) * rows), G(static_cast<size_t>(b) * rows),
           LM(static_cast<size_t>(rows) * rows), W(static_cast<size_t>(nsat) * rows), s2(nsat), part_v(nparts);
       DevBuf<int> part_i(nparts);
       Pss.alloc(static_cast<size_t>((q + 127) / 128) * 128 * dim);  // sized once: no reallocation between rounds
-      T.zero(s);
       const size_t smem_round = (static_cast<size_t>(kWarps) * b * 32 + static_cast<size_t>(kWarps) * b) * sizeof(double);
       for (int k = 0; k + 1 < q; ++k) {
         const int m = (k + 1) * b;
-        double* Tk = T.p + static_cast<size_t>(k) * ldb * n;
+        double* Tk = T.p + static_cast<size_t>(k) * b * n;
         lcb_gather_kernel<<<1, 32, 0, s>>>(dCand.p, dim, dSel.p + k, Psel.p + static_cast<size_t>(k) * dim);
         count_launch();
         build_mix_covariance(spec, gp->dX.p, N, Psel.p + static_cast<size_t>(k) * dim, 1, dDer.p, spec.g, Tk, s);
-        trsm_lower(gp->dK.p, n, Tk, n, ldb, false, s);  // T_k = L^-1 K(X, s_k rows)
-        CMOE_CUDA(cudaMemcpyAsync(B.p, Tk, static_cast<size_t>(ldb) * n * sizeof(double), cudaMemcpyDeviceToDevice, s));
-        trsm_lower(gp->dK.p, n, B.p, n, ldb, true, s);  // B = K^-1 K(X, s_k rows)
+        trsm_lower_blocked(gp->dK.p, n, Tk, n, b, false, s);  // T_k = L^-1 K(X, s_k rows)
+        CMOE_CUDA(cudaMemcpyAsync(B.p, Tk, static_cast<size_t>(b) * n * sizeof(double), cudaMemcpyDeviceToDevice, s));
+        trsm_lower_blocked(gp->dK.p, n, B.p, n, b, true, s);  // B = K^-1 K(X, s_k rows)
         scale_points(*gp, Psel.p, k + 1, Pss, s);
         CMOE_CUDA(cudaMemsetAsync(Kp.p, 0, static_cast<size_t>(m) * m * sizeof(double), s));
         build_covariance(spec, Psel.p, Pss.p, k + 1, gp->dnoise.p, Kp.p, s);  // K(S, S) + D, as append_points
-        lcb_cross_kernel<<<m * b, 256, 0, s>>>(T.p, n, ldb, b, k, G.p, dSt.p);
+        lcb_cross_kernel<<<m * b, 256, 0, s>>>(T.p, n, b, k, G.p, dSt.p);
         lcb_border_kernel<<<1, 256, 0, s>>>(Kp.p, G.p, b, k, LM.p, rows, n, dSt.p);
         lcb_round_kernel<<<nparts, kWarps * 32, smem_round, s>>>(spec, gp->dX.p, N, dCand.p, dSat.p, nsat, B.p, n,
                                                                  Psel.p + static_cast<size_t>(k) * dim, LM.p, rows, k,

@@ -822,6 +822,11 @@ void trsm_lower(const double* L, int n, double* X, int ldx, int nrhs, bool trans
     }
     return;
   }
+  trsm_lower_blocked(L, n, X, ldx, nrhs, trans, s);
+}
+
+void trsm_lower_blocked(const double* L, int n, double* X, int ldx, int nrhs, bool trans, cudaStream_t s) {
+  if (n == 0 || nrhs == 0) return;
   const int grid = (nrhs + kTrsmNB - 1) / kTrsmNB;
   if (trans) {
     trsm_kernel<true><<<grid, 256, 0, s>>>(L, n, X, ldx, nrhs);

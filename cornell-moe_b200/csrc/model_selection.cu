@@ -477,6 +477,13 @@ LmlWork& lml_workspace(int device) {
   return ws;
 }
 
+// bytes of one set in a likelihood-list chunk without the gradient: K and its factor, the staged diagonal factors, the
+// noise variances, the value, the spec and the failure flag
+size_t lml_set_bytes(int n, int b) {
+  const size_t nsteps = (n + NB - 1) / NB;
+  return sizeof(double) * (static_cast<size_t>(n) * n + nsteps * NB * NB + b + 1) + sizeof(KernelSpec) + sizeof(int);
+}
+
 }  // namespace
 }  // namespace cmoe
 
@@ -600,13 +607,10 @@ void lml_list(int kernel, const double* hyperparameters, int num_sets, const dou
     const int nsteps = (n + NB - 1) / NB;
     // the gradient adds L^-1 (n x n), a, the contraction's CTA partials and the [1 + nh] output row per set
     const int gx = (N + kHgTx - 1) / kHgTx, nctas = gx * ((N + kHgTy - 1) / kHgTy);
-    size_t per_set = sizeof(double) * (static_cast<size_t>(n) * n + static_cast<size_t>(nsteps) * NB * NB + b + 1) +
-                     sizeof(KernelSpec) + sizeof(int);
+    size_t per_set = lml_set_bytes(n, b);
     if (grads)
       per_set += sizeof(double) * (static_cast<size_t>(n) * n + n + static_cast<size_t>(nctas) * (dim + 1) + 1 + nh);
-    const int chunk = static_cast<int>(std::max<size_t>(
-        1, std::min<size_t>({kSampleWorkspaceBytes / per_set, static_cast<size_t>(num_sets),
-                             static_cast<size_t>(kMaxChunkSets)})));
+    const int chunk = static_cast<int>(chunk_items(num_sets, kSampleWorkspaceBytes, per_set, kMaxChunkSets));
     w.X.upload(points_sampled, static_cast<size_t>(N) * dim, s);
     w.r.upload(rc.data(), n, s);
     w.specs.ensure(chunk);
@@ -878,10 +882,8 @@ void hyper_mcmc(int kernel, int prior, int noisy, const double* initial_position
   CMOE_REQUIRE(W >= 2 * nh, CMOE_ERR_BOUNDS, "num_walkers must be at least twice the number of hyperparameters");
   CMOE_REQUIRE(num_steps >= 1, CMOE_ERR_BOUNDS, "num_steps must be >= 1");
   const int n = N * b, nsteps = (n + NB - 1) / NB;
-  // the half-ensemble is one K10 chunk (lml_list's per-set bytes without the gradient)
-  const size_t per_set = sizeof(double) * (static_cast<size_t>(n) * n + static_cast<size_t>(nsteps) * NB * NB + b + 1) +
-                         sizeof(KernelSpec) + sizeof(int);
-  const size_t chunk = std::max<size_t>(1, std::min<size_t>(kSampleWorkspaceBytes / per_set, kMaxChunkSets));
+  // the half-ensemble is one K10 chunk of lml_list without the gradient
+  const size_t chunk = chunk_items(kMaxChunkSets, kSampleWorkspaceBytes, lml_set_bytes(n, b));
   CMOE_REQUIRE(static_cast<size_t>(Wh) <= chunk, CMOE_ERR_BOUNDS,
                "num_walkers / 2 = " + std::to_string(Wh) + " sets exceed one likelihood chunk (" +
                    std::to_string(chunk) + " sets at n = " + std::to_string(n) + ")");

@@ -19,6 +19,7 @@
 #include <queue>
 #include <thread>
 
+#include "device_math.cuh"
 #include "internal.cuh"
 
 using namespace cmoe;  // NOLINT
@@ -27,23 +28,6 @@ namespace {
 
 constexpr int kTopK = 20;  // hard-coded in the reference (gpp_knowledge_gradient_optimization.hpp:901, gpp_math.hpp:1765)
 
-// TensorProductDomain::LimitUpdate for one coordinate (gpp_domain.cpp:64-104)
-double limit_step_host(double step, double x, double lo, double hi, double mrc) {
-  double dist = std::fmin(x - lo, hi - x);
-  if (std::fabs(step) > mrc * dist) step = std::copysign(mrc * dist, step);
-  const double next = x + step;
-  if (next < lo || next > hi) {
-    if (next < lo) {
-      dist = lo - x;
-      step = (x + step * 0.5 < lo) ? dist * 0.5 : step * 0.5;
-    } else {
-      dist = hi - x;
-      step = (x + step * 0.5 > hi) ? dist * 0.5 : step * 0.5;
-    }
-  }
-  return step;
-}
-
 // SimplexIntersectTensorProductDomain::LimitUpdate (gpp_domain.cpp:234-289) for one point: box limited to [0,1]^dim
 // (constructor, :107-139), tensor-product limit first, then half the distance to the diagonal face if the limited step
 // would leave the simplex.
@@ -51,7 +35,7 @@ void limit_update_simplex_host(const double* bounds, int dim, double mrc, const 
   if (mrc == 1.0) mrc -= 4.0 * std::numeric_limits<double>::epsilon();  // kRelativeChangeEpsilonTweak
   for (int d = 0; d < dim; ++d) {
     const double lo = std::fmax(bounds[2 * d], 0.0), hi = std::fmin(bounds[2 * d + 1], 1.0);
-    upd[d] = limit_step_host(upd[d], x[d], lo, hi, mrc);
+    upd[d] = limit_step(upd[d], x[d], lo, hi, mrc);
   }
   double norm = 0.0;
   for (int d = 0; d < dim; ++d) norm += upd[d] * upd[d];
@@ -113,7 +97,7 @@ void gradient_descent_batch(const BatchEval& eval, const cmoe_gd_params& gd, con
           std::copy(x.begin() + static_cast<size_t>(cur[k]) * ps, x.begin() + static_cast<size_t>(cur[k] + 1) * ps,
                     pts.begin() + static_cast<size_t>(k) * ps);
         eval(pts.data(), nc, vals.data(), grads.data());
-        const double alpha = gd.pre_mult * std::pow(static_cast<double>(i + 1), -gd.gamma);
+        const double alpha = gd_step_size(gd.pre_mult, gd.gamma, i);
         for (int k = 0; k < nc; ++k) {
           double* xs = x.data() + static_cast<size_t>(cur[k]) * ps;
           const double* g = grads.data() + static_cast<size_t>(k) * ps;
@@ -132,7 +116,7 @@ void gradient_descent_batch(const BatchEval& eval, const cmoe_gd_params& gd, con
           } else {
             for (int j = 0; j < ps; ++j) {
               const int d = j % dim;
-              const double step = limit_step_host(alpha * g[j], xs[j], domain_bounds[2 * d], domain_bounds[2 * d + 1],
+              const double step = limit_step(alpha * g[j], xs[j], domain_bounds[2 * d], domain_bounds[2 * d + 1],
                                                   gd.max_relative_change);
               xs[j] += step;
               ns2 += step * step;
@@ -515,7 +499,7 @@ int cmoe_limit_update(int domain_type, const double* domain_bounds, int dim, dou
     } else {
       CMOE_REQUIRE(domain_type == CMOE_DOMAIN_TENSOR_PRODUCT, CMOE_ERR_INVALID_VALUE, "unknown domain type");
       for (int d = 0; d < dim; ++d)
-        update[d] = limit_step_host(update[d], current_point[d], domain_bounds[2 * d], domain_bounds[2 * d + 1],
+        update[d] = limit_step(update[d], current_point[d], domain_bounds[2 * d], domain_bounds[2 * d + 1],
                                     max_relative_change);
     }
   });

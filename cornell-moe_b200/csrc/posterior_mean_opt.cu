@@ -32,22 +32,6 @@ struct PmDescent {
   double lo[CMOE_MAX_DIM], hi[CMOE_MAX_DIM];
 };
 
-__device__ __forceinline__ double limit_step_pm(double step, double x, double lo, double hi, double mrc) {
-  double dist = fmin(x - lo, hi - x);
-  if (fabs(step) > mrc * dist) step = copysign(mrc * dist, step);
-  const double next = x + step;
-  if (next < lo || next > hi) {
-    if (next < lo) {
-      dist = lo - x;
-      step = (x + step * 0.5 < lo) ? dist * 0.5 : step * 0.5;
-    } else {
-      dist = hi - x;
-      step = (x + step * 0.5 > hi) ? dist * 0.5 : step * 0.5;
-    }
-  }
-  return step;
-}
-
 // One thread's share of k(x, X) . beta (and, if g != null, of its gradient on the first ps coordinates) for one GP
 // (spec, N sampled points X, beta = K^-1 (y - mean)): the rows row0, row0 + stride, ... added in ascending order.
 __device__ __forceinline__ void pm_rows(const KernelSpec& spec, int N, int ps, const double* __restrict__ X,
@@ -107,7 +91,7 @@ __device__ __forceinline__ double pm_descend(const PmDescent& prm, int dim, cons
           search += 1;
         }
         for (int d = 0; d < dim; ++d)
-          step[d] = (d < ps) ? limit_step_pm(alpha * gb[d], x[d], prm.lo[d], prm.hi[d], prm.mrc) : 0.0;
+          step[d] = (d < ps) ? limit_step(alpha * gb[d], x[d], prm.lo[d], prm.hi[d], prm.mrc) : 0.0;
         for (int d = 0; d < dim; ++d) xt[d] = x[d] + step[d];
         obj = eval(xt, nullptr);
         if (obj <= fb || search == 30) break;
@@ -351,12 +335,9 @@ __global__ void __launch_bounds__(kPmScreenParts) pm_members_screen_kernel(const
   if (threadIdx.x == 0) V[static_cast<size_t>(m) * len + i] = mu;
 }
 
-// (value, index) order of the argmin: the smaller value, and among equal values the lower index
-__device__ __forceinline__ bool pm_less(double v, int i, double w, int j) { return v < w || (v == w && i < j); }
-
-// grid.x = num_gp.  Each thread scans its indices of the chunk in ascending order, then a fixed tree combines the
-// threads; the chunk's winner replaces the running one only if it is strictly smaller, so the result is np.argmin's
-// (first occurrence) however the screen is chunked.  The winner's coordinates become the member's start.
+// grid.x = num_gp.  Each thread scans its indices of the chunk, then block_best combines the threads; the chunk's winner
+// replaces the running one only if it is strictly smaller, so the result is np.argmin's (first occurrence) however the
+// screen is chunked.  The winner's coordinates become the member's start.
 __global__ void __launch_bounds__(kPmOptimaThreads) pm_members_argmin_kernel(const PmMember* __restrict__ members,
                                                                              int ps, const double* __restrict__ pts,
                                                                              int per_member, int num_points,
@@ -364,8 +345,8 @@ __global__ void __launch_bounds__(kPmOptimaThreads) pm_members_argmin_kernel(con
                                                                              int num_given,
                                                                              const double* __restrict__ V,
                                                                              double* __restrict__ state) {
-  __shared__ double sv[kPmOptimaThreads];
-  __shared__ int si[kPmOptimaThreads];
+  __shared__ double sv[kPmOptimaThreads / 32];
+  __shared__ int si[kPmOptimaThreads / 32];
   const int m = blockIdx.x, tid = threadIdx.x;
   const PmMember& mb = members[m];
   const int cnt = min(len, num_points + (include_sampled ? mb.N : 0) - i0);
@@ -374,30 +355,21 @@ __global__ void __launch_bounds__(kPmOptimaThreads) pm_members_argmin_kernel(con
   double bv = Vm[0];  // a chunk whose values are all NaN still names a point
   int bi = 0;
   for (int i = tid; i < cnt; i += kPmOptimaThreads)
-    if (pm_less(Vm[i], i, bv, bi)) {
+    if (beats<false>(Vm[i], i, bv, bi)) {
       bv = Vm[i];
       bi = i;
     }
-  sv[tid] = bv;
-  si[tid] = bi;
-  __syncthreads();
-  for (int h = kPmOptimaThreads / 2; h > 0; h >>= 1) {
-    if (tid < h && pm_less(sv[tid + h], si[tid + h], sv[tid], si[tid])) {
-      sv[tid] = sv[tid + h];
-      si[tid] = si[tid + h];
-    }
-    __syncthreads();
-  }
+  block_best<false>(bv, bi, sv, si);
   double* row = state + static_cast<size_t>(m) * (kPmStateHead + 2 * ps);
-  const bool take = i0 == 0 || sv[0] < row[0];
+  const bool take = i0 == 0 || bv < row[0];
   __syncthreads();  // every thread has read the running minimum before thread 0 replaces it
   if (!take) return;
-  const int gi = i0 + si[0];
-  const double* src = (gi < num_points) ? pts + (static_cast<size_t>(per_member ? m : 0) * num_given + si[0]) * ps
+  const int gi = i0 + bi;
+  const double* src = (gi < num_points) ? pts + (static_cast<size_t>(per_member ? m : 0) * num_given + bi) * ps
                                         : mb.X + static_cast<size_t>(gi - num_points) * mb.spec.dim;
   if (tid < ps) row[kPmStateHead + tid] = src[tid];
   if (tid == 0) {
-    row[0] = sv[0];
+    row[0] = bv;
     row[1] = static_cast<double>(gi);
   }
 }
@@ -523,7 +495,7 @@ extern "C" int cmoe_posterior_mean_optimization(const cmoe_gp* gp, int num_fidel
     }
     std::vector<double> a0(std::max(1, params->max_num_steps)), x0(dim, 1.0), res(ps + 1);
     for (int i = 0; i < params->max_num_steps; ++i)
-      a0[i] = params->pre_mult * std::pow(static_cast<double>(i + 1), -params->gamma);
+      a0[i] = gd_step_size(params->pre_mult, params->gamma, i);
     for (int d = 0; d < ps; ++d) x0[d] = initial_guess[d];
     DevBuf<double> dA0, dX0, dOut(ps + 1);
     dA0.upload(a0.data(), a0.size(), s);
@@ -637,7 +609,7 @@ extern "C" int cmoe_posterior_mean_mcmc_optimization(const cmoe_gp* const* gps, 
 
     // alpha_k = pre_mult k^-gamma on the host, as numpy.power computes it
     std::vector<double> a(prm.steps);
-    for (int k = 1; k <= prm.steps; ++k) a[k - 1] = params->pre_mult * std::pow(static_cast<double>(k), -params->gamma);
+    for (int i = 0; i < prm.steps; ++i) a[i] = gd_step_size(params->pre_mult, params->gamma, i);
     const size_t ns = num_starts;
     DevBuf<PmMember> dMem;
     DevBuf<double> dA, dStarts, dOut(ns * (ps + 1));
@@ -727,7 +699,7 @@ extern "C" int cmoe_posterior_mean_optima_mcmc(const cmoe_gp* const* gps, int nu
       std::memcpy(stage.data() + m * (sizeof(PmMember) / sizeof(double)), &mb, sizeof(PmMember));
     }
     for (size_t i = 0; i < steps; ++i)
-      stage[o_alpha + i] = params->pre_mult * std::pow(static_cast<double>(i + 1), -params->gamma);
+      stage[o_alpha + i] = gd_step_size(params->pre_mult, params->gamma, i);
     std::copy(shared_discrete, shared_discrete + static_cast<size_t>(num_shared) * ps, stage.begin() + o_shared);
     const size_t W = kPmStateHead + 2 * ps;
     DevBuf<double> dIn(stage.size()), dV(M * chunk), dState(M * W);

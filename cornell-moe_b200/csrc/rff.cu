@@ -12,7 +12,7 @@
 //   L L^T = Gram                                      potrf_batched
 //   theta                                             rff_theta_kernel: one CTA per sample, fixed-order GEMVs and
 //                                                     blocked substitutions (cta_forward_subst / cta_backward_subst)
-//   f on the grid, per-CTA argmin partials           rff_grid_kernel, rff_argmin_kernel
+//   f on the grid, per-CTA argmin partials           rff_grid_kernel, best_of_parts_kernel
 //   projected Newton from the grid argmin            rff_opt_kernel: one warp per sample
 // Every kernel treats the samples of a chunk independently and every reduction has a fixed order, so a sample's result
 // is a pure function of its randomness, not of num_points or the chunking.  cmoe_gp_sample_rff_functions stops after
@@ -310,8 +310,8 @@ __global__ void __launch_bounds__(kRffThreads) rff_grid_kernel(const __grid_cons
                                                                const double* __restrict__ theta,
                                                                double* __restrict__ part_v, int* __restrict__ part_i) {
   extern __shared__ double gs[];  // [kRffGridTile][d] W, [kRffGridTile] b, [kRffGridTile] theta
-  __shared__ double bv[kRffThreads];
-  __shared__ int bi[kRffThreads];
+  __shared__ double bv[kRffThreads / 32];
+  __shared__ int bi[kRffThreads / 32];
   const int s = blockIdx.y, tid = threadIdx.x, F = sh.F, d = sh.d;
   double* Wt = gs;
   double* bt = Wt + kRffGridTile * d;
@@ -345,37 +345,11 @@ __global__ void __launch_bounds__(kRffThreads) rff_grid_kernel(const __grid_cons
       bidx = j;
     }
   }
-  bv[tid] = best;
-  bi[tid] = bidx;
-  __syncthreads();
+  block_best<false>(best, bidx, bv, bi);
   if (tid == 0) {
-    for (int t = 1; t < kRffThreads; ++t)
-      if (bv[t] < best || (bv[t] == best && bi[t] < bidx)) {
-        best = bv[t];
-        bidx = bi[t];
-      }
     part_v[static_cast<size_t>(s) * gridDim.x + blockIdx.x] = best;
     part_i[static_cast<size_t>(s) * gridDim.x + blockIdx.x] = bidx;
   }
-}
-
-// first minimum over the grid kernel's CTAs of each sample, in CTA order (no finite value: index 0, value +inf)
-__global__ void rff_argmin_kernel(int ns, int nparts, const double* __restrict__ part_v,
-                                  const int* __restrict__ part_i, int* __restrict__ amin, double* __restrict__ vmin) {
-  const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s >= ns) return;
-  double best = INFINITY;
-  int bidx = INT_MAX;
-  for (int p = 0; p < nparts; ++p) {
-    const double v = part_v[static_cast<size_t>(s) * nparts + p];
-    const int k = part_i[static_cast<size_t>(s) * nparts + p];
-    if (v < best || (v == best && k < bidx)) {
-      best = v;
-      bidx = k;
-    }
-  }
-  amin[s] = (bidx == INT_MAX) ? 0 : bidx;
-  vmin[s] = best;
 }
 
 // f (and with G, the gradient, into gout: shared, d values) of one sample at x (shared, d values), lanes striding over the features and combined by
@@ -733,10 +707,8 @@ void rff_sample(const cmoe_gp* gp, int F, int P, bool optima, const double* doma
                                        (table ? static_cast<size_t>(F) * (d + 2) + M : 0) +
                                        (tchi2 ? static_cast<size_t>(F) : 0)) +
                      sizeof(int) * (static_cast<size_t>(gx) + 2);
-  const int chunk = static_cast<int>(std::max<size_t>(
-      1, std::min<size_t>({kSampleWorkspaceBytes / per, static_cast<size_t>(P), static_cast<size_t>(kMaxChunkSets)})));
-  if (!gp->sample_ws) gp->sample_ws = std::make_shared<SampleWork>();
-  SampleWork& w = *static_cast<SampleWork*>(gp->sample_ws.get());
+  const int chunk = static_cast<int>(chunk_items(P, kSampleWorkspaceBytes, per, kMaxChunkSets));
+  SampleWork& w = sample_work(*gp);
   w.V.ensure(static_cast<size_t>(chunk) * phi);
   w.A.ensure(static_cast<size_t>(chunk) * gram);
   w.fail.ensure(chunk);
@@ -788,7 +760,7 @@ void rff_sample(const cmoe_gp* gp, int F, int P, bool optima, const double* doma
     if (optima) {
       rff_grid_kernel<<<dim3(gx, nc), kRffThreads, smem_grid, s>>>(sh, dgrid.p, G, dW.p, db.p, dth.p, w.part_v.p,
                                                                    w.part_i.p);
-      rff_argmin_kernel<<<(nc + 127) / 128, 128, 0, s>>>(nc, gx, w.part_v.p, w.part_i.p, w.amin.p, dvmin.p);
+      best_of_parts_kernel<false><<<(nc + 127) / 128, 128, 0, s>>>(nc, gx, w.part_v.p, w.part_i.p, w.amin.p, dvmin.p);
       rff_opt_kernel<<<(nc + kRffOptWarps - 1) / kRffOptWarps, kRffOptWarps * 32, 0, s>>>(
           sh, nc, box, dgrid.p, w.amin.p, dvmin.p, dW.p, db.p, dth.p, dwc.p, dpts.p, dvals.p);
       count_launch(3);

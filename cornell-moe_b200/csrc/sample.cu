@@ -12,7 +12,7 @@
 //   mu                                 post_mean_only_kernel (posterior_mean_points)
 //   Var = K(P, P) - V^T V (+ jitter I) cov_tile_kernel: DMMA m16n8k4, the prior block is evaluated in the epilogue
 //   L L^T = Var                        batched blocked Cholesky, every launch covers all sets of the chunk
-//   y = mu + L w, argmin               sample_rows_kernel + argmin_kernel
+//   y = mu + L w, argmin               sample_rows_kernel + best_of_parts_kernel
 // The reference forms Var as (K^-1 K*)^T K* with two triangular solves; V^T V needs one solve (half the solve work)
 // and its product is exactly symmetric.  The two differ by rounding only.
 //
@@ -278,7 +278,7 @@ __global__ void __launch_bounds__(kTileThreads) chol_update_kernel(double* __res
 // --------------------------------------------------------------------------------------------------------------
 // y = mu + L w for 256 rows of one set per CTA (grid (row blocks, sets)); row i sums its i+1 products in ascending
 // order.  w: Philox draw (draw0 + set), normals 2k, 2k+1 from call k (cmoe_philox_normals), or row `set` of the table.
-// Each CTA leaves the lowest-index minimum of its value rows in (part_v, part_i); argmin_kernel combines them in order.
+// Each CTA leaves the lowest-index minimum of its value rows in (part_v, part_i); best_of_parts_kernel combines them.
 // --------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kRowThreads) sample_rows_kernel(int Q, int bs, const double* __restrict__ mu,
                                                                   const double* __restrict__ L, uint64_t seed,
@@ -286,8 +286,8 @@ __global__ void __launch_bounds__(kRowThreads) sample_rows_kernel(int Q, int bs,
                                                                   double* __restrict__ y, double* __restrict__ part_v,
                                                                   int* __restrict__ part_i) {
   extern __shared__ double w[];  // [rows this CTA needs]
-  __shared__ double bv[kRowThreads];
-  __shared__ int bi[kRowThreads];
+  __shared__ double bv[kRowThreads / 32];
+  __shared__ int bi[kRowThreads / 32];
   const int set = blockIdx.y, tid = threadIdx.x;
   const int row_end = min(Q, static_cast<int>(blockIdx.x + 1) * kRowThreads);
   if (table) {
@@ -315,36 +315,11 @@ __global__ void __launch_bounds__(kRowThreads) sample_rows_kernel(int Q, int bs,
       bidx = i / bs;
     }
   }
-  bv[tid] = best;
-  bi[tid] = bidx;
-  __syncthreads();
+  block_best<false>(best, bidx, bv, bi);
   if (tid == 0) {
-    for (int t = 1; t < kRowThreads; ++t)
-      if (bv[t] < best || (bv[t] == best && bi[t] < bidx)) {
-        best = bv[t];
-        bidx = bi[t];
-      }
     part_v[static_cast<size_t>(set) * gridDim.x + blockIdx.x] = best;
     part_i[static_cast<size_t>(set) * gridDim.x + blockIdx.x] = bidx;
   }
-}
-
-// argmin over the row blocks of each set, in block order (ties: lowest point index; no finite value: 0)
-__global__ void argmin_kernel(int nsets, int nparts, const double* __restrict__ part_v, const int* __restrict__ part_i,
-                              int* __restrict__ amin) {
-  const int set = blockIdx.x * blockDim.x + threadIdx.x;
-  if (set >= nsets) return;
-  double best = INFINITY;
-  int bidx = INT_MAX;
-  for (int p = 0; p < nparts; ++p) {
-    const double v = part_v[static_cast<size_t>(set) * nparts + p];
-    const int k = part_i[static_cast<size_t>(set) * nparts + p];
-    if (v < best || (v == best && k < bidx)) {
-      best = v;
-      bidx = k;
-    }
-  }
-  amin[set] = (bidx == INT_MAX) ? 0 : bidx;
 }
 
 // points_optima[set] = P[set][amin[set]]
@@ -404,13 +379,9 @@ void sample_chunk(const cmoe_gp& gp, SampleWork& w, int nc, int num, int gs, uin
                   const double* dtable, double jitter, cudaStream_t s) {
   const KernelSpec& spec = gp.spec;
   const int Q = num * (1 + gs), n = gp.n;
-  const size_t cols = static_cast<size_t>(nc) * Q;
-  // at least 5 right-hand sides: trsm_lower sends up to 4 columns of a large factor to a different solver, and a set
-  // must be solved by the same kernel however many sets share its chunk
-  const size_t nrhs = std::max<size_t>(cols, 5);
-  if (nrhs > cols) CMOE_CUDA(cudaMemsetAsync(w.V.p + cols * n, 0, (nrhs - cols) * n * sizeof(double), s));
   build_mix_covariance(spec, gp.dX.p, gp.N, w.P.p, nc * num, w.dPs.p, gs, w.V.p, s);
-  trsm_lower(gp.dK.p, n, w.V.p, n, static_cast<int>(nrhs), false, s);
+  // the blocked kernel whatever the column count, so a set's solve does not depend on how many sets share its chunk
+  trsm_lower_blocked(gp.dK.p, n, w.V.p, n, nc * Q, false, s);
   posterior_mean_points(gp, w.P.p, static_cast<size_t>(nc) * num, w.dPs.p, gs, w.mu.p, nullptr, s);
   const int t = (Q + NB - 1) / NB;
   const size_t smem_cov = (2 * static_cast<size_t>(NB) * LDT + 2 * static_cast<size_t>(NB) * spec.dim) * sizeof(double);
@@ -427,7 +398,7 @@ void sample_chunk(const cmoe_gp& gp, SampleWork& w, int nc, int num, int gs, uin
                                  static_cast<int>(smem_rows)));
   sample_rows_kernel<<<dim3(rb, nc), kRowThreads, smem_rows, s>>>(Q, 1 + gs, w.mu.p, w.A.p, seed, draw0, dtable, w.y.p,
                                                                   w.part_v.p, w.part_i.p);
-  argmin_kernel<<<(nc + 127) / 128, 128, 0, s>>>(nc, rb, w.part_v.p, w.part_i.p, w.amin.p);
+  best_of_parts_kernel<false><<<(nc + 127) / 128, 128, 0, s>>>(nc, rb, w.part_v.p, w.part_i.p, w.amin.p, nullptr);
   count_launch(2);
   CMOE_CUDA(cudaGetLastError());
 }
@@ -443,15 +414,12 @@ void run_sampling(const cmoe_gp& gp, int num_sets, int num, const int* derivs_s,
   const size_t per_set = sizeof(double) * (static_cast<size_t>(n) * Q + static_cast<size_t>(Q) * Q + 3 * Q +
                                            static_cast<size_t>(num) * dim) +
                          sizeof(double) * static_cast<size_t>((Q + NB - 1) / NB) * NB * NB + sizeof(int) * 2;
-  const int chunk = static_cast<int>(
-      std::max<size_t>(1, std::min<size_t>({kSampleWorkspaceBytes / per_set, static_cast<size_t>(num_sets),
-                                            static_cast<size_t>(kMaxChunkSets)})));
+  const int chunk = static_cast<int>(chunk_items(num_sets, kSampleWorkspaceBytes, per_set, kMaxChunkSets));
   const size_t cq = static_cast<size_t>(chunk) * Q;
   const int rb = (Q + kRowThreads - 1) / kRowThreads;
-  if (!gp.sample_ws) gp.sample_ws = std::make_shared<SampleWork>();
-  SampleWork& w = *static_cast<SampleWork*>(gp.sample_ws.get());
+  SampleWork& w = sample_work(gp);
   w.P.ensure(static_cast<size_t>(chunk) * num * dim);
-  w.V.ensure(std::max<size_t>(cq, 5) * n);
+  w.V.ensure(cq * n);
   w.A.ensure(cq * Q);
   w.mu.ensure(cq);
   w.y.ensure(cq);

@@ -29,7 +29,7 @@ SHAPES = [(20, 2, 0), (150, 2, 2), (500, 8, 0)]
 FS, PS, GS = [256, 1000, 4096], [16, 200, 1024], [1000, 10000, 100000]
 STAGES = {"design": ("rff_features_kernel", "rff_design_kernel"), "gram": ("rff_gram_kernel",),
           "factor": ("chol_panel_kernel", "chol_update_kernel", "chol_diag_writeback_kernel"),
-          "theta": ("rff_theta_kernel",), "grid": ("rff_grid_kernel", "rff_argmin_kernel"), "opt": ("rff_opt_kernel",)}
+          "theta": ("rff_theta_kernel",), "grid": ("rff_grid_kernel", "best_of_parts_kernel"), "opt": ("rff_opt_kernel",)}
 
 
 def card():

@@ -12,7 +12,7 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BUILD = os.path.join(ROOT, "cornell-moe_b200", "build")
 LOG = os.path.join(BUILD, "rff.ptxas.log")
-NO_LOCAL = ("rff_design_kernel", "rff_gram_kernel", "rff_theta_kernel", "rff_grid_kernel", "rff_argmin_kernel",
+NO_LOCAL = ("rff_design_kernel", "rff_gram_kernel", "rff_theta_kernel", "rff_grid_kernel", "best_of_parts_kernel",
             "rff_opt_kernel")
 
 
