@@ -143,9 +143,9 @@ __device__ __forceinline__ double exp_tab(double t) {
 // (kFastPathRadius), no per-call guard: n = round(t 2048 / ln2) no longer fits the low word for |t| >= 7.3e5, so the
 // exponent k = n >> 11 is taken from both words of the shifted double with one funnel shift (the shift's bias
 // 2^51 >> 11 = 2^40 vanishes mod 2^32); k is exact for |t| < 2^31 ln2 = 1.5e9 and clamped on the integer side like
-// exp_tab's.  Used by the tile rounds of kg_mc_kernel<SE,8,8> where its operands leave room for the table
-// (KgDispatchEntry::mc_big).  Arguments and error as exp_tab's: max relative error 4.0e-16 over [-1000 ln2, 700]
-// (tests/test_gpu_fast_math.py), exp(0) = 1 exactly.
+// exp_tab's.  Used by the union rows of kg_acc_tile_kernel; the tile rows of that kernel and of the BIG build of
+// kg_mc_kernel<SE,8,8> take the same table through exp2k_shifted below.  Arguments and error as exp_tab's: max relative
+// error 4.0e-16 over [-1000 ln2, 700] (tests/test_gpu_fast_math.py), exp(0) = 1 exactly.
 __device__ const double kExp2Table2k[2048] = {
 #include "exp2_table2048.inc"
 };
@@ -154,26 +154,66 @@ __device__ __forceinline__ void exp_table2k_stage() {
   for (int i = threadIdx.x; i < 2048; i += blockDim.x) g_exp_tab2k[i] = kExp2Table2k[i];
   __syncthreads();
 }
+constexpr double kExp2kShift = 6755399441055744.0;  // 1.5 2^52: t + kExp2kShift rounds t to an integer in the low bits
+constexpr double kKappa = 2048.0 * 1.4426950408889634;  // 2048 log2(e): natural units -> 2048ths of a binary exponent
+// exponent n (of 2^(n/2048)) from the shifted double nfs = n + 1.5 2^52: table index from the low word, k = n >> 11 from
+// both words with one funnel shift, clamped on the integer side
+__device__ __forceinline__ int exp2k_index(double nfs) { return __double2loint(nfs) & 2047; }
+__device__ __forceinline__ int exp2k_exponent(double nfs) {
+  const unsigned lo = static_cast<unsigned>(__double2loint(nfs)), hi = static_cast<unsigned>(__double2hiint(nfs));
+  return max(static_cast<int>(__funnelshift_r(lo, hi, 11)), -1000);
+}
+// 2^(n/2048) (1 + c1 r + c2 r^2 + c3 r^3): the polynomial, the table multiply and the exponent patch of the 2048-entry
+// exps
+__device__ __forceinline__ double exp2k_tail(double r, double c1, double c2, double c3, double nfs) {
+  double p = c3;
+  p = fma(p, r, c2);
+  p = fma(p, r, c1);
+  p = fma(p, r, 1.0);
+  p *= g_exp_tab2k[exp2k_index(nfs)];
+  return __hiloint2double(__double2hiint(p) + (exp2k_exponent(nfs) << 20), __double2loint(p));
+}
+__device__ __forceinline__ double exp_tab2k_round(double t) { return fma(t, kKappa, kExp2kShift); }
 __device__ __forceinline__ double exp_tab2k(double t) {
-  const double kShift = 6755399441055744.0;
-  double nf = fma(t, 2048.0 * 1.4426950408889634, kShift);
-  const int lo = __double2loint(nf), hi = __double2hiint(nf);
-  nf -= kShift;
+  const double nfs = exp_tab2k_round(t);
+  const double nf = nfs - kExp2kShift;
   double r = fma(nf, -6.93147180369123816490e-01 / 2048.0, t);
   r = fma(nf, -1.90821492927058770002e-10 / 2048.0, r);
-  double p = 1.6666666666666666e-01;
-  p = fma(p, r, 0.5);
-  p = fma(p, r, 1.0);
-  p = fma(p, r, 1.0);
-  p *= g_exp_tab2k[lo & 2047];
-  const int k = max(static_cast<int>(__funnelshift_r(static_cast<unsigned>(lo), static_cast<unsigned>(hi), 11)), -1000);
-  return __hiloint2double(__double2hiint(p) + (k << 20), __double2loint(p));
+  return exp2k_tail(r, 1.0, 0.5, 1.6666666666666666e-01, nfs);
 }
-// the exp of the tile rounds: exp_tab2k where the kernel staged the 2048-entry table (BIG), else exp_tab
+// 2^((t + H) / 2048) for an integer H, |H| < 2^51, passed as the rounding constant C = 1.5 2^52 + H (exp2k_split): the
+// same table, polynomial and exponent patch as exp_tab2k, with the argument already in 2048ths of a binary exponent
+// (t = kKappa x the natural one).  nfs = t + C rounds t + H to the integer n in the low bits; m = nfs - C = n - H and
+// r = t - m (|r| <= 1/2) are exact, so there is no Cody-Waite pair: 7 FP64-pipe instructions.  Arguments: t + H down to
+// kKappa x the range contract of exp_tab2k (|t + H| < 2^31 x 2048 keeps k exact); t alone may be anything below 2^51.
+// Max relative error 4.0e-16 (exp_tab2k's bound) over t + H in kKappa x [-1000 ln2, 700], against 2^((t + H) / 2048)
+// (tests/test_gpu_fast_math_exp2k.py), exactly 1 at t = 0, H = 0.  Relative to exp((t + H) / kKappa) the result carries
+// the rounding of kKappa (1.4e-17 relative) times |t + H| / kKappa: an argument error of the order of rounding the
+// argument itself.
+constexpr double kExp2kC1 = 6.93147180559945309417e-01 / 2048.0;  // (ln2 / 2048)^k / k!
+constexpr double kExp2kC2 = kExp2kC1 * kExp2kC1 / 2.0;
+constexpr double kExp2kC3 = kExp2kC1 * kExp2kC1 * kExp2kC1 / 6.0;
+__device__ __forceinline__ double exp2k_shifted(double t, double C) {
+  const double nfs = t + C;
+  const double r = t - (nfs - C);
+  return exp2k_tail(r, kExp2kC1, kExp2kC2, kExp2kC3, nfs);
+}
+// A per-sample exponent term h (natural units) as exp2k_shifted's rounding constant C = 1.5 2^52 + rint(kKappa h) and the
+// factor f = 2^((kKappa h - rint(kKappa h)) / 2048) that the rounding leaves, |kKappa h - rint| <= 1/2 (exact):
+// exp2k_shifted(kKappa t, C) f = exp(t + h), and no partial exponent can overflow.
+__device__ __forceinline__ void exp2k_split(double h, double& C, double& f) {
+  const double H = kKappa * h, Hi = rint(H);
+  C = kExp2kShift + Hi;
+  const double r = H - Hi;
+  f = fma(fma(fma(kExp2kC3, r, kExp2kC2), r, kExp2kC1), r, 1.0);
+}
+// The exp of the tile rounds, exp(t + h) for a row's exponent t and a sample's h (hs: the sample's term as the tile
+// rounds pass it).  BIG (the kernel staged the 2048-entry table): t comes from kKappa-scaled operands and hs is
+// exp2k_split's rounding constant, and the caller applies the split's factor f to its sums; else exp_tab(t + h).
 template <bool BIG>
-__device__ __forceinline__ double exp_row(double t) {
-  if (BIG) return exp_tab2k(t);
-  return exp_tab(t);
+__device__ __forceinline__ double exp_row(double t, double hs) {
+  if (BIG) return exp2k_shifted(t, hs);
+  return exp_tab(t + hs);
 }
 template <bool TAB>
 __device__ __forceinline__ double exp_sel(double t) {
@@ -383,12 +423,15 @@ __device__ __forceinline__ void tile_posterior(const double* __restrict__ Xt, co
   constexpr int KD = (DIM + 3) / 4, KQ = (QP + 3) / 4, ND = (DIM + 7) / 8;
   const int lane = threadIdx.x & 31, g = lane >> 2;
   double xa[2][KD][2], ca[2][KQ][2], hqr[2][2];
+  // BIG: exponents in kKappa units (e_j staged scaled, x~ scaled here); hq enters as exp2k_split's (C, f)
+  double hs = hq, f = 1.0;
+  if (BIG) exp2k_split(hq, hs, f);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    tile_frag<DIM, false>(xq, nullptr, h, xa[h]);
+    tile_frag<DIM, false, BIG>(xq, nullptr, h, xa[h], kKappa, kKappa);
     // a = beta + (-c) . B: the negation is exact, each product is the scalar one
     tile_frag<QP, true>(c, nullptr, h, ca[h]);
-    tile_rows(hq, h, hqr[h][0], hqr[h][1]);
+    tile_rows(hs, h, hqr[h][0], hqr[h][1]);
   }
   double s0[2][2], sacc[2][ND][4];
 #pragma unroll
@@ -420,7 +463,7 @@ __device__ __forceinline__ void tile_posterior(const double* __restrict__ Xt, co
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const double ai = ((i & 1) ? r.v1 : r.v0) ? a[i] : 0.0;
-        const double kv = exp_row<BIG>(dot[i] + hqr[h][i >> 1]);
+        const double kv = exp_row<BIG>(dot[i], hqr[h][i >> 1]);
         s0[h][i >> 1] = fma(ai, kv, s0[h][i >> 1]);
         w[i] = ai * kv;
       }
@@ -449,6 +492,12 @@ __device__ __forceinline__ void tile_posterior(const double* __restrict__ Xt, co
       v[h] = (lane & 8) ? vh : vl;
     }
     s[d] = (lane >> 4) ? v[1] : v[0];
+  }
+  if (BIG) {
+    // the factor exp2k_split left out of every kv of this lane (before eval_posterior adds the union rows)
+    S0 *= f;
+#pragma unroll
+    for (int d = 0; d < DIM; ++d) s[d] *= f;
   }
 }
 
@@ -547,14 +596,19 @@ __device__ __forceinline__ void tile_line(const double* __restrict__ Xt, const d
                                           double alpha_min, const double (&c)[QP], double hq, double xga,
                                           double (&S)[kLineBatch], int& pmax_hi) {
   constexpr int KD = (DIM + 3) / 4, KQ = (QP + 3) / 4, KB = kLineBatch;
+  // BIG: exponents and slopes in kKappa units (e_j staged scaled; x~, a_min and xga scaled here, so p_j and pmax_hi
+  // are kKappa a_min p_j); hq enters as exp2k_split's (C, f)
+  double hs = hq, f = 1.0;
+  if (BIG) exp2k_split(hq, hs, f);
+  const double am = BIG ? kKappa * alpha_min : alpha_min, xgs = BIG ? kKappa * xga : xga;
 #pragma unroll 1
   for (int h = 0; h < 2; ++h) {
     double xa[KD][2], gf[KD][2], ca[KQ][2];
     double hq0, hq1, xg0, xg1, am0, am1;
-    tile_rows(hq, h, hq0, hq1);
-    tile_rows(xga, h, xg0, xg1);
-    tile_rows(alpha_min, h, am0, am1);
-    tile_frag<DIM, false>(xr, inv_len, h, xa);
+    tile_rows(hs, h, hq0, hq1);
+    tile_rows(xgs, h, xg0, xg1);
+    tile_rows(am, h, am0, am1);
+    tile_frag<DIM, false, BIG>(xr, inv_len, h, xa, kKappa, kKappa);
     tile_frag<DIM, false, true>(gr, inv_len, h, gf, am0, am1);
     tile_frag<QP, true>(c, nullptr, h, ca);
     double Sp[2][KB];
@@ -578,8 +632,8 @@ __device__ __forceinline__ void tile_line(const double* __restrict__ Xt, const d
         const bool v = (i & 1) ? r.v1 : r.v0;
         const double pj = v ? p[i] : 0.0;
         pm[i >> 1] = max(pm[i >> 1], __double2hiint(pj) & 0x7fffffff);
-        const double w = (v ? a[i] : 0.0) * exp_row<BIG>(dot[i] + ((i < 2) ? hq0 : hq1));
-        double G = exp_row<BIG>(pj);
+        const double w = (v ? a[i] : 0.0) * exp_row<BIG>(dot[i], (i < 2) ? hq0 : hq1);
+        double G = BIG ? exp2k_shifted(pj, kExp2kShift) : exp_tab(pj);
 #pragma unroll
         for (int k = KB - 1; k >= 0; --k) {
           Sp[i >> 1][k] = fma(w, G, Sp[i >> 1][k]);
@@ -591,8 +645,14 @@ __device__ __forceinline__ void tile_line(const double* __restrict__ Xt, const d
 #pragma unroll 1
     for (int j0 = 0; j0 < nfull; j0 += 8) block(j0, std::false_type());
     if (nfull < N) block(nfull, std::true_type());
+    if (BIG) {
+      // the owner's factor exp2k_split left out of its w's, applied before the sums join the union rows' (natural)
 #pragma unroll
-    for (int k = 0; k < KB; ++k) S[k] = tile_to_owner<true>(quad_sum(Sp[0][k]), quad_sum(Sp[1][k]), h, S[k]);
+      for (int k = 0; k < KB; ++k) S[k] = fma(f, tile_to_owner(quad_sum(Sp[0][k]), quad_sum(Sp[1][k]), h, 0.0), S[k]);
+    } else {
+#pragma unroll
+      for (int k = 0; k < KB; ++k) S[k] = tile_to_owner<true>(quad_sum(Sp[0][k]), quad_sum(Sp[1][k]), h, S[k]);
+    }
 #pragma unroll
     for (int m = 1; m < 4; m <<= 1) {
       pm[0] = max(pm[0], __shfl_xor_sync(0xffffffffu, pm[0], m));
@@ -668,7 +728,8 @@ __device__ __forceinline__ void eval_line(const double* __restrict__ Xt, const d
 #pragma unroll
     for (int v = 0; v < QP; ++v)
       if (v == u) cu = c[v];
-    pmax_hi = max(pmax_hi, __double2hiint(pj) & 0x7fffffff);
+    // BIG: pmax_hi is kept in the tile rows' kKappa units
+    pmax_hi = max(pmax_hi, __double2hiint(BIG ? kKappa * pj : pj) & 0x7fffffff);
     const double w = cu * exp_sel<SMEM>(dot + (h.x + hq));
     double G = exp_sel<SMEM>(pj);
 #pragma unroll
@@ -1394,11 +1455,12 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
       if (state == ST_LINE) {
         n_line += 1;
         // safe iff a_0 |p_j| = 2^(KB-1) |a_min p_j| < 512 for every row: every factor exp(a_k p_j) stays in range
+        // (BIG: pmax_hi in kKappa units, so is the bound; the high word of the bound is at most the bound)
         if (!TILE) {
 #pragma unroll
           for (int d = 0; d < DIM; ++d) nb2 = fma(xt[d], xt[d], nb2);
         }
-        if (pmax_hi >= __double2hiint(512.0 / kTop) || !(nb2 <= kFarRadius * kFarRadius)) {
+        if (pmax_hi >= __double2hiint((BIG ? kKappa : 1.0) * 512.0 / kTop) || !(nb2 <= kFarRadius * kFarRadius)) {
           state = ST_TRIAL;  // factors could leave the double range: this step backtracks one evaluation at a time
         } else {
           int kacc = -1;
@@ -1585,7 +1647,8 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
   }
 }
 
-// BIG: the tile rounds use exp_tab2k, whose 2048-entry table takes 16 KB of static shared memory next to the operands.
+// BIG: the tile rounds use exp2k_shifted, whose 2048-entry table takes 16 KB of static shared memory next to the
+// operands, with their exponents in kKappa units.
 // Only the tile instantiation has a BIG build.  The host launches it on the shared-memory path only, where it does not
 // lower the residency (cmoe_kg_plan_create), so the BIG build has no global-memory branch.
 template <int KERNEL, int DIM, int QP, bool BIG = false>
@@ -1621,6 +1684,12 @@ __global__ void __launch_bounds__(kMcThreads, (kg_mc_min_blocks<KERNEL, DIM, QP>
       tma_bulk_g2s(sXu, gXu, bU, &mbar);
     }
     mbar_wait(&mbar, 0);
+    if (BIG) {
+      // the tile rounds' exponents are in kKappa units (exp2k_shifted); tile_posterior and tile_line are the only
+      // readers of e_j in this build (the union rows' e_u stay natural)
+      for (int j = threadIdx.x; j < N; j += blockDim.x) sPk[j * (QP + 2)] *= kKappa;
+      __syncthreads();
+    }
     kg_mc_body<KERNEL, DIM, QP, true, false, false, BIG>(prm, sXt, sPk, sXu, cand, s_begin, s_end, &next_sample);
   } else {
     __syncthreads();
@@ -1691,6 +1760,7 @@ constexpr int kAccTile = 64;  // samples per shared-memory tile of the accumulat
 // Streams candidate `cand`'s sample records (minimiser, c, -|x*|^2/2) through shared memory in double-buffered tiles
 // of kAccTile samples (LDGSTS, 16-byte chunks) and calls body(sx, sc, sh, cnt) once per tile, in sample order:
 // sx = [kAccTile][DIM], sc = [kAccTile][QP], sh = [kAccTile], cnt = valid samples.  Slots past num_mc are zero-filled.
+// The body may rewrite the tile in place (kg_acc_tile_rows), behind a barrier of its own.
 // sbuf: 2 * kAccTile * (DIM + QP + 1) doubles.  Every thread of the CTA must call it.
 template <int DIM, int QP, typename F>
 __device__ __forceinline__ void acc_stream_samples(const KgAccParams& prm, int cand, double* __restrict__ sbuf,
@@ -1728,8 +1798,8 @@ __device__ __forceinline__ void acc_stream_samples(const KgAccParams& prm, int c
     cp_async_commit();
     cp_async_wait<1>();
     __syncthreads();
-    const double* sx = sbuf + buf * kBuf;
-    const double* sc = sx + TS * DIM;
+    double* sx = sbuf + buf * kBuf;
+    double* sc = sx + TS * DIM;
     body(sx, sc, sc + TS * QP, min(TS, num_mc - tile * TS));
     __syncthreads();  // the buffer is refilled two tiles later
   }
@@ -1850,8 +1920,9 @@ __global__ void __launch_bounds__(128) kg_acc_kernel(const __grid_constant__ KgA
 // ---------------------------------------------------------------------------------------------------------------
 // Tile accumulation of the training rows (kg_tile_path instantiation, shared-memory fast path; DESIGN.md K6).
 //   R^T[row][a] = sum_i exp(X~_row . x~*_i + e_row + h_i) c_ia ,   e_row = ln(alpha) - |X~_row|^2 / 2,  h_i = -|x~*_i|^2/2
-// is two FP64 DMMA m16n8k4 products per 16 rows x 8 samples: the exponents (M = 16 rows, N = 8 samples, K = DIM,
-// accumulator seeded with e_row + h_i) and, after the element-wise exp, R^T += KV C (K = the 8 samples, N = QP).  The
+// is two FP64 DMMA m16n8k4 products per 16 rows x 8 samples: the exponents in kKappa units (M = 16 rows, N = 8 samples,
+// K = DIM, A = kKappa X~, accumulator seeded with kKappa e_row; h_i enters the element-wise exp2k_shifted as its
+// rounding constant, the factor exp2k_split leaves goes into c_i) and R^T += KV C (K = the 8 samples, N = QP).  The
 // second product takes KV's accumulator layout as its A operand, k-step 0 = the even columns, k-step 1 = the odd ones.
 // Column n of a sample group s0 is sample s0 + (n >> 1) + 4 (n & 1), so that lane (g, t) holds samples s0 + t and
 // s0 + t + 4, and its C operands c[s0 + t][g], c[s0 + t + 4][g] are two conflict-free LDS.  The K order of the exponent
@@ -1890,13 +1961,23 @@ __device__ __forceinline__ void kg_acc_tile_rows(const KgAccParams& prm, double*
       double nrm = 0.0;
 #pragma unroll
       for (int d = 0; d < DIM; ++d) nrm = fma(x[d], x[d], nrm);
-      e[k][h] = lna - 0.5 * nrm;
-      xa[k][0][h] = x[2 * t];
-      xa[k][1][h] = x[2 * t + 1];
+      // the exponents in kKappa units (exp2k_shifted)
+      e[k][h] = kKappa * (lna - 0.5 * nrm);
+      xa[k][0][h] = kKappa * x[2 * t];
+      xa[k][1][h] = kKappa * x[2 * t + 1];
     }
     acc[k][0] = acc[k][1] = acc[k][2] = acc[k][3] = 0.0;
   }
-  acc_stream_samples<DIM, QP>(prm, cand, sbuf, [&](const double* sx, const double* sc, const double* sh, int cnt) {
+  acc_stream_samples<DIM, QP>(prm, cand, sbuf, [&](const double* sx, double* sc, double* sh, int cnt) {
+    // once per sample and CTA: h_i becomes exp2k_split's rounding constant C_i, and its factor f_i goes into c_i (every
+    // slot, so that the zero-filled ones past num_mc get a finite exponent)
+    for (int i = threadIdx.x; i < kAccTile; i += blockDim.x) {
+      double f;
+      exp2k_split(sh[i], sh[i], f);
+#pragma unroll
+      for (int a = 0; a < QP; ++a) sc[i * QP + a] *= f;
+    }
+    __syncthreads();
 #pragma unroll 1
     for (int s0 = 0; s0 < cnt; s0 += 8) {
       const double2 xb = *reinterpret_cast<const double2*>(sx + (s0 + (g >> 1) + 4 * (g & 1)) * DIM + 2 * t);
@@ -1904,10 +1985,12 @@ __device__ __forceinline__ void kg_acc_tile_rows(const KgAccParams& prm, double*
       const double c0 = sc[(s0 + t) * QP + g], c1 = sc[(s0 + t + 4) * QP + g];
 #pragma unroll
       for (int k = 0; k < T; ++k) {
-        double kv[4] = {e[k][0] + h0, e[k][0] + h1, e[k][1] + h0, e[k][1] + h1};
+        double kv[4] = {e[k][0], e[k][0], e[k][1], e[k][1]};
         dmma_m16n8k8(kv[0], kv[1], kv[2], kv[3], xa[k][0][0], xa[k][0][1], xa[k][1][0], xa[k][1][1], xb.x, xb.y);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) kv[i] = exp_tab2k(kv[i]);
+        kv[0] = exp2k_shifted(kv[0], h0);
+        kv[1] = exp2k_shifted(kv[1], h1);
+        kv[2] = exp2k_shifted(kv[2], h0);
+        kv[3] = exp2k_shifted(kv[3], h1);
         dmma_m16n8k8(acc[k][0], acc[k][1], acc[k][2], acc[k][3], kv[0], kv[2], kv[1], kv[3], c0, c1);
       }
     }

@@ -4,7 +4,8 @@
 //
 //   int cmoe_probe_eval(int routine, const double* in, long long n, double* out, int device)
 //
-// in and out are host arrays: in holds n arguments (n (p, a) pairs for the pivot step), out receives n results of
+// in and out are host arrays: in holds n arguments (n (p, a) pairs for the pivot step, n (t, H) pairs for
+// exp2k_shifted), out receives n results of
 // kProbeOut[routine] doubles each (see ProbeRoutine).  Returns 0, or -1 for an unknown routine / bad size, or the
 // cudaError_t of the first CUDA call that failed.
 #include <cuda_runtime.h>
@@ -23,10 +24,12 @@ enum ProbeRoutine {
   kSincos = 4,      // rff_sincos(a)                               -> (sin, cos)
   kSqrtRsqrt = 5,   // sqrt_rsqrt(p)                               -> (l, y)
   kPivotFast = 6,   // chol_pivot_fast(p, a), chol_pivot_recip     -> (l, q, 1/l)
-  kNumRoutines = 7,
+  kExp2kShifted = 7,  // exp2k_shifted(t, 1.5 2^52 + H), table staged -> (value, n, k) of its shifted double
+  kExpTab2kNk = 8,    // exp_tab2k's shifted double of t               -> (n, k)
+  kNumRoutines = 9,
 };
-constexpr int kProbeIn[kNumRoutines] = {1, 1, 1, 1, 1, 1, 2};
-constexpr int kProbeOut[kNumRoutines] = {1, 1, 1, 1, 2, 2, 3};
+constexpr int kProbeIn[kNumRoutines] = {1, 1, 1, 1, 1, 1, 2, 2, 1};
+constexpr int kProbeOut[kNumRoutines] = {1, 1, 1, 1, 2, 2, 3, 3, 2};
 constexpr int kProbeThreads = 256;
 // cov.cu's kCovExp2Table (it lives in that translation unit only), from the same file
 __device__ const double kCovExp2Table[64] = {
@@ -38,7 +41,7 @@ __global__ void __launch_bounds__(kProbeThreads) probe_kernel(int routine, const
   __shared__ double cov_tab[64];
   // staging: block-uniform, every thread reaches the barriers
   if (routine == kExpTab) cmoe::exp_table_stage();
-  if (routine == kExpTab2k) cmoe::exp_table2k_stage();
+  if (routine == kExpTab2k || routine == kExp2kShifted) cmoe::exp_table2k_stage();
   if (routine == kExpTabCov) {
     if (threadIdx.x < 64) cov_tab[threadIdx.x] = kCovExp2Table[threadIdx.x];
     __syncthreads();
@@ -56,6 +59,20 @@ __global__ void __launch_bounds__(kProbeThreads) probe_kernel(int routine, const
       cmoe::chol_pivot_fast(in[2 * i], in[2 * i + 1], out[3 * i], out[3 * i + 1]);
       out[3 * i + 2] = cmoe::chol_pivot_recip(in[2 * i], out[3 * i]);
       break;
+    case kExp2kShifted: {
+      // n = round(t + H) (its low word) and k = n >> 11, clamped, as exp2k_shifted forms them
+      const double t = in[2 * i], C = cmoe::kExp2kShift + in[2 * i + 1], nfs = t + C;
+      out[3 * i] = cmoe::exp2k_shifted(t, C);
+      out[3 * i + 1] = __double2loint(nfs);
+      out[3 * i + 2] = cmoe::exp2k_exponent(nfs);
+      break;
+    }
+    case kExpTab2kNk: {
+      const double nfs = cmoe::exp_tab2k_round(in[i]);
+      out[2 * i] = __double2loint(nfs);
+      out[2 * i + 1] = cmoe::exp2k_exponent(nfs);
+      break;
+    }
     default: break;
   }
 }
