@@ -298,6 +298,21 @@ constexpr bool kg_tile_path() {
   return KERNEL == CMOE_KERNEL_SQUARE_EXPONENTIAL && DIM == 8 && QP == 8;
 }
 
+// Trial step sizes per LINE batch of the SquareExponential kernel (eval_line, eval_line_gen).  Each trial costs one
+// squaring and one accumulating FMA per row, and a step whose accepted trial lies past the batch costs its lane a
+// second LINE round (and, out of phase with its warp, an idle POINT round).  The scalar row loops and the d-KG path
+// keep 8.  The tile rounds of <SE,8,8>, where the chain is half of a LINE row's FP64 instructions, take 6: at the
+// bench shape no step accepted a trial past index 5 (the accepted-trial histogram in DESIGN.md K6).
+constexpr int kLineBatch = 8;
+#ifndef CMOE_LINE_BATCH_TILE
+#define CMOE_LINE_BATCH_TILE 6
+#endif
+template <int KERNEL, int DIM, int QP>
+constexpr int kg_line_batch() {
+  return kg_tile_path<KERNEL, DIM, QP>() ? CMOE_LINE_BATCH_TILE : kLineBatch;
+}
+static_assert(CMOE_LINE_BATCH_TILE >= 1 && CMOE_LINE_BATCH_TILE <= kLineBatch, "1 <= tile LINE batch <= kLineBatch");
+
 // CTAs of kMcThreads per SM that kg_mc_kernel's launch bounds ask for.  The tile instantiation takes 2, so that it gets
 // up to 255 registers (it uses 240 and spills nothing; the 168 that 3 CTAs leave spilled its round-level state).  Its
 // operands (72.6 KB at N = 500) leave room for 2 CTAs.  Every other instantiation keeps 3 CTAs (168 registers).
@@ -582,20 +597,20 @@ __device__ __forceinline__ void eval_posterior(const double* __restrict__ Xt, co
 // two exps per training point give all KB trial values by repeated squaring (1 mul + 1 fma per trial) instead of one
 // full evaluation (dot + weights + exp) per trial.  S[k] = sum_j a_j k(x, X_j) exp(a_k p_j) for a_k = a_min 2^(KB-1-k'),
 // returned in trial order (S[0] <-> largest step); pmax_hi (high word of max_j |a_min p_j|) lets the caller reject
-// batches whose factors could leave the double range (it then falls back to one-at-a-time evaluations).
-constexpr int kLineBatch = 8;  // trial step sizes per batch (6 measured +1.5 %, but a second batch costs a whole pass)
+// batches whose factors could leave the double range (it then falls back to one-at-a-time evaluations).  KB is the
+// instantiation's kg_line_batch.
 
 // LINE round (SquareExponential) over the training rows, added to S[k] and pmax_hi as eval_line computes them.  The
 // lanes' operands come from their unscaled state: base point xr, gradient gr (x~ = xr / l, a_min g~ = a_min (gr / l)),
 // with hq = -|x~|^2 / 2 and xga = -a_min x~ . g~.  Unlike tile_posterior, the halves sweep the rows one after the other:
 // one sweep for both (twice the 16 trial sums and the fragments live) measured slower on the H100, by 1.8 % per bench
 // step even with the lane state parked in shared memory to keep it from spilling (DESIGN.md K6).
-template <int DIM, int QP, bool BIG>
+template <int DIM, int QP, int KB, bool BIG>
 __device__ __forceinline__ void tile_line(const double* __restrict__ Xt, const double* __restrict__ Pk, int N,
                                           const double (&xr)[DIM], const double (&gr)[DIM], const double* inv_len,
                                           double alpha_min, const double (&c)[QP], double hq, double xga,
-                                          double (&S)[kLineBatch], int& pmax_hi) {
-  constexpr int KD = (DIM + 3) / 4, KQ = (QP + 3) / 4, KB = kLineBatch;
+                                          double (&S)[KB], int& pmax_hi) {
+  constexpr int KD = (DIM + 3) / 4, KQ = (QP + 3) / 4;
   // BIG: exponents and slopes in kKappa units (e_j staged scaled; x~, a_min and xga scaled here, so p_j and pmax_hi
   // are kKappa a_min p_j); hq enters as exp2k_split's (C, f)
   double hs = hq, f = 1.0;
@@ -664,11 +679,11 @@ __device__ __forceinline__ void tile_line(const double* __restrict__ Xt, const d
   }
 }
 
-template <int DIM, int QP, bool SMEM, bool TILE = false, bool BIG = false>
+template <int DIM, int QP, int KB, bool SMEM, bool TILE = false, bool BIG = false>
 __device__ __forceinline__ void eval_line(const double* __restrict__ Xt, const double* __restrict__ Pk,
                                           const double* __restrict__ Xu, int N, int U, const double (&xb)[DIM],
                                           const double (&gt)[DIM], const double (&c)[QP], double alpha_min,
-                                          double (&S)[kLineBatch], int& pmax_hi, const double (&xr)[DIM],
+                                          double (&S)[KB], int& pmax_hi, const double (&xr)[DIM],
                                           const double (&gr)[DIM], const double* inv_len) {
   double nq = 0.0, xg = 0.0;
 #pragma unroll
@@ -682,7 +697,7 @@ __device__ __forceinline__ void eval_line(const double* __restrict__ Xt, const d
   for (int d = 0; d < DIM; ++d) ga[d] = alpha_min * gt[d];
   const double xga = -alpha_min * xg;
 #pragma unroll
-  for (int k = 0; k < kLineBatch; ++k) S[k] = 0.0;
+  for (int k = 0; k < KB; ++k) S[k] = 0.0;
   pmax_hi = 0;  // max over rows of the high word of |a_min p_j| (integer ALU; monotone in |p|, NaN/inf sort last)
 #pragma unroll 2
   for (int j = 0; j < (TILE ? 0 : N); ++j) {
@@ -703,7 +718,7 @@ __device__ __forceinline__ void eval_line(const double* __restrict__ Xt, const d
     const double w = a * exp_sel<SMEM>(dot + (h.x + hq));
     double G = exp_sel<SMEM>(pj);
 #pragma unroll
-    for (int k = kLineBatch - 1; k >= 0; --k) {
+    for (int k = KB - 1; k >= 0; --k) {
       S[k] = fma(w, G, S[k]);
       if (k > 0) G *= G;
     }
@@ -733,13 +748,13 @@ __device__ __forceinline__ void eval_line(const double* __restrict__ Xt, const d
     const double w = cu * exp_sel<SMEM>(dot + (h.x + hq));
     double G = exp_sel<SMEM>(pj);
 #pragma unroll
-    for (int k = kLineBatch - 1; k >= 0; --k) {
+    for (int k = KB - 1; k >= 0; --k) {
       S[k] = fma(w, G, S[k]);
       if (k > 0) G *= G;
     }
   }
   // tile path: the training rows last, so that the scaled operands above are dead during the row loop
-  if (TILE) tile_line<DIM, QP, BIG>(Xt, Pk, N, xr, gr, inv_len, alpha_min, c, hq, xga, S, pmax_hi);
+  if (TILE) tile_line<DIM, QP, KB, BIG>(Xt, Pk, N, xr, gr, inv_len, alpha_min, c, hq, xga, S, pmax_hi);
 }
 
 // Batched backtracking for the Matern-5/2 kernel.  No factorisation along the line here, but the trial points
@@ -1304,6 +1319,30 @@ __device__ __forceinline__ void start_from_table(const KgMcParams& prm, const do
 
 enum : int { ST_FETCH = 0, ST_INIT = 1, ST_TRIAL = 2, ST_LIMIT = 3, ST_DONE = 4, ST_LINE = 5 };
 
+#ifdef CMOE_KG_TRIAL_HIST
+// Probe build only (profiles/build_variants.sh, read by profiles/kg_trial_hist_probe.py; one translation unit per
+// library): how the LINE batches of kg_mc_body end.  Bins [step][index] count accepted trials by the inner step index
+// (capped) and the trial index counted from a_0 (search + k); then batches run, batches with no passing trial, range
+// fallbacks to ST_TRIAL, warp rounds, warp rounds whose vote left lanes idle, and idle lanes summed over those rounds.
+constexpr int kHistSteps = 16, kHistTrials = 32;
+enum : int {
+  H_BATCHES = kHistSteps * kHistTrials, H_ALL_FAIL, H_RANGE, H_ROUNDS, H_IDLE_ROUNDS, H_IDLE_LANES, kHistSize
+};
+__device__ unsigned long long kg_trial_hist[kHistSize];
+__device__ __forceinline__ void hist_add(int i, unsigned v = 1) { atomicAdd(kg_trial_hist + i, v); }
+}  // namespace cmoe
+// copies the kHistSize counters to out and, with reset != 0, zeroes them; returns a cudaError_t
+extern "C" int cmoe_kg_trial_hist(unsigned long long* out, int reset) {
+  cudaError_t e = cudaMemcpyFromSymbol(out, cmoe::kg_trial_hist, sizeof(cmoe::kg_trial_hist));
+  if (e == cudaSuccess && reset) {
+    static const unsigned long long zero[cmoe::kHistSize] = {};
+    e = cudaMemcpyToSymbol(cmoe::kg_trial_hist, zero, sizeof(zero));
+  }
+  return static_cast<int>(e);
+}
+namespace cmoe {
+#endif
+
 
 // The per-lane line-search state machine.  Live across evaluations: c, the base point xb with f and grad f there,
 // the step size and a few counters; the start point of the current restart run is parked in the sample's output slot.
@@ -1322,7 +1361,7 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
                                            const double* __restrict__ Wt = nullptr, double* ring = nullptr) {
   constexpr bool SE = (KERNEL == CMOE_KERNEL_SQUARE_EXPONENTIAL);
   constexpr bool LINE = SE || !GEN;  // Matern-5/2 batches its trials too (eval_line_matern) unless derivative rows exist
-  constexpr int KB = SE ? kLineBatch : kLineBatchM;  // trial step sizes per LINE round
+  constexpr int KB = !SE ? kLineBatchM : GEN ? kLineBatch : kg_line_batch<KERNEL, DIM, QP>();  // trials per LINE round
   constexpr int ST_SEARCH = LINE ? ST_LINE : ST_TRIAL;  // how a step's backtracking starts
   constexpr bool TILE = SMEM && !GEN && kg_tile_path<KERNEL, DIM, QP>();  // DMMA tiles for the training rows
   const int N = prm.N, U = prm.U;
@@ -1422,11 +1461,21 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
       const unsigned wl = __ballot_sync(0xffffffffu, state == ST_LINE);
       const unsigned wp = __ballot_sync(0xffffffffu, state == ST_INIT || state == ST_TRIAL || state == ST_LIMIT);
       line_round = __popc(wl) > __popc(wp);
+#ifdef CMOE_KG_TRIAL_HIST
+      if ((threadIdx.x & 31) == 0 && (wl | wp)) {
+        const int idle = __popc(line_round ? wp : wl);
+        hist_add(H_ROUNDS);
+        if (idle) {
+          hist_add(H_IDLE_ROUNDS);
+          hist_add(H_IDLE_LANES, idle);
+        }
+      }
+#endif
     }
 
     if (LINE && line_round) {
       // ---- all backtracking trials of this step in one pass (warp-uniform) ----
-      double xt[DIM], gt[DIM], S[kLineBatch];
+      double xt[DIM], gt[DIM], S[SE ? KB : kLineBatch];
       int pmax_hi;
       double gg = 0.0;
 #pragma unroll
@@ -1442,26 +1491,34 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
       }
       constexpr double kTop = static_cast<double>(1 << (KB - 1));
       double T[GEN ? kLineBatch : 1];
-      if (!SE) {
+      if constexpr (!SE) {
         pmax_hi = 0;  // no factor can leave the double range on this path
         eval_line_matern<DIM, QP, SMEM>(Xt, Pk, Xu, N, U, prm.alpha, xt, gt, c, alpha_n, S);
-      } else if (GEN) {
+      } else if constexpr (GEN) {
         eval_line_gen<DIM, QP, SMEM, WIDE>(prm, Xt, Pk, Xu, xt, gt, aw, ring, cl, alpha_n * (1.0 / kTop), S,
                                reinterpret_cast<double (&)[kLineBatch]>(T), pmax_hi);
       } else {
-        eval_line<DIM, QP, SMEM, TILE, BIG>(Xt, Pk, Xu, N, U, xt, gt, c, alpha_n * (1.0 / kTop), S, pmax_hi, xb,
-                                             gb, prm.inv_len);
+        eval_line<DIM, QP, KB, SMEM, TILE, BIG>(Xt, Pk, Xu, N, U, xt, gt, c, alpha_n * (1.0 / kTop), S, pmax_hi, xb,
+                                                 gb, prm.inv_len);
       }
       if (state == ST_LINE) {
         n_line += 1;
         // safe iff a_0 |p_j| = 2^(KB-1) |a_min p_j| < 512 for every row: every factor exp(a_k p_j) stays in range
-        // (BIG: pmax_hi in kKappa units, so is the bound; the high word of the bound is at most the bound)
+        // (BIG: pmax_hi in kKappa units, so is the bound; the high word of the bound is at most the bound).  a_min
+        // and the bound 512 / kTop are a_0 and 512 scaled by the same power of two, which moves both high words by the
+        // same exponent step: the test decides a_0 |p_j| < 512 exactly as conservatively whatever KB is.
         if (!TILE) {
 #pragma unroll
           for (int d = 0; d < DIM; ++d) nb2 = fma(xt[d], xt[d], nb2);
         }
+#ifdef CMOE_KG_TRIAL_HIST
+        hist_add(H_BATCHES);
+#endif
         if (pmax_hi >= __double2hiint((BIG ? kKappa : 1.0) * 512.0 / kTop) || !(nb2 <= kFarRadius * kFarRadius)) {
           state = ST_TRIAL;  // factors could leave the double range: this step backtracks one evaluation at a time
+#ifdef CMOE_KG_TRIAL_HIST
+          hist_add(H_RANGE);
+#endif
         } else {
           int kacc = -1;
           double ak = alpha_n, a_acc = alpha_n;
@@ -1477,6 +1534,10 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
             }
             ak *= 0.5;
           }
+#ifdef CMOE_KG_TRIAL_HIST
+          hist_add(kacc < 0 ? H_ALL_FAIL
+                            : min(step_i, kHistSteps - 1) * kHistTrials + min(search + kacc, kHistTrials - 1));
+#endif
           if (kacc >= 0) {
             n_evals += kacc + 1;
             search += kacc;
