@@ -922,7 +922,6 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
       m.lo[d] = -1.0e300;
       m.hi[d] = 1.0e300;
       m.inv_len[d] = (d < dim) ? spec.inv_len[d] : 0.0;
-      m.len[d] = (d < dim) ? 1.0 / spec.inv_len[d] : 0.0;
     }
     for (int d = 0; d < ps; ++d) {  // the frame of A (kg_pack_kernel)
       m.lo[d] = inner_bounds[2 * d] - gp->centre[d];

@@ -85,7 +85,7 @@ struct KgMcParams {
   int chunks;        // work items per candidate
   int work_total;    // chunks * candidates of this launch
   int stage_ops;     // general path: scaled training points and e_j fit next to the ring in shared memory
-  double lo[CMOE_MAX_DIM], hi[CMOE_MAX_DIM], inv_len[CMOE_MAX_DIM], len[CMOE_MAX_DIM];  // lo, hi: minus the centre
+  double lo[CMOE_MAX_DIM], hi[CMOE_MAX_DIM], inv_len[CMOE_MAX_DIM];  // lo, hi: minus the centre
 };
 
 struct KgAccParams {
@@ -121,23 +121,7 @@ __device__ __forceinline__ void exp_table_stage() {
   if (threadIdx.x < 64) g_exp_tab[threadIdx.x] = kExp2Table[threadIdx.x];
   __syncthreads();
 }
-__device__ __forceinline__ double exp_tab(double t) {
-  const double kShift = 6755399441055744.0;
-  double nf = fma(t, 64.0 * 1.4426950408889634, kShift);
-  const int n = __double2loint(nf);
-  nf -= kShift;
-  double r = fma(nf, -6.93147180369123816490e-01 / 64.0, t);
-  r = fma(nf, -1.90821492927058770002e-10 / 64.0, r);
-  double p = 8.3333333333333332e-03;
-  p = fma(p, r, 4.1666666666666664e-02);
-  p = fma(p, r, 1.6666666666666666e-01);
-  p = fma(p, r, 0.5);
-  p = fma(p, r, 1.0);
-  p = fma(p, r, 1.0);
-  p *= g_exp_tab[n & 63];
-  const int k = max(n >> 6, -1000);
-  return __hiloint2double(__double2hiint(p) + (k << 20), __double2loint(p));
-}
+__device__ __forceinline__ double exp_tab(double t) { return exp_tab64(t, g_exp_tab); }
 // exp(t) = 2^k * 2^(i/2048) * e^r with |r| <= ln2/4096: 2048-entry table (16 KB of shared memory) + degree-3 Taylor
 // polynomial (truncation r^4/24 <= 3.4e-17 relative).  8 FP64-pipe instructions.  Same range contract as exp_tab
 // (kFastPathRadius), no per-call guard: n = round(t 2048 / ln2) no longer fits the low word for |t| >= 7.3e5, so the
@@ -251,6 +235,27 @@ template <bool SMEM>
 __device__ __forceinline__ double ld1(const double* p) {
   if (SMEM) return *p;
   return __ldg(p);
+}
+
+// a row's DIM scaled coordinates, as 16-byte pairs
+template <int DIM, bool SMEM>
+__device__ __forceinline__ void load_row(const double* p, double (&xv)[DIM]) {
+#pragma unroll
+  for (int d = 0; d < DIM; d += 2) {
+    const double2 v = ld2<SMEM>(p + d);
+    xv[d] = v.x;
+    xv[d + 1] = v.y;
+  }
+}
+
+// c[u], the weight of union row u, selected with compile-time register indices so that c stays in registers
+template <int QP>
+__device__ __forceinline__ double union_coef(const double (&c)[QP], int u) {
+  double cu = 0.0;
+#pragma unroll
+  for (int v = 0; v < QP; ++v)
+    if (v == u) cu = c[v];
+  return cu;
 }
 
 // x . y and beta - B . c over the staged operands (one dependent DFMA chain each; splitting them into even / odd
@@ -533,52 +538,35 @@ __device__ __forceinline__ void eval_posterior(const double* __restrict__ Xt, co
   for (int d = 0; d < DIM; ++d) s[d] = 0.0;
   static_assert(!TILE || KERNEL == CMOE_KERNEL_SQUARE_EXPONENTIAL, "the tile path is SquareExponential only");
   if (TILE) tile_posterior<DIM, QP, BIG>(Xt, Pk, N, xq, c, hq, S0, s);
-#pragma unroll 2
-  for (int j = 0; j < (TILE ? 0 : N); ++j) {
-    const double* xj = Xt + j * DIM;
-    const double* pk = Pk + j * (QP + 2);
-    double xv[DIM];
-#pragma unroll
-    for (int d = 0; d < DIM; d += 2) {
-      const double2 v = ld2<SMEM>(xj + d);
-      xv[d] = v.x;
-      xv[d + 1] = v.y;
-    }
-    const double2 h = ld2<SMEM>(pk);  // (e_j, beta_j)
+  // one row: scaled coordinates xv, exponent term e, weight weight(), taken before the kernel values (the training rows'
+  // weight_row loads) or, with late, after them (the union rows' register select)
+  auto row = [&](const double (&xv)[DIM], double e, auto weight, auto late) {
     const double dot = dot_dim<DIM>(xq, xv, 0.0);
-    const double a = weight_row<QP, SMEM>(pk, h.y, c);
+    double a = 0.0;
+    if constexpr (!decltype(late)::value) a = weight();
     double kv, kb;
-    kernel_pair<KERNEL, SMEM>(dot, h.x, hq, alpha, kv, kb);
+    kernel_pair<KERNEL, SMEM>(dot, e, hq, alpha, kv, kb);
+    if constexpr (decltype(late)::value) a = weight();
     S0 = fma(a, kv, S0);
     const double wb = a * kb;
     if (KERNEL != CMOE_KERNEL_SQUARE_EXPONENTIAL) SB += wb;
 #pragma unroll
     for (int d = 0; d < DIM; ++d) s[d] = fma(wb, xv[d], s[d]);
+  };
+#pragma unroll 2
+  for (int j = 0; j < (TILE ? 0 : N); ++j) {
+    const double* xj = Xt + j * DIM;
+    const double* pk = Pk + j * (QP + 2);
+    double xv[DIM];
+    load_row<DIM, SMEM>(xj, xv);
+    const double2 h = ld2<SMEM>(pk);  // (e_j, beta_j)
+    row(xv, h.x, [&] { return weight_row<QP, SMEM>(pk, h.y, c); }, std::false_type());
   }
   for (int u = 0; u < U; ++u) {
     const double* xu = Xu + u * (DIM + 2);
     double xv[DIM];
-#pragma unroll
-    for (int d = 0; d < DIM; d += 2) {
-      const double2 v = ld2<SMEM>(xu + d);
-      xv[d] = v.x;
-      xv[d + 1] = v.y;
-    }
-    const double2 h = ld2<SMEM>(xu + DIM);
-    double dot = 0.0;
-#pragma unroll
-    for (int d = 0; d < DIM; ++d) dot = fma(xq[d], xv[d], dot);
-    double kv, kb;
-    kernel_pair<KERNEL, SMEM>(dot, h.x, hq, alpha, kv, kb);
-    double cu = 0.0;
-#pragma unroll
-    for (int v = 0; v < QP; ++v)
-      if (v == u) cu = c[v];
-    S0 = fma(cu, kv, S0);
-    const double wb = cu * kb;
-    if (KERNEL != CMOE_KERNEL_SQUARE_EXPONENTIAL) SB += wb;
-#pragma unroll
-    for (int d = 0; d < DIM; ++d) s[d] = fma(wb, xv[d], s[d]);
+    load_row<DIM, SMEM>(xu, xv);
+    row(xv, ld2<SMEM>(xu + DIM).x, [&] { return union_coef<QP>(c, u); }, std::true_type());
   }
   if (KERNEL == CMOE_KERNEL_SQUARE_EXPONENTIAL) SB = S0;
   if (SMEM && nq > kFarRadius * kFarRadius) {
@@ -699,59 +687,39 @@ __device__ __forceinline__ void eval_line(const double* __restrict__ Xt, const d
 #pragma unroll
   for (int k = 0; k < KB; ++k) S[k] = 0.0;
   pmax_hi = 0;  // max over rows of the high word of |a_min p_j| (integer ALU; monotone in |p|, NaN/inf sort last)
-#pragma unroll 2
-  for (int j = 0; j < (TILE ? 0 : N); ++j) {
-    const double* xj = Xt + j * DIM;
-    const double* pk = Pk + j * (QP + 2);
-    double xv[DIM];
-#pragma unroll
-    for (int d = 0; d < DIM; d += 2) {
-      const double2 v = ld2<SMEM>(xj + d);
-      xv[d] = v.x;
-      xv[d + 1] = v.y;
-    }
-    const double2 h = ld2<SMEM>(pk);  // (e_j, beta_j)
-    const double dot = dot_dim<DIM>(xb, xv, 0.0);
-    const double pj = dot_dim<DIM>(ga, xv, xga);
-    const double a = weight_row<QP, SMEM>(pk, h.y, c);
-    pmax_hi = max(pmax_hi, __double2hiint(pj) & 0x7fffffff);
-    const double w = a * exp_sel<SMEM>(dot + (h.x + hq));
-    double G = exp_sel<SMEM>(pj);
-#pragma unroll
-    for (int k = KB - 1; k >= 0; --k) {
-      S[k] = fma(w, G, S[k]);
-      if (k > 0) G *= G;
-    }
-  }
-  for (int u = 0; u < U; ++u) {
-    const double* xu = Xu + u * (DIM + 2);
-    double xv[DIM];
-#pragma unroll
-    for (int d = 0; d < DIM; d += 2) {
-      const double2 v = ld2<SMEM>(xu + d);
-      xv[d] = v.x;
-      xv[d + 1] = v.y;
-    }
-    const double2 h = ld2<SMEM>(xu + DIM);
+  // one row: scaled coordinates xv, exponent term e, weight weight()
+  auto row = [&](const double (&xv)[DIM], double e, auto weight) {
     double dot = 0.0, pj = xga;
 #pragma unroll
     for (int d = 0; d < DIM; ++d) {
       dot = fma(xb[d], xv[d], dot);
       pj = fma(ga[d], xv[d], pj);
     }
-    double cu = 0.0;
-#pragma unroll
-    for (int v = 0; v < QP; ++v)
-      if (v == u) cu = c[v];
-    // BIG: pmax_hi is kept in the tile rows' kKappa units
+    // BIG: pmax_hi is kept in the tile rows' kKappa units (BIG implies TILE, so only union rows come here)
+    const double a = weight();
     pmax_hi = max(pmax_hi, __double2hiint(BIG ? kKappa * pj : pj) & 0x7fffffff);
-    const double w = cu * exp_sel<SMEM>(dot + (h.x + hq));
+    const double w = a * exp_sel<SMEM>(dot + (e + hq));
     double G = exp_sel<SMEM>(pj);
 #pragma unroll
     for (int k = KB - 1; k >= 0; --k) {
       S[k] = fma(w, G, S[k]);
       if (k > 0) G *= G;
     }
+  };
+#pragma unroll 2
+  for (int j = 0; j < (TILE ? 0 : N); ++j) {
+    const double* xj = Xt + j * DIM;
+    const double* pk = Pk + j * (QP + 2);
+    double xv[DIM];
+    load_row<DIM, SMEM>(xj, xv);
+    const double2 h = ld2<SMEM>(pk);  // (e_j, beta_j)
+    row(xv, h.x, [&] { return weight_row<QP, SMEM>(pk, h.y, c); });
+  }
+  for (int u = 0; u < U; ++u) {
+    const double* xu = Xu + u * (DIM + 2);
+    double xv[DIM];
+    load_row<DIM, SMEM>(xu, xv);
+    row(xv, ld2<SMEM>(xu + DIM).x, [&] { return union_coef<QP>(c, u); });
   }
   // tile path: the training rows last, so that the scaled operands above are dead during the row loop
   if (TILE) tile_line<DIM, QP, KB, BIG>(Xt, Pk, N, xr, gr, inv_len, alpha_min, c, hq, xga, S, pmax_hi);
@@ -794,7 +762,12 @@ __device__ __forceinline__ void eval_line_matern(const double* __restrict__ Xt, 
       S[k] = 0.0;
     }
   }
-  auto trials = [&](double r2b, double pj, double w) {
+  // one row: scaled coordinates xv, |X~|^2 term e, weight weight()
+  auto row = [&](const double (&xv)[DIM], double e, auto weight) {
+    const double dot = dot_dim<DIM>(xb, xv, 0.0);
+    const double pj = dot_dim<DIM>(gt, xv, -xg);
+    const double a = weight();
+    const double r2b = fmax(0.0, e - 2.0 * (hq + dot)), w = a * alpha;
 #pragma unroll
     for (int k = 0; k < KB; ++k) {
       // clamped away from 0 for the seed (Matern-5/2 is flat at r = 0: the value is unchanged to the last bit) and,
@@ -813,35 +786,15 @@ __device__ __forceinline__ void eval_line_matern(const double* __restrict__ Xt, 
     const double* xj = Xt + j * DIM;
     const double* pk = Pk + j * (QP + 2);
     double xv[DIM];
-#pragma unroll
-    for (int d = 0; d < DIM; d += 2) {
-      const double2 v = ld2<SMEM>(xj + d);
-      xv[d] = v.x;
-      xv[d + 1] = v.y;
-    }
+    load_row<DIM, SMEM>(xj, xv);
     const double2 h = ld2<SMEM>(pk);  // (|X~_j|^2, beta_j)
-    const double dot = dot_dim<DIM>(xb, xv, 0.0);
-    const double pj = dot_dim<DIM>(gt, xv, -xg);
-    const double a = weight_row<QP, SMEM>(pk, h.y, c);
-    trials(fmax(0.0, h.x - 2.0 * (hq + dot)), pj, a * alpha);
+    row(xv, h.x, [&] { return weight_row<QP, SMEM>(pk, h.y, c); });
   }
   for (int u = 0; u < U; ++u) {
     const double* xu = Xu + u * (DIM + 2);
     double xv[DIM];
-#pragma unroll
-    for (int d = 0; d < DIM; d += 2) {
-      const double2 v = ld2<SMEM>(xu + d);
-      xv[d] = v.x;
-      xv[d + 1] = v.y;
-    }
-    const double2 h = ld2<SMEM>(xu + DIM);
-    const double dot = dot_dim<DIM>(xb, xv, 0.0);
-    const double pj = dot_dim<DIM>(gt, xv, -xg);
-    double cu = 0.0;
-#pragma unroll
-    for (int v = 0; v < QP; ++v)
-      if (v == u) cu = c[v];
-    trials(fmax(0.0, h.x - 2.0 * (hq + dot)), pj, cu * alpha);
+    load_row<DIM, SMEM>(xu, xv);
+    row(xv, ld2<SMEM>(xu + DIM).x, [&] { return union_coef<QP>(c, u); });
   }
 }
 
@@ -1012,12 +965,7 @@ __device__ __forceinline__ void eval_posterior_gen(const KgMcParams& prm, const 
     const double* xj = Xt + static_cast<size_t>(j) * DIM;
     const double* pk = Pk + static_cast<size_t>(j) * stride;
     double xv[DIM];
-#pragma unroll
-    for (int d = 0; d < DIM; d += 2) {
-      const double2 v = ld2<XS>(xj + d);
-      xv[d] = v.x;
-      xv[d + 1] = v.y;
-    }
+    load_row<DIM, XS>(xj, xv);
     double dot = 0.0;
 #pragma unroll
     for (int d = 0; d < DIM; ++d) dot = fma(xq[d], xv[d], dot);
@@ -1056,12 +1004,7 @@ __device__ __forceinline__ void eval_posterior_gen(const KgMcParams& prm, const 
   for (int u = 0; u < U; ++u) {
     const double* xu = Xu + static_cast<size_t>(u) * (DIM + 2);
     double xv[DIM];
-#pragma unroll
-    for (int d = 0; d < DIM; d += 2) {
-      const double2 v = ld2<false>(xu + d);
-      xv[d] = v.x;
-      xv[d + 1] = v.y;
-    }
+    load_row<DIM, false>(xu, xv);
     double dot = 0.0;
 #pragma unroll
     for (int d = 0; d < DIM; ++d) dot = fma(xq[d], xv[d], dot);
@@ -1146,12 +1089,7 @@ __device__ __forceinline__ void eval_line_gen(const KgMcParams& prm, const doubl
     const double* xj = Xt + static_cast<size_t>(j) * DIM;
     const double* pk = Pk + static_cast<size_t>(j) * stride;
     double xv[DIM];
-#pragma unroll
-    for (int d = 0; d < DIM; d += 2) {
-      const double2 v = ld2<XS>(xj + d);
-      xv[d] = v.x;
-      xv[d + 1] = v.y;
-    }
+    load_row<DIM, XS>(xj, xv);
     double dot = 0.0, pj = xga;
 #pragma unroll
     for (int d = 0; d < DIM; ++d) {
@@ -1195,12 +1133,7 @@ __device__ __forceinline__ void eval_line_gen(const KgMcParams& prm, const doubl
   for (int u = 0; u < U; ++u) {
     const double* xu = Xu + static_cast<size_t>(u) * (DIM + 2);
     double xv[DIM];
-#pragma unroll
-    for (int d = 0; d < DIM; d += 2) {
-      const double2 v = ld2<false>(xu + d);
-      xv[d] = v.x;
-      xv[d + 1] = v.y;
-    }
+    load_row<DIM, false>(xu, xv);
     double dot = 0.0, pj = xga;
 #pragma unroll
     for (int d = 0; d < DIM; ++d) {
