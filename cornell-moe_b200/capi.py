@@ -288,6 +288,42 @@ class GaussianProcess:
         _check(rc, info.value)
         return (ei, g) if grad else ei
 
+    def ei_large(self, candidates, Xp, num_mc, best_so_far, seed=0, table=None, grad=False):
+        """cmoe_ei_eval_large: ``ei`` for union sets of up to 8192 rows (q + p), same draws."""
+        cand = _f64(candidates)
+        if cand.ndim == 2:
+            cand = cand[None]
+        nc, q, _ = cand.shape
+        Xp = _f64(Xp).reshape(-1, self.dim) if Xp is not None and len(Xp) else np.zeros((0, self.dim))
+        table = _f64(table).ravel() if table is not None else None
+        if table is not None and table.size < num_mc * (q + Xp.shape[0]):
+            raise BoundsError(ERR_BOUNDS, f"normals table needs num_mc*(q+p) = {num_mc * (q + Xp.shape[0])} values")
+        ei = np.empty(nc)
+        g = np.empty((nc, q, self.dim)) if grad else None
+        info = ctypes.c_int(0)
+        rc = lib().cmoe_ei_eval_large(self.h, _d(cand), nc, q, _d(Xp), Xp.shape[0], int(num_mc),
+                                      ctypes.c_double(best_so_far), ctypes.c_uint64(seed), _d(table), _d(ei), _d(g),
+                                      ctypes.byref(info))
+        _check(rc, info.value)
+        return (ei, g) if grad else ei
+
+    def posterior_large(self, sets, derivs_s=None, want=("mean", "var")):
+        """cmoe_gp_posterior_large: mean [num_sets, Q], var and chol_var [num_sets, Q*Q] (column-major, as
+        ``posterior``) for Q = num_pts (1 + len(derivs_s)) up to 8192."""
+        sets = _f64(sets)
+        if sets.ndim == 2:
+            sets = sets[None]
+        ns, num, _ = sets.shape
+        ds = _i32(derivs_s)
+        Q = num * (1 + len(ds))
+        shapes = {"mean": (ns, Q), "var": (ns, Q * Q), "chol_var": (ns, Q * Q)}
+        bufs = {k: (np.empty(shapes[k]) if k in want else None) for k in shapes}
+        info = ctypes.c_int(0)
+        rc = lib().cmoe_gp_posterior_large(self.h, _d(sets), ns, num, _i(ds), len(ds), _d(bufs["mean"]),
+                                           _d(bufs["var"]), _d(bufs["chol_var"]), ctypes.byref(info))
+        _check(rc, info.value)
+        return {k: v for k, v in bufs.items() if v is not None}
+
     def kg(self, candidates, Xp, num_mc, best_so_far, inner, inner_bounds, discrete_pts, num_fidelity=0, seed=0,
            table=None, grad=False, stats=False):
         cand = _f64(candidates)

@@ -249,8 +249,12 @@ struct GaussianProcess {
     const int Q = Qs(n);
     std::vector<double> v(static_cast<size_t>(Q) * Q);
     int info = 0;
-    check(cmoe_gp_posterior(h, P.data(), 1, n, derivatives_.data(), num_derivatives_, nullptr, nullptr, v.data(),
-                            nullptr, nullptr, nullptr, &info), info);
+    if (Q > CMOE_MAX_SET_ROWS)
+      check(cmoe_gp_posterior_large(h, P.data(), 1, n, derivatives_.data(), num_derivatives_, nullptr, v.data(), nullptr,
+                                    &info), info);
+    else
+      check(cmoe_gp_posterior(h, P.data(), 1, n, derivatives_.data(), num_derivatives_, nullptr, nullptr, v.data(),
+                              nullptr, nullptr, nullptr, &info), info);
     py::list out;
     for (int i = 0; i < Q; ++i)
       for (int j = 0; j < Q; ++j) out.append(v[static_cast<size_t>(j) * Q + i]);
@@ -261,8 +265,12 @@ struct GaussianProcess {
     const int Q = Qs(n);
     std::vector<double> v(static_cast<size_t>(Q) * Q);
     int info = 0;
-    check(cmoe_gp_posterior(h, P.data(), 1, n, derivatives_.data(), num_derivatives_, nullptr, nullptr, nullptr,
-                            v.data(), nullptr, nullptr, &info), info);
+    if (Q > CMOE_MAX_SET_ROWS)
+      check(cmoe_gp_posterior_large(h, P.data(), 1, n, derivatives_.data(), num_derivatives_, nullptr, nullptr,
+                                    v.data(), &info), info);
+    else
+      check(cmoe_gp_posterior(h, P.data(), 1, n, derivatives_.data(), num_derivatives_, nullptr, nullptr, nullptr,
+                              v.data(), nullptr, nullptr, &info), info);
     py::list out;
     for (int i = 0; i < Q; ++i)
       for (int j = 0; j < Q; ++j) out.append(v[static_cast<size_t>(j) * Q + i]);
@@ -317,6 +325,11 @@ py::object RandomFeatureSample::call(const py::object& x, bool gradient) const {
 std::vector<double> full_bounds(const py::list& domain_bounds, int dim) { return to_vec(domain_bounds, 2 * static_cast<size_t>(dim)); }
 
 // ---- EI ---------------------------------------------------------------------------------------------------------------
+// The q-EI evaluator for a union of q + p rows: the per-set kernels up to 96 rows, the tiled path past them.
+using EiEvalFn = int (*)(const cmoe_gp*, const double*, int, int, const double*, int, int, double, uint64_t,
+                         const double*, double*, double*, int*);
+EiEvalFn ei_eval_for(int q, int p) { return q + p > CMOE_MAX_SET_ROWS ? cmoe_ei_eval_large : cmoe_ei_eval; }
+
 double compute_expected_improvement(const GaussianProcess& gp, const py::list& pts, const py::list& being, int q, int p,
                                     int max_int_steps, double best_so_far, bool /*force_monte_carlo*/,
                                     RandomnessSourceContainer& rnd) {
@@ -324,7 +337,7 @@ double compute_expected_improvement(const GaussianProcess& gp, const py::list& p
   const auto Xp = to_vec(being, static_cast<size_t>(p) * gp.dim_);
   double ei = 0.0;
   int info = 0;
-  check(cmoe_ei_eval(gp.h, X.data(), 1, q, Xp.data(), p, max_int_steps, best_so_far, rnd.seed0(), nullptr, &ei, nullptr,
+  check(ei_eval_for(q, p)(gp.h, X.data(), 1, q, Xp.data(), p, max_int_steps, best_so_far, rnd.seed0(), nullptr, &ei, nullptr,
                      &info), info);
   return ei;
 }
@@ -337,7 +350,7 @@ py::list compute_grad_expected_improvement(const GaussianProcess& gp, const py::
   double ei = 0.0;
   std::vector<double> g(static_cast<size_t>(q) * gp.dim_);
   int info = 0;
-  check(cmoe_ei_eval(gp.h, X.data(), 1, q, Xp.data(), p, max_int_steps, best_so_far, rnd.seed0(), nullptr, &ei, g.data(),
+  check(ei_eval_for(q, p)(gp.h, X.data(), 1, q, Xp.data(), p, max_int_steps, best_so_far, rnd.seed0(), nullptr, &ei, g.data(),
                      &info), info);
   return to_list(g);
 }
@@ -415,7 +428,7 @@ py::list multistart_expected_improvement_optimization(const py::object& optimize
     const int n = optimizer_parameters.attr("num_random_samples").cast<int>();
     const auto starts = make_starts(n);
     std::vector<double> vals(n);
-    check(cmoe_ei_eval(gp.h, starts.data(), n, q, Xp.data(), p, max_int_steps, best_so_far, rnd.seed0(), nullptr,
+    check(ei_eval_for(q, p)(gp.h, starts.data(), n, q, Xp.data(), p, max_int_steps, best_so_far, rnd.seed0(), nullptr,
                        vals.data(), nullptr, &info), info);
     double bv = -1.0;
     std::copy(starts.begin(), starts.begin() + static_cast<size_t>(q) * dim, best.begin());
@@ -454,7 +467,7 @@ py::list evaluate_EI_at_point_list(const GaussianProcess& gp, const py::list& in
   if (q == 1 && p == 0)  // closed-form 1-EI, as EvaluateEIAtPointList does (gpp_math.cpp:2317)
     check(cmoe_ei_analytic(gp.h, starts.data(), num_multistarts, best_so_far, vals.data(), nullptr, &info), info);
   else
-    check(cmoe_ei_eval(gp.h, starts.data(), num_multistarts, q, Xp.data(), p, max_int_steps, best_so_far, rnd.seed0(),
+    check(ei_eval_for(q, p)(gp.h, starts.data(), num_multistarts, q, Xp.data(), p, max_int_steps, best_so_far, rnd.seed0(),
                        nullptr, vals.data(), nullptr, &info), info);
   bool found = false;
   for (double v : vals) found = found || (v > -1.0);

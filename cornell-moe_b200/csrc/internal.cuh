@@ -226,6 +226,13 @@ inline SampleWork& sample_work(const cmoe_gp& gp) {
   if (!gp.sample_ws) gp.sample_ws = std::make_shared<SampleWork>();
   return *static_cast<SampleWork*>(gp.sample_ws.get());
 }
+// The K8 posterior stages for the nc sets whose points are in w.P (num points, gs derivative rows dPs = w.dPs each,
+// Q = num (1 + gs) <= 8192): V = L^-1 K(X, P) in w.V (n x nc Q, ld n), the mean in w.mu and the lower triangle of
+// Var = K(P, P) - V^T V + jitter I in w.A ([nc][Q][Q] column-major; the upper triangle is not written).  Asynchronous.
+void posterior_cov_large(const cmoe_gp& gp, SampleWork& w, int nc, int num, int gs, double jitter, cudaStream_t s);
+// upper triangle of nsets Q x Q column-major matrices <- 0 (zero_upper) or <- the lower triangle (mirror_lower)
+void zero_upper(int nsets, int Q, double* A, cudaStream_t s);
+void mirror_lower(int nsets, int Q, double* A, cudaStream_t s);
 
 // Items per chunk of a batched call: as many as fit in `budget` bytes at `bytes_per_item` each, at most `total` and
 // `cap` (a grid-dimension or set-count limit), and at least one.
@@ -281,6 +288,10 @@ void upload_union_sets(PosteriorBatch& pb, const double* candidates, int nc, int
                        cudaStream_t s);
 void ei_eval_batch(const cmoe_gp& gp, const double* candidates, int nc, int q, const double* Xp, int p, int num_mc,
                    double best_so_far, uint64_t seed, const double* dtable, double* ei_host, double* grad_host);
+// ---- ei_large.cu: the same evaluation for 1 <= q + p <= kMaxSampleQ (DESIGN.md K16) ----
+void ei_large_eval_batch(const cmoe_gp& gp, const double* candidates, int nc, int q, const double* Xp, int p,
+                         int num_mc, double best_so_far, uint64_t seed, const double* dtable, double* ei_host,
+                         double* grad_host);
 
 // ---- cov.cu --------------------------------------------------------------------------------------------------
 // Lower triangle of K(X,X) + diag(noise by observation type), n*n column-major.

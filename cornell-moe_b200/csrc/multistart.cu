@@ -275,9 +275,11 @@ BatchEval make_ei_eval(const cmoe_gp* gp, int q, const double* Xp, int p, int nu
       analytic_ei(gp, pts, nc, best_so_far, values, grads);
     };
   }
+  // union sets past the per-set kernels' 96 rows take the tiled path of ei_large.cu
+  const auto batch = q + p <= kMaxQ ? ei_eval_batch : ei_large_eval_batch;
   return [=](const double* pts, int nc, double* values, double* grads) {
     require_device(gp->device);  // may run on a worker thread of the multi-device driver
-    ei_eval_batch(*gp, pts, nc, q, Xp, p, num_mc, best_so_far, seed, dtable, values, grads);
+    batch(*gp, pts, nc, q, Xp, p, num_mc, best_so_far, seed, dtable, values, grads);
   };
 }
 
@@ -462,6 +464,7 @@ void make_kg_ensemble(KgEnsembleEvaluator& ens, const cmoe_gp* const* gps, int n
 
 BatchEval make_ei_ensemble(const cmoe_gp* const* gps, int num_gp, int q, const double* Xp, int p, int num_mc,
                            const double* best_so_far, uint64_t seed) {
+  CMOE_REQUIRE(q >= 1 && p >= 0 && q + p <= kMaxQ, CMOE_ERR_BOUNDS, "(q+p)*(1+num_derivatives) must be in [1, 96]");
   std::vector<BatchEval> members;
   for (int m = 0; m < num_gp; ++m) members.push_back(make_ei_eval(gps[m], q, Xp, p, num_mc, best_so_far[m], seed));
   const size_t ps = static_cast<size_t>(q) * gps[0]->spec.dim;

@@ -341,6 +341,17 @@ __global__ void zero_upper_kernel(int nsets, int Q, double* __restrict__ A) {
   }
 }
 
+// strictly upper triangle of every Q x Q matrix <- its lower triangle (a full symmetric matrix from the lower half)
+__global__ void mirror_lower_kernel(int nsets, int Q, double* __restrict__ A) {
+  const size_t total = static_cast<size_t>(nsets) * Q * Q;
+  for (size_t e = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; e < total;
+       e += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const size_t o = e % (static_cast<size_t>(Q) * Q), base = e - o;
+    const int r = static_cast<int>(o % Q), c = static_cast<int>(o / Q);
+    if (r < c) A[e] = A[base + static_cast<size_t>(r) * Q + c];
+  }
+}
+
 size_t panel_smem_bytes() {
   return (static_cast<size_t>(NB) * LTS + NB + 128 + NB + NB * (NB + 1)) * sizeof(double);
 }
@@ -372,11 +383,7 @@ void potrf_batched(double* A, int Q, int nsets, int* fail, DevBuf<double>& stage
   CMOE_CUDA(cudaGetLastError());
 }
 
-namespace {
-
-// One chunk of nc sets whose points are in w.P: fills w.mu, w.A (factor), w.y, w.amin and w.fail.
-void sample_chunk(const cmoe_gp& gp, SampleWork& w, int nc, int num, int gs, uint64_t seed, uint64_t draw0,
-                  const double* dtable, double jitter, cudaStream_t s) {
+void posterior_cov_large(const cmoe_gp& gp, SampleWork& w, int nc, int num, int gs, double jitter, cudaStream_t s) {
   const KernelSpec& spec = gp.spec;
   const int Q = num * (1 + gs), n = gp.n;
   build_mix_covariance(spec, gp.dX.p, gp.N, w.P.p, nc * num, w.dPs.p, gs, w.V.p, s);
@@ -390,6 +397,28 @@ void sample_chunk(const cmoe_gp& gp, SampleWork& w, int nc, int num, int gs, uin
   cov_tile_kernel<<<dim3(t * (t + 1) / 2, 1, nc), kTileThreads, smem_cov, s>>>(spec, w.V.p, n, Q, w.P.p, num, w.dPs.p,
                                                                               gs, jitter, w.A.p);
   count_launch();
+  CMOE_CUDA(cudaGetLastError());
+}
+
+void zero_upper(int nsets, int Q, double* A, cudaStream_t s) {
+  zero_upper_kernel<<<1024, 256, 0, s>>>(nsets, Q, A);
+  count_launch();
+  CMOE_CUDA(cudaGetLastError());
+}
+
+void mirror_lower(int nsets, int Q, double* A, cudaStream_t s) {
+  mirror_lower_kernel<<<1024, 256, 0, s>>>(nsets, Q, A);
+  count_launch();
+  CMOE_CUDA(cudaGetLastError());
+}
+
+namespace {
+
+// One chunk of nc sets whose points are in w.P: fills w.mu, w.A (factor), w.y, w.amin and w.fail.
+void sample_chunk(const cmoe_gp& gp, SampleWork& w, int nc, int num, int gs, uint64_t seed, uint64_t draw0,
+                  const double* dtable, double jitter, cudaStream_t s) {
+  const int Q = num * (1 + gs);
+  posterior_cov_large(gp, w, nc, num, gs, jitter, s);
   CMOE_CUDA(cudaMemsetAsync(w.fail.p, 0, nc * sizeof(int), s));
   potrf_batched(w.A.p, Q, nc, w.fail.p, w.stage, s);
   const int rb = (Q + kRowThreads - 1) / kRowThreads;
@@ -513,13 +542,68 @@ extern "C" int cmoe_gp_sample_joint(const cmoe_gp* gp, const double* sets, int n
           if (argmin) w.amin.download(argmin + c0, nc, s);
           if (mean) w.mu.download(mean + off, cnt, s);
           if (chol) {
-            zero_upper_kernel<<<1024, 256, 0, s>>>(nc, Q, w.A.p);
-            count_launch();
-            CMOE_CUDA(cudaGetLastError());
+            zero_upper(nc, Q, w.A.p, s);
             w.A.download(chol + off * Q, cnt * Q, s);
           }
           CMOE_CUDA(cudaStreamSynchronize(s));
         });
+  });
+}
+
+extern "C" int cmoe_gp_posterior_large(const cmoe_gp* gp, const double* sets, int num_sets, int num_pts,
+                                       const int* derivs_s, int g_s, double* mean, double* var, double* chol_var,
+                                       int* info) {
+  return guarded(info, [&] {
+    CMOE_REQUIRE(gp != nullptr, CMOE_ERR_INVALID_VALUE, "gp is NULL");
+    CMOE_REQUIRE(num_sets >= 1 && num_pts >= 1, CMOE_ERR_BOUNDS, "num_sets and num_pts must be >= 1");
+    CMOE_REQUIRE(g_s >= 0 && g_s <= gp->spec.dim, CMOE_ERR_BOUNDS, "g_s out of range");
+    for (int k = 0; k < g_s; ++k)
+      CMOE_REQUIRE(derivs_s[k] >= 0 && derivs_s[k] < gp->spec.dim, CMOE_ERR_BOUNDS, "derivative index out of range");
+    CMOE_REQUIRE(static_cast<long long>(num_pts) * (1 + g_s) <= kMaxSampleQ, CMOE_ERR_BOUNDS,
+                 "num_pts*(1+g_s) must be <= 8192");
+    require_device(gp->device);
+    const int Q = num_pts * (1 + g_s), n = gp->n, dim = gp->spec.dim;
+    cudaStream_t s = gp->stream;
+    const size_t per_set = sizeof(double) * (static_cast<size_t>(n) * Q + static_cast<size_t>(Q) * Q + Q +
+                                             static_cast<size_t>(num_pts) * dim +
+                                             static_cast<size_t>((Q + NB - 1) / NB) * NB * NB) +
+                           sizeof(int);
+    const int chunk = static_cast<int>(chunk_items(num_sets, kSampleWorkspaceBytes, per_set, kMaxChunkSets));
+    SampleWork& w = sample_work(*gp);
+    w.P.ensure(static_cast<size_t>(chunk) * num_pts * dim);
+    w.V.ensure(static_cast<size_t>(chunk) * Q * n);
+    w.A.ensure(static_cast<size_t>(chunk) * Q * Q);
+    w.mu.ensure(static_cast<size_t>(chunk) * Q);
+    w.fail.ensure(chunk);
+    w.dPs.ensure(g_s > 0 ? g_s : 1);
+    if (g_s > 0) w.dPs.upload(derivs_s, g_s, s);
+    std::vector<int> hfail(chunk);
+    for (int c0 = 0; c0 < num_sets; c0 += chunk) {
+      const int nc = std::min(chunk, num_sets - c0);
+      const size_t off = static_cast<size_t>(c0) * Q, cnt = static_cast<size_t>(nc) * Q;
+      w.P.upload(sets + static_cast<size_t>(c0) * num_pts * dim, static_cast<size_t>(nc) * num_pts * dim, s);
+      posterior_cov_large(*gp, w, nc, num_pts, g_s, 0.0, s);
+      if (mean) w.mu.download(mean + off, cnt, s);
+      if (var) {
+        mirror_lower(nc, Q, w.A.p, s);
+        w.A.download(var + off * Q, cnt * Q, s);
+      }
+      if (chol_var) {
+        CMOE_CUDA(cudaMemsetAsync(w.fail.p, 0, nc * sizeof(int), s));
+        potrf_batched(w.A.p, Q, nc, w.fail.p, w.stage, s);
+        w.fail.download(hfail.data(), nc, s);
+        CMOE_CUDA(cudaStreamSynchronize(s));
+        for (int c = 0; c < nc; ++c)
+          if (hfail[c] != 0)
+            throw Error(CMOE_ERR_SINGULAR,
+                        "GP-Variance matrix singular. Check for duplicate points_to_sample or points_to_sample "
+                        "duplicating points_sampled with 0 noise.",
+                        hfail[c]);
+        zero_upper(nc, Q, w.A.p, s);
+        w.A.download(chol_var + off * Q, cnt * Q, s);
+      }
+      CMOE_CUDA(cudaStreamSynchronize(s));
+    }
   });
 }
 

@@ -196,6 +196,18 @@ int cmoe_gp_fit_timings(const cmoe_gp* gp, double* usec3);
 int cmoe_gp_posterior(const cmoe_gp* gp, const double* sets, int num_sets, int num_pts, const int* derivs_s, int g_s,
                       double* mean, double* grad_mean, double* var, double* chol_var, double* grad_var,
                       double* grad_chol, int* info);
+/* Largest Q = num_pts (1 + g_s) of cmoe_gp_posterior's variance outputs and largest q + p of cmoe_ei_eval. */
+#define CMOE_MAX_SET_ROWS 96
+/* Largest Q of cmoe_gp_posterior_large and largest q + p of cmoe_ei_eval_large. */
+#define CMOE_MAX_LARGE_SET_ROWS 8192
+/* cmoe_gp_posterior's mean, var and chol_var for 1 <= Q = num_pts (1 + g_s) <= 8192, in its layouts (any output may be
+ * NULL).  Computed by the stages of cmoe_gp_sample_joint: Var = K(P,P) - V^T V with V = L^-1 K(X,P), factored by the
+ * batched blocked Cholesky (the reference's (K^-1 K*)^T K* differs by rounding).  Sets run in chunks that fit the handle's
+ * 2 GiB sampling workspace; a set's result does not depend on the chunking.  chol failure -> CMOE_ERR_SINGULAR,
+ * *info = leading minor of the first failing set.  The gradients of Var and of its factor are not offered here: they
+ * hold num_pts Q^2 dim doubles per set (8.6 GB at Q = 512, dim = 8). */
+int cmoe_gp_posterior_large(const cmoe_gp* gp, const double* sets, int num_sets, int num_pts, const int* derivs_s,
+                            int g_s, double* mean, double* var, double* chol_var, int* info);
 
 /* ---- joint posterior draws, batched over point sets ------------------------------------------------------------
  * Joint posterior draws over point sets: GaussianProcess::SamplePointsFromGP (gpp_math.cpp:1803-1848) batched over sets;
@@ -367,6 +379,17 @@ int cmoe_lcb_select(const cmoe_gp* gp, const double* candidates, int num_candida
 int cmoe_ei_eval(const cmoe_gp* gp, const double* candidates, int num_candidates, int q,
                  const double* points_being_sampled, int p, int num_mc, double best_so_far, uint64_t seed,
                  const double* normals_table, double* ei, double* grad_ei, int* info);
+/* cmoe_ei_eval for 1 <= U = q + p <= 8192 (CMOE_ERR_BOUNDS past it, or when the num_mc U normals exceed 2 GiB), same
+ * arguments, same draws: sample s uses the normals 2k, 2k+1 of Philox call (seed, draw s, k), or row s of the
+ * [num_mc][U] table.  At U <= 96 the two calls differ only in summation order.  y - mu = C W runs as FP64 tensor-core
+ * tiles; the gradient is taken in reverse mode through the Cholesky factor (DESIGN.md K16), so no q U^2 dim tensor is
+ * formed: O(n U + U^2) device memory per candidate.  Candidates run in chunks that fit 2 GiB; a candidate's result does
+ * not depend on the batch.  A failed factorisation -> CMOE_ERR_SINGULAR, *info = leading minor of the first failing
+ * candidate.  The multistart q-EI drivers (cmoe_multistart_ei(_ex), cmoe_ei_gradient_descent) evaluate through this
+ * call when q + p > 96 and through cmoe_ei_eval otherwise. */
+int cmoe_ei_eval_large(const cmoe_gp* gp, const double* candidates, int num_candidates, int q,
+                       const double* points_being_sampled, int p, int num_mc, double best_so_far, uint64_t seed,
+                       const double* normals_table, double* ei, double* grad_ei, int* info);
 
 /* ---- q-KG / d-KG Monte Carlo, batched over candidates -----------------------------------------------------------
  * Replaces KnowledgeGradientEvaluator::ComputeKnowledgeGradient / ComputeGradKnowledgeGradient
