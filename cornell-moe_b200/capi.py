@@ -344,6 +344,36 @@ class GaussianProcess:
                                 ctypes.c_double(best_so_far), ctypes.c_uint64(seed), _d(table), _d(kg), _d(g),
                                 ctypes.byref(st), ctypes.byref(info))
         _check(rc, info.value)
+        return self._kg_result(kg, g, st, grad, stats)
+
+    def kg_large(self, candidates, Xp, num_mc, best_so_far, inner, inner_bounds, discrete_pts, num_fidelity=0, seed=0,
+                 table=None, grad=False, stats=False):
+        """cmoe_kg_eval_large: ``kg`` for unions of up to 1024 rows ((q + p)(1 + g)), same arguments and draws."""
+        cand = _f64(candidates)
+        if cand.ndim == 2:
+            cand = cand[None]
+        nc, q, _ = cand.shape
+        Xp = _f64(Xp).reshape(-1, self.dim) if Xp is not None and len(Xp) else np.zeros((0, self.dim))
+        Q = (q + Xp.shape[0]) * (1 + self.g)
+        table = _f64(table).ravel() if table is not None else None
+        if table is not None and table.size < ((num_mc + 1) // 2) * Q:
+            raise BoundsError(ERR_BOUNDS, f"normals table needs ((num_mc+1)/2)*Q = {((num_mc + 1) // 2) * Q} values")
+        inner = GDParams.from_seq(inner)
+        inner_bounds = _f64(inner_bounds).ravel()
+        disc = _f64(discrete_pts).reshape(-1, self.dim - num_fidelity)
+        kg = np.empty(nc)
+        g = np.empty((nc, q, self.dim)) if grad else None
+        st = KGStats()
+        info = ctypes.c_int(0)
+        rc = lib().cmoe_kg_eval_large(self.h, int(num_fidelity), ctypes.byref(inner), _d(inner_bounds), _d(disc),
+                                      disc.shape[0], _d(cand), nc, q, _d(Xp), Xp.shape[0], int(num_mc),
+                                      ctypes.c_double(best_so_far), ctypes.c_uint64(seed), _d(table), _d(kg), _d(g),
+                                      ctypes.byref(st), ctypes.byref(info))
+        _check(rc, info.value)
+        return self._kg_result(kg, g, st, grad, stats)
+
+    @staticmethod
+    def _kg_result(kg, g, st, grad, stats):
         res = [kg]
         if grad:
             res.append(g)

@@ -290,6 +290,8 @@ __global__ void __launch_bounds__(kTileThreads) ei_ctc_kernel(int U, const doubl
       }
 }
 
+constexpr size_t kTileSmem = 2 * static_cast<size_t>(NB) * LDT * sizeof(double);
+
 // out = in^T for nsets U x U matrices
 __global__ void __launch_bounds__(256) transpose_kernel(int U, const double* __restrict__ in,
                                                         double* __restrict__ out) {
@@ -390,7 +392,6 @@ __global__ void __launch_bounds__(kGradThreads) ei_grad_kernel(const __grid_cons
   }
 }
 
-constexpr size_t kTileSmem = 2 * static_cast<size_t>(NB) * LDT * sizeof(double);
 
 // Device scratch of one chunk beyond the K8 workspace.
 struct EiLargeWork {
@@ -450,27 +451,13 @@ void ei_large_chunk(const cmoe_gp& gp, SampleWork& w, EiLargeWork& e, const doub
                                    static_cast<int>(smem_bucket)));
     ei_bucket_kernel<<<nc, kBucketThreads, smem_bucket, s>>>(U, num_mc, e.win.p, e.cnt.p, e.start.p, e.order.p);
     ei_cbar_kernel<<<dim3(gUU, nc), 256, 0, s>>>(U, num_mc, W, e.cnt.p, e.start.p, e.order.p, e.T1.p);
-    const int t = nrb;
-    CMOE_CUDA(cudaFuncSetAttribute(ei_ctc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   static_cast<int>(kTileSmem)));
-    ei_ctc_kernel<<<dim3(t * (t + 1) / 2, 1, nc), kTileThreads, kTileSmem, s>>>(U, w.A.p, e.T1.p, e.T2.p);
-    count_launch(3);
-    CMOE_CUDA(cudaGetLastError());
-    mirror_lower(nc, U, e.T2.p, s);  // S = Phi(M) + Phi(M)^T
-    for (int c = 0; c < nc; ++c)     // X = C^-T S
-      trsm_lower_blocked(w.A.p + c * UU, U, e.T2.p + c * UU, U, U, true, s);
-    transpose_kernel<<<dim3(gUU, nc), 256, 0, s>>>(U, e.T2.p, e.T1.p);
-    count_launch();
-    for (int c = 0; c < nc; ++c)  // T = C^-T X^T = C^-T S C^-1 = 2 Sigmabar
-      trsm_lower_blocked(w.A.p + c * UU, U, e.T1.p + c * UU, U, U, true, s);
+    count_launch(2);
+    cholesky_adjoint(w.A.p, U, nc, e.T1.p, e.T2.p, s);
     // R = B T[:, :q]
-    CMOE_CUDA(cudaFuncSetAttribute(gemm_nn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   static_cast<int>(kTileSmem)));
-    gemm_nn_kernel<<<dim3((n + NB - 1) / NB, (q + NB - 1) / NB, nc), kTileThreads, kTileSmem, s>>>(
-        n, q, U, w.V.p, n, static_cast<size_t>(n) * U, e.T1.p, U, UU, e.R.p, n, static_cast<size_t>(n) * q);
+    gemm_nn(n, q, U, w.V.p, n, static_cast<size_t>(n) * U, e.T1.p, U, UU, e.R.p, n, static_cast<size_t>(n) * q, nc, s);
     ei_grad_kernel<<<dim3(q, nc), kGradThreads, 0, s>>>(gp.spec, gp.N, gp.dX.p, gp.dKinvY.p, w.P.p, U, q, num_mc,
                                                         e.T1.p, e.R.p, e.cnt.p, e.grad.p);
-    count_launch(2);
+    count_launch();
     CMOE_CUDA(cudaGetLastError());
     e.grad.download(grad_host, static_cast<size_t>(nc) * q * dim, s);
   }
@@ -478,6 +465,34 @@ void ei_large_chunk(const cmoe_gp& gp, SampleWork& w, EiLargeWork& e, const doub
 }
 
 }  // namespace
+
+void gemm_nn(int m, int nn, int kd, const double* A, int lda, size_t sa, const double* B, int ldb, size_t sb,
+             double* Out, int ldo, size_t so, int batch, cudaStream_t s) {
+  CMOE_CUDA(cudaFuncSetAttribute(gemm_nn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 static_cast<int>(kTileSmem)));
+  gemm_nn_kernel<<<dim3((m + NB - 1) / NB, (nn + NB - 1) / NB, batch), kTileThreads, kTileSmem, s>>>(
+      m, nn, kd, A, lda, sa, B, ldb, sb, Out, ldo, so);
+  count_launch();
+  CMOE_CUDA(cudaGetLastError());
+}
+
+void cholesky_adjoint(const double* C, int U, int nc, double* T1, double* T2, cudaStream_t s) {
+  const size_t UU = static_cast<size_t>(U) * U;
+  const unsigned gUU = static_cast<unsigned>((UU + 255) / 256);
+  const int t = (U + NB - 1) / NB;
+  CMOE_CUDA(cudaFuncSetAttribute(ei_ctc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 static_cast<int>(kTileSmem)));
+  ei_ctc_kernel<<<dim3(t * (t + 1) / 2, 1, nc), kTileThreads, kTileSmem, s>>>(U, C, T1, T2);
+  count_launch();
+  CMOE_CUDA(cudaGetLastError());
+  mirror_lower(nc, U, T2, s);  // S = Phi(M) + Phi(M)^T
+  for (int c = 0; c < nc; ++c)  // X = C^-T S
+    trsm_lower_blocked(C + c * UU, U, T2 + c * UU, U, U, true, s);
+  transpose_kernel<<<dim3(gUU, nc), 256, 0, s>>>(U, T2, T1);
+  count_launch();
+  for (int c = 0; c < nc; ++c)  // T = C^-T X^T = C^-T S C^-1 = 2 Sigmabar
+    trsm_lower_blocked(C + c * UU, U, T1 + c * UU, U, U, true, s);
+}
 
 void ei_large_eval_batch(const cmoe_gp& gp, const double* candidates, int nc, int q, const double* Xp, int p,
                          int num_mc, double best_so_far, uint64_t seed, const double* dtable, double* ei_host,

@@ -518,6 +518,15 @@ py::list compute_grad_posterior_mean(const GaussianProcess& gp, int num_fidelity
   return to_list(out);
 }
 
+// ---- q-KG ---------------------------------------------------------------------------------------------------------------
+// The q-KG evaluator for a union of (q + p)(1 + g) rows: the 32-row call up to its bound, cmoe_kg_eval_large past it.
+using KgEvalFn = int (*)(const cmoe_gp*, int, const cmoe_gd_params*, const double*, const double*, int, const double*,
+                         int, int, const double*, int, int, double, uint64_t, const double*, double*, double*,
+                         cmoe_kg_stats*, int*);
+KgEvalFn kg_eval_for(const GaussianProcess& gp, int q, int p) {
+  return static_cast<long long>(q + p) * (1 + gp.num_derivatives_) > 32 ? cmoe_kg_eval_large : cmoe_kg_eval;
+}
+
 double compute_knowledge_gradient(const GaussianProcess& gp, int num_fidelity, const py::object& optimizer_parameters,
                                   const py::list& domain_bounds, const py::list& discrete_pts, const py::list& pts,
                                   const py::list& being, int num_pts, int q, int p, int max_int_steps, double best_so_far,
@@ -530,8 +539,10 @@ double compute_knowledge_gradient(const GaussianProcess& gp, int num_fidelity, c
   const cmoe_gd_params inner = gd_of(optimizer_parameters);
   double kg = 0.0;
   int info = 0;
-  check(cmoe_kg_eval(gp.h, num_fidelity, &inner, inner_bounds.data(), D.data(), num_pts, X.data(), 1, q, Xp.data(), p,
-                     max_int_steps, best_so_far, rnd.seed0(), nullptr, &kg, nullptr, nullptr, &info), info);
+  check(kg_eval_for(gp, q, p)(gp.h, num_fidelity, &inner, inner_bounds.data(), D.data(), num_pts, X.data(), 1, q,
+                              Xp.data(), p, max_int_steps, best_so_far, rnd.seed0(), nullptr, &kg, nullptr, nullptr,
+                              &info),
+        info);
   return kg;
 }
 
@@ -549,8 +560,10 @@ py::list compute_grad_knowledge_gradient(const GaussianProcess& gp, int num_fide
   double kg = 0.0;
   std::vector<double> g(static_cast<size_t>(q) * dim);
   int info = 0;
-  check(cmoe_kg_eval(gp.h, num_fidelity, &inner, inner_bounds.data(), D.data(), num_pts, X.data(), 1, q, Xp.data(), p,
-                     max_int_steps, best_so_far, rnd.seed0(), nullptr, &kg, g.data(), nullptr, &info), info);
+  check(kg_eval_for(gp, q, p)(gp.h, num_fidelity, &inner, inner_bounds.data(), D.data(), num_pts, X.data(), 1, q,
+                              Xp.data(), p, max_int_steps, best_so_far, rnd.seed0(), nullptr, &kg, g.data(), nullptr,
+                              &info),
+        info);
   return to_list(g);
 }
 
@@ -581,8 +594,10 @@ py::list multistart_knowledge_gradient_optimization(const py::object& optimizer_
     const int n = optimizer_parameters.attr("num_random_samples").cast<int>();
     const auto starts = lhc_starts(bounds, dim, q, n, rnd.uniform_engine);
     std::vector<double> vals(n);
-    check(cmoe_kg_eval(gp.h, num_fidelity, &inner, inner_bounds.data(), D.data(), num_pts, starts.data(), n, q, Xp.data(),
-                       p, max_int_steps, best_so_far, rnd.seed0(), nullptr, vals.data(), nullptr, nullptr, &info), info);
+    check(kg_eval_for(gp, q, p)(gp.h, num_fidelity, &inner, inner_bounds.data(), D.data(), num_pts, starts.data(), n,
+                                q, Xp.data(), p, max_int_steps, best_so_far, rnd.seed0(), nullptr, vals.data(), nullptr,
+                                nullptr, &info),
+          info);
     double bv = -INFINITY;
     std::copy(starts.begin(), starts.begin() + static_cast<size_t>(q) * dim, best.begin());
     for (int i = 0; i < n; ++i)
@@ -627,8 +642,9 @@ py::list evaluate_KG_at_point_list(const GaussianProcess& gp, int num_fidelity, 
   const cmoe_gd_params inner = gd_of(optimizer_parameters);
   std::vector<double> vals(num_multistarts);
   int info = 0;
-  check(cmoe_kg_eval(gp.h, num_fidelity, &inner, inner_bounds.data(), D.data(), num_pts, starts.data(), num_multistarts, q,
-                     Xp.data(), p, max_int_steps, best_so_far, rnd.seed0(), nullptr, vals.data(), nullptr, nullptr, &info),
+  check(kg_eval_for(gp, q, p)(gp.h, num_fidelity, &inner, inner_bounds.data(), D.data(), num_pts, starts.data(),
+                              num_multistarts, q, Xp.data(), p, max_int_steps, best_so_far, rnd.seed0(), nullptr,
+                              vals.data(), nullptr, nullptr, &info),
         info);
   bool found = false;
   for (double v : vals) found = found || std::isfinite(v);

@@ -155,6 +155,8 @@ struct cmoe_gp {
   mutable std::vector<cmoe_gp*> replicas;
   // device workspace of the joint-sampling calls (sample.cu), grown on demand and kept until the handle is destroyed
   mutable std::shared_ptr<void> sample_ws;
+  // device workspace of cmoe_kg_eval_large (kg_large.cu), grown on demand and kept until the handle is destroyed
+  mutable std::shared_ptr<void> kg_large_ws;
   mutable uint64_t replicas_generation = 0;
   ~cmoe_gp();
 };
@@ -292,6 +294,22 @@ void ei_eval_batch(const cmoe_gp& gp, const double* candidates, int nc, int q, c
 void ei_large_eval_batch(const cmoe_gp& gp, const double* candidates, int nc, int q, const double* Xp, int p,
                          int num_mc, double best_so_far, uint64_t seed, const double* dtable, double* ei_host,
                          double* grad_host);
+// ---- kg_large.cu: cmoe_kg_eval for 1 <= (q + p)(1 + g) <= CMOE_MAX_KG_LARGE_ROWS (DESIGN.md K17) ----
+// stale_union (q points or NULL): the discretisation set's union part keeps these q points (the reference drivers'
+// quirk, cmoe_kg_plan_set_stale_union); normals_table: ((num_mc + 1) / 2) (q + p)(1 + g) values or NULL.  Throws Error.
+void kg_large_eval(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_params* inner, const double* inner_bounds,
+                   const double* discrete_pts, int num_pts, const double* candidates, int num_candidates, int q,
+                   const double* points_being_sampled, int p, int num_mc, double best_so_far, uint64_t seed,
+                   const double* normals_table, const double* stale_union, double* kg, double* grad_kg,
+                   cmoe_kg_stats* stats);
+// Out = A B for `batch` column-major problems (A m x kd, B kd x nn; batch z at A + z sa, B + z sb, Out + z so), 64 x 64
+// DMMA tiles.  Asynchronous on `s`.
+void gemm_nn(int m, int nn, int kd, const double* A, int lda, size_t sa, const double* B, int ldb, size_t sb,
+             double* Out, int ldo, size_t so, int batch, cudaStream_t s);
+// Reverse mode through nc Cholesky factors C (U x U, column-major, upper triangle zero): T1 holds Cbar on entry (the
+// adjoint of C, lower triangle) and 2 Sigmabar on exit, Sigmabar the adjoint of Sigma = C C^T (symmetric).  T2 is
+// scratch of the same size.  Asynchronous on `s`.
+void cholesky_adjoint(const double* C, int U, int nc, double* T1, double* T2, cudaStream_t s);
 
 // ---- cov.cu --------------------------------------------------------------------------------------------------
 // Lower triangle of K(X,X) + diag(noise by observation type), n*n column-major.

@@ -544,6 +544,51 @@ const KgDispatchEntry* find_kg_entry(int kernel, int dim, int Q, int g) {
   return best;
 }
 
+namespace {
+std::vector<KgLargeEntry>& kg_large_table() {
+  static std::vector<KgLargeEntry> t;
+  return t;
+}
+}  // namespace
+
+bool register_kg_large_entries(std::initializer_list<KgLargeEntry> entries) {
+  kg_large_table().insert(kg_large_table().end(), entries);
+  return true;
+}
+
+const KgLargeEntry* find_kg_large_entry(int kernel, int dim, int g) {
+  const bool wide = g > kMaxG;
+  const KgLargeEntry* best = nullptr;
+  for (const auto& e : kg_large_table()) {
+    if (e.kernel != kernel || e.dim < dim || e.wide != wide) continue;
+    if (!best || e.dim < best->dim) best = &e;
+  }
+  return best;
+}
+
+void kg_value(int nb, int num_mc, const double* outVal, const double* best_post, const int* fail, double* kg,
+              cudaStream_t s) {
+  kg_value_kernel<<<nb, 256, 0, s>>>(num_mc, outVal, best_post, fail, kg);
+  count_launch();
+}
+
+void kg_fill_points(const KernelSpec& spec, const Centre& ctr, int samples, int DIMP, double* outX, double* outH,
+                    cudaStream_t s) {
+  kg_fill_point_kernel<<<(samples + 255) / 256, 256, 0, s>>>(spec, ctr, samples, DIMP, outX, outH);
+  count_launch();
+}
+
+void kg_tprime(int nb, int n, int Q, int QP, const double* R, const double* B, double* Tp, cudaStream_t s) {
+  kg_tprime_kernel<<<nb, 256, 0, s>>>(n, Q, QP, R, B, Tp);
+  count_launch();
+}
+
+void kg_g1(const KernelSpec& spec, const Centre& ctr, int nb, int U, int q, int QP, int DIMP, int num_mc,
+           const double* P, const double* recC, const double* outX, double* G1, cudaStream_t s) {
+  kg_g1_kernel<<<nb, 256, 0, s>>>(spec, ctr, U, q, QP, DIMP, num_mc, P, recC, outX, G1);
+  count_launch();
+}
+
 }  // namespace cmoe
 
 using namespace cmoe;  // NOLINT

@@ -1219,6 +1219,23 @@ __device__ __forceinline__ void fill_own_weights(const double* __restrict__ Wt, 
   }
 }
 
+// Large-union build (PRE): the sample's whole weight column is precomputed (kg_large.cu, [num_mc][R] per candidate), so
+// the warp copies the column of each requesting lane into that lane's scratch column, rows strided over the lanes so
+// that the reads are coalesced.
+__device__ __forceinline__ void copy_sample_weights(const double* __restrict__ Wt, int R, double* aw_warp, unsigned want,
+                                                    int sample, int lane) {
+  while (want) {
+    const int b = __ffs(want) - 1;
+    want &= want - 1;
+    const int sb = __shfl_sync(0xffffffffu, sample, b);
+    const double* src = Wt + static_cast<size_t>(sb) * R;
+    double* col = aw_warp + b;
+#pragma unroll 4
+    for (int r = lane; r < R; r += 32) col[static_cast<size_t>(r) * kMcThreads] = __ldg(src + r);
+  }
+  __syncwarp();
+}
+
 // Value and gradient of mu+ at a sample's start point, from the start-point table instead of a POINT round (g == 0).
 // mu+ - m and the POINT round's sums S0, SB, s_d are affine in c, so kg_start_kernel tabulates, per discretisation
 // point, row 0 (the beta part) and rows 1+u (the union point u's part: k(a, Xu_u) - sum_j B_ju k(a, X_j)), columns
@@ -1287,7 +1304,9 @@ namespace cmoe {
 // observations a sample's start evaluation comes from the start-point table (start_from_table) when the lane takes the
 // sample, so a new sample's first round is a LINE round, in phase with the lanes that continue; only the general path
 // (GEN) spends a POINT round on it (ST_INIT).
-template <int KERNEL, int DIM, int QP, bool SMEM, bool GEN, bool WIDE = false, bool BIG = false>
+// PRE (GEN only): the large-union build of kg_mc_large_kernel; Wt holds the precomputed weight columns of the
+// candidate's samples (copy_sample_weights) and c is not read.
+template <int KERNEL, int DIM, int QP, bool SMEM, bool GEN, bool WIDE = false, bool BIG = false, bool PRE = false>
 __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* __restrict__ Xt,
                                            const double* __restrict__ Pk, const double* __restrict__ Xu, int cand,
                                            int s_begin, int s_end, int* next_sample, double* aw = nullptr,
@@ -1324,11 +1343,13 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
       if (sample < s_end) {
         if (prm.max_restarts > 0) {
           took_sample = true;
+          if constexpr (!PRE) {
 #pragma unroll
-          for (int u = 0; u < QP; ++u) c[u] = recC[static_cast<size_t>(sample) * QP + u];
-          if (GEN) {
+            for (int u = 0; u < QP; ++u) c[u] = recC[static_cast<size_t>(sample) * QP + u];
+            if (GEN) {
 #pragma unroll
-            for (int u = 0; u < QP; ++u) cl[GEN ? u : 0] = c[u];
+              for (int u = 0; u < QP; ++u) cl[GEN ? u : 0] = c[u];
+            }
           }
           const double* a0 = A + static_cast<size_t>(recStart[sample]) * DIM;
 #pragma unroll
@@ -1378,7 +1399,9 @@ __device__ __forceinline__ void kg_mc_body(const KgMcParams& prm, const double* 
     if (__all_sync(0xffffffffu, state == ST_DONE)) break;
     if (GEN) {
       const unsigned want = __ballot_sync(0xffffffffu, took_sample);
-      if (__popc(want) >= kOwnFillLanes) {
+      if constexpr (PRE) {
+        if (want) copy_sample_weights(Wt, prm.N * (1 + prm.g), aw - (threadIdx.x & 31), want, sample, threadIdx.x & 31);
+      } else if (__popc(want) >= kOwnFillLanes) {
         // many lanes at once (samples with equal round counts keep a warp's lanes in cohorts): every requesting lane
         // forms its own column from warp-uniform (broadcast) table loads; the column stores are full lines
         if (took_sample) fill_own_weights<QP>(Wt, prm.N * (1 + prm.g), c, aw);
@@ -1739,6 +1762,37 @@ __global__ void __launch_bounds__(kMcThreads, CMOE_MC_GEN_MINBLOCKS)
       kg_mc_body<KERNEL, DIM, QP, false, true, WIDE>(prm, prm.Xt, gPk, gXu, cand, s_begin, s_end, &next_sample, aw,
                                                      gWt, gen_ring + threadIdx.x);
     }
+    __syncthreads();  // next_sample / work_item are rewritten by thread 0
+  }
+}
+
+// Large-union build (kg_large.cu, DESIGN.md K17): the same state machine with the union points as ordinary weighted
+// points after the training points (prm.N = N + U, prm.U = 0).  Every point operand is per candidate (prm.Xt
+// [nc][N+U][DIM], prm.Pk [nc][N+U][pk_stride]) and the weight columns [beta - B c ; c] (~ convention) of every sample are
+// precomputed (prm.Wt [nc][num_mc][(N+U)(1+g)]), so the union size only sizes that table.  g == 0 is one row per point.
+template <int KERNEL, int DIM, bool WIDE>
+__global__ void __launch_bounds__(kMcThreads, CMOE_MC_GEN_MINBLOCKS)
+    kg_mc_large_kernel(const __grid_constant__ KgMcParams prm) {
+  extern __shared__ __align__(16) double gen_ring[];  // [kRingRows + kRingDepth][kMcThreads]
+  __shared__ int next_sample;
+  __shared__ int work_item;
+  const int R = prm.N * (1 + prm.g);
+  double* aw = prm.aw + static_cast<size_t>(blockIdx.x) * R * kMcThreads + threadIdx.x;
+  while (true) {
+    if (threadIdx.x == 0) work_item = atomicAdd(prm.work, 1);
+    __syncthreads();
+    const int w = work_item;
+    if (w >= prm.work_total) break;
+    const int cand = w / prm.chunks;
+    const int s_begin = (w % prm.chunks) * prm.chunk;
+    const int s_end = min(prm.num_mc, s_begin + prm.chunk);
+    if (threadIdx.x == 0) next_sample = s_begin + blockDim.x;
+    __syncthreads();
+    const double* gXt = prm.Xt + static_cast<size_t>(cand) * prm.N * DIM;
+    const double* gPk = prm.Pk + static_cast<size_t>(cand) * prm.N * prm.pk_stride;
+    const double* gWt = prm.Wt + static_cast<size_t>(cand) * prm.num_mc * R;
+    kg_mc_body<KERNEL, DIM, 2, false, true, WIDE, false, true>(prm, gXt, gPk, nullptr, cand, s_begin, s_end,
+                                                                &next_sample, aw, gWt, gen_ring + threadIdx.x);
     __syncthreads();  // next_sample / work_item are rewritten by thread 0
   }
 }
@@ -2128,6 +2182,19 @@ void launch_kg_mc_gen(const KgMcParams& p, int, int, cudaStream_t s) {
   const int grid = std::max(1, std::min(std::min(p.aw_slots, p.work_total), sms * std::max(1, per_sm)));
   kg_mc_gen_kernel<KERNEL, DIM, QP, WIDE><<<grid, kMcThreads, ring_bytes, s>>>(p);
 }
+// persistent grid over the p.work_total work items, at most one CTA per scratch slot
+template <int KERNEL, int DIM, bool WIDE>
+void launch_kg_mc_large(const KgMcParams& p, cudaStream_t s) {
+  int dev = 0, sms = 1, per_sm = 1;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const size_t ring_bytes = static_cast<size_t>(kRingRows + kRingDepth) * kMcThreads * sizeof(double);
+  cudaFuncSetAttribute(kg_mc_large_kernel<KERNEL, DIM, WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                       static_cast<int>(ring_bytes));
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kg_mc_large_kernel<KERNEL, DIM, WIDE>, kMcThreads, ring_bytes);
+  const int grid = std::max(1, std::min(std::min(p.aw_slots, p.work_total), sms * std::max(1, per_sm)));
+  kg_mc_large_kernel<KERNEL, DIM, WIDE><<<grid, kMcThreads, ring_bytes, s>>>(p);
+}
 // grid (128-row CTAs, candidates) over the (N + U) (1 + g) rows
 template <int KERNEL, int DIM, int QP, bool GEN>
 void launch_kg_acc(const KgAccParams& p, int nb, cudaStream_t s) {
@@ -2220,5 +2287,32 @@ const KgDispatchEntry* find_kg_entry(int kernel, int dim, int Q, int g);
 #define CMOE_KG_WIDE_ENTRIES_FOR_DIM(D)                                                                    \
   kg_entry<0, D, 16, kKgWide>(), kg_entry<0, D, 24, kKgWide>(), kg_entry<0, D, 32, kKgWide>(),             \
       kg_entry<1, D, 16, kKgWide>(), kg_entry<1, D, 24, kKgWide>(), kg_entry<1, D, 32, kKgWide>()
+
+// The large-union build's run-time dispatch table (kg_large.cu): one entry per kernel, padded dimension and ring kind.
+using KgLargeLaunch = void (*)(const KgMcParams&, cudaStream_t);
+struct KgLargeEntry {
+  int kernel, dim;
+  bool wide;  // 9 <= g <= 31 (stream_point_weights_wide)
+  KgLargeLaunch mc;
+};
+bool register_kg_large_entries(std::initializer_list<KgLargeEntry> entries);
+const KgLargeEntry* find_kg_large_entry(int kernel, int dim, int g);
+#define CMOE_KG_LARGE_ENTRIES_FOR_DIM(D) \
+  KgLargeEntry{0, D, false, &launch_kg_mc_large<0, D, false>}, KgLargeEntry{1, D, false, &launch_kg_mc_large<1, D, false>}
+#define CMOE_KG_LARGE_WIDE_ENTRIES_FOR_DIM(D) \
+  KgLargeEntry{0, D, true, &launch_kg_mc_large<0, D, true>}, KgLargeEntry{1, D, true, &launch_kg_mc_large<1, D, true>}
+
+// kg.cu's per-candidate stages that the large-union path shares (asynchronous on s)
+// KG[c] = best_posterior[c] + mean of outVal[c][:], NaN where fail[c] != 0 (kg_value_kernel)
+void kg_value(int nb, int num_mc, const double* outVal, const double* best_post, const int* fail, double* kg,
+              cudaStream_t s);
+// every sample's minimiser <- the max_num_restarts <= 0 fill value, in the operands' frame (kg_fill_point_kernel)
+void kg_fill_points(const KernelSpec& spec, const Centre& ctr, int samples, int DIMP, double* outX, double* outH,
+                    cudaStream_t s);
+// Tp[c][a'][a] = R[c][a'][n + a] - sum_j R[c][a'][j] B[c][a][j]  (kg_tprime_kernel); R [nb][QP][n + Q], B [nb][Q][n]
+void kg_tprime(int nb, int n, int Q, int QP, const double* R, const double* B, double* Tp, cudaStream_t s);
+// G1[c][p][d] = sum_i sum_m c_i,(p,m) d K(Xu_p row m, x*_i) / d Xu_p,d  (kg_g1_kernel); recC [nb][num_mc][QP]
+void kg_g1(const KernelSpec& spec, const Centre& ctr, int nb, int U, int q, int QP, int DIMP, int num_mc,
+           const double* P, const double* recC, const double* outX, double* G1, cudaStream_t s);
 
 }  // namespace cmoe

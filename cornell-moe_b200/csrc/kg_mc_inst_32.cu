@@ -5,5 +5,6 @@
 namespace cmoe {
 namespace {
 const bool registered = register_kg_entries({CMOE_KG_ENTRIES_FOR_DIM(32)});
+const bool registered_large = register_kg_large_entries({CMOE_KG_LARGE_ENTRIES_FOR_DIM(32)});
 }  // namespace
 }  // namespace cmoe

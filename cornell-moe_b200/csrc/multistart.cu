@@ -190,9 +190,19 @@ void multistart_common(const BatchEval& eval, const cmoe_gd_params& outer, const
   if (found_flag) *found_flag = found;
 }
 
+// The q-KG evaluator of the drivers: two plans (values, gradients) for unions of up to 32 rows, (q + p)(1 + g), and
+// cmoe_kg_eval_large's stages (kg_large_eval) past them, with the same normals table and stale union.
 struct KgEvaluator {
   cmoe_kg_plan* vplan = nullptr;
   cmoe_kg_plan* gplan = nullptr;
+  // large path: the evaluation's arguments (host copies)
+  bool large = false;
+  const cmoe_gp* gp = nullptr;
+  int nf = 0, num_pts = 0, q = 0, p = 0, num_mc = 0;
+  double best_so_far = 0.0;
+  uint64_t seed = 0;
+  cmoe_gd_params inner{};
+  std::vector<double> inner_bounds, discrete, Xp, stale, table;
   ~KgEvaluator() {
     cmoe_kg_plan_destroy(vplan);
     cmoe_kg_plan_destroy(gplan);
@@ -200,7 +210,25 @@ struct KgEvaluator {
   static void check(int rc, int info = 0) {
     if (rc != CMOE_OK) throw Error(rc, cmoe_last_error(), info);
   }
+  // replays `t` (NormalRNGSimulator semantics) in every evaluation
+  void set_table(const double* t, size_t len) {
+    if (!large) {
+      check(cmoe_kg_plan_set_table(vplan, t, static_cast<int>(len)));
+      check(cmoe_kg_plan_set_table(gplan, t, static_cast<int>(len)));
+      return;
+    }
+    const size_t need = static_cast<size_t>((num_mc + 1) / 2) * (q + p) * (1 + gp->spec.g);
+    CMOE_REQUIRE(len >= need, CMOE_ERR_INVALID_VALUE, "All random numbers stored in the RNG have been used up!");
+    table.assign(t, t + need);
+  }
   void operator()(const double* pts, int nc, double* values, double* grads) {
+    if (large) {
+      require_device(gp->device);  // may run on a worker thread of the multi-device driver
+      kg_large_eval(gp, nf, &inner, inner_bounds.data(), discrete.data(), num_pts, pts, nc, q, Xp.data(), p, num_mc,
+                    best_so_far, seed, table.empty() ? nullptr : table.data(), stale.empty() ? nullptr : stale.data(),
+                    values, grads, nullptr);
+      return;
+    }
     cmoe_kg_plan* pl = grads ? gplan : vplan;
     int info = 0;
     check(cmoe_kg_plan_upload(pl, pts, nc));
@@ -213,7 +241,27 @@ struct KgEvaluator {
 void make_kg_evaluator(KgEvaluator& ev, const cmoe_gp* gp, int nf, const cmoe_gd_params* inner,
                        const double* inner_bounds, const double* discrete_pts, int num_pts, int max_value_cands,
                        int max_grad_cands, int q, const double* Xp, int p, int num_mc, double best_so_far,
-                       uint64_t seed, const double* stale_union = nullptr) {
+                       uint64_t seed, const double* stale_union = nullptr, bool allow_large = true) {
+  // the ensemble calls keep the plans' 32-row bound (cmoe_kg_plan_create refuses larger unions)
+  if (allow_large && static_cast<long long>(q + p) * (1 + gp->spec.g) > 32) {
+    const int dim = gp->spec.dim, ps = dim - nf;
+    CMOE_REQUIRE(nf >= 0 && ps >= 1 && num_pts >= 0, CMOE_ERR_BOUNDS, "num_fidelity out of range");
+    ev.large = true;
+    ev.gp = gp;
+    ev.nf = nf;
+    ev.num_pts = num_pts;
+    ev.q = q;
+    ev.p = p;
+    ev.num_mc = num_mc;
+    ev.best_so_far = best_so_far;
+    ev.seed = seed;
+    ev.inner = *inner;
+    ev.inner_bounds.assign(inner_bounds, inner_bounds + 2 * static_cast<size_t>(ps));
+    ev.discrete.assign(discrete_pts, discrete_pts + static_cast<size_t>(num_pts) * ps);
+    if (p) ev.Xp.assign(Xp, Xp + static_cast<size_t>(p) * dim);
+    if (stale_union) ev.stale.assign(stale_union, stale_union + static_cast<size_t>(q) * dim);
+    return;
+  }
   KgEvaluator::check(cmoe_kg_plan_create(gp, nf, inner, inner_bounds, discrete_pts, num_pts, max_value_cands, q, Xp, p,
                                          num_mc, best_so_far, seed, 0, &ev.vplan));
   KgEvaluator::check(cmoe_kg_plan_create(gp, nf, inner, inner_bounds, discrete_pts, num_pts, max_grad_cands, q, Xp, p,
@@ -458,7 +506,7 @@ void make_kg_ensemble(KgEnsembleEvaluator& ens, const cmoe_gp* const* gps, int n
     ens.evs.emplace_back(new KgEvaluator());
     make_kg_evaluator(*ens.evs.back(), gps[m], nf, inner, inner_bounds,
                       discrete_pts + static_cast<size_t>(m) * num_pts * (dim - nf), num_pts, max_value_cands,
-                      max_grad_cands, q, Xp, p, num_mc, best_so_far[m], seed);
+                      max_grad_cands, q, Xp, p, num_mc, best_so_far[m], seed, nullptr, false);
   }
 }
 
@@ -535,10 +583,7 @@ int cmoe_multistart_kg_ex(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_par
       make_kg_evaluator(w.kg, w.gp, num_fidelity, inner, inner_bounds, discrete_pts, num_pts, (num_starts + G - 1) / G,
                         (std::min(kTopK, num_starts) + G - 1) / G, q, points_being_sampled, p, num_mc, best_so_far, seed,
                         stale);
-      if (opts && opts->normals_table) {
-        KgEvaluator::check(cmoe_kg_plan_set_table(w.kg.vplan, opts->normals_table, static_cast<int>(opts->table_len)));
-        KgEvaluator::check(cmoe_kg_plan_set_table(w.kg.gplan, opts->normals_table, static_cast<int>(opts->table_len)));
-      }
+      if (opts && opts->normals_table) w.kg.set_table(opts->normals_table, opts->table_len);
       w.eval = std::ref(w.kg);
     }
     BatchEval f = std::ref(sh);

@@ -404,6 +404,24 @@ int cmoe_kg_eval(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_params* inne
                  const double* discrete_pts, int num_pts, const double* candidates, int num_candidates, int q,
                  const double* points_being_sampled, int p, int num_mc, double best_so_far, uint64_t seed,
                  const double* normals_table, double* kg, double* grad_kg, cmoe_kg_stats* stats, int* info);
+/* Largest Q = (q + p)(1 + num_derivatives) of cmoe_kg_eval_large. */
+#define CMOE_MAX_KG_LARGE_ROWS 1024
+/* cmoe_kg_eval for 1 <= Q = (q + p)(1 + g) <= CMOE_MAX_KG_LARGE_ROWS: same arguments, same draws, same argument checks
+ * (g <= 31, distinct partials past 8).  The fantasised posterior of each sample is a GP mean over the training points
+ * followed by the union points with per-sample weights (DESIGN.md K17), so the union size only sizes dense products;
+ * the inner optimiser is cmoe_kg_eval's line-search descent, and the gradient is taken in reverse mode through the union's
+ * Cholesky factor.  The call's device workspace (the draws, the inner optimiser's scratch, chunks of candidates) is at
+ * most 2 GiB, kept on the handle; a candidate's value and gradient do not depend on num_candidates or the chunking.
+ * CMOE_ERR_BOUNDS, before any device work, when one candidate's workspace does not fit.  A singular union covariance -> CMOE_ERR_SINGULAR, *info = leading minor of
+ * the first failing candidate.  stats: mc_samples exact, posterior_evals and line_search_steps as cmoe_kg_stats,
+ * point_evals and line_batches what this call's kernel executed.  num_mc <= 65535 * 64.  The multistart q-KG drivers
+ * (cmoe_multistart_kg(_ex), cmoe_kg_gradient_descent(_ex)) evaluate through these stages when (q + p)(1 + g) > 32 and
+ * through the plans otherwise.  Not covered: the cmoe_kg_plan_* API, the ensemble calls (cmoe_kg_eval_mcmc,
+ * cmoe_multistart_kg_mcmc, cmoe_kg_gradient_descent_mcmc) and multigpu.py keep the 32-row bound of cmoe_kg_eval. */
+int cmoe_kg_eval_large(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_params* inner, const double* inner_bounds,
+                       const double* discrete_pts, int num_pts, const double* candidates, int num_candidates, int q,
+                       const double* points_being_sampled, int p, int num_mc, double best_so_far, uint64_t seed,
+                       const double* normals_table, double* kg, double* grad_kg, cmoe_kg_stats* stats, int* info);
 
 /* ---- device-resident plan for the q-KG path (what bench.py times as `value`) ------------------------------------
  * Same computation as cmoe_kg_eval, split so that inputs can be made resident in HBM before the timed region:
