@@ -121,7 +121,7 @@ def _i(a):
 
 
 def set_option(name, value):
-    """cmoe_set_option: 'legacy_linalg' / 'cov_tma' (0 or 1)."""
+    """cmoe_set_option: 'legacy_linalg' / 'cov_tma' (0 or 1), 'ensemble_members_in_flight' (k >= 0; 0 = no cap)."""
     _check(lib().cmoe_set_option(name.encode(), int(value)))
 
 

@@ -393,75 +393,116 @@ __global__ void __launch_bounds__(kGradThreads) ei_grad_kernel(const __grid_cons
 }
 
 
-// Device scratch of one chunk beyond the K8 workspace.
-struct EiLargeWork {
-  DevBuf<double> part_v, imp, ei, T1, T2, R, grad;
-  DevBuf<int> part_i, win, cnt, start, order;
+// Device pointers of one GP's run: the chunk workspace (chunk candidates)
+struct EiLargeBufs {
+  int chunk = 0;
+  double *P, *V, *A, *mu, *stage, *part_v, *imp, *ei;
+  double *T1 = nullptr, *T2 = nullptr, *R = nullptr, *grad = nullptr;
+  int *fail, *part_i, *win, *dPs;
+  int *cnt = nullptr, *start = nullptr, *order = nullptr;
 };
 
-void ei_large_chunk(const cmoe_gp& gp, SampleWork& w, EiLargeWork& e, const double* candidates, int nc, int q,
-                    const double* Xp, int p, int num_mc, double best_so_far, const double* W, double* ei_host,
-                    double* grad_host) {
-  cudaStream_t s = gp.stream;
-  const int U = q + p, dim = gp.spec.dim, n = gp.n;
-  const bool want_grad = grad_host != nullptr;
-  {
-    std::vector<double> h(static_cast<size_t>(nc) * U * dim);
-    for (int c = 0; c < nc; ++c) {
-      double* dst = h.data() + static_cast<size_t>(c) * U * dim;
-      std::copy(candidates + static_cast<size_t>(c) * q * dim, candidates + static_cast<size_t>(c + 1) * q * dim, dst);
-      if (p) std::copy(Xp, Xp + static_cast<size_t>(p) * dim, dst + static_cast<size_t>(q) * dim);
-    }
-    w.P.upload(h.data(), h.size(), s);
-    CMOE_CUDA(cudaStreamSynchronize(s));  // h goes out of scope
-  }
-  // mu, Var + 1e-6 I (gpp_math.cpp:2000-2002) and its factor C, upper triangle zero
-  posterior_cov_large(gp, w, nc, U, 0, 1.0e-6, s);
-  CMOE_CUDA(cudaMemsetAsync(w.fail.p, 0, nc * sizeof(int), s));
-  potrf_batched(w.A.p, U, nc, w.fail.p, w.stage, s);
-  std::vector<int> hfail(nc);
-  w.fail.download(hfail.data(), nc, s);
-  CMOE_CUDA(cudaStreamSynchronize(s));
-  for (int c = 0; c < nc; ++c)
-    if (hfail[c] != 0)
-      throw Error(CMOE_ERR_SINGULAR,
-                  "GP-Variance matrix singular. Check for duplicate points_to_sample/being_sampled or "
-                  "points_to_sample/being_sampled duplicating points_sampled with 0 noise.",
-                  hfail[c]);
-  zero_upper(nc, U, w.A.p, s);
-  // forward
-  const int nrb = (U + NB - 1) / NB, nsb = (num_mc + NB - 1) / NB;
-  CMOE_CUDA(cudaFuncSetAttribute(ei_mc_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 static_cast<int>(kTileSmem)));
-  ei_mc_tile_kernel<<<dim3(nsb, nrb, nc), kTileThreads, kTileSmem, s>>>(U, num_mc, best_so_far, W, w.mu.p, w.A.p,
-                                                                        e.part_v.p, e.part_i.p);
-  ei_winner_kernel<<<dim3((num_mc + 255) / 256, nc), 256, 0, s>>>(num_mc, nrb, e.part_v.p, e.part_i.p, e.imp.p,
-                                                                  e.win.p);
-  ei_value_kernel<<<nc, 256, 0, s>>>(num_mc, e.imp.p, e.ei.p);
-  count_launch(3);
-  CMOE_CUDA(cudaGetLastError());
-  e.ei.download(ei_host, nc, s);
+// Lays out one GP's chunk workspace for `chunk` candidates at cv.
+void ei_large_carve(int n, int U, int q, int dim, int num_mc, bool want_grad, int chunk, Carve& cv, EiLargeBufs& b) {
+  const size_t ch = static_cast<size_t>(chunk), UU = static_cast<size_t>(U) * U, nrb = (U + NB - 1) / NB;
+  b.chunk = chunk;
+  b.P = cv.take<double>(ch * U * dim);
+  b.V = cv.take<double>(ch * U * n);
+  b.A = cv.take<double>(ch * UU);
+  b.mu = cv.take<double>(ch * U);
+  b.stage = cv.take<double>(ch * nrb * NB * NB);
+  b.fail = cv.take<int>(ch);
+  b.dPs = cv.take<int>(1);
+  b.part_v = cv.take<double>(ch * nrb * num_mc);
+  b.part_i = cv.take<int>(ch * nrb * num_mc);
+  b.imp = cv.take<double>(ch * num_mc);
+  b.win = cv.take<int>(ch * num_mc);
+  b.ei = cv.take<double>(ch);
   if (want_grad) {
-    const size_t UU = static_cast<size_t>(U) * U;
-    const unsigned gUU = static_cast<unsigned>((UU + 255) / 256);
-    // B = K^-1 K(X, P) = L^-T V in place of V (cov_tile_kernel has consumed V)
-    trsm_lower_blocked(gp.dK.p, n, w.V.p, n, nc * U, true, s);
-    const size_t smem_bucket = static_cast<size_t>(U) * sizeof(int);
-    CMOE_CUDA(cudaFuncSetAttribute(ei_bucket_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   static_cast<int>(smem_bucket)));
-    ei_bucket_kernel<<<nc, kBucketThreads, smem_bucket, s>>>(U, num_mc, e.win.p, e.cnt.p, e.start.p, e.order.p);
-    ei_cbar_kernel<<<dim3(gUU, nc), 256, 0, s>>>(U, num_mc, W, e.cnt.p, e.start.p, e.order.p, e.T1.p);
-    count_launch(2);
-    cholesky_adjoint(w.A.p, U, nc, e.T1.p, e.T2.p, s);
-    // R = B T[:, :q]
-    gemm_nn(n, q, U, w.V.p, n, static_cast<size_t>(n) * U, e.T1.p, U, UU, e.R.p, n, static_cast<size_t>(n) * q, nc, s);
-    ei_grad_kernel<<<dim3(q, nc), kGradThreads, 0, s>>>(gp.spec, gp.N, gp.dX.p, gp.dKinvY.p, w.P.p, U, q, num_mc,
-                                                        e.T1.p, e.R.p, e.cnt.p, e.grad.p);
-    count_launch();
-    CMOE_CUDA(cudaGetLastError());
-    e.grad.download(grad_host, static_cast<size_t>(nc) * q * dim, s);
+    b.T1 = cv.take<double>(ch * UU);
+    b.T2 = cv.take<double>(ch * UU);
+    b.R = cv.take<double>(ch * n * q);
+    b.grad = cv.take<double>(ch * q * dim);
+    b.cnt = cv.take<int>(ch * U);
+    b.start = cv.take<int>(ch * U);
+    b.order = cv.take<int>(ch * num_mc);
   }
-  CMOE_CUDA(cudaStreamSynchronize(s));
+}
+
+size_t ei_large_chunk_bytes(int n, int U, int q, int dim, int num_mc, bool want_grad, int chunk) {
+  Carve cv;
+  EiLargeBufs b;
+  ei_large_carve(n, U, q, dim, num_mc, want_grad, chunk, cv, b);
+  return cv.off;
+}
+
+// the union sets of one chunk, P [nb][q + p][dim]: each candidate's q points, then the pending points
+__global__ void __launch_bounds__(256) ei_sets_kernel(int q, int p, int dim, const double* __restrict__ cand,
+                                                      const double* __restrict__ Xp, double* __restrict__ P) {
+  const int c = blockIdx.x, U = q + p;
+  for (int e = threadIdx.x; e < U * dim; e += blockDim.x) {
+    const int u = e / dim, d = e % dim;
+    P[static_cast<size_t>(c) * U * dim + e] =
+        u < q ? cand[(static_cast<size_t>(c) * q + u) * dim + d] : Xp[static_cast<size_t>(u - q) * dim + d];
+  }
+}
+
+void ei_large_run(const cmoe_gp& gp, const EiLargeBufs& b, const double* cand, const double* Xp, int nc, int q, int p,
+                  int num_mc, double best_so_far, const double* W, cudaStream_t s, double* ei_out, double* grad_out,
+                  int* fail_out) {
+  const int U = q + p, dim = gp.spec.dim, n = gp.n;
+  const bool want_grad = grad_out != nullptr;
+  const int nrb = (U + NB - 1) / NB, nsb = (num_mc + NB - 1) / NB;
+  const size_t UU = static_cast<size_t>(U) * U;
+  const unsigned gUU = static_cast<unsigned>((UU + 255) / 256);
+  for (int c0 = 0; c0 < nc; c0 += b.chunk) {
+    const int nb = std::min(b.chunk, nc - c0);
+    const double* P = b.P;
+    ei_sets_kernel<<<nb, 256, 0, s>>>(q, p, dim, cand + static_cast<size_t>(c0) * q * dim, Xp, b.P);
+    count_launch();
+    // mu, Var + 1e-6 I (gpp_math.cpp:2000-2002) and its factor C, upper triangle zero
+    posterior_cov_large(gp, P, b.dPs, b.V, b.mu, b.A, nb, U, 0, 1.0e-6, s);
+    CMOE_CUDA(cudaMemsetAsync(b.fail, 0, nb * sizeof(int), s));
+    potrf_batched(b.A, U, nb, b.fail, b.stage, s);
+    CMOE_CUDA(cudaMemcpyAsync(fail_out + c0, b.fail, nb * sizeof(int), cudaMemcpyDeviceToDevice, s));
+    zero_upper(nb, U, b.A, s);
+    // forward
+    CMOE_CUDA(cudaFuncSetAttribute(ei_mc_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   static_cast<int>(kTileSmem)));
+    ei_mc_tile_kernel<<<dim3(nsb, nrb, nb), kTileThreads, kTileSmem, s>>>(U, num_mc, best_so_far, W, b.mu, b.A,
+                                                                          b.part_v, b.part_i);
+    ei_winner_kernel<<<dim3((num_mc + 255) / 256, nb), 256, 0, s>>>(num_mc, nrb, b.part_v, b.part_i, b.imp, b.win);
+    ei_value_kernel<<<nb, 256, 0, s>>>(num_mc, b.imp, b.ei);
+    count_launch(3);
+    CMOE_CUDA(cudaGetLastError());
+    CMOE_CUDA(cudaMemcpyAsync(ei_out + c0, b.ei, nb * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    if (want_grad) {
+      // B = K^-1 K(X, P) = L^-T V in place of V (cov_tile_kernel has consumed V)
+      trsm_lower_blocked(gp.dK.p, n, b.V, n, nb * U, true, s);
+      const size_t smem_bucket = static_cast<size_t>(U) * sizeof(int);
+      CMOE_CUDA(cudaFuncSetAttribute(ei_bucket_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     static_cast<int>(smem_bucket)));
+      ei_bucket_kernel<<<nb, kBucketThreads, smem_bucket, s>>>(U, num_mc, b.win, b.cnt, b.start, b.order);
+      ei_cbar_kernel<<<dim3(gUU, nb), 256, 0, s>>>(U, num_mc, W, b.cnt, b.start, b.order, b.T1);
+      count_launch(2);
+      cholesky_adjoint(b.A, U, nb, b.T1, b.T2, s);
+      // R = B T[:, :q]
+      gemm_nn(n, q, U, b.V, n, static_cast<size_t>(n) * U, b.T1, U, UU, b.R, n, static_cast<size_t>(n) * q, nb, s);
+      ei_grad_kernel<<<dim3(q, nb), kGradThreads, 0, s>>>(gp.spec, gp.N, gp.dX.p, gp.dKinvY.p, P, U, q, num_mc, b.T1,
+                                                          b.R, b.cnt, b.grad);
+      count_launch();
+      CMOE_CUDA(cudaGetLastError());
+      CMOE_CUDA(cudaMemcpyAsync(grad_out + static_cast<size_t>(c0) * q * dim, b.grad,
+                                static_cast<size_t>(nb) * q * dim * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    }
+  }
+}
+
+void check_ei_large_sizes(int q, int p, int num_mc) {
+  CMOE_REQUIRE(q >= 1 && p >= 0 && num_mc >= 1, CMOE_ERR_BOUNDS, "q >= 1, p >= 0, num_mc >= 1 required");
+  CMOE_REQUIRE(static_cast<long long>(q) + p <= kMaxSampleQ, CMOE_ERR_BOUNDS, "q + p must be <= 8192");
+  CMOE_REQUIRE(static_cast<size_t>(num_mc) * (q + p) <= kSampleWorkspaceBytes / sizeof(double), CMOE_ERR_BOUNDS,
+               "num_mc * (q + p) normals must fit in 2 GiB");
 }
 
 }  // namespace
@@ -497,10 +538,7 @@ void cholesky_adjoint(const double* C, int U, int nc, double* T1, double* T2, cu
 void ei_large_eval_batch(const cmoe_gp& gp, const double* candidates, int nc, int q, const double* Xp, int p,
                          int num_mc, double best_so_far, uint64_t seed, const double* dtable, double* ei_host,
                          double* grad_host) {
-  CMOE_REQUIRE(q >= 1 && p >= 0 && num_mc >= 1, CMOE_ERR_BOUNDS, "q >= 1, p >= 0, num_mc >= 1 required");
-  CMOE_REQUIRE(static_cast<long long>(q) + p <= kMaxSampleQ, CMOE_ERR_BOUNDS, "q + p must be <= 8192");
-  CMOE_REQUIRE(static_cast<size_t>(num_mc) * (q + p) <= kSampleWorkspaceBytes / sizeof(double), CMOE_ERR_BOUNDS,
-               "num_mc * (q + p) normals must fit in 2 GiB");
+  check_ei_large_sizes(q, p, num_mc);
   cudaStream_t s = gp.stream;
   const int U = q + p, dim = gp.spec.dim, n = gp.n;
   const bool want_grad = grad_host != nullptr;
@@ -511,42 +549,93 @@ void ei_large_eval_batch(const cmoe_gp& gp, const double* candidates, int nc, in
     philox_normals_device(seed, 0, num_mc, U, Wgen.p, s);
     W = Wgen.p;
   }
-  const size_t UU = static_cast<size_t>(U) * U, nrb = (U + NB - 1) / NB;
-  const size_t per_cand =
-      sizeof(double) * (static_cast<size_t>(n) * U + UU + U + static_cast<size_t>(U) * dim + nrb * NB * NB + 1 +
-                        nrb * num_mc + num_mc) +
-      sizeof(int) * (2 + nrb * num_mc + num_mc) +
-      (want_grad ? sizeof(double) * (2 * UU + static_cast<size_t>(n) * q + static_cast<size_t>(q) * dim) +
-                       sizeof(int) * (2 * static_cast<size_t>(U) + num_mc)
-                 : 0);
-  const int chunk = static_cast<int>(chunk_items(nc, kSampleWorkspaceBytes, per_cand, kMaxChunkSets));
+  // the candidates and the pending points, uploaded once; each chunk forms its union sets on the device
+  DevBuf<double> dcand, dXp;
+  dcand.upload(candidates, static_cast<size_t>(nc) * q * dim, s);
+  if (p) dXp.upload(Xp, static_cast<size_t>(p) * dim, s);
+  // chunks of the 2 GiB workspace, a region on the handle (SampleWork::ei_large)
+  const size_t per_cand = ei_large_chunk_bytes(n, U, q, dim, num_mc, want_grad, 1);
+  const int chunk = static_cast<int>(chunk_items(nc, kSampleWorkspaceBytes - kCarveSlack, per_cand, kMaxChunkSets));
   SampleWork& w = sample_work(gp);
-  w.P.ensure(static_cast<size_t>(chunk) * U * dim);
-  w.V.ensure(static_cast<size_t>(chunk) * U * n);
-  w.A.ensure(static_cast<size_t>(chunk) * UU);
-  w.mu.ensure(static_cast<size_t>(chunk) * U);
-  w.fail.ensure(chunk);
-  w.dPs.ensure(1);
-  EiLargeWork e;
-  e.part_v.alloc(static_cast<size_t>(chunk) * nrb * num_mc);
-  e.part_i.alloc(static_cast<size_t>(chunk) * nrb * num_mc);
-  e.imp.alloc(static_cast<size_t>(chunk) * num_mc);
-  e.win.alloc(static_cast<size_t>(chunk) * num_mc);
-  e.ei.alloc(chunk);
-  if (want_grad) {
-    e.T1.alloc(static_cast<size_t>(chunk) * UU);
-    e.T2.alloc(static_cast<size_t>(chunk) * UU);
-    e.R.alloc(static_cast<size_t>(chunk) * n * q);
-    e.grad.alloc(static_cast<size_t>(chunk) * q * dim);
-    e.cnt.alloc(static_cast<size_t>(chunk) * U);
-    e.start.alloc(static_cast<size_t>(chunk) * U);
-    e.order.alloc(static_cast<size_t>(chunk) * num_mc);
-  }
-  for (int c0 = 0; c0 < nc; c0 += chunk) {
-    const int nb = std::min(chunk, nc - c0);
-    ei_large_chunk(gp, w, e, candidates + static_cast<size_t>(c0) * q * dim, nb, q, Xp, p, num_mc, best_so_far, W,
-                   ei_host + c0, want_grad ? grad_host + static_cast<size_t>(c0) * q * dim : nullptr);
-  }
+  w.ei_large.ensure((ei_large_chunk_bytes(n, U, q, dim, num_mc, want_grad, chunk) + sizeof(double) - 1) /
+                    sizeof(double));
+  EiLargeBufs b;
+  Carve cv{reinterpret_cast<char*>(w.ei_large.p)};
+  ei_large_carve(n, U, q, dim, num_mc, want_grad, chunk, cv, b);
+  // the call's results, read back once
+  DevBuf<double> dei(nc), dgrad(want_grad ? static_cast<size_t>(nc) * q * dim : 0);
+  DevBuf<int> dfail(nc);
+  ei_large_run(gp, b, dcand.p, dXp.p, nc, q, p, num_mc, best_so_far, W, s, dei.p, want_grad ? dgrad.p : nullptr,
+               dfail.p);
+  std::vector<int> hfail(nc);
+  dfail.download(hfail.data(), nc, s);
+  dei.download(ei_host, nc, s);
+  if (want_grad) dgrad.download(grad_host, static_cast<size_t>(nc) * q * dim, s);
+  CMOE_CUDA(cudaStreamSynchronize(s));
+  for (int c = 0; c < nc; ++c)
+    if (hfail[c] != 0) throw_singular_union(hfail[c]);
+}
+
+void ei_large_ensemble_eval(const cmoe_gp* const* gps, int num_gp, const double* candidates, int nc, int q,
+                            const double* Xp, int p, int num_mc, const double* best_so_far, uint64_t seed,
+                            const double* normals_table, double* values, double* grads) {
+  check_ei_large_sizes(q, p, num_mc);
+  require_device(gps[0]->device);
+  const int U = q + p, dim = gps[0]->spec.dim;
+  const bool want_grad = grads != nullptr;
+  // the normals are counted once; the W members in flight share the rest of the 2 GiB.  As in the single call, a
+  // candidate that alone needs more is not refused: it runs alone, one member at a time.
+  const size_t w_count = static_cast<size_t>(num_mc) * U;
+  const size_t budget = kSampleWorkspaceBytes - w_count * sizeof(double);
+  size_t per = 0;
+  for (int m = 0; m < num_gp; ++m)
+    per = std::max(per, ei_large_chunk_bytes(gps[m]->n, U, q, dim, num_mc, want_grad, 1));
+  size_t width = std::min<size_t>(num_gp, budget / (per + kCarveSlack));
+  if (ensemble_members_in_flight() > 0) width = std::min<size_t>(width, ensemble_members_in_flight());
+  width = std::max<size_t>(1, width);
+  const size_t share = budget / width;
+  const int chunk = static_cast<int>(chunk_items(nc, share > kCarveSlack ? share - kCarveSlack : 0, per, kMaxChunkSets));
+  size_t slot_bytes = 0;
+  for (int m = 0; m < num_gp; ++m)
+    slot_bytes = std::max(slot_bytes, ei_large_chunk_bytes(gps[m]->n, U, q, dim, num_mc, want_grad, chunk));
+  slot_bytes = (slot_bytes + 255) & ~size_t(255);
+  // one region on the first member's handle: the normals, the candidates and pending points, every member's results,
+  // the W slots
+  const size_t ps = static_cast<size_t>(q) * dim;
+  double *Wd = nullptr, *dcand = nullptr, *dXp = nullptr, *dval = nullptr, *dgrad = nullptr;
+  int* dfail = nullptr;
+  char* slots = nullptr;
+  auto layout = [&](Carve& cv) {
+    Wd = cv.take<double>(w_count);
+    dcand = cv.take<double>(static_cast<size_t>(nc) * ps);
+    dXp = cv.take<double>(static_cast<size_t>(std::max(1, p)) * dim);
+    dval = cv.take<double>(static_cast<size_t>(num_gp) * nc);
+    dgrad = want_grad ? cv.take<double>(static_cast<size_t>(num_gp) * nc * ps) : nullptr;
+    dfail = cv.take<int>(static_cast<size_t>(num_gp) * nc);
+    slots = cv.take<char>(slot_bytes * width);
+  };
+  Carve cv;
+  layout(cv);
+  EnsembleWork& ew = ensemble_work(*gps[0], cv.off);
+  cv = Carve{reinterpret_cast<char*>(ew.arena.p)};
+  layout(cv);
+  cudaStream_t s0 = gps[0]->stream;
+  if (normals_table)
+    CMOE_CUDA(cudaMemcpyAsync(Wd, normals_table, w_count * sizeof(double), cudaMemcpyHostToDevice, s0));
+  else
+    philox_normals_device(seed, 0, num_mc, U, Wd, s0);
+  CMOE_CUDA(cudaMemcpyAsync(dcand, candidates, static_cast<size_t>(nc) * ps * sizeof(double), cudaMemcpyHostToDevice,
+                            s0));
+  if (p) CMOE_CUDA(cudaMemcpyAsync(dXp, Xp, static_cast<size_t>(p) * dim * sizeof(double), cudaMemcpyHostToDevice, s0));
+  CMOE_CUDA(cudaStreamSynchronize(s0));
+  run_members(gps, num_gp, static_cast<int>(width), ew, [&](int m, int slot) {
+    EiLargeBufs b;
+    Carve sc{slots + slot * slot_bytes};
+    ei_large_carve(gps[m]->n, U, q, dim, num_mc, want_grad, chunk, sc, b);
+    ei_large_run(*gps[m], b, dcand, dXp, nc, q, p, num_mc, best_so_far[m], Wd, gps[m]->stream, dval + m * nc,
+                 want_grad ? dgrad + m * nc * ps : nullptr, dfail + m * nc);
+  });
+  drain_members(s0, num_gp, nc, ps, dval, dgrad, dfail, values, grads);
 }
 
 }  // namespace cmoe

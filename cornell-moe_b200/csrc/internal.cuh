@@ -9,6 +9,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <stdexcept>
 #include <string>
@@ -157,6 +158,9 @@ struct cmoe_gp {
   mutable std::shared_ptr<void> sample_ws;
   // device workspace of cmoe_kg_eval_large (kg_large.cu), grown on demand and kept until the handle is destroyed
   mutable std::shared_ptr<void> kg_large_ws;
+  // device workspace of the ensemble evaluations past the per-set bounds whose first member is this handle
+  // (cmoe::EnsembleWork), grown on demand up to one evaluation's need and kept until the handle is destroyed
+  mutable std::shared_ptr<void> ensemble_ws;
   mutable uint64_t replicas_generation = 0;
   ~cmoe_gp();
 };
@@ -216,11 +220,14 @@ constexpr int kMaxChunkSets = 4096;
 // zero on entry and receives 0 or the 1-based leading minor of the first pivot that fails `> 1e-16`.  `stage` holds the
 // diagonal factors until the end (nsets * ceil(Q/64) * 64 * 64 doubles).  Asynchronous on `s`.
 void potrf_batched(double* A, int Q, int nsets, int* fail, DevBuf<double>& stage, cudaStream_t s);
+// the same with the caller's stage buffer (at least nsets * ceil(Q/64) * 64 * 64 doubles)
+void potrf_batched(double* A, int Q, int nsets, int* fail, double* stage, cudaStream_t s);
 // Device workspace of the sampling calls and of the LCB screen (lcb.cu), kept on the GP handle (cmoe_gp::sample_ws) and
 // grown on demand, so repeated calls do not allocate and free up to kSampleWorkspaceBytes each time.  Released with the
 // handle.
 struct SampleWork {
   DevBuf<double> P, V, A, mu, y, part_v, opt, stage, table;
+  DevBuf<double> ei_large;  // the chunk workspace of ei_large_eval_batch, carved by ei_large.cu
   DevBuf<int> dPs, fail, part_i, amin;
 };
 // the handle's SampleWork, created on first use
@@ -232,6 +239,9 @@ inline SampleWork& sample_work(const cmoe_gp& gp) {
 // Q = num (1 + gs) <= 8192): V = L^-1 K(X, P) in w.V (n x nc Q, ld n), the mean in w.mu and the lower triangle of
 // Var = K(P, P) - V^T V + jitter I in w.A ([nc][Q][Q] column-major; the upper triangle is not written).  Asynchronous.
 void posterior_cov_large(const cmoe_gp& gp, SampleWork& w, int nc, int num, int gs, double jitter, cudaStream_t s);
+// the same on the caller's buffers (P, dPs read; V, mu, A written)
+void posterior_cov_large(const cmoe_gp& gp, const double* P, const int* dPs, double* V, double* mu, double* A, int nc,
+                         int num, int gs, double jitter, cudaStream_t s);
 // upper triangle of nsets Q x Q column-major matrices <- 0 (zero_upper) or <- the lower triangle (mirror_lower)
 void zero_upper(int nsets, int Q, double* A, cudaStream_t s);
 void mirror_lower(int nsets, int Q, double* A, cudaStream_t s);
@@ -302,6 +312,58 @@ void kg_large_eval(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_params* in
                    const double* points_being_sampled, int p, int num_mc, double best_so_far, uint64_t seed,
                    const double* normals_table, const double* stale_union, double* kg, double* grad_kg,
                    cmoe_kg_stats* stats);
+// Ensemble form (DESIGN.md K18): the num_gp members' kg_large_eval results for one draw set Z, made once; values[nc]
+// and grads[nc][q][dim] (or NULL) receive the member-ordered sums.  The large-stage workspace of the evaluation (Z, the
+// inner optimisers' scratch, the members' chunks) is at most 2 GiB, on gps[0]'s handle (ensemble_work).  A singular
+// union throws CMOE_ERR_SINGULAR with the leading minor of the first failing candidate of the first failing member.
+void kg_large_ensemble_eval(const cmoe_gp* const* gps, int num_gp, int num_fidelity, const cmoe_gd_params* inner,
+                            const double* inner_bounds, const double* discrete_pts, int num_pts,
+                            const double* candidates, int num_candidates, int q, const double* points_being_sampled,
+                            int p, int num_mc, const double* best_so_far, uint64_t seed, const double* normals_table,
+                            double* values, double* grads);
+// The same for q-EI past the per-set kernels (ei_large_eval_batch per member); normals_table: host [num_mc][q + p] or
+// NULL (Philox), checked before it is uploaded.
+void ei_large_ensemble_eval(const cmoe_gp* const* gps, int num_gp, const double* candidates, int num_candidates, int q,
+                            const double* points_being_sampled, int p, int num_mc, const double* best_so_far,
+                            uint64_t seed, const double* normals_table, double* values, double* grads);
+// Consecutive 256-byte aligned pieces of one device region (the large-union stages' workspaces); with base == NULL it
+// only counts the bytes.
+struct Carve {
+  char* base = nullptr;
+  size_t off = 0;
+  template <typename T>
+  T* take(size_t count) {
+    off = (off + 255) & ~size_t(255);
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off += count * sizeof(T);
+    return p;
+  }
+};
+// Bound on the alignment padding of one carved chunk workspace (at most 64 pieces of up to 255 bytes each): a chunk of
+// c candidates takes at most c times the one-candidate layout plus kCarveSlack.
+constexpr size_t kCarveSlack = 64 * 256;
+// CMOE_ERR_SINGULAR for a singular union covariance, *info = minor (the 1-based leading minor that failed)
+[[noreturn]] void throw_singular_union(int minor);
+// The region the ensemble evaluations above carve their buffers from, on the first member's handle, and one event per
+// member.  Every evaluation ends with its members' streams synchronised, so the next one may reuse the region.
+struct EnsembleWork {
+  DevBuf<double> arena;
+  std::vector<cudaEvent_t> done;
+  EnsembleWork() = default;
+  EnsembleWork(const EnsembleWork&) = delete;
+  EnsembleWork& operator=(const EnsembleWork&) = delete;
+  ~EnsembleWork();
+};
+// gp's EnsembleWork with an arena of at least `bytes` (grown by replacement, never kept larger than one evaluation's need)
+EnsembleWork& ensemble_work(const cmoe_gp& gp, size_t bytes);
+// Enqueues run(m, m % width) for m = 0 .. num_gp - 1 on member m's stream; member m waits for member m - width, whose
+// slot it reuses.  Returns once every member's stream has finished, also when run throws.
+void run_members(const cmoe_gp* const* gps, int num_gp, int width, EnsembleWork& ew,
+                 const std::function<void(int, int)>& run);
+// Reads back the members' device results dval [num_gp][nc], dgrad [num_gp][nc][ps] (or NULL) and dfail [num_gp][nc] on
+// `s`; throws CMOE_ERR_SINGULAR for the first failing member in member order, else sums the members in member order.
+void drain_members(cudaStream_t s, int num_gp, int nc, size_t ps, const double* dval, const double* dgrad,
+                   const int* dfail, double* values, double* grads);
 // Out = A B for `batch` column-major problems (A m x kd, B kd x nn; batch z at A + z sa, B + z sb, Out + z so), 64 x 64
 // DMMA tiles.  Asynchronous on `s`.
 void gemm_nn(int m, int nn, int kd, const double* A, int lda, size_t sa, const double* B, int ldb, size_t sb,
@@ -331,6 +393,9 @@ bool legacy_linalg();
 // it measures 62 us against 52 us for the LDGSTS kernel (see DESIGN.md K1)
 bool cov_tma_enabled();
 int set_option(const char* name, int value);
+// cmoe_set_option("ensemble_members_in_flight", k): at most k ensemble members in flight on the large-union stages
+// (0, the default: as many as the 2 GiB workspace holds)
+int ensemble_members_in_flight();
 
 int launches_issued();        // global counter of kernel launches made by this library (host side)
 void count_launch(int n = 1);

@@ -304,35 +304,425 @@ __global__ void __launch_bounds__(kGradThreads) kgl_grad_kernel(const __grid_con
 
 }  // namespace
 
-// Device workspace of cmoe_kg_eval_large beyond the K8 buffers of SampleWork, kept on the handle (cmoe_gp::kg_large_ws)
-// and grown on demand.
+namespace {
+
+// Device workspace of cmoe_kg_eval_large, kept on the handle (cmoe_gp::kg_large_ws): one region, carved as
+// kg_large_carve_slot and kg_large_carve_io lay it out, grown to the largest call's need.
 struct KgLargeWork {
-  DevBuf<double> Z, D, KD, alpha0, Xt, Pk, Afull, A, KAu, Bt, Wd, WdT, muA, S, C, Wts, outVal, outX, outH, best, kg;
-  DevBuf<double> aw, stale;
-  DevBuf<double> Kx, Ct, Rm, Tp, T1, T2, R2, G1, grad;
-  DevBuf<int> start, winner, work;
-  DevBuf<unsigned long long> stats;
+  DevBuf<double> region;
 };
 
-namespace {
+// samples of one call: the sample axis of the scan product is grid.y of gemm_nn (64 samples per CTA row, <= 65535)
+constexpr long long kMaxKgLargeSamples = 65535LL * 64;
+
+// the size bounds of cmoe_kg_eval_large, which need no handle
+void kg_large_check_sizes(int num_candidates, int q, int p, int num_mc) {
+  CMOE_REQUIRE(num_candidates >= 1, CMOE_ERR_BOUNDS, "num_candidates must be >= 1");
+  CMOE_REQUIRE(q >= 1 && p >= 0 && num_mc >= 1, CMOE_ERR_BOUNDS, "q >= 1, p >= 0, num_mc >= 1 required");
+  CMOE_REQUIRE(static_cast<long long>(q) + p <= CMOE_MAX_KG_LARGE_ROWS, CMOE_ERR_BOUNDS,
+               "(q+p)*(1+num_derivatives) must be <= 1024");
+  CMOE_REQUIRE(num_mc <= kMaxKgLargeSamples, CMOE_ERR_BOUNDS, "num_mc must be <= 4194240");
+}
+
+// Shape and sizes of one GP's evaluation (kg_large_shape)
+struct KgLargeShape {
+  const KgLargeEntry* entry = nullptr;
+  int nf, ps, q, p, U, dim, g, bs, num_pts, num_mc, DIMP, N, n, Q, Np, R, M, qb;
+  bool want_grad;
+  size_t per_bytes;  // one candidate's chunk workspace
+  size_t z_bytes;    // the draws Z
+  size_t budget;     // what one GP's chunks may use: 2 GiB less the draws, the inner optimiser's scratch and kCarveSlack
+};
+
+// Device inputs of one evaluation, shared by every GP that evaluates it
+struct KgLargeInputs {
+  const double *Z, *alpha0, *cand, *Xp, *stale;
+};
 
 KgLargeWork& kg_large_work(const cmoe_gp& gp) {
   if (!gp.kg_large_ws) gp.kg_large_ws = std::make_shared<KgLargeWork>();
   return *static_cast<KgLargeWork*>(gp.kg_large_ws.get());
 }
 
-// Argument checks that need no handle (the size bounds of cmoe_kg_eval_large)
-// samples of one call: the sample axis of the scan product is grid.y of gemm_nn (64 samples per CTA row, <= 65535)
-constexpr long long kMaxKgLargeSamples = 65535LL * 64;
 // inner-optimiser scratch (kg_mc_large_kernel's per-lane weight columns), counted in the 2 GiB budget
 constexpr size_t kKgLargeScratchBytes = size_t(256) << 20;
 
-void check_sizes(int num_candidates, int q, int p, int num_mc) {
-  CMOE_REQUIRE(num_candidates >= 1, CMOE_ERR_BOUNDS, "num_candidates must be >= 1");
-  CMOE_REQUIRE(q >= 1 && p >= 0 && num_mc >= 1, CMOE_ERR_BOUNDS, "q >= 1, p >= 0, num_mc >= 1 required");
-  CMOE_REQUIRE(static_cast<long long>(q) + p <= CMOE_MAX_KG_LARGE_ROWS, CMOE_ERR_BOUNDS,
+// candidates with a singular union factor get the identity instead, so every later stage of the chunk works on finite
+// numbers; their value is NaN (kg_value) and the evaluation reports the failure
+__global__ void __launch_bounds__(256) kgl_sanitize_kernel(int Q, const int* __restrict__ fail, double* __restrict__ A) {
+  const int c = blockIdx.y;
+  if (fail[c] == 0) return;
+  const size_t QQ = static_cast<size_t>(Q) * Q;
+  for (size_t o = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; o < QQ;
+       o += static_cast<size_t>(gridDim.x) * blockDim.x)
+    A[c * QQ + o] = (o % Q == o / Q) ? 1.0 : 0.0;
+}
+
+// Device pointers of one GP's run: the slot (the chunk workspace of `chunk` candidates and the inner optimiser's
+// scratch) and the GP's inputs and counters
+struct KgLargeBufs {
+  int chunk = 0, aw_slots = 0;
+  double *P, *V, *A, *mu, *stage, *Xt, *Pk, *Afull, *Ad, *KAu, *Bt, *Wd, *WdT, *muA, *S, *C, *Wts, *outVal, *outX,
+      *outH, *best, *kg;
+  double *Kx = nullptr, *Ct = nullptr, *Rm = nullptr, *Tp = nullptr, *T1 = nullptr, *T2 = nullptr, *R2 = nullptr,
+         *G1 = nullptr, *grad = nullptr;
+  int *fail, *start, *winner, *work, *dPs;
+  double *aw, *D, *KD;
+  unsigned long long* stats;
+};
+
+// scratch column sets (R rows x kMcThreads lanes) of the inner optimiser: one per resident CTA, at most 3 per SM and
+// `bytes` in total, at least one
+int kg_large_aw_slots(const KgLargeShape& sh, size_t bytes, int sms) {
+  const size_t slot = static_cast<size_t>(sh.R) * kMcThreads * sizeof(double);
+  return static_cast<int>(std::max<size_t>(1, std::min<size_t>(3 * static_cast<size_t>(sms), bytes / slot)));
+}
+
+// Lays out a slot for `chunk` candidates and `aw_slots` scratch column sets at cv: what the 2 GiB budget counts.
+void kg_large_carve_slot(const KgLargeShape& sh, int chunk, int aw_slots, Carve& cv, KgLargeBufs& b) {
+  const size_t ch = static_cast<size_t>(chunk), mc = static_cast<size_t>(sh.num_mc), Q = sh.Q, n = sh.n;
+  const size_t QQ = Q * Q;
+  b.chunk = chunk;
+  b.aw_slots = aw_slots;
+  b.P = cv.take<double>(ch * sh.U * sh.dim);
+  b.V = cv.take<double>(ch * Q * n);
+  b.A = cv.take<double>(ch * QQ);
+  b.mu = cv.take<double>(ch * Q);
+  b.stage = cv.take<double>(ch * ((Q + NB - 1) / NB) * NB * NB);
+  b.Xt = cv.take<double>(ch * sh.Np * sh.DIMP);
+  b.Pk = cv.take<double>(ch * sh.Np * 2);
+  b.Afull = cv.take<double>(ch * sh.U * sh.dim);
+  b.Ad = cv.take<double>(ch * sh.M * sh.DIMP);
+  b.KAu = cv.take<double>(ch * n * sh.U);
+  b.Bt = cv.take<double>(ch * n * Q);
+  b.Wd = cv.take<double>(ch * Q * sh.M);
+  b.WdT = cv.take<double>(ch * Q * sh.M);
+  b.muA = cv.take<double>(ch * sh.M);
+  b.S = cv.take<double>(ch * mc * sh.M);
+  b.C = cv.take<double>(ch * mc * Q);
+  b.Wts = cv.take<double>(ch * mc * sh.R);
+  b.outVal = cv.take<double>(ch * mc);
+  b.outX = cv.take<double>(ch * mc * sh.DIMP);
+  b.outH = cv.take<double>(ch * mc);
+  b.best = cv.take<double>(ch);
+  b.kg = cv.take<double>(ch);
+  b.fail = cv.take<int>(ch);
+  b.start = cv.take<int>(ch * mc);
+  b.winner = cv.take<int>(ch);
+  if (sh.want_grad) {
+    b.Kx = cv.take<double>(ch * mc * sh.R);
+    b.Ct = cv.take<double>(ch * mc * Q);
+    b.Rm = cv.take<double>(ch * sh.R * Q);
+    b.Tp = cv.take<double>(ch * QQ);
+    b.T1 = cv.take<double>(ch * QQ);
+    b.T2 = cv.take<double>(ch * QQ);
+    b.R2 = cv.take<double>(ch * n * sh.qb);
+    b.G1 = cv.take<double>(ch * sh.q * sh.dim);
+    b.grad = cv.take<double>(ch * sh.q * sh.dim);
+  }
+  b.aw = cv.take<double>(static_cast<size_t>(aw_slots) * sh.R * kMcThreads);
+}
+
+size_t kg_large_slot_bytes(const KgLargeShape& sh, int chunk, int aw_slots) {
+  Carve cv;
+  KgLargeBufs b;
+  kg_large_carve_slot(sh, chunk, aw_slots, cv, b);
+  return cv.off;
+}
+
+// Lays out one GP's inputs and counters at cv (beside the budget, as the call's other inputs and outputs): the
+// discrete points, K(X, D), the derivative indices, the work counter and the statistics.
+void kg_large_carve_io(const KgLargeShape& sh, Carve& cv, KgLargeBufs& b) {
+  b.D = cv.take<double>(static_cast<size_t>(std::max(1, sh.num_pts)) * sh.dim);
+  b.KD = cv.take<double>(static_cast<size_t>(sh.n) * std::max(1, sh.num_pts));
+  b.dPs = cv.take<int>(std::max(1, sh.g));
+  b.work = cv.take<int>(1);
+  b.stats = cv.take<unsigned long long>(4);
+}
+
+// Every argument check of cmoe_kg_eval_large, in its order, and the workspace sizes; CMOE_ERR_BOUNDS when one
+// candidate's workspace does not fit the 2 GiB beside the draws and the scratch.
+KgLargeShape kg_large_shape(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_params* inner,
+                            const double* inner_bounds, int num_pts, int num_candidates, int q, int p, int num_mc,
+                            bool want_grad) {
+  kg_large_check_sizes(num_candidates, q, p, num_mc);
+  CMOE_REQUIRE(gp != nullptr, CMOE_ERR_INVALID_VALUE, "gp is NULL");
+  const KernelSpec& spec = gp->spec;
+  const int dim = spec.dim, g = spec.g, bs = 1 + g, U = q + p;
+  CMOE_REQUIRE(static_cast<long long>(U) * bs <= CMOE_MAX_KG_LARGE_ROWS, CMOE_ERR_BOUNDS,
                "(q+p)*(1+num_derivatives) must be <= 1024");
-  CMOE_REQUIRE(num_mc <= kMaxKgLargeSamples, CMOE_ERR_BOUNDS, "num_mc must be <= 4194240");
+  CMOE_REQUIRE(num_pts >= 0, CMOE_ERR_BOUNDS, "bad sizes");
+  CMOE_REQUIRE(num_fidelity >= 0 && num_fidelity < dim, CMOE_ERR_BOUNDS, "num_fidelity out of range");
+  CMOE_REQUIRE(g <= kMaxGWide, CMOE_ERR_BOUNDS, "at most 31 derivative observations per point in the q-KG kernel");
+  if (g > kMaxG) {
+    for (int a = 0; a < g; ++a)
+      for (int b = 0; b < a; ++b)
+        CMOE_REQUIRE(spec.derivs[a] != spec.derivs[b], CMOE_ERR_BOUNDS,
+                     "a partial derivative is observed twice per point (q-KG with more than 8 derivative observations)");
+  }
+  CMOE_REQUIRE(inner->max_num_steps <= 4096, CMOE_ERR_BOUNDS, "inner max_num_steps must be <= 4096");
+  const int ps = dim - num_fidelity;
+  for (int d = 0; d < ps; ++d)
+    CMOE_REQUIRE(inner_bounds[2 * d] <= inner_bounds[2 * d + 1], CMOE_ERR_BOUNDS, "Tensor product region is EMPTY.");
+  const KgLargeEntry* entry = find_kg_large_entry(spec.kernel, dim, g);
+  CMOE_REQUIRE(entry != nullptr, CMOE_ERR_BOUNDS, "dim exceeds the largest compiled q-KG kernel (32 dims)");
+  KgLargeShape sh;
+  sh.entry = entry;
+  sh.nf = num_fidelity;
+  sh.ps = ps;
+  sh.q = q;
+  sh.p = p;
+  sh.U = U;
+  sh.dim = dim;
+  sh.g = g;
+  sh.bs = bs;
+  sh.num_pts = num_pts;
+  sh.num_mc = num_mc;
+  sh.want_grad = want_grad;
+  sh.DIMP = entry->dim;
+  sh.N = gp->N;
+  sh.n = gp->n;
+  sh.Q = U * bs;
+  sh.Np = sh.N + U;
+  sh.R = sh.Np * bs;
+  sh.M = U + num_pts;
+  sh.qb = q * bs;
+  // device workspace of one candidate: the slot's layout for one candidate.  A chunk of c candidates takes at most
+  // c per_bytes + kCarveSlack, since the alignment padding of its pieces does not grow with c.
+  sh.per_bytes = kg_large_slot_bytes(sh, 1, 0);
+  // per call: the draws Z and the inner optimiser's scratch; the chunks get the rest of the 2 GiB
+  sh.z_bytes = static_cast<size_t>(num_mc) * sh.Q * sizeof(double);
+  const size_t fixed = sh.z_bytes + kKgLargeScratchBytes + kCarveSlack;
+  sh.budget = kSampleWorkspaceBytes > fixed ? kSampleWorkspaceBytes - fixed : 0;
+  if (sh.per_bytes > sh.budget) {
+    char msg[320];
+    snprintf(msg, sizeof(msg),
+             "one candidate's q-KG workspace (%zu bytes: Q = %d rows, N + U = %d points, num_mc = %d) does not fit "
+             "the %zu bytes left of 2 GiB beside the call's normals and scratch",
+             sh.per_bytes, sh.Q, sh.Np, num_mc, sh.budget);
+    throw Error(CMOE_ERR_BOUNDS, msg);
+  }
+  return sh;
+}
+
+// doubles of kg_large_setup's region: Z [num_mc][Q], the step sizes, the candidates, the pending and the stale points
+size_t kg_large_setup_doubles(const KgLargeShape& sh, const cmoe_gd_params* inner, int num_candidates) {
+  return static_cast<size_t>(sh.num_mc) * sh.Q + std::max(1, inner->max_num_steps) +
+         static_cast<size_t>(num_candidates) * sh.q * sh.dim + static_cast<size_t>(std::max(1, sh.p)) * sh.dim +
+         static_cast<size_t>(sh.q) * sh.dim;
+}
+
+// The per-evaluation setup on `s` (returns once it has completed): the draws Z (Philox or the table, kg_prep_kernel's
+// layout), the step sizes, the candidates, the pending and the stale points, in `dev` (kg_large_setup_doubles).
+KgLargeInputs kg_large_setup(const KgLargeShape& sh, const cmoe_gd_params* inner, const double* candidates,
+                             int num_candidates, const double* points_being_sampled, uint64_t seed,
+                             const double* normals_table, const double* stale_union, double* dev, cudaStream_t s) {
+  const size_t mc = static_cast<size_t>(sh.num_mc);
+  KgLargeInputs in;
+  double* Z = dev;
+  double* alpha0 = Z + mc * sh.Q;
+  double* cand = alpha0 + std::max(1, inner->max_num_steps);
+  double* Xp = cand + static_cast<size_t>(num_candidates) * sh.q * sh.dim;
+  double* stale = Xp + static_cast<size_t>(std::max(1, sh.p)) * sh.dim;
+  DevBuf<double> dtable;
+  if (normals_table) dtable.upload(normals_table, ((mc + 1) / 2) * sh.Q, s);
+  kgl_normals_kernel<<<static_cast<unsigned>((mc * sh.Q + 255) / 256), 256, 0, s>>>(
+      sh.Q, sh.num_mc, seed, normals_table ? dtable.p : nullptr, Z);
+  count_launch();
+  std::vector<double> a0(std::max(1, inner->max_num_steps));
+  for (int i = 0; i < inner->max_num_steps; ++i) a0[i] = gd_step_size(inner->pre_mult, inner->gamma, i);
+  CMOE_CUDA(cudaMemcpyAsync(alpha0, a0.data(), a0.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+  CMOE_CUDA(cudaMemcpyAsync(cand, candidates, static_cast<size_t>(num_candidates) * sh.q * sh.dim * sizeof(double),
+                            cudaMemcpyHostToDevice, s));
+  if (sh.p)
+    CMOE_CUDA(cudaMemcpyAsync(Xp, points_being_sampled, static_cast<size_t>(sh.p) * sh.dim * sizeof(double),
+                              cudaMemcpyHostToDevice, s));
+  if (stale_union)
+    CMOE_CUDA(cudaMemcpyAsync(stale, stale_union, static_cast<size_t>(sh.q) * sh.dim * sizeof(double),
+                              cudaMemcpyHostToDevice, s));
+  // the host copies above are staged before the calls return; the table upload completes before dtable is freed
+  CMOE_CUDA(cudaStreamSynchronize(s));
+  in.Z = Z;
+  in.alpha0 = alpha0;
+  in.cand = cand;
+  in.Xp = Xp;
+  in.stale = stale_union ? stale : nullptr;
+  return in;
+}
+
+// Enqueues one GP's evaluation of the nc candidates on `s` in chunks of b.chunk; nothing is read back.  kg_out[nc],
+// grad_out[nc][q][dim] (if sh.want_grad) and fail_out[nc] (0 or the leading minor of a singular union) are device
+// arrays.  hD / hderivs hold the host data of the asynchronous uploads until the caller has synchronised `s`.
+void kg_large_run(const cmoe_gp& gp, const KgLargeShape& sh, const cmoe_gd_params* inner, const double* inner_bounds,
+                  const KgLargeInputs& in, const KgLargeBufs& b, const double* discrete_pts, double best_so_far,
+                  int num_candidates, cudaStream_t s, double* kg_out, double* grad_out, int* fail_out,
+                  std::vector<double>& hD, std::vector<int>& hderivs) {
+  const KernelSpec& spec = gp.spec;
+  const int dim = sh.dim, g = sh.g, bs = sh.bs, U = sh.U, q = sh.q, ps = sh.ps, num_pts = sh.num_pts;
+  const int num_mc = sh.num_mc, DIMP = sh.DIMP, N = sh.N, n = sh.n, Q = sh.Q, Np = sh.Np, R = sh.R, M = sh.M;
+  const int qb = sh.qb, chunk = b.chunk;
+  const bool want_grad = sh.want_grad;
+  const size_t QQ = static_cast<size_t>(Q) * Q, mc = static_cast<size_t>(num_mc);
+  const Centre ctr = centre_of(gp);
+  // per GP: the discrete points (fidelity coordinates 1), K(X, D), the derivative indices
+  hD.assign(static_cast<size_t>(std::max(1, num_pts)) * dim, 1.0);
+  for (int j = 0; j < num_pts; ++j)
+    for (int d = 0; d < ps; ++d) hD[static_cast<size_t>(j) * dim + d] = discrete_pts[static_cast<size_t>(j) * ps + d];
+  CMOE_CUDA(cudaMemcpyAsync(b.D, hD.data(), hD.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+  if (num_pts > 0) build_mix_covariance(spec, gp.dX.p, N, b.D, num_pts, nullptr, 0, b.KD, s);
+  hderivs.assign(std::max(1, g), 0);
+  for (int a = 0; a < g; ++a) hderivs[a] = spec.derivs[a];
+  CMOE_CUDA(cudaMemcpyAsync(b.dPs, hderivs.data(), hderivs.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  CMOE_CUDA(cudaMemsetAsync(b.stats, 0, 4 * sizeof(unsigned long long), s));
+
+  KgMcParams m{};
+  m.N = Np;
+  m.U = 0;
+  m.ps = ps;
+  m.dim = dim;
+  m.M = M;
+  m.num_mc = num_mc;
+  m.use_smem = 0;
+  m.g = g;
+  m.Q = 0;
+  m.pk_stride = 2;
+  for (int a = 0; a < CMOE_MAX_DIM; ++a) {
+    m.derivs[a] = (a < g) ? spec.derivs[a] : 0;
+    m.drow[a] = 0;
+  }
+  for (int a = 0; a < g; ++a) m.drow[spec.derivs[a]] = 1 + a;
+  m.max_steps = inner->max_num_steps;
+  m.max_restarts = inner->max_num_restarts;
+  m.mean = gp.mean;
+  m.mrc = inner->max_relative_change;
+  m.tol = inner->tolerance;
+  m.step_tol = inner->max_num_steps > 0 ? inner->tolerance / static_cast<double>(inner->max_num_steps) : 0.0;
+  m.alpha = spec.alpha;
+  m.alpha0 = in.alpha0;
+  for (int d = 0; d < CMOE_MAX_DIM; ++d) {
+    m.lo[d] = -1.0e300;
+    m.hi[d] = 1.0e300;
+    m.inv_len[d] = (d < dim) ? spec.inv_len[d] : 0.0;
+  }
+  for (int d = 0; d < ps; ++d) {  // the frame of A
+    m.lo[d] = inner_bounds[2 * d] - gp.centre[d];
+    m.hi[d] = inner_bounds[2 * d + 1] - gp.centre[d];
+  }
+  m.stats = b.stats;
+  m.aw = b.aw;
+  m.aw_slots = b.aw_slots;
+  m.work = b.work;
+  m.stage_ops = 0;
+
+  for (int c0 = 0; c0 < num_candidates; c0 += chunk) {
+    const int nb = std::min(chunk, num_candidates - c0);
+    kgl_pack_kernel<<<nb, 256, 0, s>>>(spec, ctr, N, U, q, ps, num_pts, DIMP, gp.dX.p,
+                                       in.cand + static_cast<size_t>(c0) * q * dim, in.Xp, b.D, in.stale, b.P, b.Xt,
+                                       b.Pk, b.Afull, b.Ad);
+    count_launch();
+    // posterior of the union: V = L^-1 K*, mu, Var + noise[type], L_U, B = L^-T V
+    posterior_cov_large(gp, b.P, b.dPs, b.V, b.mu, b.A, nb, U, g, 0.0, s);
+    kgl_noise_kernel<<<static_cast<unsigned>((static_cast<size_t>(nb) * Q + 255) / 256), 256, 0, s>>>(
+        nb, Q, bs, gp.dnoise.p, b.A);
+    count_launch();
+    CMOE_CUDA(cudaMemsetAsync(b.fail, 0, nb * sizeof(int), s));
+    potrf_batched(b.A, Q, nb, b.fail, b.stage, s);
+    CMOE_CUDA(cudaMemcpyAsync(fail_out + c0, b.fail, nb * sizeof(int), cudaMemcpyDeviceToDevice, s));
+    zero_upper(nb, Q, b.A, s);
+    kgl_sanitize_kernel<<<dim3(static_cast<unsigned>(std::min<size_t>((QQ + 255) / 256, 1024)), nb), 256, 0, s>>>(
+        Q, b.fail, b.A);
+    count_launch();
+    trsm_lower_blocked(gp.dK.p, n, b.V, n, nb * Q, true, s);
+    kgl_best_kernel<<<(nb + 127) / 128, 128, 0, s>>>(nb, U, bs, best_so_far, b.mu, b.best, b.winner);
+    count_launch();
+    // discretisation set: W = L_U^-1 Cov_n(Xu rows, A), mu_n(A); starts = first strict arg-min of mu_A + W^T z
+    build_mix_covariance(spec, gp.dX.p, N, b.Afull, nb * U, nullptr, 0, b.KAu, s);
+    // B^T K(X, A) on DMMA: B^T [Q][n] per candidate, then the union part and the shared discrete part of A
+    kgl_transpose_kernel<<<dim3(static_cast<unsigned>((static_cast<size_t>(n) * Q + 255) / 256), nb), 256, 0, s>>>(
+        n, Q, b.V, b.Bt);
+    count_launch();
+    gemm_nn(Q, U, n, b.Bt, Q, static_cast<size_t>(Q) * n, b.KAu, n, static_cast<size_t>(n) * U, b.Wd, Q,
+            static_cast<size_t>(Q) * M, nb, s);
+    if (num_pts > 0)
+      gemm_nn(Q, num_pts, n, b.Bt, Q, static_cast<size_t>(Q) * n, b.KD, n, 0, b.Wd + static_cast<size_t>(U) * Q, Q,
+              static_cast<size_t>(Q) * M, nb, s);
+    const size_t nwd = static_cast<size_t>(M) * (Q + 1);
+    kgl_disc_cov_kernel<<<dim3(static_cast<unsigned>((nwd + 255) / 256), nb), 256, 0, s>>>(
+        spec, n, U, num_pts, gp.mean, gp.dKinvY.p, b.P, b.Afull, b.D, b.KAu, b.KD, b.Wd, b.muA);
+    count_launch();
+    for (int c = 0; c < nb; ++c)
+      trsm_lower_blocked(b.A + c * QQ, Q, b.Wd + static_cast<size_t>(c) * Q * M, Q, M, false, s);
+    kgl_transpose_kernel<<<dim3(static_cast<unsigned>((static_cast<size_t>(Q) * M + 255) / 256), nb), 256, 0, s>>>(
+        Q, M, b.Wd, b.WdT);
+    count_launch();
+    gemm_nn(M, num_mc, Q, b.WdT, M, static_cast<size_t>(M) * Q, in.Z, Q, 0, b.S, M, mc * M, nb, s);
+    kgl_argmin_kernel<<<dim3((num_mc + 255) / 256, nb), 256, 0, s>>>(M, num_mc, b.muA, b.S, b.start);
+    count_launch();
+    // C = L_U^-T Z and the weight columns
+    for (int c = 0; c < nb; ++c) {
+      double* Cc = b.C + static_cast<size_t>(c) * mc * Q;
+      CMOE_CUDA(cudaMemcpyAsync(Cc, in.Z, mc * Q * sizeof(double), cudaMemcpyDeviceToDevice, s));
+      trsm_lower_blocked(b.A + c * QQ, Q, Cc, Q, num_mc, true, s);
+    }
+    gemm_nn(n, num_mc, Q, b.V, n, static_cast<size_t>(n) * Q, b.C, Q, mc * Q, b.Wts, R, mc * R, nb, s);
+    kgl_weights_kernel<<<dim3(static_cast<unsigned>((mc * R + 255) / 256), nb), 256, 0, s>>>(spec, n, Q, num_mc,
+                                                                                          gp.dKinvY.p, b.C, b.Wts);
+    count_launch();
+    // inner optimisation of every sample
+    KgMcParams prm = m;
+    {
+      // samples per work item: aim for >= ~8 waves of 3 CTAs per SM over the chunk, 2 to 16 samples per lane
+      const long long target = 8LL * sms * 3;
+      long long sc = (static_cast<long long>(nb) * num_mc + target - 1) / target;
+      sc = std::max<long long>(2 * kMcThreads, std::min<long long>(sc, 16 * kMcThreads));
+      sc = (sc + kMcThreads - 1) / kMcThreads * kMcThreads;
+      prm.chunk = static_cast<int>(std::min<long long>(sc, (num_mc + kMcThreads - 1) / kMcThreads * kMcThreads));
+    }
+    prm.chunks = (num_mc + prm.chunk - 1) / prm.chunk;
+    prm.work_total = prm.chunks * nb;
+    prm.Xt = b.Xt;
+    prm.Pk = b.Pk;
+    prm.A = b.Ad;
+    prm.recC = b.C;  // not read by the large-union build
+    prm.recStart = b.start;
+    prm.Wt = b.Wts;
+    prm.outVal = b.outVal;
+    prm.outX = b.outX;
+    prm.outH = b.outH;
+    CMOE_CUDA(cudaMemsetAsync(b.work, 0, sizeof(int), s));
+    sh.entry->mc(prm, s);
+    count_launch();
+    CMOE_CUDA(cudaGetLastError());
+    if (inner->max_num_restarts <= 0) kg_fill_points(spec, ctr, nb * num_mc, DIMP, b.outX, b.outH, s);
+    kg_value(nb, num_mc, b.outVal, b.best, b.fail, b.kg, s);
+    CMOE_CUDA(cudaMemcpyAsync(kg_out + c0, b.kg, nb * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    if (want_grad) {
+      // R = Kx C^T over the samples, [Q][R] (column a of length R = n + Q)
+      kgl_kx_kernel<<<dim3(static_cast<unsigned>((mc * R + 255) / 256), nb), 256, 0, s>>>(
+          spec, ctr, N, U, num_mc, DIMP, gp.dX.p, b.P, b.outX, b.Kx);
+      kgl_transpose_kernel<<<dim3(static_cast<unsigned>((mc * Q + 255) / 256), nb), 256, 0, s>>>(Q, num_mc, b.C, b.Ct);
+      count_launch(2);
+      gemm_nn(R, Q, num_mc, b.Kx, R, mc * R, b.Ct, num_mc, mc * Q, b.Rm, R, static_cast<size_t>(R) * Q, nb, s);
+      kg_tprime(nb, n, Q, Q, b.Rm, b.V, b.Tp, s);
+      potrs_lower(gp.dK.p, n, b.Rm, R, nb * Q, s);
+      kg_g1(spec, ctr, nb, U, q, Q, DIMP, num_mc, b.P, b.C, b.outX, b.G1, s);
+      // Lbar = tril(T' L_U^-T) / num_mc, then 2 Sigmabar through the Cholesky adjoint, and R2 = B 2 Sigmabar
+      for (int c = 0; c < nb; ++c) trsm_lower_blocked(b.A + c * QQ, Q, b.Tp + c * QQ, Q, Q, false, s);
+      kgl_lbar_kernel<<<dim3(static_cast<unsigned>((QQ + 255) / 256), nb), 256, 0, s>>>(Q, num_mc, b.Tp, b.T1);
+      count_launch();
+      cholesky_adjoint(b.A, Q, nb, b.T1, b.T2, s);
+      gemm_nn(n, qb, Q, b.V, n, static_cast<size_t>(n) * Q, b.T1, Q, QQ, b.R2, n, static_cast<size_t>(n) * qb, nb, s);
+      kgl_grad_kernel<<<dim3(q, nb), kGradThreads, 0, s>>>(spec, N, U, q, num_mc, gp.dX.p, gp.dKinvY.p, b.P, b.Rm,
+                                                          b.T1, b.R2, b.G1, b.winner, b.grad);
+      count_launch();
+      CMOE_CUDA(cudaGetLastError());
+      CMOE_CUDA(cudaMemcpyAsync(grad_out + static_cast<size_t>(c0) * q * dim, b.grad,
+                                static_cast<size_t>(nb) * q * dim * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    }
+  }
 }
 
 }  // namespace
@@ -342,296 +732,122 @@ void kg_large_eval(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_params* in
                    const double* points_being_sampled, int p, int num_mc, double best_so_far, uint64_t seed,
                    const double* normals_table, const double* stale_union, double* kg, double* grad_kg,
                    cmoe_kg_stats* stats) {
-    check_sizes(num_candidates, q, p, num_mc);
-    CMOE_REQUIRE(gp != nullptr, CMOE_ERR_INVALID_VALUE, "gp is NULL");
-    const KernelSpec& spec = gp->spec;
-    const int dim = spec.dim, g = spec.g, bs = 1 + g, U = q + p;
-    CMOE_REQUIRE(static_cast<long long>(U) * bs <= CMOE_MAX_KG_LARGE_ROWS, CMOE_ERR_BOUNDS,
-                 "(q+p)*(1+num_derivatives) must be <= 1024");
-    CMOE_REQUIRE(num_pts >= 0, CMOE_ERR_BOUNDS, "bad sizes");
-    CMOE_REQUIRE(num_fidelity >= 0 && num_fidelity < dim, CMOE_ERR_BOUNDS, "num_fidelity out of range");
-    CMOE_REQUIRE(g <= kMaxGWide, CMOE_ERR_BOUNDS, "at most 31 derivative observations per point in the q-KG kernel");
-    if (g > kMaxG) {
-      for (int a = 0; a < g; ++a)
-        for (int b = 0; b < a; ++b)
-          CMOE_REQUIRE(spec.derivs[a] != spec.derivs[b], CMOE_ERR_BOUNDS,
-                       "a partial derivative is observed twice per point (q-KG with more than 8 derivative observations)");
-    }
-    CMOE_REQUIRE(inner->max_num_steps <= 4096, CMOE_ERR_BOUNDS, "inner max_num_steps must be <= 4096");
-    const int ps = dim - num_fidelity;
-    for (int d = 0; d < ps; ++d)
-      CMOE_REQUIRE(inner_bounds[2 * d] <= inner_bounds[2 * d + 1], CMOE_ERR_BOUNDS, "Tensor product region is EMPTY.");
-    const KgLargeEntry* entry = find_kg_large_entry(spec.kernel, dim, g);
-    CMOE_REQUIRE(entry != nullptr, CMOE_ERR_BOUNDS, "dim exceeds the largest compiled q-KG kernel (32 dims)");
-    const int DIMP = entry->dim, N = gp->N, n = gp->n, Q = U * bs, Np = N + U, R = Np * bs, M = U + num_pts;
-    const int qb = q * bs;
-    const bool want_grad = grad_kg != nullptr;
-    const size_t QQ = static_cast<size_t>(Q) * Q, mc = static_cast<size_t>(num_mc);
-    // device workspace of one candidate (doubles; ints counted as doubles)
-    const size_t nb64 = static_cast<size_t>((Q + NB - 1) / NB) * NB * NB;
-    size_t per = static_cast<size_t>(U) * dim * 2 + static_cast<size_t>(n) * Q + QQ + Q + nb64 + 1 +
-                 static_cast<size_t>(Np) * (DIMP + 2) + static_cast<size_t>(M) * (DIMP + 1) +
-                 static_cast<size_t>(n) * U + 2 * static_cast<size_t>(Q) * M + mc * (M + Q + R + DIMP + 3) + 4;
-    if (want_grad) per += mc * (R + Q) + static_cast<size_t>(R) * Q + 3 * QQ + static_cast<size_t>(n) * qb +
-                          2 * static_cast<size_t>(q) * dim;
-    per += static_cast<size_t>(n) * Q;  // B^T for the discretisation product
-    const size_t per_bytes = per * sizeof(double);
-    // per call: the draws Z and the inner optimiser's scratch; the chunks get the rest of the 2 GiB
-    const size_t fixed = mc * Q * sizeof(double) + kKgLargeScratchBytes;
-    const size_t budget = kSampleWorkspaceBytes > fixed ? kSampleWorkspaceBytes - fixed : 0;
-    if (per_bytes > budget) {
-      char msg[320];
-      snprintf(msg, sizeof(msg),
-               "one candidate's q-KG workspace (%zu bytes: Q = %d rows, N + U = %d points, num_mc = %d) does not fit "
-               "the %zu bytes left of 2 GiB beside the call's normals and scratch",
-               per_bytes, Q, Np, num_mc, budget);
-      throw Error(CMOE_ERR_BOUNDS, msg);
-    }
-    require_device(gp->device);
-    cudaStream_t s = gp->stream;
-    const Centre ctr = centre_of(*gp);
-    const int chunk = static_cast<int>(chunk_items(num_candidates, budget, per_bytes, kMaxChunkSets));
-    SampleWork& w = sample_work(*gp);
-    KgLargeWork& k = kg_large_work(*gp);
-    // per call: the draws, the discrete points (fidelity coordinates 1), K(X, D), the step sizes
-    k.Z.ensure(mc * Q);
-    DevBuf<double> dtable;
-    if (normals_table) dtable.upload(normals_table, ((mc + 1) / 2) * Q, s);
-    kgl_normals_kernel<<<static_cast<unsigned>((mc * Q + 255) / 256), 256, 0, s>>>(
-        Q, num_mc, seed, normals_table ? dtable.p : nullptr, k.Z.p);
-    count_launch();
-    std::vector<double> hD(static_cast<size_t>(std::max(1, num_pts)) * dim, 1.0);
-    for (int j = 0; j < num_pts; ++j)
-      for (int d = 0; d < ps; ++d) hD[static_cast<size_t>(j) * dim + d] = discrete_pts[static_cast<size_t>(j) * ps + d];
-    k.D.upload(hD.data(), hD.size(), s);
-    k.KD.ensure(static_cast<size_t>(n) * std::max(1, num_pts));
-    if (num_pts > 0) build_mix_covariance(spec, gp->dX.p, N, k.D.p, num_pts, nullptr, 0, k.KD.p, s);
-    std::vector<double> a0(std::max(1, inner->max_num_steps));
-    for (int i = 0; i < inner->max_num_steps; ++i) a0[i] = gd_step_size(inner->pre_mult, inner->gamma, i);
-    k.alpha0.upload(a0.data(), a0.size(), s);
-    std::vector<int> hderivs(std::max(1, g), 0);
-    for (int a = 0; a < g; ++a) hderivs[a] = spec.derivs[a];
-    w.dPs.upload(hderivs.data(), hderivs.size(), s);
-    DevBuf<double> dcand, dXp;
-    dcand.upload(candidates, static_cast<size_t>(num_candidates) * q * dim, s);
-    if (p) dXp.upload(points_being_sampled, static_cast<size_t>(p) * dim, s);
-    if (stale_union) k.stale.upload(stale_union, static_cast<size_t>(q) * dim, s);
-    // chunk workspace
-    w.P.ensure(static_cast<size_t>(chunk) * U * dim);
-    w.V.ensure(static_cast<size_t>(chunk) * Q * n);
-    w.A.ensure(static_cast<size_t>(chunk) * QQ);
-    w.mu.ensure(static_cast<size_t>(chunk) * Q);
-    w.fail.ensure(chunk);
-    k.Xt.ensure(static_cast<size_t>(chunk) * Np * DIMP);
-    k.Pk.ensure(static_cast<size_t>(chunk) * Np * 2);
-    k.Afull.ensure(static_cast<size_t>(chunk) * U * dim);
-    k.A.ensure(static_cast<size_t>(chunk) * M * DIMP);
-    k.KAu.ensure(static_cast<size_t>(chunk) * n * U);
-    k.Bt.ensure(static_cast<size_t>(chunk) * n * Q);
-    k.Wd.ensure(static_cast<size_t>(chunk) * Q * M);
-    k.WdT.ensure(static_cast<size_t>(chunk) * Q * M);
-    k.muA.ensure(static_cast<size_t>(chunk) * M);
-    k.S.ensure(static_cast<size_t>(chunk) * mc * M);
-    k.C.ensure(static_cast<size_t>(chunk) * mc * Q);
-    k.Wts.ensure(static_cast<size_t>(chunk) * mc * R);
-    k.outVal.ensure(static_cast<size_t>(chunk) * mc);
-    k.outX.ensure(static_cast<size_t>(chunk) * mc * DIMP);
-    k.outH.ensure(static_cast<size_t>(chunk) * mc);
-    k.best.ensure(chunk);
-    k.kg.ensure(chunk);
-    k.start.ensure(static_cast<size_t>(chunk) * mc);
-    k.winner.ensure(chunk);
-    k.work.ensure(1);
-    k.stats.ensure(4);
-    if (want_grad) {
-      k.Kx.ensure(static_cast<size_t>(chunk) * mc * R);
-      k.Ct.ensure(static_cast<size_t>(chunk) * mc * Q);
-      k.Rm.ensure(static_cast<size_t>(chunk) * R * Q);
-      k.Tp.ensure(static_cast<size_t>(chunk) * QQ);
-      k.T1.ensure(static_cast<size_t>(chunk) * QQ);
-      k.T2.ensure(static_cast<size_t>(chunk) * QQ);
-      k.R2.ensure(static_cast<size_t>(chunk) * n * qb);
-      k.G1.ensure(static_cast<size_t>(chunk) * q * dim);
-      k.grad.ensure(static_cast<size_t>(chunk) * q * dim);
-    }
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    {
-      // one scratch column set (R rows x kMcThreads lanes) per resident CTA, at most 3 per SM and
-      // kKgLargeScratchBytes in total
-      const size_t slot = static_cast<size_t>(R) * kMcThreads;
-      const size_t slots = std::max<size_t>(1, std::min<size_t>(3 * static_cast<size_t>(sms),
-                                                                kKgLargeScratchBytes / (slot * sizeof(double))));
-      k.aw.ensure(slot * slots);
-    }
-    const int aw_slots = static_cast<int>(k.aw.count / (static_cast<size_t>(R) * kMcThreads));
-    CMOE_CUDA(cudaMemsetAsync(k.stats.p, 0, 4 * sizeof(unsigned long long), s));
+  const KgLargeShape sh = kg_large_shape(gp, num_fidelity, inner, inner_bounds, num_pts, num_candidates, q, p, num_mc,
+                                         grad_kg != nullptr);
+  require_device(gp->device);
+  cudaStream_t s = gp->stream;
+  const int dim = sh.dim, chunk = static_cast<int>(chunk_items(num_candidates, sh.budget, sh.per_bytes, kMaxChunkSets));
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  // per call: the draws, the step sizes, the candidates, the pending and the stale points
+  DevBuf<double> in_buf(kg_large_setup_doubles(sh, inner, num_candidates));
+  const KgLargeInputs in = kg_large_setup(sh, inner, candidates, num_candidates, points_being_sampled, seed,
+                                          normals_table, stale_union, in_buf.p, s);
+  // the handle's region: the slot (chunk workspace and scratch), then the GP's inputs and counters
+  const int aw_slots = kg_large_aw_slots(sh, kKgLargeScratchBytes, sms);
+  KgLargeBufs b;
+  Carve cv;
+  kg_large_carve_slot(sh, chunk, aw_slots, cv, b);
+  kg_large_carve_io(sh, cv, b);
+  KgLargeWork& k = kg_large_work(*gp);
+  k.region.ensure((cv.off + sizeof(double) - 1) / sizeof(double));
+  cv = Carve{reinterpret_cast<char*>(k.region.p)};
+  kg_large_carve_slot(sh, chunk, aw_slots, cv, b);
+  kg_large_carve_io(sh, cv, b);
+  // the call's results, read back once
+  DevBuf<double> dkg(num_candidates), dgrad(sh.want_grad ? static_cast<size_t>(num_candidates) * q * dim : 0);
+  DevBuf<int> dfail(num_candidates);
+  std::vector<double> hD;
+  std::vector<int> hderivs;
+  kg_large_run(*gp, sh, inner, inner_bounds, in, b, discrete_pts, best_so_far, num_candidates, s, dkg.p, dgrad.p,
+               dfail.p, hD, hderivs);
+  std::vector<int> hfail(num_candidates);
+  unsigned long long st[4] = {0, 0, 0, 0};
+  dfail.download(hfail.data(), num_candidates, s);
+  dkg.download(kg, num_candidates, s);
+  if (sh.want_grad) dgrad.download(grad_kg, static_cast<size_t>(num_candidates) * q * dim, s);
+  CMOE_CUDA(cudaMemcpyAsync(st, b.stats, sizeof(st), cudaMemcpyDeviceToHost, s));
+  CMOE_CUDA(cudaStreamSynchronize(s));
+  for (int c = 0; c < num_candidates; ++c)
+    if (hfail[c] != 0) throw_singular_union(hfail[c]);
+  if (stats) {
+    stats->mc_samples = static_cast<uint64_t>(num_candidates) * num_mc;
+    stats->posterior_evals = st[0];
+    stats->line_search_steps = st[1];
+    stats->point_evals = st[2];
+    stats->line_batches = st[3];
+  }
+}
 
-    KgMcParams m{};
-    m.N = Np;
-    m.U = 0;
-    m.ps = ps;
-    m.dim = dim;
-    m.M = M;
-    m.num_mc = num_mc;
-    m.use_smem = 0;
-    m.g = g;
-    m.Q = 0;
-    m.pk_stride = 2;
-    for (int a = 0; a < CMOE_MAX_DIM; ++a) {
-      m.derivs[a] = (a < g) ? spec.derivs[a] : 0;
-      m.drow[a] = 0;
-    }
-    for (int a = 0; a < g; ++a) m.drow[spec.derivs[a]] = 1 + a;
-    m.max_steps = inner->max_num_steps;
-    m.max_restarts = inner->max_num_restarts;
-    m.mean = gp->mean;
-    m.mrc = inner->max_relative_change;
-    m.tol = inner->tolerance;
-    m.step_tol = inner->max_num_steps > 0 ? inner->tolerance / static_cast<double>(inner->max_num_steps) : 0.0;
-    m.alpha = spec.alpha;
-    m.alpha0 = k.alpha0.p;
-    for (int d = 0; d < CMOE_MAX_DIM; ++d) {
-      m.lo[d] = -1.0e300;
-      m.hi[d] = 1.0e300;
-      m.inv_len[d] = (d < dim) ? spec.inv_len[d] : 0.0;
-    }
-    for (int d = 0; d < ps; ++d) {  // the frame of A
-      m.lo[d] = inner_bounds[2 * d] - gp->centre[d];
-      m.hi[d] = inner_bounds[2 * d + 1] - gp->centre[d];
-    }
-    m.stats = k.stats.p;
-    m.aw = k.aw.p;
-    m.aw_slots = aw_slots;
-    m.work = k.work.p;
-    m.stage_ops = 0;
-
-    std::vector<int> hfail(chunk);
-    for (int c0 = 0; c0 < num_candidates; c0 += chunk) {
-      const int nb = std::min(chunk, num_candidates - c0);
-      kgl_pack_kernel<<<nb, 256, 0, s>>>(spec, ctr, N, U, q, ps, num_pts, DIMP, gp->dX.p,
-                                         dcand.p + static_cast<size_t>(c0) * q * dim, dXp.p, k.D.p,
-                                         stale_union ? k.stale.p : nullptr, w.P.p, k.Xt.p,
-                                         k.Pk.p, k.Afull.p, k.A.p);
-      count_launch();
-      // posterior of the union: V = L^-1 K*, mu, Var + noise[type], L_U, B = L^-T V
-      posterior_cov_large(*gp, w, nb, U, g, 0.0, s);
-      kgl_noise_kernel<<<static_cast<unsigned>((static_cast<size_t>(nb) * Q + 255) / 256), 256, 0, s>>>(
-          nb, Q, bs, gp->dnoise.p, w.A.p);
-      count_launch();
-      CMOE_CUDA(cudaMemsetAsync(w.fail.p, 0, nb * sizeof(int), s));
-      potrf_batched(w.A.p, Q, nb, w.fail.p, w.stage, s);
-      w.fail.download(hfail.data(), nb, s);
-      CMOE_CUDA(cudaStreamSynchronize(s));
-      for (int c = 0; c < nb; ++c)
-        if (hfail[c] != 0)
-          throw Error(CMOE_ERR_SINGULAR,
-                      "GP-Variance matrix singular. Check for duplicate points_to_sample/being_sampled or "
-                      "points_to_sample/being_sampled duplicating points_sampled with 0 noise.",
-                      hfail[c]);
-      zero_upper(nb, Q, w.A.p, s);
-      trsm_lower_blocked(gp->dK.p, n, w.V.p, n, nb * Q, true, s);
-      kgl_best_kernel<<<(nb + 127) / 128, 128, 0, s>>>(nb, U, bs, best_so_far, w.mu.p, k.best.p, k.winner.p);
-      count_launch();
-      // discretisation set: W = L_U^-1 Cov_n(Xu rows, A), mu_n(A); starts = first strict arg-min of mu_A + W^T z
-      build_mix_covariance(spec, gp->dX.p, N, k.Afull.p, nb * U, nullptr, 0, k.KAu.p, s);
-      // B^T K(X, A) on DMMA: B^T [Q][n] per candidate, then the union part and the shared discrete part of A
-      kgl_transpose_kernel<<<dim3(static_cast<unsigned>((static_cast<size_t>(n) * Q + 255) / 256), nb), 256, 0, s>>>(
-          n, Q, w.V.p, k.Bt.p);
-      count_launch();
-      gemm_nn(Q, U, n, k.Bt.p, Q, static_cast<size_t>(Q) * n, k.KAu.p, n, static_cast<size_t>(n) * U, k.Wd.p, Q,
-              static_cast<size_t>(Q) * M, nb, s);
-      if (num_pts > 0)
-        gemm_nn(Q, num_pts, n, k.Bt.p, Q, static_cast<size_t>(Q) * n, k.KD.p, n, 0, k.Wd.p + static_cast<size_t>(U) * Q,
-                Q, static_cast<size_t>(Q) * M, nb, s);
-      const size_t nwd = static_cast<size_t>(M) * (Q + 1);
-      kgl_disc_cov_kernel<<<dim3(static_cast<unsigned>((nwd + 255) / 256), nb), 256, 0, s>>>(
-          spec, n, U, num_pts, gp->mean, gp->dKinvY.p, w.P.p, k.Afull.p, k.D.p, k.KAu.p, k.KD.p, k.Wd.p, k.muA.p);
-      count_launch();
-      for (int c = 0; c < nb; ++c)
-        trsm_lower_blocked(w.A.p + c * QQ, Q, k.Wd.p + static_cast<size_t>(c) * Q * M, Q, M, false, s);
-      kgl_transpose_kernel<<<dim3(static_cast<unsigned>((static_cast<size_t>(Q) * M + 255) / 256), nb), 256, 0, s>>>(
-          Q, M, k.Wd.p, k.WdT.p);
-      count_launch();
-      gemm_nn(M, num_mc, Q, k.WdT.p, M, static_cast<size_t>(M) * Q, k.Z.p, Q, 0, k.S.p, M, mc * M, nb, s);
-      kgl_argmin_kernel<<<dim3((num_mc + 255) / 256, nb), 256, 0, s>>>(M, num_mc, k.muA.p, k.S.p, k.start.p);
-      count_launch();
-      // C = L_U^-T Z and the weight columns
-      for (int c = 0; c < nb; ++c) {
-        double* Cc = k.C.p + static_cast<size_t>(c) * mc * Q;
-        CMOE_CUDA(cudaMemcpyAsync(Cc, k.Z.p, mc * Q * sizeof(double), cudaMemcpyDeviceToDevice, s));
-        trsm_lower_blocked(w.A.p + c * QQ, Q, Cc, Q, num_mc, true, s);
-      }
-      gemm_nn(n, num_mc, Q, w.V.p, n, static_cast<size_t>(n) * Q, k.C.p, Q, mc * Q, k.Wts.p, R, mc * R, nb, s);
-      kgl_weights_kernel<<<dim3(static_cast<unsigned>((mc * R + 255) / 256), nb), 256, 0, s>>>(spec, n, Q, num_mc,
-                                                                                            gp->dKinvY.p, k.C.p,
-                                                                                            k.Wts.p);
-      count_launch();
-      // inner optimisation of every sample
-      KgMcParams prm = m;
-      {
-        // samples per work item: aim for >= ~8 waves of 3 CTAs per SM over the chunk, 2 to 16 samples per lane
-        const long long target = 8LL * sms * 3;
-        long long sc = (static_cast<long long>(nb) * num_mc + target - 1) / target;
-        sc = std::max<long long>(2 * kMcThreads, std::min<long long>(sc, 16 * kMcThreads));
-        sc = (sc + kMcThreads - 1) / kMcThreads * kMcThreads;
-        prm.chunk = static_cast<int>(std::min<long long>(sc, (num_mc + kMcThreads - 1) / kMcThreads * kMcThreads));
-      }
-      prm.chunks = (num_mc + prm.chunk - 1) / prm.chunk;
-      prm.work_total = prm.chunks * nb;
-      prm.Xt = k.Xt.p;
-      prm.Pk = k.Pk.p;
-      prm.A = k.A.p;
-      prm.recC = k.C.p;  // not read by the large-union build
-      prm.recStart = k.start.p;
-      prm.Wt = k.Wts.p;
-      prm.outVal = k.outVal.p;
-      prm.outX = k.outX.p;
-      prm.outH = k.outH.p;
-      CMOE_CUDA(cudaMemsetAsync(k.work.p, 0, sizeof(int), s));
-      entry->mc(prm, s);
-      count_launch();
-      CMOE_CUDA(cudaGetLastError());
-      if (inner->max_num_restarts <= 0) kg_fill_points(spec, ctr, nb * num_mc, DIMP, k.outX.p, k.outH.p, s);
-      kg_value(nb, num_mc, k.outVal.p, k.best.p, w.fail.p, k.kg.p, s);
-      k.kg.download(kg + c0, nb, s);
-      if (want_grad) {
-        // R = Kx C^T over the samples, [Q][R] (column a of length R = n + Q)
-        kgl_kx_kernel<<<dim3(static_cast<unsigned>((mc * R + 255) / 256), nb), 256, 0, s>>>(
-            spec, ctr, N, U, num_mc, DIMP, gp->dX.p, w.P.p, k.outX.p, k.Kx.p);
-        kgl_transpose_kernel<<<dim3(static_cast<unsigned>((mc * Q + 255) / 256), nb), 256, 0, s>>>(Q, num_mc, k.C.p,
-                                                                                                 k.Ct.p);
-        count_launch(2);
-        gemm_nn(R, Q, num_mc, k.Kx.p, R, mc * R, k.Ct.p, num_mc, mc * Q, k.Rm.p, R, static_cast<size_t>(R) * Q, nb, s);
-        kg_tprime(nb, n, Q, Q, k.Rm.p, w.V.p, k.Tp.p, s);
-        potrs_lower(gp->dK.p, n, k.Rm.p, R, nb * Q, s);
-        kg_g1(spec, ctr, nb, U, q, Q, DIMP, num_mc, w.P.p, k.C.p, k.outX.p, k.G1.p, s);
-        // Lbar = tril(T' L_U^-T) / num_mc, then 2 Sigmabar through the Cholesky adjoint, and R2 = B 2 Sigmabar
-        for (int c = 0; c < nb; ++c) trsm_lower_blocked(w.A.p + c * QQ, Q, k.Tp.p + c * QQ, Q, Q, false, s);
-        kgl_lbar_kernel<<<dim3(static_cast<unsigned>((QQ + 255) / 256), nb), 256, 0, s>>>(Q, num_mc, k.Tp.p, k.T1.p);
-        count_launch();
-        cholesky_adjoint(w.A.p, Q, nb, k.T1.p, k.T2.p, s);
-        gemm_nn(n, qb, Q, w.V.p, n, static_cast<size_t>(n) * Q, k.T1.p, Q, QQ, k.R2.p, n, static_cast<size_t>(n) * qb,
-                nb, s);
-        kgl_grad_kernel<<<dim3(q, nb), kGradThreads, 0, s>>>(spec, N, U, q, num_mc, gp->dX.p, gp->dKinvY.p, w.P.p,
-                                                            k.Rm.p, k.T1.p, k.R2.p, k.G1.p, k.winner.p, k.grad.p);
-        count_launch();
-        CMOE_CUDA(cudaGetLastError());
-        k.grad.download(grad_kg + static_cast<size_t>(c0) * q * dim, static_cast<size_t>(nb) * q * dim, s);
-      }
-      CMOE_CUDA(cudaStreamSynchronize(s));
-    }
-    unsigned long long st[4] = {0, 0, 0, 0};
-    CMOE_CUDA(cudaMemcpyAsync(st, k.stats.p, sizeof(st), cudaMemcpyDeviceToHost, s));
-    CMOE_CUDA(cudaStreamSynchronize(s));
-    if (stats) {
-      stats->mc_samples = static_cast<uint64_t>(num_candidates) * num_mc;
-      stats->posterior_evals = st[0];
-      stats->line_search_steps = st[1];
-      stats->point_evals = st[2];
-      stats->line_batches = st[3];
-    }
+void kg_large_ensemble_eval(const cmoe_gp* const* gps, int num_gp, int num_fidelity, const cmoe_gd_params* inner,
+                            const double* inner_bounds, const double* discrete_pts, int num_pts,
+                            const double* candidates, int num_candidates, int q, const double* points_being_sampled,
+                            int p, int num_mc, const double* best_so_far, uint64_t seed, const double* normals_table,
+                            double* values, double* grads) {
+  const bool want_grad = grads != nullptr;
+  std::vector<KgLargeShape> sh;
+  size_t per = 0;
+  for (int m = 0; m < num_gp; ++m) {
+    sh.push_back(kg_large_shape(gps[m], num_fidelity, inner, inner_bounds, num_pts, num_candidates, q, p, num_mc,
+                                want_grad));
+    per = std::max(per, sh.back().per_bytes);
+  }
+  require_device(gps[0]->device);
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  // W members in flight: each gets 1/W of the chunks' budget and of the scratch, W as large as one candidate of every
+  // member (and one scratch column set) still fits.  A slot then takes at most (budget + kCarveSlack) / W + scratch,
+  // so Z and the W slots stay within 2 GiB.
+  const KgLargeShape& s0 = sh[0];
+  size_t slot_max = 0;
+  for (const KgLargeShape& x : sh) slot_max = std::max(slot_max, static_cast<size_t>(x.R) * kMcThreads * sizeof(double));
+  size_t width = std::min<size_t>({static_cast<size_t>(num_gp), (s0.budget + kCarveSlack) / (per + kCarveSlack),
+                                   kKgLargeScratchBytes / slot_max});
+  if (ensemble_members_in_flight() > 0) width = std::min<size_t>(width, ensemble_members_in_flight());
+  width = std::max<size_t>(1, width);
+  const int W = static_cast<int>(width);
+  const size_t scratch = kKgLargeScratchBytes / width;
+  const size_t chunk_budget = (s0.budget + kCarveSlack) / width - kCarveSlack;
+  const int chunk = static_cast<int>(chunk_items(num_candidates, chunk_budget, per, kMaxChunkSets));
+  size_t slot_bytes = 0;
+  for (const KgLargeShape& x : sh)
+    slot_bytes = std::max(slot_bytes, kg_large_slot_bytes(x, chunk, kg_large_aw_slots(x, scratch, sms)));
+  slot_bytes = (slot_bytes + 255) & ~size_t(255);
+  // one region on the first member's handle: the evaluation's inputs (Z first), every member's results, inputs and
+  // counters, then the W slots
+  const size_t ps = static_cast<size_t>(q) * s0.dim, nc = num_candidates;
+  std::vector<KgLargeBufs> io(num_gp);
+  double *in_dev = nullptr, *dval = nullptr, *dgrad = nullptr;
+  int* dfail = nullptr;
+  char* slots = nullptr;
+  auto layout = [&](Carve& cv) {
+    in_dev = cv.take<double>(kg_large_setup_doubles(s0, inner, num_candidates));
+    dval = cv.take<double>(static_cast<size_t>(num_gp) * nc);
+    dgrad = want_grad ? cv.take<double>(static_cast<size_t>(num_gp) * nc * ps) : nullptr;
+    dfail = cv.take<int>(static_cast<size_t>(num_gp) * nc);
+    for (int m = 0; m < num_gp; ++m) kg_large_carve_io(sh[m], cv, io[m]);
+    slots = cv.take<char>(slot_bytes * width);
+  };
+  Carve cv;
+  layout(cv);
+  EnsembleWork& ew = ensemble_work(*gps[0], cv.off);
+  cv = Carve{reinterpret_cast<char*>(ew.arena.p)};
+  layout(cv);
+  const KgLargeInputs in = kg_large_setup(s0, inner, candidates, num_candidates, points_being_sampled, seed,
+                                          normals_table, nullptr, in_dev, gps[0]->stream);
+  std::vector<std::vector<double>> hD(num_gp);
+  std::vector<std::vector<int>> hderivs(num_gp);
+  run_members(gps, num_gp, W, ew, [&](int m, int slot) {
+    KgLargeBufs b = io[m];
+    Carve sc{slots + slot * slot_bytes};
+    kg_large_carve_slot(sh[m], chunk, kg_large_aw_slots(sh[m], scratch, sms), sc, b);
+    kg_large_run(*gps[m], sh[m], inner, inner_bounds, in, b, discrete_pts + static_cast<size_t>(m) * num_pts * s0.ps,
+                 best_so_far[m], num_candidates, gps[m]->stream, dval + m * nc, want_grad ? dgrad + m * nc * ps : nullptr,
+                 dfail + m * nc, hD[m], hderivs[m]);
+  });
+  drain_members(gps[0]->stream, num_gp, num_candidates, ps, dval, dgrad, dfail, values, grads);
 }
 
 }  // namespace cmoe

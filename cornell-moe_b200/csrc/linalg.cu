@@ -680,8 +680,13 @@ int& opt_cov_tma() {
   }();
   return v;
 }
+int& opt_members_in_flight() {
+  static int v = 0;
+  return v;
+}
 }  // namespace
 bool legacy_linalg() { return opt_legacy() != 0; }
+int ensemble_members_in_flight() { return opt_members_in_flight(); }
 bool cov_tma_enabled() { return opt_cov_tma() != 0; }
 int set_option(const char* name, int value) {
   const std::string n(name ? name : "");
@@ -689,6 +694,9 @@ int set_option(const char* name, int value) {
     opt_legacy() = value ? 1 : 0;
   } else if (n == "cov_tma") {
     opt_cov_tma() = value ? 1 : 0;
+  } else if (n == "ensemble_members_in_flight") {
+    if (value < 0) return -1;
+    opt_members_in_flight() = value;
   } else {
     return -1;
   }

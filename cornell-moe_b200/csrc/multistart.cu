@@ -241,9 +241,8 @@ struct KgEvaluator {
 void make_kg_evaluator(KgEvaluator& ev, const cmoe_gp* gp, int nf, const cmoe_gd_params* inner,
                        const double* inner_bounds, const double* discrete_pts, int num_pts, int max_value_cands,
                        int max_grad_cands, int q, const double* Xp, int p, int num_mc, double best_so_far,
-                       uint64_t seed, const double* stale_union = nullptr, bool allow_large = true) {
-  // the ensemble calls keep the plans' 32-row bound (cmoe_kg_plan_create refuses larger unions)
-  if (allow_large && static_cast<long long>(q + p) * (1 + gp->spec.g) > 32) {
+                       uint64_t seed, const double* stale_union = nullptr) {
+  if (static_cast<long long>(q + p) * (1 + gp->spec.g) > 32) {
     const int dim = gp->spec.dim, ps = dim - nf;
     CMOE_REQUIRE(nf >= 0 && ps >= 1 && num_pts >= 0, CMOE_ERR_BOUNDS, "num_fidelity out of range");
     ev.large = true;
@@ -451,12 +450,28 @@ void apply_fidelity_cost(const double* pts, int nc, int q, int dim, int nf, int 
   }
 }
 
+// Past 32 union rows the members run cmoe_kg_eval_large's stages (kg_large_ensemble_eval) with the evaluation's
+// arguments kept here; up to 32 rows each member has its two plans.
 struct KgEnsembleEvaluator {
   std::vector<std::unique_ptr<KgEvaluator>> evs;
   int q = 0, dim = 0, nf = 0;
   std::vector<double> tv, tg;
+  // large path
+  bool large = false;
+  std::vector<const cmoe_gp*> gps;
+  int num_pts = 0, p = 0, num_mc = 0;
+  uint64_t seed = 0;
+  cmoe_gd_params inner{};
+  std::vector<double> inner_bounds, discrete, Xp, best;
   void operator()(const double* pts, int nc, double* values, double* grads) {
     const size_t ps = static_cast<size_t>(q) * dim;
+    if (large) {
+      kg_large_ensemble_eval(gps.data(), static_cast<int>(gps.size()), nf, &inner, inner_bounds.data(),
+                             discrete.data(), num_pts, pts, nc, q, Xp.data(), p, num_mc, best.data(), seed, nullptr,
+                             values, grads);
+      apply_fidelity_cost(pts, nc, q, dim, nf, static_cast<int>(gps.size()), values, grads);
+      return;
+    }
     // phase 1: enqueue every member on its own stream; phase 2: drain in member order (fixed summation order)
     for (auto& ev : evs) {
       cmoe_kg_plan* pl = grads ? ev->gplan : ev->vplan;
@@ -492,7 +507,76 @@ void cmoe::check_ensemble(const cmoe_gp* const* gps, int num_gp) {
   }
 }
 
+cmoe::EnsembleWork::~EnsembleWork() {
+  for (cudaEvent_t e : done) cudaEventDestroy(e);
+}
+
+cmoe::EnsembleWork& cmoe::ensemble_work(const cmoe_gp& gp, size_t bytes) {
+  if (!gp.ensemble_ws) gp.ensemble_ws = std::make_shared<EnsembleWork>();
+  EnsembleWork& ew = *static_cast<EnsembleWork*>(gp.ensemble_ws.get());
+  ew.arena.ensure((bytes + sizeof(double) - 1) / sizeof(double));
+  return ew;
+}
+
+void cmoe::run_members(const cmoe_gp* const* gps, int num_gp, int width, EnsembleWork& ew,
+                       const std::function<void(int, int)>& run) {
+  while (ew.done.size() < static_cast<size_t>(num_gp)) {
+    cudaEvent_t e;
+    CMOE_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    ew.done.push_back(e);
+  }
+  // the members' streams are drained however the loop ends: the next evaluation reuses the region
+  struct Drain {
+    const cmoe_gp* const* gps;
+    int n = 0;
+    ~Drain() {
+      for (int m = 0; m < n; ++m) cudaStreamSynchronize(gps[m]->stream);
+    }
+  } drain{gps};
+  for (int m = 0; m < num_gp; ++m) {
+    cudaStream_t s = gps[m]->stream;
+    if (m >= width) CMOE_CUDA(cudaStreamWaitEvent(s, ew.done[m - width], 0));
+    drain.n = m + 1;
+    run(m, m % width);
+    CMOE_CUDA(cudaEventRecord(ew.done[m], s));
+  }
+  drain.n = 0;
+  for (int m = 0; m < num_gp; ++m) CMOE_CUDA(cudaStreamSynchronize(gps[m]->stream));
+}
+
+void cmoe::throw_singular_union(int minor) {
+  throw Error(CMOE_ERR_SINGULAR,
+              "GP-Variance matrix singular. Check for duplicate points_to_sample/being_sampled or "
+              "points_to_sample/being_sampled duplicating points_sampled with 0 noise.",
+              minor);
+}
+
+void cmoe::drain_members(cudaStream_t s, int num_gp, int nc, size_t ps, const double* dval, const double* dgrad,
+                         const int* dfail, double* values, double* grads) {
+  const size_t all = static_cast<size_t>(num_gp) * nc;
+  std::vector<int> f(all);
+  std::vector<double> v(all), g(grads ? all * ps : 0);
+  CMOE_CUDA(cudaMemcpyAsync(f.data(), dfail, all * sizeof(int), cudaMemcpyDeviceToHost, s));
+  CMOE_CUDA(cudaMemcpyAsync(v.data(), dval, all * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (grads) CMOE_CUDA(cudaMemcpyAsync(g.data(), dgrad, all * ps * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CMOE_CUDA(cudaStreamSynchronize(s));
+  for (size_t e = 0; e < all; ++e)
+    if (f[e] != 0) throw_singular_union(f[e]);
+  std::fill(values, values + nc, 0.0);
+  if (grads) std::fill(grads, grads + nc * ps, 0.0);
+  for (int m = 0; m < num_gp; ++m) {
+    for (int c = 0; c < nc; ++c) values[c] += v[static_cast<size_t>(m) * nc + c];
+    if (grads)
+      for (size_t k = 0; k < nc * ps; ++k) grads[k] += g[static_cast<size_t>(m) * nc * ps + k];
+  }
+}
+
 namespace {
+
+// union rows of an ensemble's q-KG: up to 32 the plans and cmoe_kg_eval, past them cmoe_kg_eval_large's stages
+bool kg_ensemble_large(const cmoe_gp* const* gps, int q, int p) {
+  return static_cast<long long>(q + p) * (1 + gps[0]->spec.g) > 32;
+}
 
 void make_kg_ensemble(KgEnsembleEvaluator& ens, const cmoe_gp* const* gps, int num_gp, int nf,
                       const cmoe_gd_params* inner, const double* inner_bounds, const double* discrete_pts, int num_pts,
@@ -502,17 +586,47 @@ void make_kg_ensemble(KgEnsembleEvaluator& ens, const cmoe_gp* const* gps, int n
   ens.q = q;
   ens.dim = dim;
   ens.nf = nf;
+  if (kg_ensemble_large(gps, q, p)) {
+    const int ps = dim - nf;
+    CMOE_REQUIRE(nf >= 0 && ps >= 1 && num_pts >= 0, CMOE_ERR_BOUNDS, "num_fidelity out of range");
+    ens.large = true;
+    ens.gps.assign(gps, gps + num_gp);
+    ens.num_pts = num_pts;
+    ens.p = p;
+    ens.num_mc = num_mc;
+    ens.seed = seed;
+    ens.inner = *inner;
+    ens.inner_bounds.assign(inner_bounds, inner_bounds + 2 * static_cast<size_t>(ps));
+    ens.discrete.assign(discrete_pts, discrete_pts + static_cast<size_t>(num_gp) * num_pts * ps);
+    if (p) ens.Xp.assign(Xp, Xp + static_cast<size_t>(p) * dim);
+    ens.best.assign(best_so_far, best_so_far + num_gp);
+    return;
+  }
   for (int m = 0; m < num_gp; ++m) {
     ens.evs.emplace_back(new KgEvaluator());
     make_kg_evaluator(*ens.evs.back(), gps[m], nf, inner, inner_bounds,
                       discrete_pts + static_cast<size_t>(m) * num_pts * (dim - nf), num_pts, max_value_cands,
-                      max_grad_cands, q, Xp, p, num_mc, best_so_far[m], seed, nullptr, false);
+                      max_grad_cands, q, Xp, p, num_mc, best_so_far[m], seed);
   }
 }
 
 BatchEval make_ei_ensemble(const cmoe_gp* const* gps, int num_gp, int q, const double* Xp, int p, int num_mc,
                            const double* best_so_far, uint64_t seed) {
-  CMOE_REQUIRE(q >= 1 && p >= 0 && q + p <= kMaxQ, CMOE_ERR_BOUNDS, "(q+p)*(1+num_derivatives) must be in [1, 96]");
+  CMOE_REQUIRE(q >= 1 && p >= 0 && static_cast<long long>(q) + p <= kMaxSampleQ, CMOE_ERR_BOUNDS,
+               "q + p must be in [1, 8192]");
+  if (q + p > kMaxQ) {
+    // past the per-set kernels' 96 rows: every member on the tiled path of ei_large.cu, one set of normals
+    std::vector<const cmoe_gp*> members(gps, gps + num_gp);
+    std::vector<double> best(best_so_far, best_so_far + num_gp), pending(Xp, Xp + static_cast<size_t>(p) * gps[0]->spec.dim);
+    const size_t ps = static_cast<size_t>(q) * gps[0]->spec.dim;
+    return [=](const double* pts, int nc, double* values, double* grads) {
+      ei_large_ensemble_eval(members.data(), num_gp, pts, nc, q, pending.data(), p, num_mc, best.data(), seed, nullptr,
+                             values, grads);
+      for (int c = 0; c < nc; ++c) values[c] /= static_cast<double>(num_gp);
+      if (grads)
+        for (size_t k = 0; k < nc * ps; ++k) grads[k] /= static_cast<double>(num_gp);
+    };
+  }
   std::vector<BatchEval> members;
   for (int m = 0; m < num_gp; ++m) members.push_back(make_ei_eval(gps[m], q, Xp, p, num_mc, best_so_far[m], seed));
   const size_t ps = static_cast<size_t>(q) * gps[0]->spec.dim;
@@ -695,10 +809,19 @@ int cmoe_kg_eval_mcmc(const cmoe_gp* const* gps, int num_gp, int num_fidelity, c
                       const double* best_so_far, uint64_t seed, const double* normals_table, double* values,
                       double* grads, int* info) {
   return guarded(info, [&] {
+    CMOE_REQUIRE(static_cast<long long>(q) + p <= CMOE_MAX_KG_LARGE_ROWS, CMOE_ERR_BOUNDS,
+                 "(q+p)*(1+num_derivatives) must be <= 1024");
     check_ensemble(gps, num_gp);
     CMOE_REQUIRE(num_candidates >= 1, CMOE_ERR_BOUNDS, "num_multistarts must be > 1");
     const int dim = gps[0]->spec.dim;
     const size_t ps = static_cast<size_t>(q) * dim;
+    if (kg_ensemble_large(gps, q, p)) {
+      kg_large_ensemble_eval(gps, num_gp, num_fidelity, inner, inner_bounds, discrete_pts, num_pts, candidates,
+                             num_candidates, q, points_being_sampled, p, num_mc, best_so_far, seed, normals_table,
+                             values, grads);
+      apply_fidelity_cost(candidates, num_candidates, q, dim, num_fidelity, num_gp, values, grads);
+      return;
+    }
     std::vector<double> tv(num_candidates), tg(grads ? num_candidates * ps : 0);
     std::fill(values, values + num_candidates, 0.0);
     if (grads) std::fill(grads, grads + num_candidates * ps, 0.0);
@@ -730,10 +853,21 @@ int cmoe_ei_eval_mcmc(const cmoe_gp* const* gps, int num_gp, const double* candi
                       const double* points_being_sampled, int p, int num_mc, const double* best_so_far, uint64_t seed,
                       const double* normals_table, int analytic_single, double* values, double* grads, int* info) {
   return guarded(info, [&] {
+    CMOE_REQUIRE(static_cast<long long>(q) + p <= kMaxSampleQ, CMOE_ERR_BOUNDS, "q + p must be <= 8192");
     check_ensemble(gps, num_gp);
     CMOE_REQUIRE(num_candidates >= 1, CMOE_ERR_BOUNDS, "num_multistarts must be > 1");
     require_device(gps[0]->device);
     const size_t ps = static_cast<size_t>(q) * gps[0]->spec.dim;
+    if (q + p > kMaxQ) {
+      // past the per-set kernels' 96 rows: the tiled path of ei_large.cu, every member on the same normals (the table
+      // is checked, then uploaded into the evaluation's workspace)
+      ei_large_ensemble_eval(gps, num_gp, candidates, num_candidates, q, points_being_sampled, p, num_mc, best_so_far,
+                             seed, normals_table, values, grads);
+      for (int c = 0; c < num_candidates; ++c) values[c] /= static_cast<double>(num_gp);
+      if (grads)
+        for (size_t k = 0; k < num_candidates * ps; ++k) grads[k] /= static_cast<double>(num_gp);
+      return;
+    }
     std::vector<double> tv(num_candidates), tg(grads ? num_candidates * ps : 0);
     std::fill(values, values + num_candidates, 0.0);
     if (grads) std::fill(grads, grads + num_candidates * ps, 0.0);

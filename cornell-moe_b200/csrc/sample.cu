@@ -360,6 +360,11 @@ size_t panel_smem_bytes() {
 
 // declared in internal.cuh; also factors the covariance matrices of cmoe_log_marginal_likelihood_list
 void potrf_batched(double* A, int Q, int nsets, int* fail, DevBuf<double>& stage, cudaStream_t s) {
+  stage.ensure(static_cast<size_t>(nsets) * ((Q + NB - 1) / NB) * NB * NB);
+  potrf_batched(A, Q, nsets, fail, stage.p, s);
+}
+
+void potrf_batched(double* A, int Q, int nsets, int* fail, double* stage, cudaStream_t s) {
   const size_t smem_panel = panel_smem_bytes();
   const size_t smem_tile = 2 * NB * LDT * sizeof(double);
   CMOE_CUDA(cudaFuncSetAttribute(chol_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -367,10 +372,9 @@ void potrf_batched(double* A, int Q, int nsets, int* fail, DevBuf<double>& stage
   CMOE_CUDA(cudaFuncSetAttribute(chol_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  static_cast<int>(smem_tile)));
   const int nsteps = (Q + NB - 1) / NB;
-  stage.ensure(static_cast<size_t>(nsets) * nsteps * NB * NB);
   for (int k0 = 0; k0 < Q; k0 += NB) {
     const int nb = std::min(NB, Q - k0), rem = Q - k0 - nb;
-    chol_panel_kernel<<<dim3(1 + (rem + PT - 1) / PT, 1, nsets), PT, smem_panel, s>>>(A, Q, k0, nb, fail, stage.p);
+    chol_panel_kernel<<<dim3(1 + (rem + PT - 1) / PT, 1, nsets), PT, smem_panel, s>>>(A, Q, k0, nb, fail, stage);
     count_launch();
     if (rem > 0) {
       const int t = (rem + NB - 1) / NB;
@@ -378,24 +382,29 @@ void potrf_batched(double* A, int Q, int nsets, int* fail, DevBuf<double>& stage
       count_launch();
     }
   }
-  chol_diag_writeback_kernel<<<dim3(nsteps, 1, nsets), PT, 0, s>>>(A, Q, fail, stage.p);
+  chol_diag_writeback_kernel<<<dim3(nsteps, 1, nsets), PT, 0, s>>>(A, Q, fail, stage);
   count_launch();
   CMOE_CUDA(cudaGetLastError());
 }
 
 void posterior_cov_large(const cmoe_gp& gp, SampleWork& w, int nc, int num, int gs, double jitter, cudaStream_t s) {
+  posterior_cov_large(gp, w.P.p, w.dPs.p, w.V.p, w.mu.p, w.A.p, nc, num, gs, jitter, s);
+}
+
+void posterior_cov_large(const cmoe_gp& gp, const double* P, const int* dPs, double* V, double* mu, double* A, int nc,
+                         int num, int gs, double jitter, cudaStream_t s) {
   const KernelSpec& spec = gp.spec;
   const int Q = num * (1 + gs), n = gp.n;
-  build_mix_covariance(spec, gp.dX.p, gp.N, w.P.p, nc * num, w.dPs.p, gs, w.V.p, s);
+  build_mix_covariance(spec, gp.dX.p, gp.N, P, nc * num, dPs, gs, V, s);
   // the blocked kernel whatever the column count, so a set's solve does not depend on how many sets share its chunk
-  trsm_lower_blocked(gp.dK.p, n, w.V.p, n, nc * Q, false, s);
-  posterior_mean_points(gp, w.P.p, static_cast<size_t>(nc) * num, w.dPs.p, gs, w.mu.p, nullptr, s);
+  trsm_lower_blocked(gp.dK.p, n, V, n, nc * Q, false, s);
+  posterior_mean_points(gp, P, static_cast<size_t>(nc) * num, dPs, gs, mu, nullptr, s);
   const int t = (Q + NB - 1) / NB;
   const size_t smem_cov = (2 * static_cast<size_t>(NB) * LDT + 2 * static_cast<size_t>(NB) * spec.dim) * sizeof(double);
   CMOE_CUDA(cudaFuncSetAttribute(cov_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  static_cast<int>(smem_cov)));
-  cov_tile_kernel<<<dim3(t * (t + 1) / 2, 1, nc), kTileThreads, smem_cov, s>>>(spec, w.V.p, n, Q, w.P.p, num, w.dPs.p,
-                                                                              gs, jitter, w.A.p);
+  cov_tile_kernel<<<dim3(t * (t + 1) / 2, 1, nc), kTileThreads, smem_cov, s>>>(spec, V, n, Q, P, num, dPs, gs, jitter,
+                                                                              A);
   count_launch();
   CMOE_CUDA(cudaGetLastError());
 }

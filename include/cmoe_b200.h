@@ -170,7 +170,9 @@ int cmoe_hyperparameter_mcmc(int kernel, int prior, int noisy, const double* ini
                              double* log_probabilities, int* info);
 /* Run-time switches between kernel generations (also read once from the environment: CMOE_LEGACY_LINALG, CMOE_COV_TMA):
  *   "legacy_linalg" 1 = round-1 launch-per-step Cholesky / chained trsv for large n (default 0: cooperative kernels);
- *   "cov_tma"       1 = TMA / DMMA covariance build with tensor-map tile stores (default 0: LDGSTS kernel, faster at d ~ 10). */
+ *   "cov_tma"       1 = TMA / DMMA covariance build with tensor-map tile stores (default 0: LDGSTS kernel, faster at d ~ 10);
+ *   "ensemble_members_in_flight"  k >= 1 = at most k members of an ensemble run at once on the large-union q-KG / q-EI
+ *                   stages (default 0: as many as the 2 GiB workspace holds).  Results do not depend on it. */
 int cmoe_set_option(const char* name, int value);
 void cmoe_gp_destroy(cmoe_gp* gp);
 int cmoe_gp_dim(const cmoe_gp* gp);
@@ -415,9 +417,9 @@ int cmoe_kg_eval(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_params* inne
  * CMOE_ERR_BOUNDS, before any device work, when one candidate's workspace does not fit.  A singular union covariance -> CMOE_ERR_SINGULAR, *info = leading minor of
  * the first failing candidate.  stats: mc_samples exact, posterior_evals and line_search_steps as cmoe_kg_stats,
  * point_evals and line_batches what this call's kernel executed.  num_mc <= 65535 * 64.  The multistart q-KG drivers
- * (cmoe_multistart_kg(_ex), cmoe_kg_gradient_descent(_ex)) evaluate through these stages when (q + p)(1 + g) > 32 and
- * through the plans otherwise.  Not covered: the cmoe_kg_plan_* API, the ensemble calls (cmoe_kg_eval_mcmc,
- * cmoe_multistart_kg_mcmc, cmoe_kg_gradient_descent_mcmc) and multigpu.py keep the 32-row bound of cmoe_kg_eval. */
+ * (cmoe_multistart_kg(_ex), cmoe_kg_gradient_descent(_ex)) and the ensemble calls (cmoe_kg_eval_mcmc,
+ * cmoe_multistart_kg_mcmc, cmoe_kg_gradient_descent_mcmc) evaluate through these stages when (q + p)(1 + g) > 32 and
+ * through the plans / cmoe_kg_eval otherwise.  The cmoe_kg_plan_* API keeps the 32-row bound of cmoe_kg_eval. */
 int cmoe_kg_eval_large(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_params* inner, const double* inner_bounds,
                        const double* discrete_pts, int num_pts, const double* candidates, int num_candidates, int q,
                        const double* points_being_sampled, int p, int num_mc, double best_so_far, uint64_t seed,
@@ -556,7 +558,16 @@ int cmoe_ei_analytic(const cmoe_gp* gp, const double* points, int num_points, do
  *                        and ComputeEIMCMC... (gpp_expected_improvement_mcmc_optimization.hpp:860-980): screen, top-20,
  *                        restarted gradient descent, strict-> arg-max (initial best -inf for KG, 0.0 for EI; the EI
  *                        driver uses analytic 1-EI per member when q = 1, p = 0).
- * normals_table: as in cmoe_kg_eval / cmoe_ei_eval (NULL = Philox stream keyed by seed); shared by every member. */
+ * normals_table: as in cmoe_kg_eval / cmoe_ei_eval (NULL = Philox stream keyed by seed); shared by every member.
+ *
+ * Sizes: q-KG up to (q + p)(1 + g) = 32 runs each member's cmoe_kg_eval (the drivers: its plans); past 32, up to
+ * CMOE_MAX_KG_LARGE_ROWS, each member's cmoe_kg_eval_large with num_mc, g and the inner optimiser bounded as there.
+ * q-EI up to q + p = CMOE_MAX_SET_ROWS runs each member's cmoe_ei_eval; past it, up to CMOE_MAX_LARGE_SET_ROWS, each
+ * member's cmoe_ei_eval_large.  Past the per-set bounds the draws are made once per evaluation, the members run
+ * together on their own streams, and the evaluation's large-stage workspace is at most 2 GiB per device whatever
+ * num_gp is (kept on gps[0]'s handle); each member's value and gradient are those of its single large call, summed in
+ * member order.  q + p past the large bound -> CMOE_ERR_BOUNDS before any handle is read.  A singular union ->
+ * CMOE_ERR_SINGULAR, *info = leading minor of the first failing candidate of the first failing member. */
 int cmoe_kg_eval_mcmc(const cmoe_gp* const* gps, int num_gp, int num_fidelity, const cmoe_gd_params* inner,
                       const double* inner_bounds, const double* discrete_pts, int num_pts, const double* candidates,
                       int num_candidates, int q, const double* points_being_sampled, int p, int num_mc,
