@@ -137,11 +137,7 @@ void ei_eval_chunk(const cmoe_gp& gp, const double* candidates, int nc, int q, c
   pb.run(gp, /*diag_mode=*/1, /*want_chol=*/true, want_grad, s);
   int which = 0;
   const int f = pb.first_failure(s, &which);
-  if (f != 0)
-    throw Error(CMOE_ERR_SINGULAR,
-                "GP-Variance matrix singular. Check for duplicate points_to_sample/being_sampled or "
-                "points_to_sample/being_sampled duplicating points_sampled with 0 noise.",
-                f);
+  if (f != 0) throw_singular_union(f);
   DevBuf<double> zbuf(static_cast<size_t>(nc) * num_mc * U), imp(static_cast<size_t>(nc) * num_mc);
   DevBuf<int> win(static_cast<size_t>(nc) * num_mc);
   DevBuf<double> dei(nc), dgrad(want_grad ? static_cast<size_t>(nc) * q * dim : 1);

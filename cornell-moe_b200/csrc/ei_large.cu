@@ -292,15 +292,14 @@ __global__ void __launch_bounds__(kTileThreads) ei_ctc_kernel(int U, const doubl
 
 constexpr size_t kTileSmem = 2 * static_cast<size_t>(NB) * LDT * sizeof(double);
 
-// out = in^T for nsets U x U matrices
-__global__ void __launch_bounds__(256) transpose_kernel(int U, const double* __restrict__ in,
+// out = in^T for batched column-major rows x cols matrices (out: cols x rows), one batch entry per blockIdx.y
+__global__ void __launch_bounds__(256) transpose_kernel(int rows, int cols, const double* __restrict__ in,
                                                         double* __restrict__ out) {
-  const int set = blockIdx.y;
-  const size_t o = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
-  if (o >= static_cast<size_t>(U) * U) return;
-  const size_t off = static_cast<size_t>(set) * U * U;
-  const int r = static_cast<int>(o % U), c = static_cast<int>(o / U);
-  out[off + o] = in[off + static_cast<size_t>(r) * U + c];
+  const size_t off = static_cast<size_t>(blockIdx.y) * rows * cols;
+  const size_t o = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (o >= static_cast<size_t>(rows) * cols) return;
+  const size_t r = o % cols, cc = o / cols;  // out (r, cc) = in (cc, r)
+  out[off + o] = in[off + r * rows + cc];
 }
 
 // Out = A B (column-major; A m x kd, B kd x nn), 64 x 64 DMMA tiles; grid (row blocks, column blocks, batch)
@@ -436,17 +435,6 @@ size_t ei_large_chunk_bytes(int n, int U, int q, int dim, int num_mc, bool want_
   return cv.off;
 }
 
-// the union sets of one chunk, P [nb][q + p][dim]: each candidate's q points, then the pending points
-__global__ void __launch_bounds__(256) ei_sets_kernel(int q, int p, int dim, const double* __restrict__ cand,
-                                                      const double* __restrict__ Xp, double* __restrict__ P) {
-  const int c = blockIdx.x, U = q + p;
-  for (int e = threadIdx.x; e < U * dim; e += blockDim.x) {
-    const int u = e / dim, d = e % dim;
-    P[static_cast<size_t>(c) * U * dim + e] =
-        u < q ? cand[(static_cast<size_t>(c) * q + u) * dim + d] : Xp[static_cast<size_t>(u - q) * dim + d];
-  }
-}
-
 void ei_large_run(const cmoe_gp& gp, const EiLargeBufs& b, const double* cand, const double* Xp, int nc, int q, int p,
                   int num_mc, double best_so_far, const double* W, cudaStream_t s, double* ei_out, double* grad_out,
                   int* fail_out) {
@@ -458,8 +446,7 @@ void ei_large_run(const cmoe_gp& gp, const EiLargeBufs& b, const double* cand, c
   for (int c0 = 0; c0 < nc; c0 += b.chunk) {
     const int nb = std::min(b.chunk, nc - c0);
     const double* P = b.P;
-    ei_sets_kernel<<<nb, 256, 0, s>>>(q, p, dim, cand + static_cast<size_t>(c0) * q * dim, Xp, b.P);
-    count_launch();
+    build_union_sets(cand + static_cast<size_t>(c0) * q * dim, Xp, nb, q, p, dim, b.P, s);
     // mu, Var + 1e-6 I (gpp_math.cpp:2000-2002) and its factor C, upper triangle zero
     posterior_cov_large(gp, P, b.dPs, b.V, b.mu, b.A, nb, U, 0, 1.0e-6, s);
     CMOE_CUDA(cudaMemsetAsync(b.fail, 0, nb * sizeof(int), s));
@@ -519,7 +506,6 @@ void gemm_nn(int m, int nn, int kd, const double* A, int lda, size_t sa, const d
 
 void cholesky_adjoint(const double* C, int U, int nc, double* T1, double* T2, cudaStream_t s) {
   const size_t UU = static_cast<size_t>(U) * U;
-  const unsigned gUU = static_cast<unsigned>((UU + 255) / 256);
   const int t = (U + NB - 1) / NB;
   CMOE_CUDA(cudaFuncSetAttribute(ei_ctc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  static_cast<int>(kTileSmem)));
@@ -529,110 +515,65 @@ void cholesky_adjoint(const double* C, int U, int nc, double* T1, double* T2, cu
   mirror_lower(nc, U, T2, s);  // S = Phi(M) + Phi(M)^T
   for (int c = 0; c < nc; ++c)  // X = C^-T S
     trsm_lower_blocked(C + c * UU, U, T2 + c * UU, U, U, true, s);
-  transpose_kernel<<<dim3(gUU, nc), 256, 0, s>>>(U, T2, T1);
-  count_launch();
+  transpose_batched(U, U, T2, T1, nc, s);
   for (int c = 0; c < nc; ++c)  // T = C^-T X^T = C^-T S C^-1 = 2 Sigmabar
     trsm_lower_blocked(C + c * UU, U, T1 + c * UU, U, U, true, s);
 }
 
-void ei_large_eval_batch(const cmoe_gp& gp, const double* candidates, int nc, int q, const double* Xp, int p,
-                         int num_mc, double best_so_far, uint64_t seed, const double* dtable, double* ei_host,
-                         double* grad_host) {
-  check_ei_large_sizes(q, p, num_mc);
-  cudaStream_t s = gp.stream;
-  const int U = q + p, dim = gp.spec.dim, n = gp.n;
-  const bool want_grad = grad_host != nullptr;
-  DevBuf<double> Wgen;
-  const double* W = dtable;
-  if (W == nullptr) {
-    Wgen.alloc(static_cast<size_t>(num_mc) * U);
-    philox_normals_device(seed, 0, num_mc, U, Wgen.p, s);
-    W = Wgen.p;
-  }
-  // the candidates and the pending points, uploaded once; each chunk forms its union sets on the device
-  DevBuf<double> dcand, dXp;
-  dcand.upload(candidates, static_cast<size_t>(nc) * q * dim, s);
-  if (p) dXp.upload(Xp, static_cast<size_t>(p) * dim, s);
-  // chunks of the 2 GiB workspace, a region on the handle (SampleWork::ei_large)
-  const size_t per_cand = ei_large_chunk_bytes(n, U, q, dim, num_mc, want_grad, 1);
-  const int chunk = static_cast<int>(chunk_items(nc, kSampleWorkspaceBytes - kCarveSlack, per_cand, kMaxChunkSets));
-  SampleWork& w = sample_work(gp);
-  w.ei_large.ensure((ei_large_chunk_bytes(n, U, q, dim, num_mc, want_grad, chunk) + sizeof(double) - 1) /
-                    sizeof(double));
-  EiLargeBufs b;
-  Carve cv{reinterpret_cast<char*>(w.ei_large.p)};
-  ei_large_carve(n, U, q, dim, num_mc, want_grad, chunk, cv, b);
-  // the call's results, read back once
-  DevBuf<double> dei(nc), dgrad(want_grad ? static_cast<size_t>(nc) * q * dim : 0);
-  DevBuf<int> dfail(nc);
-  ei_large_run(gp, b, dcand.p, dXp.p, nc, q, p, num_mc, best_so_far, W, s, dei.p, want_grad ? dgrad.p : nullptr,
-               dfail.p);
-  std::vector<int> hfail(nc);
-  dfail.download(hfail.data(), nc, s);
-  dei.download(ei_host, nc, s);
-  if (want_grad) dgrad.download(grad_host, static_cast<size_t>(nc) * q * dim, s);
-  CMOE_CUDA(cudaStreamSynchronize(s));
-  for (int c = 0; c < nc; ++c)
-    if (hfail[c] != 0) throw_singular_union(hfail[c]);
+void transpose_batched(int rows, int cols, const double* in, double* out, int batch, cudaStream_t s) {
+  transpose_kernel<<<dim3(static_cast<unsigned>((static_cast<size_t>(rows) * cols + 255) / 256), batch), 256, 0, s>>>(
+      rows, cols, in, out);
+  count_launch();
 }
 
-void ei_large_ensemble_eval(const cmoe_gp* const* gps, int num_gp, const double* candidates, int nc, int q,
-                            const double* Xp, int p, int num_mc, const double* best_so_far, uint64_t seed,
-                            const double* normals_table, double* values, double* grads) {
+void ei_large_eval(const cmoe_gp* const* gps, int num_gp, const double* candidates, int nc, int q, const double* Xp,
+                   int p, int num_mc, const double* best_so_far, uint64_t seed, const double* dtable, double* values,
+                   double* grads) {
   check_ei_large_sizes(q, p, num_mc);
   require_device(gps[0]->device);
   const int U = q + p, dim = gps[0]->spec.dim;
   const bool want_grad = grads != nullptr;
-  // the normals are counted once; the W members in flight share the rest of the 2 GiB.  As in the single call, a
-  // candidate that alone needs more is not refused: it runs alone, one member at a time.
+  // the normals are counted once, whether drawn here or passed in; the members in flight share the rest of the 2 GiB.
+  // A candidate that alone needs more is not refused: it runs alone, one member at a time.
   const size_t w_count = static_cast<size_t>(num_mc) * U;
-  const size_t budget = kSampleWorkspaceBytes - w_count * sizeof(double);
   size_t per = 0;
   for (int m = 0; m < num_gp; ++m)
     per = std::max(per, ei_large_chunk_bytes(gps[m]->n, U, q, dim, num_mc, want_grad, 1));
-  size_t width = std::min<size_t>(num_gp, budget / (per + kCarveSlack));
-  if (ensemble_members_in_flight() > 0) width = std::min<size_t>(width, ensemble_members_in_flight());
-  width = std::max<size_t>(1, width);
-  const size_t share = budget / width;
-  const int chunk = static_cast<int>(chunk_items(nc, share > kCarveSlack ? share - kCarveSlack : 0, per, kMaxChunkSets));
+  const MemberSchedule ms = schedule_members(num_gp, nc, kSampleWorkspaceBytes - w_count * sizeof(double), per);
   size_t slot_bytes = 0;
   for (int m = 0; m < num_gp; ++m)
-    slot_bytes = std::max(slot_bytes, ei_large_chunk_bytes(gps[m]->n, U, q, dim, num_mc, want_grad, chunk));
-  slot_bytes = (slot_bytes + 255) & ~size_t(255);
-  // one region on the first member's handle: the normals, the candidates and pending points, every member's results,
-  // the W slots
+    slot_bytes = std::max(slot_bytes, ei_large_chunk_bytes(gps[m]->n, U, q, dim, num_mc, want_grad, ms.chunk));
+  slot_bytes = slot_stride(slot_bytes);
+  // one region on the first member's handle: the normals (unless passed in), the candidates and pending points, every
+  // member's results, the slots
   const size_t ps = static_cast<size_t>(q) * dim;
   double *Wd = nullptr, *dcand = nullptr, *dXp = nullptr, *dval = nullptr, *dgrad = nullptr;
   int* dfail = nullptr;
   char* slots = nullptr;
-  auto layout = [&](Carve& cv) {
-    Wd = cv.take<double>(w_count);
+  LargeUnionWork& w = carve_large_union_work(*gps[0], [&](Carve& cv) {
+    Wd = dtable ? nullptr : cv.take<double>(w_count);
     dcand = cv.take<double>(static_cast<size_t>(nc) * ps);
     dXp = cv.take<double>(static_cast<size_t>(std::max(1, p)) * dim);
     dval = cv.take<double>(static_cast<size_t>(num_gp) * nc);
     dgrad = want_grad ? cv.take<double>(static_cast<size_t>(num_gp) * nc * ps) : nullptr;
     dfail = cv.take<int>(static_cast<size_t>(num_gp) * nc);
-    slots = cv.take<char>(slot_bytes * width);
-  };
-  Carve cv;
-  layout(cv);
-  EnsembleWork& ew = ensemble_work(*gps[0], cv.off);
-  cv = Carve{reinterpret_cast<char*>(ew.arena.p)};
-  layout(cv);
+    slots = cv.take<char>(slot_bytes * ms.width);
+  });
   cudaStream_t s0 = gps[0]->stream;
-  if (normals_table)
-    CMOE_CUDA(cudaMemcpyAsync(Wd, normals_table, w_count * sizeof(double), cudaMemcpyHostToDevice, s0));
-  else
+  const double* W = dtable;
+  if (W == nullptr) {
     philox_normals_device(seed, 0, num_mc, U, Wd, s0);
+    W = Wd;
+  }
   CMOE_CUDA(cudaMemcpyAsync(dcand, candidates, static_cast<size_t>(nc) * ps * sizeof(double), cudaMemcpyHostToDevice,
                             s0));
   if (p) CMOE_CUDA(cudaMemcpyAsync(dXp, Xp, static_cast<size_t>(p) * dim * sizeof(double), cudaMemcpyHostToDevice, s0));
   CMOE_CUDA(cudaStreamSynchronize(s0));
-  run_members(gps, num_gp, static_cast<int>(width), ew, [&](int m, int slot) {
+  run_members(gps, num_gp, ms.width, w, [&](int m, int slot) {
     EiLargeBufs b;
     Carve sc{slots + slot * slot_bytes};
-    ei_large_carve(gps[m]->n, U, q, dim, num_mc, want_grad, chunk, sc, b);
-    ei_large_run(*gps[m], b, dcand, dXp, nc, q, p, num_mc, best_so_far[m], Wd, gps[m]->stream, dval + m * nc,
+    ei_large_carve(gps[m]->n, U, q, dim, num_mc, want_grad, ms.chunk, sc, b);
+    ei_large_run(*gps[m], b, dcand, dXp, nc, q, p, num_mc, best_so_far[m], W, gps[m]->stream, dval + m * nc,
                  want_grad ? dgrad + m * nc * ps : nullptr, dfail + m * nc);
   });
   drain_members(s0, num_gp, nc, ps, dval, dgrad, dfail, values, grads);
@@ -650,10 +591,10 @@ extern "C" int cmoe_ei_eval_large(const cmoe_gp* gp, const double* candidates, i
     CMOE_REQUIRE(q >= 1 && p >= 0 && num_mc >= 1, CMOE_ERR_BOUNDS, "q >= 1, p >= 0, num_mc >= 1 required");
     CMOE_REQUIRE(static_cast<long long>(q) + p <= kMaxSampleQ, CMOE_ERR_BOUNDS, "q + p must be <= 8192");
     require_device(gp->device);
-    const int U = q + p;
+    // the table is uploaded once, beside the evaluation's workspace
     DevBuf<double> dtable;
-    if (normals_table) dtable.upload(normals_table, static_cast<size_t>(num_mc) * U, gp->stream);
-    ei_large_eval_batch(*gp, candidates, num_candidates, q, points_being_sampled, p, num_mc, best_so_far, seed,
-                        normals_table ? dtable.p : nullptr, ei, grad_ei);
+    if (normals_table) dtable.upload(normals_table, static_cast<size_t>(num_mc) * (q + p), gp->stream);
+    ei_large_eval(&gp, 1, candidates, num_candidates, q, points_being_sampled, p, num_mc, &best_so_far, seed,
+                  normals_table ? dtable.p : nullptr, ei, grad_ei);
   });
 }

@@ -325,7 +325,7 @@ py::object RandomFeatureSample::call(const py::object& x, bool gradient) const {
 std::vector<double> full_bounds(const py::list& domain_bounds, int dim) { return to_vec(domain_bounds, 2 * static_cast<size_t>(dim)); }
 
 // ---- EI ---------------------------------------------------------------------------------------------------------------
-// The q-EI evaluator for a union of q + p rows: the per-set kernels up to 96 rows, the tiled path past them.
+// The q-EI evaluator for a union of q + p rows: the per-set kernels up to CMOE_MAX_SET_ROWS, the tiled path past them.
 using EiEvalFn = int (*)(const cmoe_gp*, const double*, int, int, const double*, int, int, double, uint64_t,
                          const double*, double*, double*, int*);
 EiEvalFn ei_eval_for(int q, int p) { return q + p > CMOE_MAX_SET_ROWS ? cmoe_ei_eval_large : cmoe_ei_eval; }
@@ -519,12 +519,13 @@ py::list compute_grad_posterior_mean(const GaussianProcess& gp, int num_fidelity
 }
 
 // ---- q-KG ---------------------------------------------------------------------------------------------------------------
-// The q-KG evaluator for a union of (q + p)(1 + g) rows: the 32-row call up to its bound, cmoe_kg_eval_large past it.
+// The q-KG evaluator for a union of (q + p)(1 + g) rows: cmoe_kg_eval up to CMOE_MAX_KG_ROWS, cmoe_kg_eval_large past it.
 using KgEvalFn = int (*)(const cmoe_gp*, int, const cmoe_gd_params*, const double*, const double*, int, const double*,
                          int, int, const double*, int, int, double, uint64_t, const double*, double*, double*,
                          cmoe_kg_stats*, int*);
 KgEvalFn kg_eval_for(const GaussianProcess& gp, int q, int p) {
-  return static_cast<long long>(q + p) * (1 + gp.num_derivatives_) > 32 ? cmoe_kg_eval_large : cmoe_kg_eval;
+  return static_cast<long long>(q + p) * (1 + gp.num_derivatives_) > CMOE_MAX_KG_ROWS ? cmoe_kg_eval_large
+                                                                                       : cmoe_kg_eval;
 }
 
 double compute_knowledge_gradient(const GaussianProcess& gp, int num_fidelity, const py::object& optimizer_parameters,

@@ -40,6 +40,10 @@ void set_last_error(const std::string& msg);
     }                                                                                                    \
   } while (0)
 
+// a macro's value as a string literal
+#define CMOE_STR_(x) #x
+#define CMOE_STR(x) CMOE_STR_(x)
+
 #define CMOE_REQUIRE(cond, code, msg)                 \
   do {                                                \
     if (!(cond)) throw ::cmoe::Error((code), (msg)); \
@@ -156,11 +160,9 @@ struct cmoe_gp {
   mutable std::vector<cmoe_gp*> replicas;
   // device workspace of the joint-sampling calls (sample.cu), grown on demand and kept until the handle is destroyed
   mutable std::shared_ptr<void> sample_ws;
-  // device workspace of cmoe_kg_eval_large (kg_large.cu), grown on demand and kept until the handle is destroyed
-  mutable std::shared_ptr<void> kg_large_ws;
-  // device workspace of the ensemble evaluations past the per-set bounds whose first member is this handle
-  // (cmoe::EnsembleWork), grown on demand up to one evaluation's need and kept until the handle is destroyed
-  mutable std::shared_ptr<void> ensemble_ws;
+  // device workspace of the large-union evaluations (kg_large.cu, ei_large.cu) whose first member is this handle
+  // (cmoe::LargeUnionWork), grown on demand up to one evaluation's need and kept until the handle is destroyed
+  mutable std::shared_ptr<void> large_union_ws;
   mutable uint64_t replicas_generation = 0;
   ~cmoe_gp();
 };
@@ -227,7 +229,6 @@ void potrf_batched(double* A, int Q, int nsets, int* fail, double* stage, cudaSt
 // handle.
 struct SampleWork {
   DevBuf<double> P, V, A, mu, y, part_v, opt, stage, table;
-  DevBuf<double> ei_large;  // the chunk workspace of ei_large_eval_batch, carved by ei_large.cu
   DevBuf<int> dPs, fail, part_i, amin;
 };
 // the handle's SampleWork, created on first use
@@ -252,6 +253,14 @@ inline size_t chunk_items(size_t total, size_t budget, size_t bytes_per_item, si
   return std::max<size_t>(1, std::min<size_t>({total, budget / bytes_per_item, cap}));
 }
 
+// streaming multiprocessors of the current device
+inline int sm_count() {
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms;
+}
+
 // Step size of gradient-descent iteration i (from 0): pre_mult (i + 1)^-gamma, gpp_optimization.hpp:736
 inline double gd_step_size(double pre_mult, double gamma, int i) {
   return pre_mult * std::pow(static_cast<double>(i + 1), -gamma);
@@ -264,7 +273,7 @@ constexpr int kMaxLcbSelectedRows = 1024;
 constexpr size_t kMaxLcbRoundDoubles = kSampleWorkspaceBytes / sizeof(double);
 
 // ---- posterior.cu -------------------------------------------------------------------------------------------
-constexpr int kMaxQ = 96;  // largest (q+p)*(1+num_derivatives) handled by the per-set kernels
+constexpr int kMaxQ = CMOE_MAX_SET_ROWS;  // largest (q+p)*(1+num_derivatives) handled by the per-set kernels
 
 // Device-resident posterior quantities for a batch of nc point sets (num points each, gs derivative rows per point).
 struct PosteriorBatch {
@@ -294,38 +303,46 @@ void posterior_mean_points(const cmoe_gp& gp, const double* P, size_t npts, cons
 // ---- multistart.cu -------------------------------------------------------------------------------------------
 // An ensemble (one GP per hyper-parameter sample) is non-empty and its members share dim, g and device.
 void check_ensemble(const cmoe_gp* const* gps, int num_gp);
+// Member m's values v[nc] and gradients g[nc][ps] (g, grads NULL: none) into the ensemble's sums, called in member
+// order: member 0's start the sums (its own bits, so a one-member sum is the member's result), later members are added.
+void add_member(int m, int nc, size_t ps, const double* v, const double* g, double* values, double* grads);
+
+// The evaluation path of a union of q candidate and p pending points.  q-KG past CMOE_MAX_KG_ROWS rows,
+// (q + p)(1 + g), runs the large-union stages of kg_large.cu instead of the plans of kg.cu; q-EI past kMaxQ rows runs
+// the tiles of ei_large.cu instead of the per-set kernels of ei.cu.
+inline bool kg_union_is_large(int q, int p, int g) {
+  return static_cast<long long>(q + p) * (1 + g) > CMOE_MAX_KG_ROWS;
+}
+inline bool ei_union_is_large(int q, int p) { return q + p > kMaxQ; }
+
+// ---- kg.cu ---------------------------------------------------------------------------------------------------
+// P [nc][q + p][dim] <- each candidate's q points, then the p pending points.  Asynchronous on `s`.
+void build_union_sets(const double* cand, const double* Xp, int nc, int q, int p, int dim, double* P, cudaStream_t s);
 
 // ---- ei.cu ---------------------------------------------------------------------------------------------------
 void upload_union_sets(PosteriorBatch& pb, const double* candidates, int nc, int q, const double* Xp, int p, int dim,
                        cudaStream_t s);
 void ei_eval_batch(const cmoe_gp& gp, const double* candidates, int nc, int q, const double* Xp, int p, int num_mc,
                    double best_so_far, uint64_t seed, const double* dtable, double* ei_host, double* grad_host);
-// ---- ei_large.cu: the same evaluation for 1 <= q + p <= kMaxSampleQ (DESIGN.md K16) ----
-void ei_large_eval_batch(const cmoe_gp& gp, const double* candidates, int nc, int q, const double* Xp, int p,
-                         int num_mc, double best_so_far, uint64_t seed, const double* dtable, double* ei_host,
-                         double* grad_host);
-// ---- kg_large.cu: cmoe_kg_eval for 1 <= (q + p)(1 + g) <= CMOE_MAX_KG_LARGE_ROWS (DESIGN.md K17) ----
-// stale_union (q points or NULL): the discretisation set's union part keeps these q points (the reference drivers'
-// quirk, cmoe_kg_plan_set_stale_union); normals_table: ((num_mc + 1) / 2) (q + p)(1 + g) values or NULL.  Throws Error.
-void kg_large_eval(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_params* inner, const double* inner_bounds,
-                   const double* discrete_pts, int num_pts, const double* candidates, int num_candidates, int q,
-                   const double* points_being_sampled, int p, int num_mc, double best_so_far, uint64_t seed,
-                   const double* normals_table, const double* stale_union, double* kg, double* grad_kg,
-                   cmoe_kg_stats* stats);
-// Ensemble form (DESIGN.md K18): the num_gp members' kg_large_eval results for one draw set Z, made once; values[nc]
-// and grads[nc][q][dim] (or NULL) receive the member-ordered sums.  The large-stage workspace of the evaluation (Z, the
-// inner optimisers' scratch, the members' chunks) is at most 2 GiB, on gps[0]'s handle (ensemble_work).  A singular
-// union throws CMOE_ERR_SINGULAR with the leading minor of the first failing candidate of the first failing member.
-void kg_large_ensemble_eval(const cmoe_gp* const* gps, int num_gp, int num_fidelity, const cmoe_gd_params* inner,
-                            const double* inner_bounds, const double* discrete_pts, int num_pts,
-                            const double* candidates, int num_candidates, int q, const double* points_being_sampled,
-                            int p, int num_mc, const double* best_so_far, uint64_t seed, const double* normals_table,
-                            double* values, double* grads);
-// The same for q-EI past the per-set kernels (ei_large_eval_batch per member); normals_table: host [num_mc][q + p] or
-// NULL (Philox), checked before it is uploaded.
-void ei_large_ensemble_eval(const cmoe_gp* const* gps, int num_gp, const double* candidates, int num_candidates, int q,
-                            const double* points_being_sampled, int p, int num_mc, const double* best_so_far,
-                            uint64_t seed, const double* normals_table, double* values, double* grads);
+// ---- the large-union stages: one evaluation of an ensemble of num_gp >= 1 GPs (a single GP is the one-member ensemble)
+// values[nc] and grads[nc][q][dim] (or NULL) receive the members' results summed in member order; with one member they
+// are that member's own.  The draws are made once per evaluation and shared by every member.  The evaluation's device
+// workspace is at most 2 GiB, on gps[0]'s handle (large_union_work).  A singular union throws CMOE_ERR_SINGULAR with
+// the leading minor of the first failing candidate of the first failing member.
+// kg_large.cu: cmoe_kg_eval for 1 <= (q + p)(1 + g) <= CMOE_MAX_KG_LARGE_ROWS (DESIGN.md K17, K18).  normals_table:
+// host ((num_mc + 1) / 2) (q + p)(1 + g) values or NULL (Philox); stale_union (q points or NULL): the discretisation
+// set's union part keeps these q points (the reference drivers' quirk, cmoe_kg_plan_set_stale_union); stats (or NULL)
+// receives the members' counters summed.
+void kg_large_eval(const cmoe_gp* const* gps, int num_gp, int num_fidelity, const cmoe_gd_params* inner,
+                   const double* inner_bounds, const double* discrete_pts, int num_pts, const double* candidates,
+                   int num_candidates, int q, const double* points_being_sampled, int p, int num_mc,
+                   const double* best_so_far, uint64_t seed, const double* normals_table, const double* stale_union,
+                   double* values, double* grads, cmoe_kg_stats* stats);
+// ei_large.cu: the q-EI of ei.cu for 1 <= q + p <= kMaxSampleQ (DESIGN.md K16, K18).  dtable: device [num_mc][q + p]
+// or NULL (Philox).
+void ei_large_eval(const cmoe_gp* const* gps, int num_gp, const double* candidates, int num_candidates, int q,
+                   const double* points_being_sampled, int p, int num_mc, const double* best_so_far, uint64_t seed,
+                   const double* dtable, double* values, double* grads);
 // Consecutive 256-byte aligned pieces of one device region (the large-union stages' workspaces); with base == NULL it
 // only counts the bytes.
 struct Carve {
@@ -344,30 +361,54 @@ struct Carve {
 constexpr size_t kCarveSlack = 64 * 256;
 // CMOE_ERR_SINGULAR for a singular union covariance, *info = minor (the 1-based leading minor that failed)
 [[noreturn]] void throw_singular_union(int minor);
-// The region the ensemble evaluations above carve their buffers from, on the first member's handle, and one event per
-// member.  Every evaluation ends with its members' streams synchronised, so the next one may reuse the region.
-struct EnsembleWork {
+// The region the large-union evaluations above carve their buffers from, on the first member's handle, and one event
+// per member.  Every evaluation ends with its members' streams synchronised, so the next one may reuse the region.
+struct LargeUnionWork {
   DevBuf<double> arena;
   std::vector<cudaEvent_t> done;
-  EnsembleWork() = default;
-  EnsembleWork(const EnsembleWork&) = delete;
-  EnsembleWork& operator=(const EnsembleWork&) = delete;
-  ~EnsembleWork();
+  LargeUnionWork() = default;
+  LargeUnionWork(const LargeUnionWork&) = delete;
+  LargeUnionWork& operator=(const LargeUnionWork&) = delete;
+  ~LargeUnionWork();
 };
-// gp's EnsembleWork with an arena of at least `bytes` (grown by replacement, never kept larger than one evaluation's need)
-EnsembleWork& ensemble_work(const cmoe_gp& gp, size_t bytes);
+// gp's LargeUnionWork with an arena of at least `bytes` (grown by replacement, never kept larger than one evaluation's
+// need)
+LargeUnionWork& large_union_work(const cmoe_gp& gp, size_t bytes);
+// gp's LargeUnionWork with the arena laid out by layout(Carve&): called once to measure, once more to carve the arena
+template <class Layout>
+LargeUnionWork& carve_large_union_work(const cmoe_gp& gp, Layout&& layout) {
+  Carve cv;
+  layout(cv);
+  LargeUnionWork& w = large_union_work(gp, cv.off);
+  cv = Carve{reinterpret_cast<char*>(w.arena.p)};
+  layout(cv);
+  return w;
+}
+// How many members run at once and how many candidates each runs per chunk.  `avail` bytes hold the members' slots; a
+// slot is a chunk at `per` bytes per candidate, kCarveSlack for alignment and, after the chunk, whatever the caller
+// splits evenly between the slots.  width_cap bounds the members in flight further, as does
+// cmoe_set_option("ensemble_members_in_flight").
+struct MemberSchedule {
+  int width, chunk;
+};
+MemberSchedule schedule_members(int num_gp, int num_candidates, size_t avail, size_t per, size_t width_cap = SIZE_MAX);
+// bytes of one member's slot: the largest member's chunk workspace, rounded up so that every slot starts aligned
+inline size_t slot_stride(size_t bytes) { return (bytes + 255) & ~size_t(255); }
 // Enqueues run(m, m % width) for m = 0 .. num_gp - 1 on member m's stream; member m waits for member m - width, whose
 // slot it reuses.  Returns once every member's stream has finished, also when run throws.
-void run_members(const cmoe_gp* const* gps, int num_gp, int width, EnsembleWork& ew,
+void run_members(const cmoe_gp* const* gps, int num_gp, int width, LargeUnionWork& w,
                  const std::function<void(int, int)>& run);
 // Reads back the members' device results dval [num_gp][nc], dgrad [num_gp][nc][ps] (or NULL) and dfail [num_gp][nc] on
-// `s`; throws CMOE_ERR_SINGULAR for the first failing member in member order, else sums the members in member order.
+// `s`; throws CMOE_ERR_SINGULAR for the first failing member in member order, else sums the members in member order
+// (add_member).
 void drain_members(cudaStream_t s, int num_gp, int nc, size_t ps, const double* dval, const double* dgrad,
                    const int* dfail, double* values, double* grads);
 // Out = A B for `batch` column-major problems (A m x kd, B kd x nn; batch z at A + z sa, B + z sb, Out + z so), 64 x 64
 // DMMA tiles.  Asynchronous on `s`.
 void gemm_nn(int m, int nn, int kd, const double* A, int lda, size_t sa, const double* B, int ldb, size_t sb,
              double* Out, int ldo, size_t so, int batch, cudaStream_t s);
+// out = in^T for `batch` column-major rows x cols matrices, stored back to back (out: cols x rows).  Asynchronous on `s`.
+void transpose_batched(int rows, int cols, const double* in, double* out, int batch, cudaStream_t s);
 // Reverse mode through nc Cholesky factors C (U x U, column-major, upper triangle zero): T1 holds Cbar on entry (the
 // adjoint of C, lower triangle) and 2 Sigmabar on exit, Sigmabar the adjoint of Sigma = C C^T (symmetric).  T2 is
 // scratch of the same size.  Asynchronous on `s`.

@@ -30,7 +30,7 @@ std::vector<KgDispatchEntry>& kg_table() {
 
 __device__ __forceinline__ int row_type(int local, const int* derivs) { return local ? derivs[local - 1] : -1; }
 
-// union sets on the device: P[c] = [candidate c ; points being sampled]
+// union sets on the device: P[c] = [candidate c ; points being sampled] (build_union_sets)
 __global__ void build_union_kernel(const double* __restrict__ cand, const double* __restrict__ Xp, int nc, int q, int p,
                                    int dim, double* __restrict__ P) {
   const size_t e = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -139,7 +139,8 @@ __global__ void __launch_bounds__(256) kg_pack_kernel(const __grid_constant__ Ke
 // batch.  fast: the MC kernel's shared-memory fast path (table exp, and all kernel values 0 beyond kFarRadius).
 constexpr int kStartThreads = 256;
 constexpr int kStartOuts = 5;  // outputs per thread: (1 + QP)(DIMP + 2) <= 33 x 34 = 1122 <= 5 x 256
-static_assert(kStartOuts * kStartThreads >= (1 + 32) * (CMOE_MAX_DIM + 2), "start table outputs per CTA (QP <= 32)");
+static_assert(kStartOuts * kStartThreads >= (1 + CMOE_MAX_KG_ROWS) * (CMOE_MAX_DIM + 2),
+              "start table outputs per CTA (QP <= CMOE_MAX_KG_ROWS)");
 __global__ void __launch_bounds__(kStartThreads) kg_start_kernel(const __grid_constant__ KernelSpec spec, int N, int U,
                                                                  int M, int DIMP, int QP, int fast,
                                                                  const double* __restrict__ Xt,
@@ -566,6 +567,80 @@ const KgLargeEntry* find_kg_large_entry(int kernel, int dim, int g) {
   return best;
 }
 
+void build_union_sets(const double* cand, const double* Xp, int nc, int q, int p, int dim, double* P, cudaStream_t s) {
+  const size_t tot = static_cast<size_t>(nc) * (q + p) * dim;
+  build_union_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256, 0, s>>>(cand, Xp, nc, q, p, dim, P);
+  count_launch();
+}
+
+void kg_check_inner(const KernelSpec& spec, int num_fidelity, const cmoe_gd_params* inner, const double* inner_bounds) {
+  CMOE_REQUIRE(num_fidelity >= 0 && num_fidelity < spec.dim, CMOE_ERR_BOUNDS, "num_fidelity out of range");
+  CMOE_REQUIRE(spec.g <= kMaxGWide, CMOE_ERR_BOUNDS, "at most 31 derivative observations per point in the q-KG kernel");
+  if (spec.g > kMaxG) {
+    // the wide kernel visits the derivative rows by coordinate (KgMcParams::drow)
+    for (int a = 0; a < spec.g; ++a)
+      for (int b = 0; b < a; ++b)
+        CMOE_REQUIRE(spec.derivs[a] != spec.derivs[b], CMOE_ERR_BOUNDS,
+                     "a partial derivative is observed twice per point (q-KG with more than 8 derivative observations)");
+  }
+  CMOE_REQUIRE(inner->max_num_steps <= 4096, CMOE_ERR_BOUNDS, "inner max_num_steps must be <= 4096");
+  for (int d = 0; d < spec.dim - num_fidelity; ++d)
+    CMOE_REQUIRE(inner_bounds[2 * d] <= inner_bounds[2 * d + 1], CMOE_ERR_BOUNDS, "Tensor product region is EMPTY.");
+}
+
+KgMcParams kg_inner_params(const cmoe_gp& gp, int ps, int M, int num_mc, const cmoe_gd_params& inner,
+                           const double* inner_bounds, const double* alpha0) {
+  const KernelSpec& spec = gp.spec;
+  const int dim = spec.dim;
+  KgMcParams m{};
+  m.ps = ps;
+  m.dim = dim;
+  m.M = M;
+  m.num_mc = num_mc;
+  m.g = spec.g;
+  for (int k = 0; k < CMOE_MAX_DIM; ++k) m.derivs[k] = (k < spec.g) ? spec.derivs[k] : 0;
+  for (int k = 0; k < spec.g; ++k) m.drow[spec.derivs[k]] = 1 + k;
+  m.max_steps = inner.max_num_steps;
+  m.max_restarts = inner.max_num_restarts;
+  m.mean = gp.mean;
+  m.mrc = inner.max_relative_change;
+  m.tol = inner.tolerance;
+  m.step_tol = inner.max_num_steps > 0 ? inner.tolerance / static_cast<double>(inner.max_num_steps) : 0.0;
+  m.alpha = spec.alpha;
+  m.alpha0 = alpha0;
+  for (int d = 0; d < CMOE_MAX_DIM; ++d) {
+    m.lo[d] = -1.0e300;
+    m.hi[d] = 1.0e300;
+    m.inv_len[d] = (d < dim) ? spec.inv_len[d] : 0.0;
+  }
+  for (int d = 0; d < ps; ++d) {  // the frame of A (kg_pack_kernel, kgl_pack_kernel)
+    m.lo[d] = inner_bounds[2 * d] - gp.centre[d];
+    m.hi[d] = inner_bounds[2 * d + 1] - gp.centre[d];
+  }
+  return m;
+}
+
+std::vector<double> kg_step_sizes(const cmoe_gd_params& inner) {
+  std::vector<double> a0(std::max(1, inner.max_num_steps));
+  for (int i = 0; i < inner.max_num_steps; ++i) a0[i] = gd_step_size(inner.pre_mult, inner.gamma, i);
+  return a0;
+}
+
+std::vector<double> kg_pinned_discrete(const double* discrete_pts, int num_pts, int ps, int dim) {
+  std::vector<double> hD(static_cast<size_t>(std::max(1, num_pts)) * dim, 1.0);
+  for (int j = 0; j < num_pts; ++j)
+    for (int d = 0; d < ps; ++d) hD[static_cast<size_t>(j) * dim + d] = discrete_pts[static_cast<size_t>(j) * ps + d];
+  return hD;
+}
+
+int kg_samples_per_item(long long candidates, int num_mc, int sms, int ctas_per_sm) {
+  const long long target_ctas = 8LL * sms * ctas_per_sm;
+  long long chunk = (candidates * num_mc + target_ctas - 1) / target_ctas;
+  chunk = std::max<long long>(2 * kMcThreads, std::min<long long>(chunk, 16 * kMcThreads));
+  chunk = (chunk + kMcThreads - 1) / kMcThreads * kMcThreads;
+  return static_cast<int>(std::min<long long>(chunk, (num_mc + kMcThreads - 1) / kMcThreads * kMcThreads));
+}
+
 void kg_value(int nb, int num_mc, const double* outVal, const double* best_post, const int* fail, double* kg,
               cudaStream_t s) {
   kg_value_kernel<<<nb, 256, 0, s>>>(num_mc, outVal, best_post, fail, kg);
@@ -659,12 +734,7 @@ void plan_run_batch(cmoe_kg_plan& pl, int c0, int nb, size_t ev_idx) {
   const Centre ctr = centre_of(gp);
   PosteriorBatch& pb = pl.pb;
   pb.configure(gp, nb, U, spec.derivs, spec.g, pl.want_grad ? q : 0, s);
-  {
-    const size_t tot = static_cast<size_t>(nb) * U * dim;
-    build_union_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256, 0, s>>>(
-        pl.dCand.p + static_cast<size_t>(c0) * q * dim, pl.dXp.p, nb, q, p, dim, pb.P.p);
-    count_launch();
-  }
+  build_union_sets(pl.dCand.p + static_cast<size_t>(c0) * q * dim, pl.dXp.p, nb, q, p, dim, pb.P.p, s);
   pb.run(gp, /*diag_mode=*/2, /*want_chol=*/true, pl.want_grad, s);
   CMOE_CUDA(cudaMemcpyAsync(pl.dFailAll.p + c0, pb.fail.p, nb * sizeof(int), cudaMemcpyDeviceToDevice, s));
 
@@ -779,17 +849,7 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     CMOE_REQUIRE(q >= 1 && p >= 0 && num_mc >= 1 && num_pts >= 0, CMOE_ERR_BOUNDS, "bad sizes");
     const KernelSpec& spec = gp->spec;
     const int dim = spec.dim;
-    CMOE_REQUIRE(num_fidelity >= 0 && num_fidelity < dim, CMOE_ERR_BOUNDS, "num_fidelity out of range");
-    CMOE_REQUIRE(spec.g <= kMaxGWide, CMOE_ERR_BOUNDS,
-                 "at most 31 derivative observations per point in the q-KG kernel");
-    if (spec.g > kMaxG) {
-      // the wide kernel visits the derivative rows by coordinate (KgMcParams::drow)
-      for (int a = 0; a < spec.g; ++a)
-        for (int b = 0; b < a; ++b)
-          CMOE_REQUIRE(spec.derivs[a] != spec.derivs[b], CMOE_ERR_BOUNDS,
-                       "a partial derivative is observed twice per point (q-KG with more than 8 derivative observations)");
-    }
-    CMOE_REQUIRE(inner->max_num_steps <= 4096, CMOE_ERR_BOUNDS, "inner max_num_steps must be <= 4096");
+    kg_check_inner(spec, num_fidelity, inner, inner_bounds);
     require_device(gp->device);
     std::unique_ptr<cmoe_kg_plan> pl(new cmoe_kg_plan());
     pl->gp = gp;
@@ -811,12 +871,11 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     pl->h_discrete.assign(discrete_pts, discrete_pts + static_cast<size_t>(num_pts) * pl->ps);
     if (p) pl->h_Xp.assign(points_being_sampled, points_being_sampled + static_cast<size_t>(p) * dim);
     const int U = pl->U, N = gp->N, n = gp->n, ps = pl->ps;
-    for (int d = 0; d < ps; ++d)
-      CMOE_REQUIRE(inner_bounds[2 * d] <= inner_bounds[2 * d + 1], CMOE_ERR_BOUNDS, "Tensor product region is EMPTY.");
     pl->Q = pl->U * (1 + spec.g);
     const KgDispatchEntry* entry = find_kg_entry(spec.kernel, dim, pl->Q, spec.g);
     CMOE_REQUIRE(entry != nullptr, CMOE_ERR_BOUNDS,
-                 "(q+p)*(1+num_derivatives) or dim exceeds the largest compiled q-KG kernel (32 rows, 32 dims)");
+                 "(q+p)*(1+num_derivatives) or dim exceeds the largest compiled q-KG kernel (" CMOE_STR(CMOE_MAX_KG_ROWS)
+                 " rows, 32 dims)");
     pl->select = entry->select;
     pl->DIMP = entry->dim;
     pl->QP = entry->qp;
@@ -828,9 +887,7 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     pl->dXt.alloc(static_cast<size_t>(N) * DIMP);
     const Centre ctr = centre_of(*gp);
     pack_xt_kernel<<<(N * DIMP + 255) / 256, 256, 0, s>>>(spec, ctr, gp->dX.p, N, DIMP, pl->dXt.p);
-    std::vector<double> hD(static_cast<size_t>(std::max(1, num_pts)) * dim, 1.0);
-    for (int j = 0; j < num_pts; ++j)
-      for (int d = 0; d < ps; ++d) hD[static_cast<size_t>(j) * dim + d] = discrete_pts[static_cast<size_t>(j) * ps + d];
+    const std::vector<double> hD = kg_pinned_discrete(discrete_pts, num_pts, ps, dim);
     pl->dD.upload(hD.data(), hD.size(), s);
     pl->dKD.alloc(static_cast<size_t>(n) * std::max(1, num_pts));
     pl->dMuD.alloc(std::max(1, num_pts));
@@ -839,9 +896,7 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
       mean_of_points_kernel<<<(num_pts + 127) / 128, 128, 0, s>>>(n, num_pts, gp->mean, pl->dKD.p, gp->dKinvY.p,
                                                                   pl->dMuD.p);
     }
-    std::vector<double> a0(std::max(1, inner->max_num_steps));
-    for (int i = 0; i < inner->max_num_steps; ++i)
-      a0[i] = gd_step_size(inner->pre_mult, inner->gamma, i);
+    const std::vector<double> a0 = kg_step_sizes(*inner);
     pl->dAlpha0.upload(a0.data(), a0.size(), s);
     std::vector<double> hXp(static_cast<size_t>(std::max(1, p)) * dim, 0.0);
     if (p) std::copy(points_being_sampled, points_being_sampled + static_cast<size_t>(p) * dim, hXp.begin());
@@ -850,9 +905,7 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     CMOE_CUDA(cudaStreamSynchronize(s));
 
     // work decomposition
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = sm_count();
     {
       // The shared-memory fast path evaluates exp without per-call range guards; that is valid while every scaled
       // coordinate vector it can meet lies within kFastPathRadius length scales of the origin of the kernels' frame,
@@ -880,15 +933,8 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
                             static_cast<size_t>(n) * Q * 4 * sizeof(double) +
                             (spec.g == 0 ? static_cast<size_t>(pl->M) * (1 + QP) * (DIMP + 2) * sizeof(double) : 0);
     pl->batch = static_cast<int>(chunk_items(max_candidates, size_t(3) << 30, per_cand, kMaxGridY));
-    // samples per CTA: aim for >= ~8 waves of CTAs over the whole batch, between 2 and 16 samples per lane.  A wave is
-    // the selected path's residency (kg_select; 2 CTAs per SM for the tile instantiation at the bench shape).
-    {
-      const long long target_ctas = 8LL * sms * pl->path.ctas_per_sm;
-      long long chunk = (static_cast<long long>(pl->batch) * num_mc + target_ctas - 1) / target_ctas;
-      chunk = std::max<long long>(2 * kMcThreads, std::min<long long>(chunk, 16 * kMcThreads));
-      chunk = (chunk + kMcThreads - 1) / kMcThreads * kMcThreads;
-      pl->chunk = static_cast<int>(std::min<long long>(chunk, (num_mc + kMcThreads - 1) / kMcThreads * kMcThreads));
-    }
+    // a wave is the selected path's residency (kg_select; 2 CTAs per SM for the tile instantiation at the bench shape)
+    pl->chunk = kg_samples_per_item(pl->batch, num_mc, sms, pl->path.ctas_per_sm);
     const int B = pl->batch;
     pl->dPk.alloc(static_cast<size_t>(B) * N * pl->stride);
     pl->dXu.alloc(static_cast<size_t>(B) * U * (DIMP + 2));
@@ -934,44 +980,18 @@ int cmoe_kg_plan_create(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_param
     }
 
     KgMcParams& m = pl->mcp;
+    m = kg_inner_params(*gp, ps, pl->M, num_mc, *inner, inner_bounds, pl->dAlpha0.p);
     m.N = N;
     m.U = U;
-    m.ps = ps;
-    m.dim = dim;
-    m.M = pl->M;
-    m.num_mc = num_mc;
     m.chunk = pl->chunk;
     m.use_smem = pl->path.use_smem ? 1 : 0;
-    m.g = spec.g;
     m.Q = Q;
     m.pk_stride = pl->stride;
     // general path: park the scaled training points + e_j behind the weight ring when they are small enough to leave room
     // for two CTAs per SM (2 x (90 KB ring + 20 KB) < 227 KB)
     m.stage_ops = (spec.g > 0 && static_cast<size_t>(N) * (DIMP + 2) * sizeof(double) <= 20 * 1024) ? 1 : 0;
     if (const char* e = std::getenv("CMOE_GEN_STAGE")) m.stage_ops = m.stage_ops && std::atoi(e) != 0;
-    for (int k = 0; k < CMOE_MAX_DIM; ++k) {
-      m.derivs[k] = (k < spec.g) ? spec.derivs[k] : 0;
-      m.drow[k] = 0;
-    }
-    for (int k = 0; k < spec.g; ++k) m.drow[spec.derivs[k]] = 1 + k;
-    m.max_steps = inner->max_num_steps;
-    m.max_restarts = inner->max_num_restarts;
-    m.mean = gp->mean;
-    m.mrc = inner->max_relative_change;
-    m.tol = inner->tolerance;
-    m.step_tol = inner->max_num_steps > 0 ? inner->tolerance / static_cast<double>(inner->max_num_steps) : 0.0;
-    m.alpha = spec.alpha;
     m.Xt = pl->dXt.p;
-    m.alpha0 = pl->dAlpha0.p;
-    for (int d = 0; d < CMOE_MAX_DIM; ++d) {
-      m.lo[d] = -1.0e300;
-      m.hi[d] = 1.0e300;
-      m.inv_len[d] = (d < dim) ? spec.inv_len[d] : 0.0;
-    }
-    for (int d = 0; d < ps; ++d) {  // the frame of A (kg_pack_kernel)
-      m.lo[d] = inner_bounds[2 * d] - gp->centre[d];
-      m.hi[d] = inner_bounds[2 * d + 1] - gp->centre[d];
-    }
     *plan_out = pl.release();
   });
 }
@@ -1053,11 +1073,7 @@ int cmoe_kg_plan_sync(cmoe_kg_plan* plan, int* info) {
     plan->dFailAll.download(f.data(), plan->nc, s);
     CMOE_CUDA(cudaStreamSynchronize(s));
     for (int c = 0; c < plan->nc; ++c)
-      if (f[c] != 0)
-        throw Error(CMOE_ERR_SINGULAR,
-                    "GP-Variance matrix singular. Check for duplicate points_to_sample/being_sampled or "
-                    "points_to_sample/being_sampled duplicating points_sampled with 0 noise.",
-                    f[c]);
+      if (f[c] != 0) throw_singular_union(f[c]);
   });
 }
 

@@ -160,16 +160,6 @@ __global__ void __launch_bounds__(256) kgl_disc_cov_kernel(const __grid_constant
   *w = cov_entry(spec, kp, pa, aj, rtype(a % bs, spec.derivs), -1) - *w;
 }
 
-// out = in^T for nb column-major rows x cols matrices (out: cols x rows)
-__global__ void __launch_bounds__(256) kgl_transpose_kernel(int rows, int cols, const double* __restrict__ in,
-                                                            double* __restrict__ out) {
-  const size_t off = static_cast<size_t>(blockIdx.y) * rows * cols;
-  const size_t o = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (o >= static_cast<size_t>(rows) * cols) return;
-  const size_t r = o % cols, cc = o / cols;  // out (r, cc) = in (cc, r)
-  out[off + o] = in[off + r * rows + cc];
-}
-
 // each sample's start: first strict arg-min over j of mu_A[j] + S[s][j], S = W^T Z [num_mc][M]
 __global__ void __launch_bounds__(256) kgl_argmin_kernel(int M, int num_mc, const double* __restrict__ muA,
                                                          const double* __restrict__ S, int* __restrict__ start) {
@@ -306,12 +296,6 @@ __global__ void __launch_bounds__(kGradThreads) kgl_grad_kernel(const __grid_con
 
 namespace {
 
-// Device workspace of cmoe_kg_eval_large, kept on the handle (cmoe_gp::kg_large_ws): one region, carved as
-// kg_large_carve_slot and kg_large_carve_io lay it out, grown to the largest call's need.
-struct KgLargeWork {
-  DevBuf<double> region;
-};
-
 // samples of one call: the sample axis of the scan product is grid.y of gemm_nn (64 samples per CTA row, <= 65535)
 constexpr long long kMaxKgLargeSamples = 65535LL * 64;
 
@@ -338,11 +322,6 @@ struct KgLargeShape {
 struct KgLargeInputs {
   const double *Z, *alpha0, *cand, *Xp, *stale;
 };
-
-KgLargeWork& kg_large_work(const cmoe_gp& gp) {
-  if (!gp.kg_large_ws) gp.kg_large_ws = std::make_shared<KgLargeWork>();
-  return *static_cast<KgLargeWork*>(gp.kg_large_ws.get());
-}
 
 // inner-optimiser scratch (kg_mc_large_kernel's per-lane weight columns), counted in the 2 GiB budget
 constexpr size_t kKgLargeScratchBytes = size_t(256) << 20;
@@ -452,18 +431,8 @@ KgLargeShape kg_large_shape(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_p
   CMOE_REQUIRE(static_cast<long long>(U) * bs <= CMOE_MAX_KG_LARGE_ROWS, CMOE_ERR_BOUNDS,
                "(q+p)*(1+num_derivatives) must be <= 1024");
   CMOE_REQUIRE(num_pts >= 0, CMOE_ERR_BOUNDS, "bad sizes");
-  CMOE_REQUIRE(num_fidelity >= 0 && num_fidelity < dim, CMOE_ERR_BOUNDS, "num_fidelity out of range");
-  CMOE_REQUIRE(g <= kMaxGWide, CMOE_ERR_BOUNDS, "at most 31 derivative observations per point in the q-KG kernel");
-  if (g > kMaxG) {
-    for (int a = 0; a < g; ++a)
-      for (int b = 0; b < a; ++b)
-        CMOE_REQUIRE(spec.derivs[a] != spec.derivs[b], CMOE_ERR_BOUNDS,
-                     "a partial derivative is observed twice per point (q-KG with more than 8 derivative observations)");
-  }
-  CMOE_REQUIRE(inner->max_num_steps <= 4096, CMOE_ERR_BOUNDS, "inner max_num_steps must be <= 4096");
+  kg_check_inner(spec, num_fidelity, inner, inner_bounds);
   const int ps = dim - num_fidelity;
-  for (int d = 0; d < ps; ++d)
-    CMOE_REQUIRE(inner_bounds[2 * d] <= inner_bounds[2 * d + 1], CMOE_ERR_BOUNDS, "Tensor product region is EMPTY.");
   const KgLargeEntry* entry = find_kg_large_entry(spec.kernel, dim, g);
   CMOE_REQUIRE(entry != nullptr, CMOE_ERR_BOUNDS, "dim exceeds the largest compiled q-KG kernel (32 dims)");
   KgLargeShape sh;
@@ -529,8 +498,7 @@ KgLargeInputs kg_large_setup(const KgLargeShape& sh, const cmoe_gd_params* inner
   kgl_normals_kernel<<<static_cast<unsigned>((mc * sh.Q + 255) / 256), 256, 0, s>>>(
       sh.Q, sh.num_mc, seed, normals_table ? dtable.p : nullptr, Z);
   count_launch();
-  std::vector<double> a0(std::max(1, inner->max_num_steps));
-  for (int i = 0; i < inner->max_num_steps; ++i) a0[i] = gd_step_size(inner->pre_mult, inner->gamma, i);
+  const std::vector<double> a0 = kg_step_sizes(*inner);
   CMOE_CUDA(cudaMemcpyAsync(alpha0, a0.data(), a0.size() * sizeof(double), cudaMemcpyHostToDevice, s));
   CMOE_CUDA(cudaMemcpyAsync(cand, candidates, static_cast<size_t>(num_candidates) * sh.q * sh.dim * sizeof(double),
                             cudaMemcpyHostToDevice, s));
@@ -555,7 +523,7 @@ KgLargeInputs kg_large_setup(const KgLargeShape& sh, const cmoe_gd_params* inner
 // arrays.  hD / hderivs hold the host data of the asynchronous uploads until the caller has synchronised `s`.
 void kg_large_run(const cmoe_gp& gp, const KgLargeShape& sh, const cmoe_gd_params* inner, const double* inner_bounds,
                   const KgLargeInputs& in, const KgLargeBufs& b, const double* discrete_pts, double best_so_far,
-                  int num_candidates, cudaStream_t s, double* kg_out, double* grad_out, int* fail_out,
+                  int num_candidates, int sms, cudaStream_t s, double* kg_out, double* grad_out, int* fail_out,
                   std::vector<double>& hD, std::vector<int>& hderivs) {
   const KernelSpec& spec = gp.spec;
   const int dim = sh.dim, g = sh.g, bs = sh.bs, U = sh.U, q = sh.q, ps = sh.ps, num_pts = sh.num_pts;
@@ -565,52 +533,18 @@ void kg_large_run(const cmoe_gp& gp, const KgLargeShape& sh, const cmoe_gd_param
   const size_t QQ = static_cast<size_t>(Q) * Q, mc = static_cast<size_t>(num_mc);
   const Centre ctr = centre_of(gp);
   // per GP: the discrete points (fidelity coordinates 1), K(X, D), the derivative indices
-  hD.assign(static_cast<size_t>(std::max(1, num_pts)) * dim, 1.0);
-  for (int j = 0; j < num_pts; ++j)
-    for (int d = 0; d < ps; ++d) hD[static_cast<size_t>(j) * dim + d] = discrete_pts[static_cast<size_t>(j) * ps + d];
+  hD = kg_pinned_discrete(discrete_pts, num_pts, ps, dim);
   CMOE_CUDA(cudaMemcpyAsync(b.D, hD.data(), hD.size() * sizeof(double), cudaMemcpyHostToDevice, s));
   if (num_pts > 0) build_mix_covariance(spec, gp.dX.p, N, b.D, num_pts, nullptr, 0, b.KD, s);
   hderivs.assign(std::max(1, g), 0);
   for (int a = 0; a < g; ++a) hderivs[a] = spec.derivs[a];
   CMOE_CUDA(cudaMemcpyAsync(b.dPs, hderivs.data(), hderivs.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   CMOE_CUDA(cudaMemsetAsync(b.stats, 0, 4 * sizeof(unsigned long long), s));
 
-  KgMcParams m{};
+  // the training then the union points as one row set with per-sample weight columns: no union block, no pack weights
+  KgMcParams m = kg_inner_params(gp, ps, M, num_mc, *inner, inner_bounds, in.alpha0);
   m.N = Np;
-  m.U = 0;
-  m.ps = ps;
-  m.dim = dim;
-  m.M = M;
-  m.num_mc = num_mc;
-  m.use_smem = 0;
-  m.g = g;
-  m.Q = 0;
   m.pk_stride = 2;
-  for (int a = 0; a < CMOE_MAX_DIM; ++a) {
-    m.derivs[a] = (a < g) ? spec.derivs[a] : 0;
-    m.drow[a] = 0;
-  }
-  for (int a = 0; a < g; ++a) m.drow[spec.derivs[a]] = 1 + a;
-  m.max_steps = inner->max_num_steps;
-  m.max_restarts = inner->max_num_restarts;
-  m.mean = gp.mean;
-  m.mrc = inner->max_relative_change;
-  m.tol = inner->tolerance;
-  m.step_tol = inner->max_num_steps > 0 ? inner->tolerance / static_cast<double>(inner->max_num_steps) : 0.0;
-  m.alpha = spec.alpha;
-  m.alpha0 = in.alpha0;
-  for (int d = 0; d < CMOE_MAX_DIM; ++d) {
-    m.lo[d] = -1.0e300;
-    m.hi[d] = 1.0e300;
-    m.inv_len[d] = (d < dim) ? spec.inv_len[d] : 0.0;
-  }
-  for (int d = 0; d < ps; ++d) {  // the frame of A
-    m.lo[d] = inner_bounds[2 * d] - gp.centre[d];
-    m.hi[d] = inner_bounds[2 * d + 1] - gp.centre[d];
-  }
   m.stats = b.stats;
   m.aw = b.aw;
   m.aw_slots = b.aw_slots;
@@ -641,9 +575,7 @@ void kg_large_run(const cmoe_gp& gp, const KgLargeShape& sh, const cmoe_gd_param
     // discretisation set: W = L_U^-1 Cov_n(Xu rows, A), mu_n(A); starts = first strict arg-min of mu_A + W^T z
     build_mix_covariance(spec, gp.dX.p, N, b.Afull, nb * U, nullptr, 0, b.KAu, s);
     // B^T K(X, A) on DMMA: B^T [Q][n] per candidate, then the union part and the shared discrete part of A
-    kgl_transpose_kernel<<<dim3(static_cast<unsigned>((static_cast<size_t>(n) * Q + 255) / 256), nb), 256, 0, s>>>(
-        n, Q, b.V, b.Bt);
-    count_launch();
+    transpose_batched(n, Q, b.V, b.Bt, nb, s);
     gemm_nn(Q, U, n, b.Bt, Q, static_cast<size_t>(Q) * n, b.KAu, n, static_cast<size_t>(n) * U, b.Wd, Q,
             static_cast<size_t>(Q) * M, nb, s);
     if (num_pts > 0)
@@ -655,9 +587,7 @@ void kg_large_run(const cmoe_gp& gp, const KgLargeShape& sh, const cmoe_gd_param
     count_launch();
     for (int c = 0; c < nb; ++c)
       trsm_lower_blocked(b.A + c * QQ, Q, b.Wd + static_cast<size_t>(c) * Q * M, Q, M, false, s);
-    kgl_transpose_kernel<<<dim3(static_cast<unsigned>((static_cast<size_t>(Q) * M + 255) / 256), nb), 256, 0, s>>>(
-        Q, M, b.Wd, b.WdT);
-    count_launch();
+    transpose_batched(Q, M, b.Wd, b.WdT, nb, s);
     gemm_nn(M, num_mc, Q, b.WdT, M, static_cast<size_t>(M) * Q, in.Z, Q, 0, b.S, M, mc * M, nb, s);
     kgl_argmin_kernel<<<dim3((num_mc + 255) / 256, nb), 256, 0, s>>>(M, num_mc, b.muA, b.S, b.start);
     count_launch();
@@ -673,14 +603,7 @@ void kg_large_run(const cmoe_gp& gp, const KgLargeShape& sh, const cmoe_gd_param
     count_launch();
     // inner optimisation of every sample
     KgMcParams prm = m;
-    {
-      // samples per work item: aim for >= ~8 waves of 3 CTAs per SM over the chunk, 2 to 16 samples per lane
-      const long long target = 8LL * sms * 3;
-      long long sc = (static_cast<long long>(nb) * num_mc + target - 1) / target;
-      sc = std::max<long long>(2 * kMcThreads, std::min<long long>(sc, 16 * kMcThreads));
-      sc = (sc + kMcThreads - 1) / kMcThreads * kMcThreads;
-      prm.chunk = static_cast<int>(std::min<long long>(sc, (num_mc + kMcThreads - 1) / kMcThreads * kMcThreads));
-    }
+    prm.chunk = kg_samples_per_item(nb, num_mc, sms, 3);  // the general path's 3 CTAs per SM
     prm.chunks = (num_mc + prm.chunk - 1) / prm.chunk;
     prm.work_total = prm.chunks * nb;
     prm.Xt = b.Xt;
@@ -703,8 +626,8 @@ void kg_large_run(const cmoe_gp& gp, const KgLargeShape& sh, const cmoe_gd_param
       // R = Kx C^T over the samples, [Q][R] (column a of length R = n + Q)
       kgl_kx_kernel<<<dim3(static_cast<unsigned>((mc * R + 255) / 256), nb), 256, 0, s>>>(
           spec, ctr, N, U, num_mc, DIMP, gp.dX.p, b.P, b.outX, b.Kx);
-      kgl_transpose_kernel<<<dim3(static_cast<unsigned>((mc * Q + 255) / 256), nb), 256, 0, s>>>(Q, num_mc, b.C, b.Ct);
-      count_launch(2);
+      count_launch();
+      transpose_batched(Q, num_mc, b.C, b.Ct, nb, s);
       gemm_nn(R, Q, num_mc, b.Kx, R, mc * R, b.Ct, num_mc, mc * Q, b.Rm, R, static_cast<size_t>(R) * Q, nb, s);
       kg_tprime(nb, n, Q, Q, b.Rm, b.V, b.Tp, s);
       potrs_lower(gp.dK.p, n, b.Rm, R, nb * Q, s);
@@ -727,127 +650,76 @@ void kg_large_run(const cmoe_gp& gp, const KgLargeShape& sh, const cmoe_gd_param
 
 }  // namespace
 
-void kg_large_eval(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_params* inner, const double* inner_bounds,
-                   const double* discrete_pts, int num_pts, const double* candidates, int num_candidates, int q,
-                   const double* points_being_sampled, int p, int num_mc, double best_so_far, uint64_t seed,
-                   const double* normals_table, const double* stale_union, double* kg, double* grad_kg,
-                   cmoe_kg_stats* stats) {
-  const KgLargeShape sh = kg_large_shape(gp, num_fidelity, inner, inner_bounds, num_pts, num_candidates, q, p, num_mc,
-                                         grad_kg != nullptr);
-  require_device(gp->device);
-  cudaStream_t s = gp->stream;
-  const int dim = sh.dim, chunk = static_cast<int>(chunk_items(num_candidates, sh.budget, sh.per_bytes, kMaxChunkSets));
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  // per call: the draws, the step sizes, the candidates, the pending and the stale points
-  DevBuf<double> in_buf(kg_large_setup_doubles(sh, inner, num_candidates));
-  const KgLargeInputs in = kg_large_setup(sh, inner, candidates, num_candidates, points_being_sampled, seed,
-                                          normals_table, stale_union, in_buf.p, s);
-  // the handle's region: the slot (chunk workspace and scratch), then the GP's inputs and counters
-  const int aw_slots = kg_large_aw_slots(sh, kKgLargeScratchBytes, sms);
-  KgLargeBufs b;
-  Carve cv;
-  kg_large_carve_slot(sh, chunk, aw_slots, cv, b);
-  kg_large_carve_io(sh, cv, b);
-  KgLargeWork& k = kg_large_work(*gp);
-  k.region.ensure((cv.off + sizeof(double) - 1) / sizeof(double));
-  cv = Carve{reinterpret_cast<char*>(k.region.p)};
-  kg_large_carve_slot(sh, chunk, aw_slots, cv, b);
-  kg_large_carve_io(sh, cv, b);
-  // the call's results, read back once
-  DevBuf<double> dkg(num_candidates), dgrad(sh.want_grad ? static_cast<size_t>(num_candidates) * q * dim : 0);
-  DevBuf<int> dfail(num_candidates);
-  std::vector<double> hD;
-  std::vector<int> hderivs;
-  kg_large_run(*gp, sh, inner, inner_bounds, in, b, discrete_pts, best_so_far, num_candidates, s, dkg.p, dgrad.p,
-               dfail.p, hD, hderivs);
-  std::vector<int> hfail(num_candidates);
-  unsigned long long st[4] = {0, 0, 0, 0};
-  dfail.download(hfail.data(), num_candidates, s);
-  dkg.download(kg, num_candidates, s);
-  if (sh.want_grad) dgrad.download(grad_kg, static_cast<size_t>(num_candidates) * q * dim, s);
-  CMOE_CUDA(cudaMemcpyAsync(st, b.stats, sizeof(st), cudaMemcpyDeviceToHost, s));
-  CMOE_CUDA(cudaStreamSynchronize(s));
-  for (int c = 0; c < num_candidates; ++c)
-    if (hfail[c] != 0) throw_singular_union(hfail[c]);
-  if (stats) {
-    stats->mc_samples = static_cast<uint64_t>(num_candidates) * num_mc;
-    stats->posterior_evals = st[0];
-    stats->line_search_steps = st[1];
-    stats->point_evals = st[2];
-    stats->line_batches = st[3];
-  }
-}
-
-void kg_large_ensemble_eval(const cmoe_gp* const* gps, int num_gp, int num_fidelity, const cmoe_gd_params* inner,
-                            const double* inner_bounds, const double* discrete_pts, int num_pts,
-                            const double* candidates, int num_candidates, int q, const double* points_being_sampled,
-                            int p, int num_mc, const double* best_so_far, uint64_t seed, const double* normals_table,
-                            double* values, double* grads) {
+void kg_large_eval(const cmoe_gp* const* gps, int num_gp, int num_fidelity, const cmoe_gd_params* inner,
+                   const double* inner_bounds, const double* discrete_pts, int num_pts, const double* candidates,
+                   int num_candidates, int q, const double* points_being_sampled, int p, int num_mc,
+                   const double* best_so_far, uint64_t seed, const double* normals_table, const double* stale_union,
+                   double* values, double* grads, cmoe_kg_stats* stats) {
   const bool want_grad = grads != nullptr;
   std::vector<KgLargeShape> sh;
-  size_t per = 0;
+  size_t per = 0, slot_max = 0;
   for (int m = 0; m < num_gp; ++m) {
     sh.push_back(kg_large_shape(gps[m], num_fidelity, inner, inner_bounds, num_pts, num_candidates, q, p, num_mc,
                                 want_grad));
     per = std::max(per, sh.back().per_bytes);
+    slot_max = std::max(slot_max, static_cast<size_t>(sh.back().R) * kMcThreads * sizeof(double));
   }
   require_device(gps[0]->device);
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  // W members in flight: each gets 1/W of the chunks' budget and of the scratch, W as large as one candidate of every
-  // member (and one scratch column set) still fits.  A slot then takes at most (budget + kCarveSlack) / W + scratch,
-  // so Z and the W slots stay within 2 GiB.
+  const int sms = sm_count();
+  // Each member in flight gets an even share of the chunks' budget and of the inner optimiser's scratch, so the members
+  // in flight are also bounded by one scratch column set each.  A slot then takes at most (budget + kCarveSlack) / width
+  // + scratch, so Z and the slots stay within 2 GiB.
   const KgLargeShape& s0 = sh[0];
-  size_t slot_max = 0;
-  for (const KgLargeShape& x : sh) slot_max = std::max(slot_max, static_cast<size_t>(x.R) * kMcThreads * sizeof(double));
-  size_t width = std::min<size_t>({static_cast<size_t>(num_gp), (s0.budget + kCarveSlack) / (per + kCarveSlack),
-                                   kKgLargeScratchBytes / slot_max});
-  if (ensemble_members_in_flight() > 0) width = std::min<size_t>(width, ensemble_members_in_flight());
-  width = std::max<size_t>(1, width);
-  const int W = static_cast<int>(width);
-  const size_t scratch = kKgLargeScratchBytes / width;
-  const size_t chunk_budget = (s0.budget + kCarveSlack) / width - kCarveSlack;
-  const int chunk = static_cast<int>(chunk_items(num_candidates, chunk_budget, per, kMaxChunkSets));
+  const MemberSchedule ms =
+      schedule_members(num_gp, num_candidates, s0.budget + kCarveSlack, per, kKgLargeScratchBytes / slot_max);
+  const size_t scratch = kKgLargeScratchBytes / ms.width;
   size_t slot_bytes = 0;
   for (const KgLargeShape& x : sh)
-    slot_bytes = std::max(slot_bytes, kg_large_slot_bytes(x, chunk, kg_large_aw_slots(x, scratch, sms)));
-  slot_bytes = (slot_bytes + 255) & ~size_t(255);
+    slot_bytes = std::max(slot_bytes, kg_large_slot_bytes(x, ms.chunk, kg_large_aw_slots(x, scratch, sms)));
+  slot_bytes = slot_stride(slot_bytes);
   // one region on the first member's handle: the evaluation's inputs (Z first), every member's results, inputs and
-  // counters, then the W slots
+  // counters, then the slots
   const size_t ps = static_cast<size_t>(q) * s0.dim, nc = num_candidates;
   std::vector<KgLargeBufs> io(num_gp);
   double *in_dev = nullptr, *dval = nullptr, *dgrad = nullptr;
   int* dfail = nullptr;
   char* slots = nullptr;
-  auto layout = [&](Carve& cv) {
+  LargeUnionWork& w = carve_large_union_work(*gps[0], [&](Carve& cv) {
     in_dev = cv.take<double>(kg_large_setup_doubles(s0, inner, num_candidates));
     dval = cv.take<double>(static_cast<size_t>(num_gp) * nc);
     dgrad = want_grad ? cv.take<double>(static_cast<size_t>(num_gp) * nc * ps) : nullptr;
     dfail = cv.take<int>(static_cast<size_t>(num_gp) * nc);
     for (int m = 0; m < num_gp; ++m) kg_large_carve_io(sh[m], cv, io[m]);
-    slots = cv.take<char>(slot_bytes * width);
-  };
-  Carve cv;
-  layout(cv);
-  EnsembleWork& ew = ensemble_work(*gps[0], cv.off);
-  cv = Carve{reinterpret_cast<char*>(ew.arena.p)};
-  layout(cv);
+    slots = cv.take<char>(slot_bytes * ms.width);
+  });
+  cudaStream_t st0 = gps[0]->stream;
   const KgLargeInputs in = kg_large_setup(s0, inner, candidates, num_candidates, points_being_sampled, seed,
-                                          normals_table, nullptr, in_dev, gps[0]->stream);
+                                          normals_table, stale_union, in_dev, st0);
   std::vector<std::vector<double>> hD(num_gp);
   std::vector<std::vector<int>> hderivs(num_gp);
-  run_members(gps, num_gp, W, ew, [&](int m, int slot) {
+  run_members(gps, num_gp, ms.width, w, [&](int m, int slot) {
     KgLargeBufs b = io[m];
     Carve sc{slots + slot * slot_bytes};
-    kg_large_carve_slot(sh[m], chunk, kg_large_aw_slots(sh[m], scratch, sms), sc, b);
+    kg_large_carve_slot(sh[m], ms.chunk, kg_large_aw_slots(sh[m], scratch, sms), sc, b);
     kg_large_run(*gps[m], sh[m], inner, inner_bounds, in, b, discrete_pts + static_cast<size_t>(m) * num_pts * s0.ps,
-                 best_so_far[m], num_candidates, gps[m]->stream, dval + m * nc, want_grad ? dgrad + m * nc * ps : nullptr,
-                 dfail + m * nc, hD[m], hderivs[m]);
+                 best_so_far[m], num_candidates, sms, gps[m]->stream, dval + m * nc,
+                 want_grad ? dgrad + m * nc * ps : nullptr, dfail + m * nc, hD[m], hderivs[m]);
   });
-  drain_members(gps[0]->stream, num_gp, num_candidates, ps, dval, dgrad, dfail, values, grads);
+  std::vector<unsigned long long> st(stats ? 4 * static_cast<size_t>(num_gp) : 0);
+  for (int m = 0; m < static_cast<int>(st.size() / 4); ++m)
+    CMOE_CUDA(cudaMemcpyAsync(st.data() + 4 * m, io[m].stats, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                              st0));
+  drain_members(st0, num_gp, num_candidates, ps, dval, dgrad, dfail, values, grads);  // synchronises st0
+  if (stats) {
+    *stats = cmoe_kg_stats{};
+    stats->mc_samples = static_cast<uint64_t>(num_gp) * num_candidates * num_mc;
+    for (int m = 0; m < num_gp; ++m) {
+      stats->posterior_evals += st[4 * m];
+      stats->line_search_steps += st[4 * m + 1];
+      stats->point_evals += st[4 * m + 2];
+      stats->line_batches += st[4 * m + 3];
+    }
+  }
 }
 
 }  // namespace cmoe
@@ -861,7 +733,7 @@ extern "C" int cmoe_kg_eval_large(const cmoe_gp* gp, int num_fidelity, const cmo
                                   uint64_t seed, const double* normals_table, double* kg, double* grad_kg,
                                   cmoe_kg_stats* stats, int* info) {
   return guarded(info, [&] {
-    kg_large_eval(gp, num_fidelity, inner, inner_bounds, discrete_pts, num_pts, candidates, num_candidates, q,
-                  points_being_sampled, p, num_mc, best_so_far, seed, normals_table, nullptr, kg, grad_kg, stats);
+    kg_large_eval(&gp, 1, num_fidelity, inner, inner_bounds, discrete_pts, num_pts, candidates, num_candidates, q,
+                  points_being_sampled, p, num_mc, &best_so_far, seed, normals_table, nullptr, kg, grad_kg, stats);
   });
 }

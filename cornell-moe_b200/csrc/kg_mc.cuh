@@ -2302,6 +2302,24 @@ const KgLargeEntry* find_kg_large_entry(int kernel, int dim, int g);
 #define CMOE_KG_LARGE_WIDE_ENTRIES_FOR_DIM(D) \
   KgLargeEntry{0, D, true, &launch_kg_mc_large<0, D, true>}, KgLargeEntry{1, D, true, &launch_kg_mc_large<1, D, true>}
 
+// The q-KG set-up that cmoe_kg_plan_create (kg.cu) and the large-union stages (kg_large.cu) share.
+// The inner optimiser's argument checks, in this order: the num_fidelity range, g <= 31, distinct partials past 8,
+// inner steps <= 4096, a non-empty inner box.  Throws CMOE_ERR_BOUNDS.
+void kg_check_inner(const KernelSpec& spec, int num_fidelity, const cmoe_gd_params* inner, const double* inner_bounds);
+// The inner optimiser's KgMcParams fields that follow from the GP, `inner` and the inner bounds (in the frame of A), for
+// ps free coordinates, M discretisation points and num_mc samples; alpha0 = the device step sizes (kg_step_sizes).
+// Every other field is zero: the caller sets the row sets (N, U, Q, pk_stride), use_smem, stage_ops, the chunk and the
+// buffers.
+KgMcParams kg_inner_params(const cmoe_gp& gp, int ps, int M, int num_mc, const cmoe_gd_params& inner,
+                           const double* inner_bounds, const double* alpha0);
+// pre_mult (i + 1)^-gamma for the inner steps i (at least one entry)
+std::vector<double> kg_step_sizes(const cmoe_gd_params& inner);
+// discrete_pts [num_pts][ps] -> [max(1, num_pts)][dim] with the fidelity coordinates pinned to 1 (...cpp:259-261, 365)
+std::vector<double> kg_pinned_discrete(const double* discrete_pts, int num_pts, int ps, int dim);
+// samples per work item of the MC kernel: aim for >= ~8 waves of ctas_per_sm CTAs per SM over `candidates`, between 2
+// and 16 samples per lane
+int kg_samples_per_item(long long candidates, int num_mc, int sms, int ctas_per_sm);
+
 // kg.cu's per-candidate stages that the large-union path shares (asynchronous on s)
 // KG[c] = best_posterior[c] + mean of outVal[c][:], NaN where fail[c] != 0 (kg_value_kernel)
 void kg_value(int nb, int num_mc, const double* outVal, const double* best_post, const int* fail, double* kg,

@@ -190,22 +190,27 @@ void multistart_common(const BatchEval& eval, const cmoe_gd_params& outer, const
   if (found_flag) *found_flag = found;
 }
 
-// The q-KG evaluator of the drivers: two plans (values, gradients) for unions of up to 32 rows, (q + p)(1 + g), and
-// cmoe_kg_eval_large's stages (kg_large_eval) past them, with the same normals table and stale union.
+// The q-KG evaluation of the drivers for an ensemble of num_gp >= 1 GPs (a single GP is the one-member ensemble): the
+// members' values and gradients summed in member order.  Up to CMOE_MAX_KG_ROWS union rows, (q + p)(1 + g), each member
+// has two plans (values, gradients); every member's plan is enqueued on its own stream before the first is drained.
+// Past them one kg_large_eval call runs every member on the large-union stages, with the evaluation's arguments kept
+// here.  Both paths use the same normals table and stale union.
 struct KgEvaluator {
-  cmoe_kg_plan* vplan = nullptr;
-  cmoe_kg_plan* gplan = nullptr;
+  std::vector<std::pair<cmoe_kg_plan*, cmoe_kg_plan*>> plans;  // (values, gradients) per member
+  size_t ps = 0;
+  std::vector<double> tv, tg;
   // large path: the evaluation's arguments (host copies)
   bool large = false;
-  const cmoe_gp* gp = nullptr;
+  std::vector<const cmoe_gp*> gps;
   int nf = 0, num_pts = 0, q = 0, p = 0, num_mc = 0;
-  double best_so_far = 0.0;
   uint64_t seed = 0;
   cmoe_gd_params inner{};
-  std::vector<double> inner_bounds, discrete, Xp, stale, table;
+  std::vector<double> inner_bounds, discrete, Xp, best, stale, table;
   ~KgEvaluator() {
-    cmoe_kg_plan_destroy(vplan);
-    cmoe_kg_plan_destroy(gplan);
+    for (auto& pp : plans) {
+      cmoe_kg_plan_destroy(pp.first);
+      cmoe_kg_plan_destroy(pp.second);
+    }
   }
   static void check(int rc, int info = 0) {
     if (rc != CMOE_OK) throw Error(rc, cmoe_last_error(), info);
@@ -213,61 +218,78 @@ struct KgEvaluator {
   // replays `t` (NormalRNGSimulator semantics) in every evaluation
   void set_table(const double* t, size_t len) {
     if (!large) {
-      check(cmoe_kg_plan_set_table(vplan, t, static_cast<int>(len)));
-      check(cmoe_kg_plan_set_table(gplan, t, static_cast<int>(len)));
+      for (auto& pp : plans) {
+        check(cmoe_kg_plan_set_table(pp.first, t, static_cast<int>(len)));
+        check(cmoe_kg_plan_set_table(pp.second, t, static_cast<int>(len)));
+      }
       return;
     }
-    const size_t need = static_cast<size_t>((num_mc + 1) / 2) * (q + p) * (1 + gp->spec.g);
+    const size_t need = static_cast<size_t>((num_mc + 1) / 2) * (q + p) * (1 + gps[0]->spec.g);
     CMOE_REQUIRE(len >= need, CMOE_ERR_INVALID_VALUE, "All random numbers stored in the RNG have been used up!");
     table.assign(t, t + need);
   }
   void operator()(const double* pts, int nc, double* values, double* grads) {
     if (large) {
-      require_device(gp->device);  // may run on a worker thread of the multi-device driver
-      kg_large_eval(gp, nf, &inner, inner_bounds.data(), discrete.data(), num_pts, pts, nc, q, Xp.data(), p, num_mc,
-                    best_so_far, seed, table.empty() ? nullptr : table.data(), stale.empty() ? nullptr : stale.data(),
-                    values, grads, nullptr);
+      require_device(gps[0]->device);  // may run on a worker thread of the multi-device driver
+      kg_large_eval(gps.data(), static_cast<int>(gps.size()), nf, &inner, inner_bounds.data(), discrete.data(),
+                    num_pts, pts, nc, q, Xp.data(), p, num_mc, best.data(), seed,
+                    table.empty() ? nullptr : table.data(), stale.empty() ? nullptr : stale.data(), values, grads,
+                    nullptr);
       return;
     }
-    cmoe_kg_plan* pl = grads ? gplan : vplan;
-    int info = 0;
-    check(cmoe_kg_plan_upload(pl, pts, nc));
-    check(cmoe_kg_plan_run(pl));
-    check(cmoe_kg_plan_sync(pl, &info), info);
-    check(cmoe_kg_plan_download(pl, values, grads, nullptr));
+    for (auto& pp : plans) {
+      cmoe_kg_plan* pl = grads ? pp.second : pp.first;
+      check(cmoe_kg_plan_upload(pl, pts, nc));
+      check(cmoe_kg_plan_run(pl));
+    }
+    tv.resize(nc);
+    if (grads) tg.resize(nc * ps);
+    for (size_t m = 0; m < plans.size(); ++m) {
+      cmoe_kg_plan* pl = grads ? plans[m].second : plans[m].first;
+      int info = 0;
+      check(cmoe_kg_plan_sync(pl, &info), info);
+      check(cmoe_kg_plan_download(pl, tv.data(), grads ? tg.data() : nullptr, nullptr));
+      add_member(static_cast<int>(m), nc, ps, tv.data(), grads ? tg.data() : nullptr, values, grads);
+    }
   }
 };
 
-void make_kg_evaluator(KgEvaluator& ev, const cmoe_gp* gp, int nf, const cmoe_gd_params* inner,
+void make_kg_evaluator(KgEvaluator& ev, const cmoe_gp* const* gps, int num_gp, int nf, const cmoe_gd_params* inner,
                        const double* inner_bounds, const double* discrete_pts, int num_pts, int max_value_cands,
-                       int max_grad_cands, int q, const double* Xp, int p, int num_mc, double best_so_far,
+                       int max_grad_cands, int q, const double* Xp, int p, int num_mc, const double* best_so_far,
                        uint64_t seed, const double* stale_union = nullptr) {
-  if (static_cast<long long>(q + p) * (1 + gp->spec.g) > 32) {
-    const int dim = gp->spec.dim, ps = dim - nf;
+  const int dim = gps[0]->spec.dim, ps = dim - nf;
+  ev.ps = static_cast<size_t>(q) * dim;
+  if (kg_union_is_large(q, p, gps[0]->spec.g)) {
     CMOE_REQUIRE(nf >= 0 && ps >= 1 && num_pts >= 0, CMOE_ERR_BOUNDS, "num_fidelity out of range");
     ev.large = true;
-    ev.gp = gp;
+    ev.gps.assign(gps, gps + num_gp);
     ev.nf = nf;
     ev.num_pts = num_pts;
     ev.q = q;
     ev.p = p;
     ev.num_mc = num_mc;
-    ev.best_so_far = best_so_far;
     ev.seed = seed;
     ev.inner = *inner;
     ev.inner_bounds.assign(inner_bounds, inner_bounds + 2 * static_cast<size_t>(ps));
-    ev.discrete.assign(discrete_pts, discrete_pts + static_cast<size_t>(num_pts) * ps);
+    ev.discrete.assign(discrete_pts, discrete_pts + static_cast<size_t>(num_gp) * num_pts * ps);
     if (p) ev.Xp.assign(Xp, Xp + static_cast<size_t>(p) * dim);
+    ev.best.assign(best_so_far, best_so_far + num_gp);
     if (stale_union) ev.stale.assign(stale_union, stale_union + static_cast<size_t>(q) * dim);
     return;
   }
-  KgEvaluator::check(cmoe_kg_plan_create(gp, nf, inner, inner_bounds, discrete_pts, num_pts, max_value_cands, q, Xp, p,
-                                         num_mc, best_so_far, seed, 0, &ev.vplan));
-  KgEvaluator::check(cmoe_kg_plan_create(gp, nf, inner, inner_bounds, discrete_pts, num_pts, max_grad_cands, q, Xp, p,
-                                         num_mc, best_so_far, seed, 1, &ev.gplan));
-  if (stale_union) {
-    KgEvaluator::check(cmoe_kg_plan_set_stale_union(ev.vplan, stale_union));
-    KgEvaluator::check(cmoe_kg_plan_set_stale_union(ev.gplan, stale_union));
+  for (int m = 0; m < num_gp; ++m) {
+    ev.plans.emplace_back(nullptr, nullptr);
+    auto& pp = ev.plans.back();
+    const double* disc = discrete_pts + static_cast<size_t>(m) * num_pts * ps;
+    KgEvaluator::check(cmoe_kg_plan_create(gps[m], nf, inner, inner_bounds, disc, num_pts, max_value_cands, q, Xp, p,
+                                           num_mc, best_so_far[m], seed, 0, &pp.first));
+    KgEvaluator::check(cmoe_kg_plan_create(gps[m], nf, inner, inner_bounds, disc, num_pts, max_grad_cands, q, Xp, p,
+                                           num_mc, best_so_far[m], seed, 1, &pp.second));
+    if (stale_union) {
+      KgEvaluator::check(cmoe_kg_plan_set_stale_union(pp.first, stale_union));
+      KgEvaluator::check(cmoe_kg_plan_set_stale_union(pp.second, stale_union));
+    }
   }
 }
 
@@ -312,22 +334,6 @@ void analytic_ei(const cmoe_gp* gp, const double* pts, int nc, double best_so_fa
       }
     }
   }
-}
-
-BatchEval make_ei_eval(const cmoe_gp* gp, int q, const double* Xp, int p, int num_mc, double best_so_far,
-                       uint64_t seed, const double* dtable = nullptr) {
-  if (q == 1 && p == 0) {
-    // special analytic case (gpp_math.hpp:1703-1749)
-    return [=](const double* pts, int nc, double* values, double* grads) {
-      analytic_ei(gp, pts, nc, best_so_far, values, grads);
-    };
-  }
-  // union sets past the per-set kernels' 96 rows take the tiled path of ei_large.cu
-  const auto batch = q + p <= kMaxQ ? ei_eval_batch : ei_large_eval_batch;
-  return [=](const double* pts, int nc, double* values, double* grads) {
-    require_device(gp->device);  // may run on a worker thread of the multi-device driver
-    batch(*gp, pts, nc, q, Xp, p, num_mc, best_so_far, seed, dtable, values, grads);
-  };
 }
 
 // ---- the parallel axis inside the call: starts strided over several GPUs ---------------------------------------------
@@ -450,51 +456,6 @@ void apply_fidelity_cost(const double* pts, int nc, int q, int dim, int nf, int 
   }
 }
 
-// Past 32 union rows the members run cmoe_kg_eval_large's stages (kg_large_ensemble_eval) with the evaluation's
-// arguments kept here; up to 32 rows each member has its two plans.
-struct KgEnsembleEvaluator {
-  std::vector<std::unique_ptr<KgEvaluator>> evs;
-  int q = 0, dim = 0, nf = 0;
-  std::vector<double> tv, tg;
-  // large path
-  bool large = false;
-  std::vector<const cmoe_gp*> gps;
-  int num_pts = 0, p = 0, num_mc = 0;
-  uint64_t seed = 0;
-  cmoe_gd_params inner{};
-  std::vector<double> inner_bounds, discrete, Xp, best;
-  void operator()(const double* pts, int nc, double* values, double* grads) {
-    const size_t ps = static_cast<size_t>(q) * dim;
-    if (large) {
-      kg_large_ensemble_eval(gps.data(), static_cast<int>(gps.size()), nf, &inner, inner_bounds.data(),
-                             discrete.data(), num_pts, pts, nc, q, Xp.data(), p, num_mc, best.data(), seed, nullptr,
-                             values, grads);
-      apply_fidelity_cost(pts, nc, q, dim, nf, static_cast<int>(gps.size()), values, grads);
-      return;
-    }
-    // phase 1: enqueue every member on its own stream; phase 2: drain in member order (fixed summation order)
-    for (auto& ev : evs) {
-      cmoe_kg_plan* pl = grads ? ev->gplan : ev->vplan;
-      KgEvaluator::check(cmoe_kg_plan_upload(pl, pts, nc));
-      KgEvaluator::check(cmoe_kg_plan_run(pl));
-    }
-    std::fill(values, values + nc, 0.0);
-    if (grads) std::fill(grads, grads + nc * ps, 0.0);
-    tv.resize(nc);
-    if (grads) tg.resize(nc * ps);
-    for (auto& ev : evs) {
-      cmoe_kg_plan* pl = grads ? ev->gplan : ev->vplan;
-      int info = 0;
-      KgEvaluator::check(cmoe_kg_plan_sync(pl, &info), info);
-      KgEvaluator::check(cmoe_kg_plan_download(pl, tv.data(), grads ? tg.data() : nullptr, nullptr));
-      for (int c = 0; c < nc; ++c) values[c] += tv[c];
-      if (grads)
-        for (size_t k = 0; k < nc * ps; ++k) grads[k] += tg[k];
-    }
-    apply_fidelity_cost(pts, nc, q, dim, nf, static_cast<int>(evs.size()), values, grads);
-  }
-};
-
 }  // namespace
 
 void cmoe::check_ensemble(const cmoe_gp* const* gps, int num_gp) {
@@ -507,18 +468,28 @@ void cmoe::check_ensemble(const cmoe_gp* const* gps, int num_gp) {
   }
 }
 
-cmoe::EnsembleWork::~EnsembleWork() {
+cmoe::LargeUnionWork::~LargeUnionWork() {
   for (cudaEvent_t e : done) cudaEventDestroy(e);
 }
 
-cmoe::EnsembleWork& cmoe::ensemble_work(const cmoe_gp& gp, size_t bytes) {
-  if (!gp.ensemble_ws) gp.ensemble_ws = std::make_shared<EnsembleWork>();
-  EnsembleWork& ew = *static_cast<EnsembleWork*>(gp.ensemble_ws.get());
-  ew.arena.ensure((bytes + sizeof(double) - 1) / sizeof(double));
-  return ew;
+cmoe::LargeUnionWork& cmoe::large_union_work(const cmoe_gp& gp, size_t bytes) {
+  if (!gp.large_union_ws) gp.large_union_ws = std::make_shared<LargeUnionWork>();
+  LargeUnionWork& w = *static_cast<LargeUnionWork*>(gp.large_union_ws.get());
+  w.arena.ensure((bytes + sizeof(double) - 1) / sizeof(double));
+  return w;
 }
 
-void cmoe::run_members(const cmoe_gp* const* gps, int num_gp, int width, EnsembleWork& ew,
+cmoe::MemberSchedule cmoe::schedule_members(int num_gp, int num_candidates, size_t avail, size_t per,
+                                            size_t width_cap) {
+  size_t width = std::min<size_t>({static_cast<size_t>(num_gp), avail / (per + kCarveSlack), width_cap});
+  if (ensemble_members_in_flight() > 0) width = std::min<size_t>(width, ensemble_members_in_flight());
+  width = std::max<size_t>(1, width);
+  const size_t share = avail / width;
+  const size_t chunk = chunk_items(num_candidates, share > kCarveSlack ? share - kCarveSlack : 0, per, kMaxChunkSets);
+  return {static_cast<int>(width), static_cast<int>(chunk)};
+}
+
+void cmoe::run_members(const cmoe_gp* const* gps, int num_gp, int width, LargeUnionWork& ew,
                        const std::function<void(int, int)>& run) {
   while (ew.done.size() < static_cast<size_t>(num_gp)) {
     cudaEvent_t e;
@@ -551,6 +522,17 @@ void cmoe::throw_singular_union(int minor) {
               minor);
 }
 
+void cmoe::add_member(int m, int nc, size_t ps, const double* v, const double* g, double* values, double* grads) {
+  if (m == 0) {
+    std::copy(v, v + nc, values);
+    if (grads) std::copy(g, g + nc * ps, grads);
+    return;
+  }
+  for (int c = 0; c < nc; ++c) values[c] += v[c];
+  if (grads)
+    for (size_t k = 0; k < nc * ps; ++k) grads[k] += g[k];
+}
+
 void cmoe::drain_members(cudaStream_t s, int num_gp, int nc, size_t ps, const double* dval, const double* dgrad,
                          const int* dfail, double* values, double* grads) {
   const size_t all = static_cast<size_t>(num_gp) * nc;
@@ -562,87 +544,67 @@ void cmoe::drain_members(cudaStream_t s, int num_gp, int nc, size_t ps, const do
   CMOE_CUDA(cudaStreamSynchronize(s));
   for (size_t e = 0; e < all; ++e)
     if (f[e] != 0) throw_singular_union(f[e]);
-  std::fill(values, values + nc, 0.0);
-  if (grads) std::fill(grads, grads + nc * ps, 0.0);
-  for (int m = 0; m < num_gp; ++m) {
-    for (int c = 0; c < nc; ++c) values[c] += v[static_cast<size_t>(m) * nc + c];
-    if (grads)
-      for (size_t k = 0; k < nc * ps; ++k) grads[k] += g[static_cast<size_t>(m) * nc * ps + k];
-  }
+  for (int m = 0; m < num_gp; ++m)
+    add_member(m, nc, ps, v.data() + static_cast<size_t>(m) * nc, grads ? g.data() + m * nc * ps : nullptr, values,
+               grads);
 }
 
 namespace {
 
-// union rows of an ensemble's q-KG: up to 32 the plans and cmoe_kg_eval, past them cmoe_kg_eval_large's stages
-bool kg_ensemble_large(const cmoe_gp* const* gps, int q, int p) {
-  return static_cast<long long>(q + p) * (1 + gps[0]->spec.g) > 32;
+// the mean of the members' sums
+void ensemble_mean(int nc, size_t ps, int num_gp, double* values, double* grads) {
+  for (int c = 0; c < nc; ++c) values[c] /= static_cast<double>(num_gp);
+  if (grads)
+    for (size_t k = 0; k < nc * ps; ++k) grads[k] /= static_cast<double>(num_gp);
 }
 
-void make_kg_ensemble(KgEnsembleEvaluator& ens, const cmoe_gp* const* gps, int num_gp, int nf,
-                      const cmoe_gd_params* inner, const double* inner_bounds, const double* discrete_pts, int num_pts,
-                      int max_value_cands, int max_grad_cands, int q, const double* Xp, int p, int num_mc,
-                      const double* best_so_far, uint64_t seed) {
+// The q-EI evaluation of the drivers for an ensemble of num_gp >= 1 GPs: the mean of the members' q-EI.  With `analytic`
+// and q = 1, p = 0 each member's is the closed-form one-point EI (gpp_math.hpp:1703-1749); otherwise the Monte-Carlo
+// estimate on the normals of dtable (device [num_mc][q + p]) or Philox, per member on the per-set kernels up to kMaxQ
+// union rows, past them one ei_large_eval call for every member.
+BatchEval make_ei_eval(const cmoe_gp* const* gps_in, int num_gp, int q, const double* Xp_in, int p, int num_mc,
+                       const double* best_in, uint64_t seed, bool analytic, const double* dtable) {
+  const std::vector<const cmoe_gp*> gps(gps_in, gps_in + num_gp);
+  const std::vector<double> best(best_in, best_in + num_gp);
   const int dim = gps[0]->spec.dim;
-  ens.q = q;
-  ens.dim = dim;
-  ens.nf = nf;
-  if (kg_ensemble_large(gps, q, p)) {
-    const int ps = dim - nf;
-    CMOE_REQUIRE(nf >= 0 && ps >= 1 && num_pts >= 0, CMOE_ERR_BOUNDS, "num_fidelity out of range");
-    ens.large = true;
-    ens.gps.assign(gps, gps + num_gp);
-    ens.num_pts = num_pts;
-    ens.p = p;
-    ens.num_mc = num_mc;
-    ens.seed = seed;
-    ens.inner = *inner;
-    ens.inner_bounds.assign(inner_bounds, inner_bounds + 2 * static_cast<size_t>(ps));
-    ens.discrete.assign(discrete_pts, discrete_pts + static_cast<size_t>(num_gp) * num_pts * ps);
-    if (p) ens.Xp.assign(Xp, Xp + static_cast<size_t>(p) * dim);
-    ens.best.assign(best_so_far, best_so_far + num_gp);
-    return;
+  const std::vector<double> Xp(Xp_in, Xp_in + static_cast<size_t>(p) * dim);
+  const size_t ps = static_cast<size_t>(q) * dim;
+  const bool closed_form = analytic && q == 1 && p == 0;
+  if (!closed_form && ei_union_is_large(q, p)) {
+    return [=](const double* pts, int nc, double* values, double* grads) {
+      ei_large_eval(gps.data(), num_gp, pts, nc, q, Xp.data(), p, num_mc, best.data(), seed, dtable, values, grads);
+      ensemble_mean(nc, ps, num_gp, values, grads);
+    };
   }
-  for (int m = 0; m < num_gp; ++m) {
-    ens.evs.emplace_back(new KgEvaluator());
-    make_kg_evaluator(*ens.evs.back(), gps[m], nf, inner, inner_bounds,
-                      discrete_pts + static_cast<size_t>(m) * num_pts * (dim - nf), num_pts, max_value_cands,
-                      max_grad_cands, q, Xp, p, num_mc, best_so_far[m], seed);
-  }
+  return [=](const double* pts, int nc, double* values, double* grads) {
+    std::vector<double> tv(nc), tg(grads ? nc * ps : 0);
+    for (int m = 0; m < num_gp; ++m) {
+      if (closed_form) {
+        analytic_ei(gps[m], pts, nc, best[m], tv.data(), grads ? tg.data() : nullptr);
+      } else {
+        require_device(gps[m]->device);  // may run on a worker thread of the multi-device driver
+        ei_eval_batch(*gps[m], pts, nc, q, Xp.data(), p, num_mc, best[m], seed, dtable, tv.data(),
+                      grads ? tg.data() : nullptr);
+      }
+      add_member(m, nc, ps, tv.data(), grads ? tg.data() : nullptr, values, grads);
+    }
+    ensemble_mean(nc, ps, num_gp, values, grads);
+  };
 }
 
+// the MCMC drivers' q-EI: Monte-Carlo, or the closed form at q = 1, p = 0
 BatchEval make_ei_ensemble(const cmoe_gp* const* gps, int num_gp, int q, const double* Xp, int p, int num_mc,
                            const double* best_so_far, uint64_t seed) {
   CMOE_REQUIRE(q >= 1 && p >= 0 && static_cast<long long>(q) + p <= kMaxSampleQ, CMOE_ERR_BOUNDS,
                "q + p must be in [1, 8192]");
-  if (q + p > kMaxQ) {
-    // past the per-set kernels' 96 rows: every member on the tiled path of ei_large.cu, one set of normals
-    std::vector<const cmoe_gp*> members(gps, gps + num_gp);
-    std::vector<double> best(best_so_far, best_so_far + num_gp), pending(Xp, Xp + static_cast<size_t>(p) * gps[0]->spec.dim);
-    const size_t ps = static_cast<size_t>(q) * gps[0]->spec.dim;
-    return [=](const double* pts, int nc, double* values, double* grads) {
-      ei_large_ensemble_eval(members.data(), num_gp, pts, nc, q, pending.data(), p, num_mc, best.data(), seed, nullptr,
-                             values, grads);
-      for (int c = 0; c < nc; ++c) values[c] /= static_cast<double>(num_gp);
-      if (grads)
-        for (size_t k = 0; k < nc * ps; ++k) grads[k] /= static_cast<double>(num_gp);
-    };
-  }
-  std::vector<BatchEval> members;
-  for (int m = 0; m < num_gp; ++m) members.push_back(make_ei_eval(gps[m], q, Xp, p, num_mc, best_so_far[m], seed));
-  const size_t ps = static_cast<size_t>(q) * gps[0]->spec.dim;
-  return [members, ps, num_gp](const double* pts, int nc, double* values, double* grads) {
-    std::vector<double> tv(nc), tg(grads ? nc * ps : 0);
-    std::fill(values, values + nc, 0.0);
-    if (grads) std::fill(grads, grads + nc * ps, 0.0);
-    for (const BatchEval& f : members) {
-      f(pts, nc, tv.data(), grads ? tg.data() : nullptr);
-      for (int c = 0; c < nc; ++c) values[c] += tv[c];
-      if (grads)
-        for (size_t k = 0; k < nc * ps; ++k) grads[k] += tg[k];
-    }
-    for (int c = 0; c < nc; ++c) values[c] /= static_cast<double>(num_gp);
-    if (grads)
-      for (size_t k = 0; k < nc * ps; ++k) grads[k] /= static_cast<double>(num_gp);
+  return make_ei_eval(gps, num_gp, q, Xp, p, num_mc, best_so_far, seed, true, nullptr);
+}
+
+// The MCMC drivers' q-KG: the members' sum divided by num_gp and the fidelity cost
+BatchEval kg_ensemble_eval(KgEvaluator& ev, int q, int dim, int nf, int num_gp) {
+  return [&ev, q, dim, nf, num_gp](const double* pts, int nc, double* values, double* grads) {
+    ev(pts, nc, values, grads);
+    apply_fidelity_cost(pts, nc, q, dim, nf, num_gp, values, grads);
   };
 }
 
@@ -694,8 +656,8 @@ int cmoe_multistart_kg_ex(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_par
       const double* stale = (opts && opts->fresh_discretisation) ? nullptr
                             : (opts && opts->stale_union)        ? opts->stale_union
                                                                  : starts;
-      make_kg_evaluator(w.kg, w.gp, num_fidelity, inner, inner_bounds, discrete_pts, num_pts, (num_starts + G - 1) / G,
-                        (std::min(kTopK, num_starts) + G - 1) / G, q, points_being_sampled, p, num_mc, best_so_far, seed,
+      make_kg_evaluator(w.kg, &w.gp, 1, num_fidelity, inner, inner_bounds, discrete_pts, num_pts, (num_starts + G - 1) / G,
+                        (std::min(kTopK, num_starts) + G - 1) / G, q, points_being_sampled, p, num_mc, &best_so_far, seed,
                         stale);
       if (opts && opts->normals_table) w.kg.set_table(opts->normals_table, opts->table_len);
       w.eval = std::ref(w.kg);
@@ -742,7 +704,7 @@ int cmoe_multistart_ei_ex(const cmoe_gp* gp, const cmoe_gd_params* outer, const 
         CMOE_CUDA(cudaStreamSynchronize(w.gp->stream));
         dtable = w.table.p;
       }
-      w.eval = make_ei_eval(w.gp, q, points_being_sampled, p, num_mc, best_so_far, seed, dtable);
+      w.eval = make_ei_eval(&w.gp, 1, q, points_being_sampled, p, num_mc, &best_so_far, seed, true, dtable);
     }
     BatchEval f = std::ref(sh);
     const int domain_type = opts ? opts->domain_type : CMOE_DOMAIN_TENSOR_PRODUCT;
@@ -773,8 +735,8 @@ int cmoe_kg_gradient_descent_ex(const cmoe_gp* gp, int num_fidelity, const cmoe_
     require_device(gp->device);
     validate_bounds(domain_bounds, gp->spec.dim);
     KgEvaluator ev;
-    make_kg_evaluator(ev, gp, num_fidelity, inner, inner_bounds, discrete_pts, num_pts, num_starts, num_starts, q,
-                      points_being_sampled, p, num_mc, best_so_far, seed, stale_union);
+    make_kg_evaluator(ev, &gp, 1, num_fidelity, inner, inner_bounds, discrete_pts, num_pts, num_starts, num_starts, q,
+                      points_being_sampled, p, num_mc, &best_so_far, seed, stale_union);
     BatchEval f = std::ref(ev);
     gradient_descent_batch(f, *outer, domain_bounds, q, gp->spec.dim, starts, num_starts, values_out, points_out);
   });
@@ -798,7 +760,7 @@ int cmoe_ei_gradient_descent(const cmoe_gp* gp, const cmoe_gd_params* outer, con
     CMOE_REQUIRE(num_starts >= 1, CMOE_ERR_BOUNDS, "num_multistarts must be > 1");
     require_device(gp->device);
     validate_bounds(domain_bounds, gp->spec.dim);
-    BatchEval f = make_ei_eval(gp, q, points_being_sampled, p, num_mc, best_so_far, seed);
+    BatchEval f = make_ei_eval(&gp, 1, q, points_being_sampled, p, num_mc, &best_so_far, seed, true, nullptr);
     gradient_descent_batch(f, *outer, domain_bounds, q, gp->spec.dim, starts, num_starts, values_out, points_out);
   });
 }
@@ -815,26 +777,22 @@ int cmoe_kg_eval_mcmc(const cmoe_gp* const* gps, int num_gp, int num_fidelity, c
     CMOE_REQUIRE(num_candidates >= 1, CMOE_ERR_BOUNDS, "num_multistarts must be > 1");
     const int dim = gps[0]->spec.dim;
     const size_t ps = static_cast<size_t>(q) * dim;
-    if (kg_ensemble_large(gps, q, p)) {
-      kg_large_ensemble_eval(gps, num_gp, num_fidelity, inner, inner_bounds, discrete_pts, num_pts, candidates,
-                             num_candidates, q, points_being_sampled, p, num_mc, best_so_far, seed, normals_table,
-                             values, grads);
-      apply_fidelity_cost(candidates, num_candidates, q, dim, num_fidelity, num_gp, values, grads);
-      return;
-    }
-    std::vector<double> tv(num_candidates), tg(grads ? num_candidates * ps : 0);
-    std::fill(values, values + num_candidates, 0.0);
-    if (grads) std::fill(grads, grads + num_candidates * ps, 0.0);
-    for (int m = 0; m < num_gp; ++m) {
-      int inf = 0;
-      const int rc = cmoe_kg_eval(gps[m], num_fidelity, inner, inner_bounds,
-                                  discrete_pts + static_cast<size_t>(m) * num_pts * (dim - num_fidelity), num_pts,
-                                  candidates, num_candidates, q, points_being_sampled, p, num_mc, best_so_far[m], seed,
-                                  normals_table, tv.data(), grads ? tg.data() : nullptr, nullptr, &inf);
-      if (rc != CMOE_OK) throw Error(rc, cmoe_last_error(), inf);
-      for (int c = 0; c < num_candidates; ++c) values[c] += tv[c];
-      if (grads)
-        for (size_t k = 0; k < num_candidates * ps; ++k) grads[k] += tg[k];
+    if (kg_union_is_large(q, p, gps[0]->spec.g)) {
+      kg_large_eval(gps, num_gp, num_fidelity, inner, inner_bounds, discrete_pts, num_pts, candidates, num_candidates,
+                    q, points_being_sampled, p, num_mc, best_so_far, seed, normals_table, nullptr, values, grads,
+                    nullptr);
+    } else {
+      // each member's cmoe_kg_eval, which reuses its handle's cached plan across calls
+      std::vector<double> tv(num_candidates), tg(grads ? num_candidates * ps : 0);
+      for (int m = 0; m < num_gp; ++m) {
+        int inf = 0;
+        const int rc = cmoe_kg_eval(gps[m], num_fidelity, inner, inner_bounds,
+                                    discrete_pts + static_cast<size_t>(m) * num_pts * (dim - num_fidelity), num_pts,
+                                    candidates, num_candidates, q, points_being_sampled, p, num_mc, best_so_far[m],
+                                    seed, normals_table, tv.data(), grads ? tg.data() : nullptr, nullptr, &inf);
+        if (rc != CMOE_OK) throw Error(rc, cmoe_last_error(), inf);
+        add_member(m, num_candidates, ps, tv.data(), grads ? tg.data() : nullptr, values, grads);
+      }
     }
     apply_fidelity_cost(candidates, num_candidates, q, dim, num_fidelity, num_gp, values, grads);
   });
@@ -857,20 +815,6 @@ int cmoe_ei_eval_mcmc(const cmoe_gp* const* gps, int num_gp, const double* candi
     check_ensemble(gps, num_gp);
     CMOE_REQUIRE(num_candidates >= 1, CMOE_ERR_BOUNDS, "num_multistarts must be > 1");
     require_device(gps[0]->device);
-    const size_t ps = static_cast<size_t>(q) * gps[0]->spec.dim;
-    if (q + p > kMaxQ) {
-      // past the per-set kernels' 96 rows: the tiled path of ei_large.cu, every member on the same normals (the table
-      // is checked, then uploaded into the evaluation's workspace)
-      ei_large_ensemble_eval(gps, num_gp, candidates, num_candidates, q, points_being_sampled, p, num_mc, best_so_far,
-                             seed, normals_table, values, grads);
-      for (int c = 0; c < num_candidates; ++c) values[c] /= static_cast<double>(num_gp);
-      if (grads)
-        for (size_t k = 0; k < num_candidates * ps; ++k) grads[k] /= static_cast<double>(num_gp);
-      return;
-    }
-    std::vector<double> tv(num_candidates), tg(grads ? num_candidates * ps : 0);
-    std::fill(values, values + num_candidates, 0.0);
-    if (grads) std::fill(grads, grads + num_candidates * ps, 0.0);
     // the kernels read the table from device memory: a host pointer is only readable by the GPU where the system
     // maps pageable host memory for it, and faults elsewhere
     DevBuf<double> dtable;
@@ -878,19 +822,8 @@ int cmoe_ei_eval_mcmc(const cmoe_gp* const* gps, int num_gp, const double* candi
       dtable.upload(normals_table, static_cast<size_t>(num_mc) * (q + p), gps[0]->stream);
       CMOE_CUDA(cudaStreamSynchronize(gps[0]->stream));  // the members evaluate on their own streams
     }
-    for (int m = 0; m < num_gp; ++m) {
-      if (analytic_single && q == 1 && p == 0)
-        analytic_ei(gps[m], candidates, num_candidates, best_so_far[m], tv.data(), grads ? tg.data() : nullptr);
-      else
-        ei_eval_batch(*gps[m], candidates, num_candidates, q, points_being_sampled, p, num_mc, best_so_far[m], seed,
-                      normals_table ? dtable.p : nullptr, tv.data(), grads ? tg.data() : nullptr);
-      for (int c = 0; c < num_candidates; ++c) values[c] += tv[c];
-      if (grads)
-        for (size_t k = 0; k < num_candidates * ps; ++k) grads[k] += tg[k];
-    }
-    for (int c = 0; c < num_candidates; ++c) values[c] /= static_cast<double>(num_gp);
-    if (grads)
-      for (size_t k = 0; k < num_candidates * ps; ++k) grads[k] /= static_cast<double>(num_gp);
+    make_ei_eval(gps, num_gp, q, points_being_sampled, p, num_mc, best_so_far, seed, analytic_single != 0,
+                 normals_table ? dtable.p : nullptr)(candidates, num_candidates, values, grads);
   });
 }
 
@@ -905,10 +838,10 @@ int cmoe_multistart_kg_mcmc(const cmoe_gp* const* gps, int num_gp, int num_fidel
     CMOE_REQUIRE(num_starts >= 1, CMOE_ERR_BOUNDS, "num_multistarts must be > 1");
     require_device(gps[0]->device);
     validate_bounds(domain_bounds, gps[0]->spec.dim);
-    KgEnsembleEvaluator ens;
-    make_kg_ensemble(ens, gps, num_gp, num_fidelity, inner, inner_bounds, discrete_pts, num_pts, num_starts,
-                     std::min(kTopK, num_starts), q, points_being_sampled, p, num_mc, best_so_far, seed);
-    BatchEval f = std::ref(ens);
+    KgEvaluator ev;
+    make_kg_evaluator(ev, gps, num_gp, num_fidelity, inner, inner_bounds, discrete_pts, num_pts, num_starts,
+                      std::min(kTopK, num_starts), q, points_being_sampled, p, num_mc, best_so_far, seed);
+    BatchEval f = kg_ensemble_eval(ev, q, gps[0]->spec.dim, num_fidelity, num_gp);
     multistart_common(f, *outer, domain_bounds, q, gps[0]->spec.dim, starts, num_starts,
                       -std::numeric_limits<double>::infinity(), start_values, best_point, best_value, found_flag);
   });
@@ -941,10 +874,10 @@ int cmoe_kg_gradient_descent_mcmc(const cmoe_gp* const* gps, int num_gp, int num
     CMOE_REQUIRE(num_starts >= 1, CMOE_ERR_BOUNDS, "num_multistarts must be > 1");
     require_device(gps[0]->device);
     validate_bounds(domain_bounds, gps[0]->spec.dim);
-    KgEnsembleEvaluator ens;
-    make_kg_ensemble(ens, gps, num_gp, num_fidelity, inner, inner_bounds, discrete_pts, num_pts, num_starts, num_starts,
-                     q, points_being_sampled, p, num_mc, best_so_far, seed);
-    BatchEval f = std::ref(ens);
+    KgEvaluator ev;
+    make_kg_evaluator(ev, gps, num_gp, num_fidelity, inner, inner_bounds, discrete_pts, num_pts, num_starts, num_starts,
+                      q, points_being_sampled, p, num_mc, best_so_far, seed);
+    BatchEval f = kg_ensemble_eval(ev, q, gps[0]->spec.dim, num_fidelity, num_gp);
     gradient_descent_batch(f, *outer, domain_bounds, q, gps[0]->spec.dim, starts, num_starts, values_out, points_out);
   });
 }

@@ -202,6 +202,8 @@ int cmoe_gp_posterior(const cmoe_gp* gp, const double* sets, int num_sets, int n
 #define CMOE_MAX_SET_ROWS 96
 /* Largest Q of cmoe_gp_posterior_large and largest q + p of cmoe_ei_eval_large. */
 #define CMOE_MAX_LARGE_SET_ROWS 8192
+/* Largest Q = (q + p)(1 + num_derivatives) of cmoe_kg_eval and the cmoe_kg_plan_* API. */
+#define CMOE_MAX_KG_ROWS 32
 /* cmoe_gp_posterior's mean, var and chol_var for 1 <= Q = num_pts (1 + g_s) <= 8192, in its layouts (any output may be
  * NULL).  Computed by the stages of cmoe_gp_sample_joint: Var = K(P,P) - V^T V with V = L^-1 K(X,P), factored by the
  * batched blocked Cholesky (the reference's (K^-1 K*)^T K* differs by rounding).  Sets run in chunks that fit the handle's
@@ -385,10 +387,11 @@ int cmoe_ei_eval(const cmoe_gp* gp, const double* candidates, int num_candidates
  * arguments, same draws: sample s uses the normals 2k, 2k+1 of Philox call (seed, draw s, k), or row s of the
  * [num_mc][U] table.  At U <= 96 the two calls differ only in summation order.  y - mu = C W runs as FP64 tensor-core
  * tiles; the gradient is taken in reverse mode through the Cholesky factor (DESIGN.md K16), so no q U^2 dim tensor is
- * formed: O(n U + U^2) device memory per candidate.  Candidates run in chunks that fit 2 GiB; a candidate's result does
- * not depend on the batch.  A failed factorisation -> CMOE_ERR_SINGULAR, *info = leading minor of the first failing
+ * formed: O(n U + U^2) device memory per candidate.  The call's device workspace (the num_mc U normals and chunks of
+ * candidates) is at most 2 GiB, kept on the handle; the table, when given, is uploaded beside it.  A candidate's result
+ * does not depend on the batch or the chunking.  A failed factorisation -> CMOE_ERR_SINGULAR, *info = leading minor of the first failing
  * candidate.  The multistart q-EI drivers (cmoe_multistart_ei(_ex), cmoe_ei_gradient_descent) evaluate through this
- * call when q + p > 96 and through cmoe_ei_eval otherwise. */
+ * call's stages when q + p > CMOE_MAX_SET_ROWS and through cmoe_ei_eval's otherwise. */
 int cmoe_ei_eval_large(const cmoe_gp* gp, const double* candidates, int num_candidates, int q,
                        const double* points_being_sampled, int p, int num_mc, double best_so_far, uint64_t seed,
                        const double* normals_table, double* ei, double* grad_ei, int* info);
@@ -418,8 +421,9 @@ int cmoe_kg_eval(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_params* inne
  * the first failing candidate.  stats: mc_samples exact, posterior_evals and line_search_steps as cmoe_kg_stats,
  * point_evals and line_batches what this call's kernel executed.  num_mc <= 65535 * 64.  The multistart q-KG drivers
  * (cmoe_multistart_kg(_ex), cmoe_kg_gradient_descent(_ex)) and the ensemble calls (cmoe_kg_eval_mcmc,
- * cmoe_multistart_kg_mcmc, cmoe_kg_gradient_descent_mcmc) evaluate through these stages when (q + p)(1 + g) > 32 and
- * through the plans / cmoe_kg_eval otherwise.  The cmoe_kg_plan_* API keeps the 32-row bound of cmoe_kg_eval. */
+ * cmoe_multistart_kg_mcmc, cmoe_kg_gradient_descent_mcmc) evaluate through these stages when (q + p)(1 + g) >
+ * CMOE_MAX_KG_ROWS and through the plans / cmoe_kg_eval otherwise.  The cmoe_kg_plan_* API keeps the
+ * CMOE_MAX_KG_ROWS bound of cmoe_kg_eval. */
 int cmoe_kg_eval_large(const cmoe_gp* gp, int num_fidelity, const cmoe_gd_params* inner, const double* inner_bounds,
                        const double* discrete_pts, int num_pts, const double* candidates, int num_candidates, int q,
                        const double* points_being_sampled, int p, int num_mc, double best_so_far, uint64_t seed,
@@ -560,13 +564,15 @@ int cmoe_ei_analytic(const cmoe_gp* gp, const double* points, int num_points, do
  *                        driver uses analytic 1-EI per member when q = 1, p = 0).
  * normals_table: as in cmoe_kg_eval / cmoe_ei_eval (NULL = Philox stream keyed by seed); shared by every member.
  *
- * Sizes: q-KG up to (q + p)(1 + g) = 32 runs each member's cmoe_kg_eval (the drivers: its plans); past 32, up to
- * CMOE_MAX_KG_LARGE_ROWS, each member's cmoe_kg_eval_large with num_mc, g and the inner optimiser bounded as there.
+ * Sizes: q-KG up to (q + p)(1 + g) = CMOE_MAX_KG_ROWS runs each member's cmoe_kg_eval (the drivers: its plans); past
+ * it, up to CMOE_MAX_KG_LARGE_ROWS, each member's cmoe_kg_eval_large with num_mc, g and the inner optimiser bounded as
+ * there.
  * q-EI up to q + p = CMOE_MAX_SET_ROWS runs each member's cmoe_ei_eval; past it, up to CMOE_MAX_LARGE_SET_ROWS, each
  * member's cmoe_ei_eval_large.  Past the per-set bounds the draws are made once per evaluation, the members run
  * together on their own streams, and the evaluation's large-stage workspace is at most 2 GiB per device whatever
  * num_gp is (kept on gps[0]'s handle); each member's value and gradient are those of its single large call, summed in
- * member order.  q + p past the large bound -> CMOE_ERR_BOUNDS before any handle is read.  A singular union ->
+ * member order (a one-member sum is the member's own result).  q + p past the large bound -> CMOE_ERR_BOUNDS before
+ * any handle is read.  A singular union ->
  * CMOE_ERR_SINGULAR, *info = leading minor of the first failing candidate of the first failing member. */
 int cmoe_kg_eval_mcmc(const cmoe_gp* const* gps, int num_gp, int num_fidelity, const cmoe_gd_params* inner,
                       const double* inner_bounds, const double* discrete_pts, int num_pts, const double* candidates,

@@ -1,5 +1,6 @@
 """Build-time check of the large-union q-KG kernels (no GPU needed, DESIGN.md K17): `-Xptxas -v` reports no more local
-memory for the stage kernels of kg_large.cu than K17 records and none for the DMMA products it shares with ei_large.cu,
+memory for the stage kernels of kg_large.cu than K17 records and none for the DMMA products and the transpose it shares
+with ei_large.cu,
 those products issue FP64 tensor-core instructions, and the inner-optimiser builds (kg_mc_large_kernel) spill no more
 than K17 records."""
 import os
@@ -11,7 +12,7 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BUILD = os.path.join(ROOT, "cornell-moe_b200", "build")
 STAGE_KERNELS = ("kgl_normals_kernel", "kgl_pack_kernel", "kgl_noise_kernel", "kgl_best_kernel",
-                 "kgl_disc_cov_kernel", "kgl_transpose_kernel", "kgl_argmin_kernel", "kgl_weights_kernel",
+                 "kgl_disc_cov_kernel", "kgl_argmin_kernel", "kgl_weights_kernel",
                  "kgl_kx_kernel", "kgl_lbar_kernel", "kgl_grad_kernel")
 # local memory the stage kernels are allowed, (stack frame, spill stores, spill loads) in bytes, as DESIGN.md K17 records:
 # the Box-Muller sine and cosine's slow-path reduction, the raw minimiser kept as an indexable array, and the gradient
@@ -19,6 +20,8 @@ STAGE_KERNELS = ("kgl_normals_kernel", "kgl_pack_kernel", "kgl_noise_kernel", "k
 STAGE_LOCAL = {"kgl_normals_kernel": (40, 0, 0), "kgl_kx_kernel": (256, 0, 0), "kgl_grad_kernel": (8, 4, 12)}
 # the scan (W^T Z), the weights (B C), R (Kx C^T), R2 (B 2 Sigmabar) and the adjoint's C^T Cbar
 SHARED_DMMA_KERNELS = ("gemm_nn_kernel", "ei_ctc_kernel")
+# every kernel of ei_large.cu that the stages launch: the DMMA products and the batched transpose (B^T, W^T, C^T)
+SHARED_KERNELS = SHARED_DMMA_KERNELS + ("transpose_kernel",)
 # spill stores (bytes) of every kg_mc_large_kernel build, (kernel, padded dim, wide) -> bytes, as DESIGN.md K17 records
 MAX_SPILL_STORES = {
     (0, 2, 0): 0, (1, 2, 0): 0, (0, 4, 0): 0, (1, 4, 0): 0, (0, 6, 0): 0, (1, 6, 0): 0, (0, 8, 0): 0, (1, 8, 0): 0,
@@ -40,14 +43,14 @@ def _usage(block):
     return tuple(int(x) for x in m.groups())
 
 
-def test_kg_large_stage_kernels_use_no_local_memory():
+def test_kg_large_stage_and_shared_kernels_use_no_local_memory():
     blocks = _blocks("kg_large.ptxas.log")
     for name in STAGE_KERNELS:
         block = next((b for b in blocks if name in b.split("\n")[0]), None)
         assert block is not None, name
         assert all(u <= a for u, a in zip(_usage(block), STAGE_LOCAL.get(name, (0, 0, 0)))), (name, block)
     blocks = _blocks("ei_large.ptxas.log")
-    for name in SHARED_DMMA_KERNELS:
+    for name in SHARED_KERNELS:
         block = next((b for b in blocks if name in b.split("\n")[0]), None)
         assert block is not None, name
         assert _usage(block) == (0, 0, 0), (name, block)

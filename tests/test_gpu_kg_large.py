@@ -166,6 +166,17 @@ def test_size_edges(capi):
     with pytest.raises(capi.BoundsError):
         dgp.kg_large(rng.uniform(size=(1, 5, 4)), rng.uniform(size=(200, 4)), 8, 0.1, DISCRETE_ONLY_GD,
                      unit_bounds(4), rng.uniform(size=(3, 4)), seed=1)
+    # cmoe_kg_eval and cmoe_kg_eval_large refuse the same bad inner arguments with the same message
+    small, long_gd, empty = rng.uniform(size=(1, 2, 2)), list(DISCRETE_ONLY_GD), unit_bounds(2).copy()
+    long_gd[1] = 4097
+    empty[0] = 2.0
+    for gd, ib in [(long_gd, unit_bounds(2)), (DISCRETE_ONLY_GD, empty)]:
+        msgs = []
+        for call in (gp.kg, gp.kg_large):
+            with pytest.raises(capi.BoundsError) as e:
+                call(small, None, 8, 0.1, gd, ib, disc, seed=1)
+            msgs.append(str(e.value))
+        assert msgs[0] == msgs[1], msgs
 
 
 def test_singular_union_reports_the_leading_minor(capi):
