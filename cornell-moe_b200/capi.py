@@ -633,6 +633,52 @@ def hyperparameter_gradient_descent(kernel, gd, bounds, starts, X, y, derivs=Non
     return best, best_v.value, bool(found.value), ends, end_v
 
 
+def grad_log_marginal_likelihood_list_exact(kernel, hypers, X, y, derivs=None, device=0):
+    """cmoe_grad_log_marginal_likelihood_list_exact: grad_log_marginal_likelihood_list with the exact gradient (every
+    entry of a Matern-5/2 derivative block contributes).  Equal to it bit for bit with g = 0 and for SE."""
+    X = _f64(X)
+    N, dim = X.shape
+    derivs = _i32(derivs)
+    H = _f64(hypers).reshape(-1, 2 + dim + derivs.size)
+    values = np.empty(H.shape[0])
+    grads = np.empty(H.shape)
+    info = ctypes.c_int()
+    rc = lib().cmoe_grad_log_marginal_likelihood_list_exact(int(kernel), _d(H), H.shape[0], _d(X), _d(_f64(y).ravel()),
+                                                            _i(derivs), derivs.size, dim, N, int(device), _d(values),
+                                                            _d(grads), ctypes.byref(info))
+    _check(rc, info.value)
+    return values, grads
+
+
+class MapOpts(ctypes.Structure):
+    """cmoe_map_opts: gtol and max_iterations (0 = 200 nh) of hyperparameter_map."""
+    _fields_ = [("gtol", ctypes.c_double), ("max_iterations", ctypes.c_int)]
+
+
+def hyperparameter_map(kernel, starts, X, y, derivs=None, noisy=True, default_prior=True, gtol=1e-5,
+                       max_iterations=None, device=0):
+    """cmoe_hyperparameter_map (DESIGN.md K19): GaussianProcessLogLikelihoodMCMC.optimize's BFGS on
+    -compute_log_likelihood from every row of ``starts`` [num_starts, 2 + dim + g] (log scale), with the analytic
+    gradient.  Returns a dict of positions, values (nll), gradients, iterations, evaluations and status
+    (0 converged, 1 max_iterations, 2 line search failed or objective not finite, 3 NaN)."""
+    X = _f64(X)
+    N, dim = X.shape
+    derivs = _i32(derivs)
+    nh = 2 + dim + derivs.size
+    S = _f64(starts).reshape(-1, nh)
+    M = S.shape[0]
+    opts = MapOpts(float(gtol), 0 if max_iterations is None else int(max_iterations))
+    pos, grads, vals = np.empty(S.shape), np.empty(S.shape), np.empty(M)
+    iters, evals, status = (np.empty(M, dtype=np.int32) for _ in range(3))
+    info = ctypes.c_int()
+    rc = lib().cmoe_hyperparameter_map(int(kernel), int(bool(default_prior)), int(bool(noisy)), _d(S), M,
+                                       ctypes.byref(opts), _d(X), _d(_f64(y).ravel()), _i(derivs), derivs.size, dim, N,
+                                       int(device), _d(pos), _d(vals), _d(grads), _i(iters), _i(evals), _i(status),
+                                       ctypes.byref(info))
+    _check(rc, info.value)
+    return dict(positions=pos, values=vals, gradients=grads, iterations=iters, evaluations=evals, status=status)
+
+
 class MCMCTable(ctypes.Structure):
     """cmoe_mcmc_table: host-supplied random numbers of hyperparameter_mcmc, each [num_steps, num_walkers]."""
     _fields_ = [("z_uniform", _dp), ("partner", _ip), ("accept_uniform", _dp)]

@@ -1417,6 +1417,39 @@ PYBIND11_MODULE(GPP, m) {
         py::arg("derivatives"), py::arg("num_derivatives"), py::arg("initial_positions"), py::arg("num_walkers"),
         py::arg("num_steps"), py::arg("noisy"), py::arg("use_default_prior"), py::arg("seed"),
         py::arg("first_step") = 0);
+  // hyperparameter_map_optimization(points_sampled, points_sampled_value, dim, num_sampled, derivatives,
+  //     num_derivatives, initial_positions, num_starts, noisy, use_default_prior, gtol, max_iterations)
+  // Not in the reference module: GaussianProcessLogLikelihoodMCMC.optimize (log_likelihood_mcmc.py:241-275), BFGS on
+  // -compute_log_likelihood from every start in one device call (cmoe_hyperparameter_map, DESIGN.md K19), with the
+  // analytic gradient.  Starts are log-scale [log alpha, log lengths..., log noise...]; max_iterations = 0 is scipy's
+  // 200 nh.  Returns (positions, values, status) as flat lists; values are the negative log-likelihood.
+  m.def("hyperparameter_map_optimization",
+        [](const py::list& points_sampled, const py::list& points_sampled_value, int dim, int num_sampled,
+           const py::list& derivatives, int num_derivatives, const py::list& initial_positions, int num_starts,
+           bool noisy, bool use_default_prior, double gtol, int max_iterations) -> py::tuple {
+          const auto X = to_vec(points_sampled, static_cast<size_t>(dim) * num_sampled);
+          const auto y = to_vec(points_sampled_value, static_cast<size_t>(num_sampled) * (1 + num_derivatives));
+          const auto derivs = to_ivec(derivatives, num_derivatives);
+          const size_t nh = static_cast<size_t>(dim) + 2 + num_derivatives, S = std::max(num_starts, 0);
+          const auto p0 = to_vec(initial_positions, nh * S);
+          std::vector<double> pos(p0.size()), grads(p0.size()), vals(S);
+          std::vector<int> iters(S), evals(S), status(S);
+          const cmoe_map_opts opts{gtol, max_iterations};
+          int info = 0;
+          // MaternNu2p5 hard-wired, as compute_log_likelihood's boundary does
+          check(cmoe_hyperparameter_map(CMOE_KERNEL_MATERN_NU_2P5,
+                                        use_default_prior ? CMOE_HYPER_PRIOR_DEFAULT : CMOE_HYPER_PRIOR_NONE,
+                                        noisy ? 1 : 0, p0.data(), num_starts, &opts, X.data(), y.data(), derivs.data(),
+                                        num_derivatives, dim, num_sampled, 0, pos.data(), vals.data(), grads.data(),
+                                        iters.data(), evals.data(), status.data(), &info),
+                info);
+          py::list st;
+          for (int v : status) st.append(v);
+          return py::make_tuple(to_list(pos), to_list(vals), st);
+        },
+        py::arg("points_sampled"), py::arg("points_sampled_value"), py::arg("dim"), py::arg("num_sampled"),
+        py::arg("derivatives"), py::arg("num_derivatives"), py::arg("initial_positions"), py::arg("num_starts"),
+        py::arg("noisy"), py::arg("use_default_prior"), py::arg("gtol") = 1.0e-5, py::arg("max_iterations") = 0);
   // lower_confidence_bound_optimization(gaussian_process, candidate_pts, num_candidates, num_to_sample)
   // Not in the reference module: the body of lower_confidence_bound.py:52-80 in one device call (cmoe_lcb_select,
   // DESIGN.md K13).  `gaussian_process` is a GaussianProcess or a wrapper holding one as `_gaussian_process`;

@@ -44,13 +44,69 @@ constexpr int kHgTx = 32, kHgTy = 8;
 
 // The hyper-gradient block of one point pair (row point j at p1, column point i at p2): acc[h], h in [0, dim], zero on
 // entry, receives sum_{m,nn} W[j*bs+m, i*bs+nn] * dK/d theta_h [j*bs+m, i*bs+nn], where Wf(row, col) returns the entry
-// of W = a a^T - K^-1.  Shared by the single-set and the list contraction kernels.
-template <class WF>
+// of W = a a^T - K^-1.  Shared by the single-set and the list contraction kernels.  kExact = false keeps the reference's
+// Matern quirk; kExact = true differentiates every entry of the Matern derivative block (the SE branch is exact either
+// way).  With g = 0 the two Matern branches are the same function, and the host launches the quirk build there.
+template <bool kExact, class WF>
 __device__ __forceinline__ void hyper_grad_pair(const KernelSpec& spec, const double* p1, const double* p2, int j, int i,
                                                 const WF& Wf, double (&acc)[CMOE_MAX_DIM + 1]) {
   const int dim = spec.dim, bs = 1 + spec.g;
   const double r2 = weighted_sqdist(spec, p1, p2);
-  if (spec.kernel != CMOE_KERNEL_SQUARE_EXPONENTIAL) {
+  if (kExact && spec.kernel != CMOE_KERNEL_SQUARE_EXPONENTIAL) {
+    // cov_entry's block at alpha = 1, (A, B, C) of kernel_parts over alpha, u_a = (p2_a - p1_a) / l_a^2:
+    //   c(0,0) = A, c(m,0) = B u_a, c(0,n) = -B u_b, c(m,n) = -C u_a u_b + [a==b] B / l_a^2
+    // d/d r^2 of (A, B, C) is (-B/2, -C/2, -sqrt(5) C / (2 r)); the last multiplies only u_a u_b = O(r^2), so it is
+    // taken as 0 at r = 0.  d r^2 / d l_k = -2 D_k^2 / l_k^3 and d u_a / d l_k = -2 [a==k] u_a / l_a.  Lengths enter
+    // through inv_len (no division in the loops).
+    const double r = sqrt(r2), arg = kSqrt5 * r, e = exp(-arg);
+    const double A1 = e * (1.0 + arg + 5.0 / 3.0 * r2), B1 = 5.0 / 3.0 * e * (1.0 + arg), C1 = 25.0 / 3.0 * e;
+    const double dC1 = r2 > 0.0 ? -0.5 * kSqrt5 * C1 / r : 0.0;
+    for (int m = 0; m < bs; ++m) {
+      const int ta = m ? spec.derivs[m - 1] : -1;
+      const double ila = ta >= 0 ? spec.inv_len[ta] : 0.0;
+      const double ua = (ta >= 0) ? (p2[ta] - p1[ta]) * ila * ila : 0.0;
+      for (int nn = 0; nn < bs; ++nn) {
+        const int tb = nn ? spec.derivs[nn - 1] : -1;
+        const double ilb = tb >= 0 ? spec.inv_len[tb] : 0.0;
+        const double ub = (tb >= 0) ? (p2[tb] - p1[tb]) * ilb * ilb : 0.0;
+        // the entry E, and dE/d l_k = cs ds_k + ([a==k] ca + [b==k] cb) / l_k
+        double E, cs, ca = 0.0, cb = 0.0;
+        if (ta < 0 && tb < 0) {
+          E = A1;
+          cs = -0.5 * B1;
+        } else if (tb < 0) {
+          E = B1 * ua;
+          cs = -0.5 * C1 * ua;
+          ca = -2.0 * B1 * ua;
+        } else if (ta < 0) {
+          E = -B1 * ub;
+          cs = 0.5 * C1 * ub;
+          cb = 2.0 * B1 * ub;
+        } else {
+          E = -C1 * ua * ub;
+          cs = -dC1 * ua * ub;
+          ca = cb = 2.0 * C1 * ua * ub;
+          if (ta == tb) {
+            const double il2 = ila * ila;
+            E += B1 * il2;
+            cs += -0.5 * C1 * il2;
+            ca += -2.0 * B1 * il2;
+          }
+        }
+        const double W = Wf(j * bs + m, i * bs + nn);
+        acc[0] = fma(W, E, acc[0]);
+        const double aW = spec.alpha * W;
+        for (int k = 0; k < dim; ++k) {
+          const double il = spec.inv_len[k];
+          const double Dl = (p1[k] - p2[k]) * il;
+          double dE = cs * (-2.0 * Dl * Dl * il);
+          if (ta == k) dE += ca * il;
+          if (tb == k) dE += cb * il;
+          acc[k + 1] = fma(aW, dE, acc[k + 1]);
+        }
+      }
+    }
+  } else if (spec.kernel != CMOE_KERNEL_SQUARE_EXPONENTIAL) {
     // value-value entry only (gpp_covariance.cpp:461-489)
     const double W = Wf(j * bs, i * bs);
     if (r2 == 0.0) {
@@ -120,8 +176,9 @@ __global__ void __launch_bounds__(kHgTx * kHgTy)
   double acc[CMOE_MAX_DIM + 1];
   for (int h = 0; h < hd; ++h) acc[h] = 0.0;
   if (i < N && j < N) {
-    hyper_grad_pair(spec, X + static_cast<size_t>(j) * dim, X + static_cast<size_t>(i) * dim, j, i,
-                    [&](int row, int col) { return a[row] * a[col] - Kinv[static_cast<size_t>(col) * n + row]; }, acc);
+    hyper_grad_pair<false>(spec, X + static_cast<size_t>(j) * dim, X + static_cast<size_t>(i) * dim, j, i,
+                           [&](int row, int col) { return a[row] * a[col] - Kinv[static_cast<size_t>(col) * n + row]; },
+                           acc);
   }
   const int cta = blockIdx.y * gridDim.x + blockIdx.x;
   for (int h = 0; h < hd; ++h) {
@@ -384,7 +441,8 @@ __global__ void __launch_bounds__(kInvThreads) inv_syrk_kernel(const double* __r
 
 // partial[set][cta][h], h in [0, dim]: hyper_grad_contract_kernel for every set, grid (point-pair tiles, 1, sets) with
 // CTA (bx, by) = (x % gx, x / gx).  The set's KernelSpec is staged in shared memory; W is read from the lower
-// triangle of K^-1 only.
+// triangle of K^-1 only.  kExact: hyper_grad_pair's exact Matern block.
+template <bool kExact>
 __global__ void __launch_bounds__(kHgTx * kHgTy)
     lml_grad_contract_kernel(const KernelSpec* __restrict__ specs, const double* __restrict__ X, int N, int gx,
                              const double* __restrict__ a, const double* __restrict__ Kinv,
@@ -408,12 +466,12 @@ __global__ void __launch_bounds__(kHgTx * kHgTy)
   double acc[CMOE_MAX_DIM + 1];
   for (int h = 0; h < hd; ++h) acc[h] = 0.0;
   if (i < N && j < N) {
-    hyper_grad_pair(spec, X + static_cast<size_t>(j) * dim, X + static_cast<size_t>(i) * dim, j, i,
-                    [&](int row, int col) {
-                      const int lo = min(row, col), hi = max(row, col);
-                      return as[row] * as[col] - Ks[static_cast<size_t>(lo) * n + hi];
-                    },
-                    acc);
+    hyper_grad_pair<kExact>(spec, X + static_cast<size_t>(j) * dim, X + static_cast<size_t>(i) * dim, j, i,
+                            [&](int row, int col) {
+                              const int lo = min(row, col), hi = max(row, col);
+                              return as[row] * as[col] - Ks[static_cast<size_t>(lo) * n + hi];
+                            },
+                            acc);
   }
   for (int h = 0; h < hd; ++h) {
     const double s = block_sum(acc[h], scratch);
@@ -484,6 +542,117 @@ size_t lml_set_bytes(int n, int b) {
   return sizeof(double) * (static_cast<size_t>(n) * n + nsteps * NB * NB + b + 1) + sizeof(KernelSpec) + sizeof(int);
 }
 
+// CTAs of one set's gradient contraction: gx point tiles along the rows times the tiles along the columns
+int lml_grad_ctas(int N, int& gx) {
+  gx = (N + kHgTx - 1) / kHgTx;
+  return gx * ((N + kHgTy - 1) / kHgTy);
+}
+
+// bytes of one set in a chunk with the gradient: lml_set_bytes plus L^-1 (n x n), a, the contraction's CTA partials and
+// the [1 + nh] output row
+size_t lml_grad_set_bytes(int N, int dim, int g) {
+  const int b = 1 + g, n = N * b;
+  int gx;
+  const int nctas = lml_grad_ctas(N, gx);
+  return lml_set_bytes(n, b) +
+         sizeof(double) * (static_cast<size_t>(n) * n + n + static_cast<size_t>(nctas) * (dim + 1) + 1 + 2 + dim + g);
+}
+
+// y - m, m = average of the function values in the reference's order (gpp_model_selection.cpp:556-560); it does not
+// depend on the set
+std::vector<double> centred_values(const double* points_sampled_value, int N, int b) {
+  double m = 0.0;
+  for (int i = 0; i < N; ++i) m += points_sampled_value[static_cast<size_t>(i) * b];
+  m /= N;
+  std::vector<double> rc(points_sampled_value, points_sampled_value + static_cast<size_t>(N) * b);
+  for (int i = 0; i < N; ++i) rc[static_cast<size_t>(i) * b] -= m;
+  return rc;
+}
+
+// Uploads the points and y - m and sizes w's buffers for chunks of `chunk` sets (with the gradient's when `grads`).
+void lml_prepare(LmlWork& w, const double* points_sampled, const double* points_sampled_value, int N, int dim, int g,
+                 int chunk, bool grads, cudaStream_t s) {
+  const int b = 1 + g, n = N * b;
+  int gx;
+  const int nctas = lml_grad_ctas(N, gx);
+  const std::vector<double> rc = centred_values(points_sampled_value, N, b);
+  w.X.upload(points_sampled, static_cast<size_t>(N) * dim, s);
+  w.r.upload(rc.data(), n, s);
+  w.specs.ensure(chunk);
+  w.noise.ensure(static_cast<size_t>(chunk) * b);
+  w.K.ensure(static_cast<size_t>(chunk) * n * n);
+  w.values.ensure(chunk);
+  w.fail.ensure(chunk);
+  const size_t smem_solve = (static_cast<size_t>(n) + NB * (NB + 1)) * sizeof(double);
+  const size_t smem_inv = 2 * NB * LDT * sizeof(double), smem_diag = 2 * NB * (NB + 1) * sizeof(double);
+  CMOE_CUDA(cudaFuncSetAttribute(lml_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 static_cast<int>(smem_solve)));
+  if (grads) {
+    w.Linv.ensure(static_cast<size_t>(chunk) * n * n);
+    w.a.ensure(static_cast<size_t>(chunk) * n);
+    w.partial.ensure(static_cast<size_t>(chunk) * nctas * (dim + 1));
+    w.gout.ensure(static_cast<size_t>(chunk) * (1 + 2 + dim + g));
+    CMOE_CUDA(cudaFuncSetAttribute(tri_inv_offdiag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   static_cast<int>(smem_inv)));
+    CMOE_CUDA(cudaFuncSetAttribute(inv_syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   static_cast<int>(smem_inv)));
+    CMOE_CUDA(cudaFuncSetAttribute(tri_inv_diag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   static_cast<int>(smem_diag)));
+  }
+}
+
+// The K10 stages, and with `grads` the K11 stages, for the nc sets whose specs, noise and failure flags (zero, or
+// preset to skip a set) are in w: values in w.values, and with `grads` the rows [value, gradient] in w.gout.
+// `exact` selects the exact Matern contraction when there are derivative rows.  Asynchronous on s.
+void lml_stages(LmlWork& w, int N, int dim, int g, int kernel, int nc, bool grads, bool exact, cudaStream_t s) {
+  const int b = 1 + g, n = N * b, t = (n + NB - 1) / NB, nh = 2 + dim + g;
+  int gx;
+  const int nctas = lml_grad_ctas(N, gx);
+  const size_t smem_cov = 2 * static_cast<size_t>(NB) * dim * sizeof(double);
+  const size_t smem_solve = (static_cast<size_t>(n) + NB * (NB + 1)) * sizeof(double);
+  const size_t smem_inv = 2 * NB * LDT * sizeof(double), smem_diag = 2 * NB * (NB + 1) * sizeof(double);
+  lml_cov_kernel<<<dim3(t * (t + 1) / 2, 1, nc), kLmlCovThreads, smem_cov, s>>>(w.specs.p, w.noise.p, w.X.p, N, w.K.p);
+  count_launch();
+  CMOE_CUDA(cudaGetLastError());
+  potrf_batched(w.K.p, n, nc, w.fail.p, w.stage, s);
+  lml_solve_kernel<<<nc, kLmlSolveThreads, smem_solve, s>>>(w.K.p, n, w.r.p, w.fail.p, w.values.p,
+                                                            grads ? w.a.p : nullptr);
+  count_launch();
+  CMOE_CUDA(cudaGetLastError());
+  if (!grads) return;
+  tri_inv_diag_kernel<<<dim3(t, 1, nc), NB, smem_diag, s>>>(w.K.p, n, w.fail.p, w.Linv.p);
+  for (int bi = 1; bi < t; ++bi)
+    tri_inv_offdiag_kernel<<<dim3(bi, 1, nc), kInvThreads, smem_inv, s>>>(w.K.p, n, bi, w.fail.p, w.Linv.p);
+  inv_syrk_kernel<<<dim3(t * (t + 1) / 2, 1, nc), kInvThreads, smem_inv, s>>>(w.Linv.p, n, w.fail.p, w.K.p);
+  // with g = 0 the exact contraction is the quirk one's function: the same build keeps the bits
+  if (exact && g > 0 && kernel == CMOE_KERNEL_MATERN_NU_2P5)
+    lml_grad_contract_kernel<true><<<dim3(nctas, 1, nc), kHgTx * kHgTy, 0, s>>>(w.specs.p, w.X.p, N, gx, w.a.p, w.K.p,
+                                                                              w.fail.p, w.partial.p);
+  else
+    lml_grad_contract_kernel<false><<<dim3(nctas, 1, nc), kHgTx * kHgTy, 0, s>>>(w.specs.p, w.X.p, N, gx, w.a.p,
+                                                                               w.K.p, w.fail.p, w.partial.p);
+  lml_grad_reduce_kernel<<<nc, ((nh + 31) / 32) * 32, 0, s>>>(w.values.p, w.partial.p, nctas, w.a.p, w.K.p, n, dim + 1,
+                                                              b, w.fail.p, w.gout.p);
+  count_launch(t + 3);
+  CMOE_CUDA(cudaGetLastError());
+}
+
+// The argument and size checks of the list calls (and of the calls built on the list stages).
+void check_lml_problem(int kernel, const double* points_sampled, const double* points_sampled_value,
+                       const int* derivatives, int num_derivatives, int dim, int num_sampled) {
+  CMOE_REQUIRE(points_sampled != nullptr && points_sampled_value != nullptr, CMOE_ERR_INVALID_VALUE, "NULL argument");
+  CMOE_REQUIRE(kernel == CMOE_KERNEL_SQUARE_EXPONENTIAL || kernel == CMOE_KERNEL_MATERN_NU_2P5,
+               CMOE_ERR_INVALID_VALUE, "unknown covariance kernel id");
+  CMOE_REQUIRE(dim >= 1 && dim <= CMOE_MAX_DIM, CMOE_ERR_BOUNDS, "dim must be in [1, CMOE_MAX_DIM]");
+  CMOE_REQUIRE(num_sampled >= 1, CMOE_ERR_BOUNDS, "num_sampled must be >= 1");
+  CMOE_REQUIRE(num_derivatives >= 0 && num_derivatives <= dim, CMOE_ERR_BOUNDS, "num_derivatives out of range");
+  CMOE_REQUIRE(num_derivatives == 0 || derivatives != nullptr, CMOE_ERR_INVALID_VALUE, "derivatives is NULL");
+  for (int k = 0; k < num_derivatives; ++k)
+    CMOE_REQUIRE(derivatives[k] >= 0 && derivatives[k] < dim, CMOE_ERR_BOUNDS, "derivative index out of range");
+  CMOE_REQUIRE(static_cast<long long>(num_sampled) * (1 + num_derivatives) <= kMaxSampleQ, CMOE_ERR_BOUNDS,
+               "num_sampled * (1 + num_derivatives) must be <= 8192");
+}
+
 }  // namespace
 }  // namespace cmoe
 
@@ -542,27 +711,16 @@ extern "C" int cmoe_grad_log_marginal_likelihood(int kernel, double alpha, const
 
 namespace {
 
-// The body of both list calls: values[num_sets], and with grads != NULL also grads[num_sets][2 + dim + g].
+// The body of the list calls: values[num_sets], and with grads != NULL also grads[num_sets][2 + dim + g] (exact: the
+// exact Matern derivative block).
 void lml_list(int kernel, const double* hyperparameters, int num_sets, const double* points_sampled,
               const double* points_sampled_value, const int* derivatives, int num_derivatives, int dim,
-              int num_sampled, int device, double* values, double* grads) {
+              int num_sampled, int device, double* values, double* grads, bool exact) {
   {
     CMOE_REQUIRE(num_sets >= 1, CMOE_ERR_BOUNDS, "num_sets must be >= 1");
-    CMOE_REQUIRE(hyperparameters != nullptr && points_sampled != nullptr && points_sampled_value != nullptr &&
-                     values != nullptr,
-                 CMOE_ERR_INVALID_VALUE, "NULL argument");
-    CMOE_REQUIRE(kernel == CMOE_KERNEL_SQUARE_EXPONENTIAL || kernel == CMOE_KERNEL_MATERN_NU_2P5,
-                 CMOE_ERR_INVALID_VALUE, "unknown covariance kernel id");
-    CMOE_REQUIRE(dim >= 1 && dim <= CMOE_MAX_DIM, CMOE_ERR_BOUNDS, "dim must be in [1, CMOE_MAX_DIM]");
-    CMOE_REQUIRE(num_sampled >= 1, CMOE_ERR_BOUNDS, "num_sampled must be >= 1");
-    CMOE_REQUIRE(num_derivatives >= 0 && num_derivatives <= dim, CMOE_ERR_BOUNDS, "num_derivatives out of range");
-    CMOE_REQUIRE(num_derivatives == 0 || derivatives != nullptr, CMOE_ERR_INVALID_VALUE, "derivatives is NULL");
-    for (int k = 0; k < num_derivatives; ++k)
-      CMOE_REQUIRE(derivatives[k] >= 0 && derivatives[k] < dim, CMOE_ERR_BOUNDS, "derivative index out of range");
+    CMOE_REQUIRE(hyperparameters != nullptr && values != nullptr, CMOE_ERR_INVALID_VALUE, "NULL argument");
+    check_lml_problem(kernel, points_sampled, points_sampled_value, derivatives, num_derivatives, dim, num_sampled);
     const int g = num_derivatives, b = 1 + g, nh = 2 + dim + g, N = num_sampled;
-    CMOE_REQUIRE(static_cast<long long>(N) * b <= kMaxSampleQ, CMOE_ERR_BOUNDS,
-                 "num_sampled * (1 + num_derivatives) must be <= 8192");
-    const int n = N * b;
     // per set: the covariance hyper-parameters as cmoe_gp_create takes them (InitializeCovariance's checks,
     // gpp_covariance.cpp:74-98, naming the set), the noise with the single call's 1e-6 added first
     std::vector<KernelSpec> specs(num_sets);
@@ -594,78 +752,24 @@ void lml_list(int kernel, const double* hyperparameters, int num_sets, const dou
       for (int t = 0; t < b; ++t) noise[static_cast<size_t>(s) * b + t] = h[1 + dim + t] + 1.0e-6;
     }
     require_device(device);
-    // y - m, m = average of the function values in the reference's order (gpp_model_selection.cpp:556-560); it does
-    // not depend on the set
-    double m = 0.0;
-    for (int i = 0; i < N; ++i) m += points_sampled_value[static_cast<size_t>(i) * b];
-    m /= N;
-    std::vector<double> rc(points_sampled_value, points_sampled_value + n);
-    for (int i = 0; i < N; ++i) rc[static_cast<size_t>(i) * b] -= m;
 
     LmlWork& w = lml_workspace(device);
     cudaStream_t s = w.stream;
-    const int nsteps = (n + NB - 1) / NB;
-    // the gradient adds L^-1 (n x n), a, the contraction's CTA partials and the [1 + nh] output row per set
-    const int gx = (N + kHgTx - 1) / kHgTx, nctas = gx * ((N + kHgTy - 1) / kHgTy);
-    size_t per_set = lml_set_bytes(n, b);
-    if (grads)
-      per_set += sizeof(double) * (static_cast<size_t>(n) * n + n + static_cast<size_t>(nctas) * (dim + 1) + 1 + nh);
+    const size_t per_set = grads ? lml_grad_set_bytes(N, dim, g) : lml_set_bytes(N * b, b);
     const int chunk = static_cast<int>(chunk_items(num_sets, kSampleWorkspaceBytes, per_set, kMaxChunkSets));
-    w.X.upload(points_sampled, static_cast<size_t>(N) * dim, s);
-    w.r.upload(rc.data(), n, s);
-    w.specs.ensure(chunk);
-    w.noise.ensure(static_cast<size_t>(chunk) * b);
-    w.K.ensure(static_cast<size_t>(chunk) * n * n);
-    w.values.ensure(chunk);
-    w.fail.ensure(chunk);
-    const size_t smem_cov = 2 * static_cast<size_t>(NB) * dim * sizeof(double);
-    const size_t smem_solve = (static_cast<size_t>(n) + NB * (NB + 1)) * sizeof(double);
-    const size_t smem_inv = 2 * NB * LDT * sizeof(double), smem_diag = 2 * NB * (NB + 1) * sizeof(double);
-    CMOE_CUDA(cudaFuncSetAttribute(lml_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   static_cast<int>(smem_solve)));
-    if (grads) {
-      w.Linv.ensure(static_cast<size_t>(chunk) * n * n);
-      w.a.ensure(static_cast<size_t>(chunk) * n);
-      w.partial.ensure(static_cast<size_t>(chunk) * nctas * (dim + 1));
-      w.gout.ensure(static_cast<size_t>(chunk) * (1 + nh));
-      CMOE_CUDA(cudaFuncSetAttribute(tri_inv_offdiag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     static_cast<int>(smem_inv)));
-      CMOE_CUDA(cudaFuncSetAttribute(inv_syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     static_cast<int>(smem_inv)));
-      CMOE_CUDA(cudaFuncSetAttribute(tri_inv_diag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     static_cast<int>(smem_diag)));
-    }
-    const int t = nsteps;
+    lml_prepare(w, points_sampled, points_sampled_value, N, dim, g, chunk, grads != nullptr, s);
     std::vector<double> hout(grads ? static_cast<size_t>(chunk) * (1 + nh) : 0);
     for (int c0 = 0; c0 < num_sets; c0 += chunk) {
       const int nc = std::min(chunk, num_sets - c0);
       w.specs.upload(specs.data() + c0, nc, s);
       w.noise.upload(noise.data() + static_cast<size_t>(c0) * b, static_cast<size_t>(nc) * b, s);
       CMOE_CUDA(cudaMemsetAsync(w.fail.p, 0, nc * sizeof(int), s));
-      lml_cov_kernel<<<dim3(t * (t + 1) / 2, 1, nc), kLmlCovThreads, smem_cov, s>>>(w.specs.p, w.noise.p, w.X.p, N,
-                                                                                  w.K.p);
-      count_launch();
-      CMOE_CUDA(cudaGetLastError());
-      potrf_batched(w.K.p, n, nc, w.fail.p, w.stage, s);
-      lml_solve_kernel<<<nc, kLmlSolveThreads, smem_solve, s>>>(w.K.p, n, w.r.p, w.fail.p, w.values.p,
-                                                                grads ? w.a.p : nullptr);
-      count_launch();
-      CMOE_CUDA(cudaGetLastError());
+      lml_stages(w, N, dim, g, kernel, nc, grads != nullptr, exact, s);
       if (!grads) {
         w.values.download(values + c0, nc, s);
         CMOE_CUDA(cudaStreamSynchronize(s));
         continue;
       }
-      tri_inv_diag_kernel<<<dim3(t, 1, nc), NB, smem_diag, s>>>(w.K.p, n, w.fail.p, w.Linv.p);
-      for (int bi = 1; bi < t; ++bi)
-        tri_inv_offdiag_kernel<<<dim3(bi, 1, nc), kInvThreads, smem_inv, s>>>(w.K.p, n, bi, w.fail.p, w.Linv.p);
-      inv_syrk_kernel<<<dim3(t * (t + 1) / 2, 1, nc), kInvThreads, smem_inv, s>>>(w.Linv.p, n, w.fail.p, w.K.p);
-      lml_grad_contract_kernel<<<dim3(nctas, 1, nc), kHgTx * kHgTy, 0, s>>>(w.specs.p, w.X.p, N, gx, w.a.p, w.K.p,
-                                                                           w.fail.p, w.partial.p);
-      lml_grad_reduce_kernel<<<nc, ((nh + 31) / 32) * 32, 0, s>>>(w.values.p, w.partial.p, nctas, w.a.p, w.K.p, n,
-                                                                  dim + 1, b, w.fail.p, w.gout.p);
-      count_launch(t + 3);
-      CMOE_CUDA(cudaGetLastError());
       w.gout.download(hout.data(), static_cast<size_t>(nc) * (1 + nh), s);
       CMOE_CUDA(cudaStreamSynchronize(s));
       for (int k = 0; k < nc; ++k) {
@@ -685,7 +789,7 @@ extern "C" int cmoe_log_marginal_likelihood_list(int kernel, const double* hyper
                                                  int num_sampled, int device, double* values, int* info) {
   return guarded(info, [&] {
     lml_list(kernel, hyperparameters, num_sets, points_sampled, points_sampled_value, derivatives, num_derivatives,
-             dim, num_sampled, device, values, nullptr);
+             dim, num_sampled, device, values, nullptr, false);
   });
 }
 
@@ -697,7 +801,20 @@ extern "C" int cmoe_grad_log_marginal_likelihood_list(int kernel, const double* 
   return guarded(info, [&] {
     CMOE_REQUIRE(grads != nullptr, CMOE_ERR_INVALID_VALUE, "NULL argument");
     lml_list(kernel, hyperparameters, num_sets, points_sampled, points_sampled_value, derivatives, num_derivatives,
-             dim, num_sampled, device, values, grads);
+             dim, num_sampled, device, values, grads, false);
+  });
+}
+
+extern "C" int cmoe_grad_log_marginal_likelihood_list_exact(int kernel, const double* hyperparameters, int num_sets,
+                                                            const double* points_sampled,
+                                                            const double* points_sampled_value,
+                                                            const int* derivatives, int num_derivatives, int dim,
+                                                            int num_sampled, int device, double* values, double* grads,
+                                                            int* info) {
+  return guarded(info, [&] {
+    CMOE_REQUIRE(grads != nullptr, CMOE_ERR_INVALID_VALUE, "NULL argument");
+    lml_list(kernel, hyperparameters, num_sets, points_sampled, points_sampled_value, derivatives, num_derivatives,
+             dim, num_sampled, device, values, grads, true);
   });
 }
 
@@ -752,6 +869,67 @@ __device__ __forceinline__ void hmc_draws(uint64_t seed, uint64_t step, int w, i
   partner = static_cast<int>(__umul64hi((static_cast<uint64_t>(d[0]) << 32) | d[1], static_cast<uint64_t>(Wh)));
 }
 
+// compute_log_likelihood's order (log_likelihood_mcmc.py:277-312) on q[nh] in place: the box (q untouched outside
+// it), with noisy == 0 the pinning of the noise entries to log(1e-8), then the prior into lp.  Returns whether the
+// likelihood is needed: false outside the box or where the prior is -inf.  With dlp != NULL, dlp[nh] receives d lp / d q
+// (zero for pinned entries and when the likelihood is skipped).  Shared by K12's proposals and K19's trial points.
+__device__ __forceinline__ bool hyper_box_prior(double* q, int nh, int dim, int b, int prior, int noisy, double& lp,
+                                                double* dlp) {
+  if (dlp)
+    for (int k = 0; k < nh; ++k) dlp[k] = 0.0;
+  bool inbox = true;
+  for (int k = 0; k < nh; ++k)
+    if (q[k] < -20.0 || q[k] > 20.0) inbox = false;
+  lp = 1.0;
+  if (inbox) {
+    if (!noisy)
+      for (int t = 0; t < b; ++t) q[1 + dim + t] = kLogNoiseFree;
+    if (prior == CMOE_HYPER_PRIOR_DEFAULT) {
+      // NormalPrior(0, 1).lnprob returns the pdf (base_prior.py:338-354); TophatPrior(-2, 3) over the lengths
+      // (:104-123); HorseshoePrior(0.1) per noise entry in order (:183-201)
+      lp = exp(-(q[0] * q[0]) / 2.0) / kSqrt2Pi;
+      if (dlp) dlp[0] = -q[0] * lp;
+      for (int k = 0; k < dim; ++k)
+        if (q[1 + k] < -2.0 || q[1 + k] > 3.0) lp = -INFINITY;
+      for (int t = 0; t < b; ++t) {
+        const double th = q[1 + dim + t];
+        const double r = 0.1 / th;
+        const double L = log(1.0 + 3.0 * (r * r));
+        lp += (th == 0.0) ? INFINITY : log(L);
+        // d/d th log(log(1 + 3 (0.1 / th)^2)) = -6 r^2 / (th (1 + 3 r^2) L), the term as written (not
+        // HorseshoePrior.gradient, which is in terms of exp(th))
+        if (dlp && noisy && th != 0.0) dlp[1 + dim + t] = -6.0 * (r * r) / (th * (1.0 + 3.0 * (r * r)) * L);
+      }
+    }
+  }
+  const bool need = inbox && lp != -INFINITY;
+  if (dlp && !need)
+    for (int k = 0; k < nh; ++k) dlp[k] = 0.0;
+  return need;
+}
+
+// The K10 inputs of one set at log-scale q as lml_list builds them on the host; a skipped set gets the finite
+// placeholder theta = 0 (its failure flag is preset, so the Cholesky skips it and lml_solve_kernel writes -inf).
+__device__ __forceinline__ void hyper_set_inputs(const double* q, bool skip, int kernel, int dim, int g,
+                                                 const int* derivs, KernelSpec& sp, double* noise) {
+  sp.kernel = kernel;
+  sp.dim = dim;
+  sp.g = g;
+  sp.alpha = exp(skip ? 0.0 : q[0]);
+  for (int k = 0; k < CMOE_MAX_DIM; ++k) {
+    double lsq = 1.0, il = 0.0;
+    if (k < dim) {
+      const double l = exp(skip ? 0.0 : q[1 + k]);
+      lsq = l * l;
+      il = 1.0 / l;
+    }
+    sp.lsq[k] = lsq;
+    sp.inv_len[k] = il;
+    sp.derivs[k] = derivs[k];
+  }
+  for (int t = 0; t < 1 + g; ++t) noise[t] = exp(skip ? 0.0 : q[1 + dim + t]) + 1.0e-6;
+}
+
 // Moving walker w = half * Wh + j.  With move == 0 the proposal is the walker itself (the initial evaluation).
 __global__ void __launch_bounds__(kHmcThreads) hmc_propose_kernel(const __grid_constant__ HmcArgs a, int half,
                                                                   int move) {
@@ -782,48 +960,10 @@ __global__ void __launch_bounds__(kHmcThreads) hmc_propose_kernel(const __grid_c
   } else {
     for (int k = 0; k < nh; ++k) q[k] = s[k];
   }
-  // compute_log_likelihood's order: the box (theta untouched outside it), the pinning, the prior
-  bool inbox = true;
-  for (int k = 0; k < nh; ++k)
-    if (q[k] < -20.0 || q[k] > 20.0) inbox = false;
-  double lp = 1.0;
-  if (inbox) {
-    if (!a.noisy)
-      for (int t = 0; t < b; ++t) q[1 + dim + t] = kLogNoiseFree;
-    if (a.prior == CMOE_HYPER_PRIOR_DEFAULT) {
-      // NormalPrior(0, 1).lnprob returns the pdf (base_prior.py:338-354); TophatPrior(-2, 3) over the lengths
-      // (:104-123); HorseshoePrior(0.1) per noise entry in order (:183-201)
-      lp = exp(-(q[0] * q[0]) / 2.0) / kSqrt2Pi;
-      for (int k = 0; k < dim; ++k)
-        if (q[1 + k] < -2.0 || q[1 + k] > 3.0) lp = -INFINITY;
-      for (int t = 0; t < b; ++t) {
-        const double th = q[1 + dim + t];
-        const double r = 0.1 / th;
-        lp += (th == 0.0) ? INFINITY : log(log(1.0 + 3.0 * (r * r)));
-      }
-    }
-  }
-  const bool skip = !inbox || lp == -INFINITY;
+  double lp;
+  const bool skip = !hyper_box_prior(q, nh, dim, b, a.prior, a.noisy, lp, nullptr);
   a.lprior[j] = skip ? -INFINITY : lp;
-  // the set's KernelSpec and noise as lml_list builds them on the host; a skipped proposal gets the finite placeholder
-  // theta = 0 and a preset failure flag, so the Cholesky skips it and lml_solve_kernel writes -inf
-  KernelSpec& sp = a.specs[j];
-  sp.kernel = a.kernel;
-  sp.dim = dim;
-  sp.g = a.g;
-  sp.alpha = exp(skip ? 0.0 : q[0]);
-  for (int k = 0; k < CMOE_MAX_DIM; ++k) {
-    double lsq = 1.0, il = 0.0;
-    if (k < dim) {
-      const double l = exp(skip ? 0.0 : q[1 + k]);
-      lsq = l * l;
-      il = 1.0 / l;
-    }
-    sp.lsq[k] = lsq;
-    sp.inv_len[k] = il;
-    sp.derivs[k] = a.derivs[k];
-  }
-  for (int t = 0; t < b; ++t) a.noise[static_cast<size_t>(j) * b + t] = exp(skip ? 0.0 : q[1 + dim + t]) + 1.0e-6;
+  hyper_set_inputs(q, skip, a.kernel, dim, a.g, a.derivs, a.specs[j], a.noise + static_cast<size_t>(j) * b);
   a.fail[j] = skip ? -1 : 0;
 }
 
@@ -898,12 +1038,7 @@ void hyper_mcmc(int kernel, int prior, int noisy, const double* initial_position
                    "table partner out of range [0, num_walkers / 2)");
   }
   require_device(device);
-  // y - m as lml_list centres it (gpp_model_selection.cpp:556-560)
-  double m = 0.0;
-  for (int i = 0; i < N; ++i) m += points_sampled_value[static_cast<size_t>(i) * b];
-  m /= N;
-  std::vector<double> rc(points_sampled_value, points_sampled_value + n);
-  for (int i = 0; i < N; ++i) rc[static_cast<size_t>(i) * b] -= m;
+  const std::vector<double> rc = centred_values(points_sampled_value, N, b);
 
   LmlWork& w = lml_workspace(device);
   cudaStream_t s = w.stream;
@@ -1001,5 +1136,493 @@ extern "C" int cmoe_hyperparameter_mcmc(int kernel, int prior, int noisy, const 
     hyper_mcmc(kernel, prior, noisy, initial_positions, num_walkers, num_steps, seed, first_step, table,
                points_sampled, points_sampled_value, derivatives, num_derivatives, dim, num_sampled, device, positions,
                log_probabilities);
+  });
+}
+
+// ---- hyper-parameter MAP fit (DESIGN.md K19) ------------------------------------------------------------------------
+// scipy's _minimize_bfgs with an analytic gradient on nll(theta) = -compute_log_likelihood(theta)
+// (log_likelihood_mcmc.py:241-312), every start in lock step.  One round evaluates one trial point of every active start:
+//   map_prep_kernel   one thread per start: the box, the pinning and the prior (hyper_box_prior) and the K10 inputs
+//   lml_stages        (K10/K11, the exact contraction) on all starts; finished or skipped starts have fail = -1
+//   map_step_kernel   one warp per start: the trial's value and gradient, one step of the strong-Wolfe line search
+//                     (scipy's scalar_search_wolfe2 and _zoom), and on acceptance the BFGS update of H and the next
+//                     direction
+// The host reads the number of active starts every kMapPoll rounds.  No sum crosses starts.
+namespace cmoe {
+namespace {
+
+constexpr int kMapWarps = 4;      // starts per CTA of map_step_kernel
+constexpr int kMapPoll = 4;       // rounds between reads of the active count
+constexpr int kMapLsIter = 10;    // bracketing steps and zoom trials of the line search
+constexpr int kMapMaxNh = 2 + 2 * CMOE_MAX_DIM;
+constexpr int kMapPer = (kMapMaxNh + 31) / 32;  // entries per lane
+constexpr double kMapC1 = 1.0e-4, kMapC2 = 0.9, kMapAmax = 1.0e100;
+
+enum MapPhase : int { kMapInit = 0, kMapBracket = 1, kMapZoom = 2, kMapDone = 3 };
+
+struct MapState {
+  double f, f_old;                 // objective at x, and at the previous iterate (old_old_fval)
+  double phi0, dphi0;              // the line search's phi(0) and phi'(0)
+  double at;                       // step of the pending trial
+  double alpha0, phi_a0, dphi_a0;  // bracketing: the previous step
+  double a_lo, a_hi, phi_lo, phi_hi, dphi_lo, a_rec, phi_rec;  // zoom
+  int phase, li, iters, evals, status;
+};
+
+struct MapArgs {
+  int S, nh, dim, g, kernel, prior, noisy, max_iter;
+  int derivs[CMOE_MAX_DIM];
+  double gtol;
+  MapState* st;
+  double* x;       // [S][nh] iterates
+  double* gr;      // [S][nh] their gradients
+  double* p;       // [S][nh] search directions
+  double* xt;      // [S][nh] pending trial points
+  double* q;       // [S][nh] the trial points after the pinning
+  double* dprior;  // [S][nh] d prior / d q
+  double* lprior;  // [S] prior, -inf when the likelihood is skipped
+  double* H;       // [S][nh][nh] inverse Hessian approximations, row-major
+  const double* out;  // [S][1 + nh] value and linear-space gradient of the likelihood (lml_grad_reduce_kernel)
+  KernelSpec* specs;
+  double* noise;
+  int* fail;
+  int* active;
+};
+
+__global__ void __launch_bounds__(kHmcThreads) map_prep_kernel(const __grid_constant__ MapArgs a) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s == 0) *a.active = 0;
+  if (s >= a.S) return;
+  const int nh = a.nh, b = 1 + a.g;
+  double* q = a.q + static_cast<size_t>(s) * nh;
+  const double* xt = a.xt + static_cast<size_t>(s) * nh;
+  for (int k = 0; k < nh; ++k) q[k] = xt[k];
+  double lp = 1.0;
+  bool need = false;
+  if (a.st[s].phase != kMapDone)
+    need = hyper_box_prior(q, nh, a.dim, b, a.prior, a.noisy, lp, a.dprior + static_cast<size_t>(s) * nh);
+  a.lprior[s] = need ? lp : -INFINITY;
+  hyper_set_inputs(q, !need, a.kernel, a.dim, a.g, a.derivs, a.specs[s], a.noise + static_cast<size_t>(s) * b);
+  a.fail[s] = need ? 0 : -1;
+}
+
+__device__ __forceinline__ double warp_sum(double v) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// scipy's _cubicmin / _quadmin: NaN where numpy would raise (a zero divisor, a negative radical) or the result is not
+// finite
+__device__ __forceinline__ double map_cubicmin(double a, double fa, double fpa, double b, double fb, double c, double fc) {
+  const double C = fpa, db = b - a, dc = c - a;
+  const double denom = (db * dc) * (db * dc) * (db - dc);
+  const double v0 = fb - fa - C * db, v1 = fc - fa - C * dc;
+  if (denom == 0.0 || !isfinite(denom)) return NAN;
+  const double A = (dc * dc * v0 - db * db * v1) / denom;
+  const double B = (-(dc * dc * dc) * v0 + db * db * db * v1) / denom;
+  const double radical = B * B - 3.0 * A * C;
+  if (A == 0.0 || !(radical >= 0.0)) return NAN;
+  const double xmin = a + (-B + sqrt(radical)) / (3.0 * A);
+  return isfinite(xmin) ? xmin : NAN;
+}
+
+__device__ __forceinline__ double map_quadmin(double a, double fa, double fpa, double b, double fb) {
+  const double db = b - a;
+  if (db * db == 0.0) return NAN;
+  const double B = (fb - fa - fpa * db) / (db * db);
+  if (B == 0.0) return NAN;
+  const double xmin = a - fpa / (2.0 * B);
+  return isfinite(xmin) ? xmin : NAN;
+}
+
+// _zoom's next trial step (trial i of this zoom)
+__device__ __forceinline__ double map_zoom_trial(const MapState& t, int i) {
+  const double dalpha = t.a_hi - t.a_lo;
+  const double lo = dalpha < 0 ? t.a_hi : t.a_lo, hi = dalpha < 0 ? t.a_lo : t.a_hi;
+  double aj = NAN;
+  if (i > 0) {
+    const double cchk = 0.2 * dalpha;
+    aj = map_cubicmin(t.a_lo, t.phi_lo, t.dphi_lo, t.a_hi, t.phi_hi, t.a_rec, t.phi_rec);
+    if (isnan(aj) || aj > hi - cchk || aj < lo + cchk) aj = NAN;
+  }
+  if (isnan(aj)) {
+    const double qchk = 0.1 * dalpha;
+    aj = map_quadmin(t.a_lo, t.phi_lo, t.dphi_lo, t.a_hi, t.phi_hi);
+    if (isnan(aj) || aj > hi - qchk || aj < lo + qchk) aj = t.a_lo + 0.5 * dalpha;
+  }
+  return aj;
+}
+
+// The line search's decision at a trial with value ft and slope dphi (scalar_search_wolfe2's loop body in the bracket
+// phase, _zoom's in the zoom phase; a +inf or NaN trial fails sufficient decrease).  Returns 1 to accept the trial, -1
+// when the line search fails, 0 with t.at = the next trial.
+__device__ __forceinline__ int map_line_search(MapState& t, double ft, double dphi) {
+  if (t.phase == kMapBracket) {
+    const double a1 = t.at;
+    if (t.li >= kMapLsIter) return 1;  // the loop ran out: scipy takes alpha1 untested
+    if (!(ft <= t.phi0 + kMapC1 * a1 * t.dphi0) || (t.li > 0 && ft >= t.phi_a0)) {
+      t.a_lo = t.alpha0; t.a_hi = a1; t.phi_lo = t.phi_a0; t.phi_hi = ft; t.dphi_lo = t.dphi_a0;
+    } else if (fabs(dphi) <= -kMapC2 * t.dphi0) {
+      return 1;
+    } else if (dphi >= 0.0) {
+      t.a_lo = a1; t.a_hi = t.alpha0; t.phi_lo = ft; t.phi_hi = t.phi_a0; t.dphi_lo = dphi;
+    } else {
+      t.alpha0 = a1;
+      t.at = fmin(2.0 * a1, kMapAmax);
+      t.phi_a0 = ft;
+      t.dphi_a0 = dphi;
+      t.li += 1;
+      return t.alpha0 > kMapAmax ? -1 : 0;
+    }
+    t.phase = kMapZoom;
+    t.phi_rec = t.phi0;
+    t.a_rec = 0.0;
+    t.li = 0;
+    t.at = map_zoom_trial(t, 0);
+    return 0;
+  }
+  const double aj = t.at;
+  if (!(ft <= t.phi0 + kMapC1 * aj * t.dphi0) || ft >= t.phi_lo) {
+    t.phi_rec = t.phi_hi; t.a_rec = t.a_hi; t.a_hi = aj; t.phi_hi = ft;
+  } else if (fabs(dphi) <= -kMapC2 * t.dphi0) {
+    return 1;
+  } else {
+    if (dphi * (t.a_hi - t.a_lo) >= 0.0) {
+      t.phi_rec = t.phi_hi; t.a_rec = t.a_hi; t.a_hi = t.a_lo; t.phi_hi = t.phi_lo;
+    } else {
+      t.phi_rec = t.phi_lo; t.a_rec = t.a_lo;
+    }
+    t.a_lo = aj; t.phi_lo = ft; t.dphi_lo = dphi;
+  }
+  t.li += 1;
+  if (t.li >= kMapLsIter) return -1;
+  t.at = map_zoom_trial(t, t.li);
+  return 0;
+}
+
+// One warp per start; lane l owns entries l + 32 m.  The scalar state is in shared memory and only lane 0 changes it
+// (no scalar then has to stay in a register across the divisions' slow-path calls); the vector work and the fixed-order
+// warp reductions are shared by all lanes, with __syncwarp between the two.
+__global__ void __launch_bounds__(kMapWarps * 32) map_step_kernel(const __grid_constant__ MapArgs a) {
+  __shared__ double sh_s[kMapWarps][kMapMaxNh], sh_v[kMapWarps][kMapMaxNh];
+  __shared__ MapState sh_t[kMapWarps];
+  __shared__ int sh_act[kMapWarps];  // 1 accept, -1 fail, 0 next trial; then 1 = start a line search
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int s = blockIdx.x * kMapWarps + warp;
+  if (s >= a.S) return;
+  MapState& t = sh_t[warp];
+  if (lane == 0) t = a.st[s];
+  __syncwarp();
+  if (t.phase == kMapDone) return;
+  const bool first = t.phase == kMapInit;
+  const int nh = a.nh, dim = a.dim;
+  const size_t off = static_cast<size_t>(s) * nh;
+  double* x = a.x + off;
+  double* gr = a.gr + off;
+  double* p = a.p + off;
+  double* xt = a.xt + off;
+  const double* q = a.q + off;
+  const double* dp = a.dprior + off;
+  const double* o = a.out + static_cast<size_t>(s) * (1 + nh);
+  double* ss = sh_s[warp];
+  double* sv = sh_v[warp];
+
+  // the trial's nll and gradient: f = -(prior + log p), g_k = -(d prior / d q_k + e^{q_k} d log p / d theta_k), with 0
+  // for pinned noise entries; the preset failure flag leaves o[0] = -inf and a zero gradient for a skipped trial
+  const double lp = a.lprior[s];
+  const double ft = -(lp + o[0]);
+  double gt[kMapPer];
+  double dphi = 0.0;
+#pragma unroll
+  for (int m = 0; m < kMapPer; ++m) {
+    const int k = lane + 32 * m;
+    double v = 0.0;
+    if (k < nh && lp != -INFINITY && !(a.noisy == 0 && k > dim)) v = -(dp[k] + exp(q[k]) * o[1 + k]);
+    gt[m] = v;
+    if (k < nh) dphi = fma(v, p[k], dphi);
+  }
+  dphi = warp_sum(dphi);
+  __syncwarp();  // every lane has read t before lane 0 changes it
+  if (lane == 0) {
+    t.evals += 1;
+    int act = 1;
+    if (!first) act = map_line_search(t, ft, dphi);
+    if (act < 0) {
+      t.status = 2;  // scipy's _LineSearchError: warnflag 2, x stays at the last iterate
+      t.phase = kMapDone;
+    }
+    sh_act[warp] = act;
+  }
+  __syncwarp();
+
+  if (sh_act[warp] == 1) {
+    // accept: s = alpha p, y = g_t - g; x = the evaluated trial, g = g_t
+    double ys = 0.0, gsq = 0.0, gmax = 0.0;
+    bool nan = false;
+#pragma unroll
+    for (int m = 0; m < kMapPer; ++m) {
+      const int k = lane + 32 * m;
+      if (k >= nh) continue;
+      if (!first) {
+        const double sk = __dmul_rn(t.at, p[k]);
+        ys = fma(gt[m] - gr[k], sk, ys);
+        ss[k] = sk;
+        sv[k] = gt[m] - gr[k];
+      }
+      x[k] = xt[k];
+      gr[k] = gt[m];
+      gsq = fma(gt[m], gt[m], gsq);
+      gmax = fmax(gmax, fabs(gt[m]));
+      nan = nan || isnan(gt[m]) || isnan(xt[k]);
+    }
+    ys = warp_sum(ys);
+    gsq = warp_sum(gsq);
+    for (int o2 = 16; o2 > 0; o2 >>= 1) gmax = fmax(gmax, __shfl_xor_sync(0xffffffffu, gmax, o2));
+    nan = __any_sync(0xffffffffu, nan) || isnan(ft);
+    __syncwarp();
+    if (lane == 0) {
+      const bool finite_t = isfinite(ft);
+      t.f_old = first ? ft + sqrt(gsq) / 2.0 : t.f;
+      t.f = ft;
+      if (!first) t.iters += 1;
+      int st = -1;
+      if (first && !finite_t) {
+        st = 2;  // the start itself is outside the box, under a -inf prior or singular
+      } else if (!nan && gmax <= a.gtol) {
+        st = 0;
+      } else if (!finite_t) {
+        st = 2;
+      } else if (t.iters >= a.max_iter) {
+        st = 1;
+      } else if (nan) {
+        st = 3;
+      }
+      t.status = st;
+      if (st >= 0) t.phase = kMapDone;
+    }
+    __syncwarp();
+    if (t.phase != kMapDone) {
+      const double* H0 = a.H + static_cast<size_t>(s) * nh * nh;
+      if (!first) {
+        // H <- (I - rho s y^T) H (I - rho y s^T) + rho s s^T, rho = 1 / y^T s (1000 when y^T s == 0), expanded:
+        // H - rho s (y^T H) - rho (H y) s^T + (rho^2 y^T H y + rho) s s^T
+        double* H = a.H + static_cast<size_t>(s) * nh * nh;
+        const double rho = ys == 0.0 ? 1000.0 : 1.0 / ys;
+        double hy[kMapPer], yh[kMapPer], yhy = 0.0;
+#pragma unroll
+        for (int m = 0; m < kMapPer; ++m) {
+          const int k = lane + 32 * m;
+          double r = 0.0, c = 0.0;
+          if (k < nh)
+            for (int jj = 0; jj < nh; ++jj) {
+              r = fma(H[static_cast<size_t>(k) * nh + jj], sv[jj], r);
+              c = fma(sv[jj], H[static_cast<size_t>(jj) * nh + k], c);
+            }
+          hy[m] = r;
+          yh[m] = c;
+          if (k < nh) yhy = fma(sv[k], r, yhy);
+        }
+        yhy = warp_sum(yhy);
+        __syncwarp();
+#pragma unroll
+        for (int m = 0; m < kMapPer; ++m) {
+          const int k = lane + 32 * m;
+          if (k < nh) sv[k] = yh[m];  // sv <- y^T H
+        }
+        __syncwarp();
+        const double css = rho * rho * yhy + rho;
+#pragma unroll
+        for (int m = 0; m < kMapPer; ++m) {
+          const int k = lane + 32 * m;
+          if (k >= nh) continue;
+          const double sk = ss[k];
+          for (int jj = 0; jj < nh; ++jj) {
+            double& h = H[static_cast<size_t>(k) * nh + jj];
+            h = h - rho * sk * sv[jj] - rho * hy[m] * ss[jj] + css * sk * ss[jj];
+          }
+        }
+        __syncwarp();
+      }
+      // p = -H g, then scalar_search_wolfe2's start
+#pragma unroll
+      for (int m = 0; m < kMapPer; ++m) {
+        const int k = lane + 32 * m;
+        if (k < nh) sv[k] = gr[k];
+      }
+      __syncwarp();
+      double d0 = 0.0;
+#pragma unroll
+      for (int m = 0; m < kMapPer; ++m) {
+        const int k = lane + 32 * m;
+        if (k >= nh) continue;
+        double r = 0.0;
+        for (int jj = 0; jj < nh; ++jj) r = fma(H0[static_cast<size_t>(k) * nh + jj], sv[jj], r);
+        p[k] = -r;
+        d0 = fma(sv[k], -r, d0);
+      }
+      d0 = warp_sum(d0);
+      __syncwarp();
+      if (lane == 0) {
+        t.phi0 = t.f;
+        t.dphi0 = d0;
+        double a1 = 1.0;
+        if (d0 != 0.0) a1 = fmin(1.0, 1.01 * 2.0 * (t.phi0 - t.f_old) / d0);
+        if (a1 < 0.0) a1 = 1.0;
+        t.at = fmin(a1, kMapAmax);
+        t.alpha0 = 0.0;
+        t.phi_a0 = t.phi0;
+        t.dphi_a0 = d0;
+        t.li = 0;
+        t.phase = kMapBracket;
+        if (t.at == 0.0) {
+          t.status = 2;  // "Rounding errors prevent the line search from converging"
+          t.phase = kMapDone;
+        }
+      }
+      __syncwarp();
+    }
+  }
+  if (t.phase != kMapDone) {
+    // the next trial x + at p, with the product rounded first as scipy's s = alpha p
+#pragma unroll
+    for (int m = 0; m < kMapPer; ++m) {
+      const int k = lane + 32 * m;
+      if (k < nh) xt[k] = __dadd_rn(x[k], __dmul_rn(t.at, p[k]));
+    }
+    if (lane == 0) atomicAdd(a.active, 1);
+  }
+  __syncwarp();
+  if (lane == 0) a.st[s] = t;
+}
+
+__global__ void map_init_kernel(const __grid_constant__ MapArgs a) {
+  const size_t e = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const size_t nh = a.nh;
+  if (e >= static_cast<size_t>(a.S) * nh * nh) return;
+  const size_t r = e % (nh * nh);
+  a.H[e] = (r / nh == r % nh) ? 1.0 : 0.0;
+}
+
+void hyper_map(int kernel, int prior, int noisy, const double* starts, int num_starts, const cmoe_map_opts* opts,
+               const double* points_sampled, const double* points_sampled_value, const int* derivatives,
+               int num_derivatives, int dim, int num_sampled, int device, double* positions, double* values,
+               double* gradients, int* iterations, int* evaluations, int* status) {
+  CMOE_REQUIRE(starts != nullptr && positions != nullptr && values != nullptr && gradients != nullptr &&
+                   iterations != nullptr && evaluations != nullptr && status != nullptr,
+               CMOE_ERR_INVALID_VALUE, "NULL argument");
+  check_lml_problem(kernel, points_sampled, points_sampled_value, derivatives, num_derivatives, dim, num_sampled);
+  CMOE_REQUIRE(prior == CMOE_HYPER_PRIOR_NONE || prior == CMOE_HYPER_PRIOR_DEFAULT, CMOE_ERR_INVALID_VALUE,
+               "prior must be CMOE_HYPER_PRIOR_NONE or CMOE_HYPER_PRIOR_DEFAULT");
+  CMOE_REQUIRE(noisy == 0 || noisy == 1, CMOE_ERR_INVALID_VALUE, "noisy must be 0 or 1");
+  const int g = num_derivatives, b = 1 + g, nh = 2 + dim + g, N = num_sampled, S = num_starts;
+  double gtol = 1.0e-5;
+  int max_iter = 200 * nh;
+  if (opts) {
+    CMOE_REQUIRE(opts->gtol >= 0.0, CMOE_ERR_INVALID_VALUE, "gtol must be >= 0");
+    CMOE_REQUIRE(opts->max_iterations >= 0, CMOE_ERR_INVALID_VALUE, "max_iterations must be >= 0 (0: 200 nh)");
+    gtol = opts->gtol;
+    if (opts->max_iterations > 0) max_iter = opts->max_iterations;
+  }
+  CMOE_REQUIRE(S >= 1, CMOE_ERR_BOUNDS, "num_starts must be >= 1");
+  // every start is one set of a K11 chunk, with its BFGS state beside it
+  const size_t per_set = lml_grad_set_bytes(N, dim, g) + sizeof(MapState) +
+                         sizeof(double) * (static_cast<size_t>(nh) * nh + 6 * static_cast<size_t>(nh) + 1);
+  const size_t chunk = chunk_items(kMaxChunkSets, kSampleWorkspaceBytes, per_set);
+  CMOE_REQUIRE(static_cast<size_t>(S) <= chunk, CMOE_ERR_BOUNDS,
+               "num_starts = " + std::to_string(S) + " exceeds one likelihood chunk (" + std::to_string(chunk) +
+                   " sets at n = " + std::to_string(N * b) + ")");
+  require_device(device);
+
+  LmlWork& w = lml_workspace(device);
+  cudaStream_t s = w.stream;
+  lml_prepare(w, points_sampled, points_sampled_value, N, dim, g, S, true, s);
+  const size_t v = static_cast<size_t>(S) * nh;
+  DevBuf<MapState> st(S);
+  DevBuf<double> x, gr(v), p(v), xt, q(v), dprior(v), lprior(S), H(v * nh);
+  DevBuf<int> active(1);
+  x.upload(starts, v, s);
+  xt.upload(starts, v, s);
+  std::vector<MapState> h0(S);
+  for (MapState& m : h0) {
+    m = MapState{};
+    m.phase = kMapInit;
+    m.status = -1;
+  }
+  st.upload(h0.data(), S, s);
+  MapArgs a{};
+  a.S = S;
+  a.nh = nh;
+  a.dim = dim;
+  a.g = g;
+  a.kernel = kernel;
+  a.prior = prior;
+  a.noisy = noisy;
+  a.max_iter = max_iter;
+  for (int k = 0; k < g; ++k) a.derivs[k] = derivatives[k];
+  a.gtol = gtol;
+  a.st = st.p;
+  a.x = x.p;
+  a.gr = gr.p;
+  a.p = p.p;
+  a.xt = xt.p;
+  a.q = q.p;
+  a.dprior = dprior.p;
+  a.lprior = lprior.p;
+  a.H = H.p;
+  a.out = w.gout.p;
+  a.specs = w.specs.p;
+  a.noise = w.noise.p;
+  a.fail = w.fail.p;
+  a.active = active.p;
+  map_init_kernel<<<static_cast<unsigned>((v * nh + 255) / 256), 256, 0, s>>>(a);
+  p.zero(s);
+  count_launch();
+  // a start makes at most 1 + 2 kMapLsIter evaluations per iteration
+  const long long max_rounds = 1 + static_cast<long long>(max_iter) * (2 * kMapLsIter + 1);
+  const unsigned prep_blocks = static_cast<unsigned>((S + kHmcThreads - 1) / kHmcThreads);
+  const unsigned step_blocks = static_cast<unsigned>((S + kMapWarps - 1) / kMapWarps);
+  int* h_active = nullptr;
+  CMOE_CUDA(cudaMallocHost(reinterpret_cast<void**>(&h_active), sizeof(int)));
+  std::unique_ptr<int, cudaError_t (*)(void*)> keep(h_active, cudaFreeHost);
+  for (long long round = 0; round < max_rounds; ++round) {
+    map_prep_kernel<<<prep_blocks, kHmcThreads, 0, s>>>(a);
+    count_launch();
+    CMOE_CUDA(cudaGetLastError());
+    lml_stages(w, N, dim, g, kernel, S, true, true, s);
+    map_step_kernel<<<step_blocks, kMapWarps * 32, 0, s>>>(a);
+    count_launch();
+    CMOE_CUDA(cudaGetLastError());
+    if ((round + 1) % kMapPoll == 0 || round + 1 == max_rounds) {
+      CMOE_CUDA(cudaMemcpyAsync(h_active, active.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+      CMOE_CUDA(cudaStreamSynchronize(s));
+      if (*h_active == 0) break;
+    }
+  }
+  std::vector<MapState> hs(S);
+  st.download(hs.data(), S, s);
+  x.download(positions, v, s);
+  gr.download(gradients, v, s);
+  CMOE_CUDA(cudaStreamSynchronize(s));
+  for (int k = 0; k < S; ++k) {
+    values[k] = hs[k].f;
+    iterations[k] = hs[k].iters;
+    evaluations[k] = hs[k].evals;
+    status[k] = hs[k].status < 0 ? 1 : hs[k].status;
+  }
+}
+
+}  // namespace
+}  // namespace cmoe
+
+extern "C" int cmoe_hyperparameter_map(int kernel, int prior, int noisy, const double* starts, int num_starts,
+                                       const cmoe_map_opts* opts, const double* points_sampled,
+                                       const double* points_sampled_value, const int* derivatives,
+                                       int num_derivatives, int dim, int num_sampled, int device, double* positions,
+                                       double* values, double* gradients, int* iterations, int* evaluations,
+                                       int* status, int* info) {
+  return guarded(info, [&] {
+    hyper_map(kernel, prior, noisy, starts, num_starts, opts, points_sampled, points_sampled_value, derivatives,
+              num_derivatives, dim, num_sampled, device, positions, values, gradients, iterations, evaluations,
+              status);
   });
 }

@@ -126,6 +126,15 @@ int cmoe_grad_log_marginal_likelihood_list(int kernel, const double* hyperparame
                                            const double* points_sampled, const double* points_sampled_value,
                                            const int* derivatives, int num_derivatives, int dim, int num_sampled,
                                            int device, double* values, double* grads, int* info);
+/* The exact hyper-parameter gradient: cmoe_grad_log_marginal_likelihood_list's signature, layout, checks and values,
+ * with grads the true d log p / d (alpha, lengths..., noise by observation type).  For Matern-5/2 with derivative
+ * observations every entry of each (1 + g) x (1 + g) derivative block contributes, coincident points included, where
+ * the quirk-keeping call uses the value-value entry only.  With g = 0, and for SquareExponential (whose branch is exact),
+ * the results equal cmoe_grad_log_marginal_likelihood_list's bit for bit. */
+int cmoe_grad_log_marginal_likelihood_list_exact(int kernel, const double* hyperparameters, int num_sets,
+                                                 const double* points_sampled, const double* points_sampled_value,
+                                                 const int* derivatives, int num_derivatives, int dim, int num_sampled,
+                                                 int device, double* values, double* grads, int* info);
 /* Maximum-likelihood fit of the hyper-parameters by restarted gradient ascent from every one of num_starts starts
  * [num_starts][nh], nh = 2 + dim + g, on the linear-space box bounds[nh][2]: MultistartGradientDescentHyperparameter-
  * Optimization (gpp_model_selection.hpp:1063-1103) with one thread, every start descending in lock step with one
@@ -168,6 +177,33 @@ int cmoe_hyperparameter_mcmc(int kernel, int prior, int noisy, const double* ini
                              const double* points_sampled, const double* points_sampled_value, const int* derivatives,
                              int num_derivatives, int dim, int num_sampled, int device, double* positions,
                              double* log_probabilities, int* info);
+/* Options of cmoe_hyperparameter_map; NULL gives the defaults. */
+typedef struct cmoe_map_opts {
+  double gtol;         /* stop at ||gradient||_inf <= gtol (scipy's default 1e-5); >= 0 */
+  int max_iterations;  /* BFGS iterations per start; 0 = 200 nh (scipy's default) */
+} cmoe_map_opts;
+/* Hyper-parameter MAP fit (DESIGN.md K19): GaussianProcessLogLikelihoodMCMC.optimize (log_likelihood_mcmc.py:241-275),
+ * scipy.optimize.minimize(nll, p0) with BFGS, from every one of num_starts starts[num_starts][nh] in one call, with the
+ * analytic gradient instead of finite differences.  theta = (log alpha, log l_1..l_dim, log noise_0..noise_g), nh =
+ * 2 + dim + g, and nll(theta) = -compute_log_likelihood(theta): +inf outside [-20, 20]^nh; with noisy == 0 the noise
+ * entries of a copy of theta are log(1e-8) (their gradient entries are 0 and positions keep the start's values); then
+ * minus (the prior, CMOE_HYPER_PRIOR_NONE = 1 or CMOE_HYPER_PRIOR_DEFAULT, plus the value of
+ * cmoe_log_marginal_likelihood_list at exp(theta)).  The likelihood gradient is the exact one of
+ * cmoe_grad_log_marginal_likelihood_list_exact.  BFGS as scipy's _minimize_bfgs (H0 = I, the first step from
+ * old_old_fval = f + ||g||_2 / 2, rho = 1000 when y^T s == 0) with scipy's strong-Wolfe line_search_wolfe2 (c1 = 1e-4,
+ * c2 = 0.9, 10 bracketing steps, at most 10 zoom trials; a +inf or NaN trial fails sufficient decrease).
+ * Outputs per start: positions[num_starts][nh], values[num_starts] = nll there, gradients[num_starts][nh],
+ * iterations, evaluations (value-and-gradient evaluations, the start's included) and status: 0 converged
+ * (||g||_inf <= gtol), 1 max_iterations, 2 line search failed or objective not finite (scipy's warnflag 2; a start
+ * outside the box gives value +inf), 3 NaN.  A start's results do not depend on the other starts.
+ * Bounds (CMOE_ERR_BOUNDS, before any device work): the K10 size contract (dim <= CMOE_MAX_DIM, so nh <= 2 + 2
+ * CMOE_MAX_DIM; num_sampled (1 + g) <= 8192), num_starts >= 1 and all starts within one K11 chunk (4096 sets and about
+ * 2 GiB).  NULL pointers, a kernel, prior or noisy value outside the defined ones and bad opts: CMOE_ERR_INVALID_VALUE. */
+int cmoe_hyperparameter_map(int kernel, int prior, int noisy, const double* starts, int num_starts,
+                            const cmoe_map_opts* opts, const double* points_sampled,
+                            const double* points_sampled_value, const int* derivatives, int num_derivatives,
+                            int dim, int num_sampled, int device, double* positions, double* values,
+                            double* gradients, int* iterations, int* evaluations, int* status, int* info);
 /* Run-time switches between kernel generations (also read once from the environment: CMOE_LEGACY_LINALG, CMOE_COV_TMA):
  *   "legacy_linalg" 1 = round-1 launch-per-step Cholesky / chained trsv for large n (default 0: cooperative kernels);
  *   "cov_tma"       1 = TMA / DMMA covariance build with tensor-map tile stores (default 0: LDGSTS kernel, faster at d ~ 10);
