@@ -575,39 +575,33 @@ def log_marginal_likelihood(kernel, alpha, lengths, X, y, noise, derivs=None, de
     return val.value
 
 
-def log_marginal_likelihood_list(kernel, hypers, X, y, derivs=None, device=0):
-    """cmoe_log_marginal_likelihood_list (EvaluateLogLikelihoodAtPointList, gpp_model_selection.hpp:1274-1308): the
-    log marginal likelihood at every row of ``hypers`` [num_sets, 2 + dim + g] = (alpha, lengths..., noise by
-    observation type) in one device call.  Returns a [num_sets] array; a set whose Cholesky fails is -inf."""
+def _lml_list(entry, grads, kernel, hypers, X, y, derivs, device):
+    """One of the cmoe_*log_marginal_likelihood_list calls: values [num_sets], and with ``grads`` also the gradients
+    [num_sets, 2 + dim + g]."""
     X = _f64(X)
     N, dim = X.shape
     derivs = _i32(derivs)
     H = _f64(hypers).reshape(-1, 2 + dim + derivs.size)
-    values = np.empty(H.shape[0])
+    out = (np.empty(H.shape[0]), np.empty(H.shape)) if grads else (np.empty(H.shape[0]),)
     info = ctypes.c_int()
-    rc = lib().cmoe_log_marginal_likelihood_list(int(kernel), _d(H), H.shape[0], _d(X), _d(_f64(y).ravel()),
-                                                 _i(derivs), derivs.size, dim, N, int(device), _d(values),
-                                                 ctypes.byref(info))
+    rc = getattr(lib(), entry)(int(kernel), _d(H), H.shape[0], _d(X), _d(_f64(y).ravel()), _i(derivs), derivs.size,
+                               dim, N, int(device), *(_d(o) for o in out), ctypes.byref(info))
     _check(rc, info.value)
-    return values
+    return out if grads else out[0]
+
+
+def log_marginal_likelihood_list(kernel, hypers, X, y, derivs=None, device=0):
+    """cmoe_log_marginal_likelihood_list (EvaluateLogLikelihoodAtPointList, gpp_model_selection.hpp:1274-1308): the
+    log marginal likelihood at every row of ``hypers`` [num_sets, 2 + dim + g] = (alpha, lengths..., noise by
+    observation type) in one device call.  Returns a [num_sets] array; a set whose Cholesky fails is -inf."""
+    return _lml_list("cmoe_log_marginal_likelihood_list", False, kernel, hypers, X, y, derivs, device)
 
 
 def grad_log_marginal_likelihood_list(kernel, hypers, X, y, derivs=None, device=0):
     """cmoe_grad_log_marginal_likelihood_list: (values [num_sets], grads [num_sets, 2 + dim + g]) at every row of
     ``hypers`` (the layout of log_marginal_likelihood_list) in one device call.  The values equal
     log_marginal_likelihood_list's bit for bit; a set whose Cholesky fails gets -inf and a zero gradient."""
-    X = _f64(X)
-    N, dim = X.shape
-    derivs = _i32(derivs)
-    H = _f64(hypers).reshape(-1, 2 + dim + derivs.size)
-    values = np.empty(H.shape[0])
-    grads = np.empty(H.shape)
-    info = ctypes.c_int()
-    rc = lib().cmoe_grad_log_marginal_likelihood_list(int(kernel), _d(H), H.shape[0], _d(X), _d(_f64(y).ravel()),
-                                                      _i(derivs), derivs.size, dim, N, int(device), _d(values),
-                                                      _d(grads), ctypes.byref(info))
-    _check(rc, info.value)
-    return values, grads
+    return _lml_list("cmoe_grad_log_marginal_likelihood_list", True, kernel, hypers, X, y, derivs, device)
 
 
 def hyperparameter_gradient_descent(kernel, gd, bounds, starts, X, y, derivs=None, device=0):
@@ -636,18 +630,7 @@ def hyperparameter_gradient_descent(kernel, gd, bounds, starts, X, y, derivs=Non
 def grad_log_marginal_likelihood_list_exact(kernel, hypers, X, y, derivs=None, device=0):
     """cmoe_grad_log_marginal_likelihood_list_exact: grad_log_marginal_likelihood_list with the exact gradient (every
     entry of a Matern-5/2 derivative block contributes).  Equal to it bit for bit with g = 0 and for SE."""
-    X = _f64(X)
-    N, dim = X.shape
-    derivs = _i32(derivs)
-    H = _f64(hypers).reshape(-1, 2 + dim + derivs.size)
-    values = np.empty(H.shape[0])
-    grads = np.empty(H.shape)
-    info = ctypes.c_int()
-    rc = lib().cmoe_grad_log_marginal_likelihood_list_exact(int(kernel), _d(H), H.shape[0], _d(X), _d(_f64(y).ravel()),
-                                                            _i(derivs), derivs.size, dim, N, int(device), _d(values),
-                                                            _d(grads), ctypes.byref(info))
-    _check(rc, info.value)
-    return values, grads
+    return _lml_list("cmoe_grad_log_marginal_likelihood_list_exact", True, kernel, hypers, X, y, derivs, device)
 
 
 class MapOpts(ctypes.Structure):

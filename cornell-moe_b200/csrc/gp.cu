@@ -100,6 +100,24 @@ void require_device(int device) {
   CMOE_CUDA(cudaSetDevice(device));
 }
 
+void fill_kernel_spec(KernelSpec& s, int kernel, int dim, int g, const int* derivs, double alpha,
+                      const double* lengths) {
+  s = KernelSpec{};
+  s.kernel = kernel;
+  s.dim = dim;
+  s.g = g;
+  s.alpha = alpha;
+  for (int k = 0; k < CMOE_MAX_DIM; ++k) {
+    s.lsq[k] = 1.0;
+    s.inv_len[k] = 0.0;
+  }
+  for (int k = 0; k < dim; ++k) {
+    s.lsq[k] = lengths[k] * lengths[k];
+    s.inv_len[k] = 1.0 / lengths[k];
+  }
+  for (int k = 0; k < g; ++k) s.derivs[k] = derivs[k];
+}
+
 void fit_gp(cmoe_gp* gp, bool mean_change) {
   drop_cached_plan(gp);  // the cached workspace refers to the previous training set
   ++gp->generation;
@@ -303,21 +321,7 @@ int cmoe_gp_create(int kernel, double alpha, const double* lengths, const double
     require_device(device);
     std::unique_ptr<cmoe_gp> gp(new cmoe_gp());
     gp->device = device;
-    KernelSpec& s = gp->spec;
-    s.kernel = kernel;
-    s.dim = dim;
-    s.g = num_derivatives;
-    s.alpha = alpha;
-    for (int k = 0; k < CMOE_MAX_DIM; ++k) {
-      s.lsq[k] = 1.0;
-      s.inv_len[k] = 0.0;
-      s.derivs[k] = 0;
-    }
-    for (int k = 0; k < dim; ++k) {
-      s.lsq[k] = lengths[k] * lengths[k];
-      s.inv_len[k] = 1.0 / lengths[k];
-    }
-    for (int k = 0; k < num_derivatives; ++k) s.derivs[k] = derivatives[k];
+    fill_kernel_spec(gp->spec, kernel, dim, num_derivatives, derivatives, alpha, lengths);
     gp->N = num_sampled;
     gp->hX.assign(points_sampled, points_sampled + static_cast<size_t>(num_sampled) * dim);
     gp->hy.assign(points_sampled_value,

@@ -917,12 +917,42 @@ py::list evaluate_EI_mcmc_at_point_list(const GaussianProcessMCMC& gp, const py:
   throw py::error_already_set();
 }
 
-// ---- hyper-parameter optimisation (gpp_python_model_selection.cpp:150-279, 343-376) ---------------------------------
-// The inputs of both entries in the reference's order: the input lists (PythonInterfaceInputContainer), the MaternNu2p5
-// constructor's checks, then the log10 domain copy.  start = (alpha, lengths..., noise by observation type).
-struct HyperInputs {
-  std::vector<double> X, y, start, log_bounds;
+// ---- model selection (gpp_python_model_selection.cpp) ---------------------------------------------------------------
+// The training data of the model-selection entries in PythonInterfaceInputContainer's order (gpp_python_common.cpp:
+// 107-129): points, values, the noise of the entries that take one, then the derivative indices.
+struct TrainingData {
+  std::vector<double> X, y, noise;
   std::vector<int> derivs;
+};
+
+TrainingData training_data(const py::list& points_sampled, const py::list& points_sampled_value, int dim,
+                           int num_sampled, const py::list& derivatives, int num_derivatives,
+                           const py::list* noise_variance = nullptr) {
+  TrainingData d;
+  d.X = to_vec(points_sampled, static_cast<size_t>(dim) * num_sampled);
+  d.y = to_vec(points_sampled_value, static_cast<size_t>(num_sampled) * (1 + num_derivatives));
+  if (noise_variance) d.noise = to_vec(*noise_variance, 1 + num_derivatives);
+  d.derivs = to_ivec(derivatives, num_derivatives);
+  return d;
+}
+
+// (alpha, lengths...) of `hyperparameters` = [alpha, [lengths]], with MaternNu2p5's constructor checks
+// (gpp_covariance.cpp:80-91)
+std::vector<double> covariance_hyperparameters(const py::list& hyperparameters, int dim) {
+  std::vector<double> h{hyperparameters[0].cast<double>()};
+  const auto lengths = to_vec(hyperparameters[1].cast<py::list>(), dim);
+  if (!(h[0] > 0.0)) raise_exc(g_exc_bounds, "Invalid hyperparameter (alpha).");
+  for (double l : lengths)
+    if (!(l > 0.0)) raise_exc(g_exc_bounds, "Invalid hyperparameter (length).");
+  h.insert(h.end(), lengths.begin(), lengths.end());
+  return h;
+}
+
+// ---- hyper-parameter optimisation (gpp_python_model_selection.cpp:150-279, 343-376) ---------------------------------
+// The inputs of both entries in the reference's order: the input lists, the MaternNu2p5 constructor's checks, then the
+// log10 domain copy.  start = (alpha, lengths..., noise by observation type).
+struct HyperInputs : TrainingData {
+  std::vector<double> start, log_bounds;
   int nh = 0;
 };
 
@@ -931,19 +961,11 @@ HyperInputs hyper_inputs(const py::list& hyperparameter_domain, const py::list& 
                          const py::list& hyperparameters, const py::list& noise_variance, const py::list& derivatives,
                          int num_derivatives) {
   HyperInputs in;
-  in.X = to_vec(points_sampled, static_cast<size_t>(dim) * num_sampled);
-  in.y = to_vec(points_sampled_value, static_cast<size_t>(num_sampled) * (1 + num_derivatives));
-  const auto noise = to_vec(noise_variance, 1 + num_derivatives);
-  in.derivs = to_ivec(derivatives, num_derivatives);
-  const double alpha = hyperparameters[0].cast<double>();
-  const auto lengths = to_vec(hyperparameters[1].cast<py::list>(), dim);
-  if (!(alpha > 0.0)) raise_exc(g_exc_bounds, "Invalid hyperparameter (alpha).");  // gpp_covariance.cpp:80-91
-  for (double l : lengths)
-    if (!(l > 0.0)) raise_exc(g_exc_bounds, "Invalid hyperparameter (length).");
+  static_cast<TrainingData&>(in) = training_data(points_sampled, points_sampled_value, dim, num_sampled, derivatives,
+                                                 num_derivatives, &noise_variance);
+  in.start = covariance_hyperparameters(hyperparameters, dim);
+  in.start.insert(in.start.end(), in.noise.begin(), in.noise.end());
   in.nh = dim + 2 + num_derivatives;
-  in.start.push_back(alpha);
-  in.start.insert(in.start.end(), lengths.begin(), lengths.end());
-  in.start.insert(in.start.end(), noise.begin(), noise.end());
   in.log_bounds = to_vec(hyperparameter_domain, 2 * static_cast<size_t>(in.nh));
   return in;
 }
@@ -1288,16 +1310,14 @@ PYBIND11_MODULE(GPP, m) {
           }
           const double alpha = hyperparameters[0].cast<double>();
           const auto lengths = to_vec(hyperparameters[1].cast<py::list>(), dim);
-          const auto X = to_vec(points_sampled, static_cast<size_t>(dim) * num_sampled);
-          const auto y = to_vec(points_sampled_value, static_cast<size_t>(num_sampled) * (1 + num_derivatives));
-          const auto noise = to_vec(noise_variance, 1 + num_derivatives);
-          const auto derivs = to_ivec(derivatives, num_derivatives);
+          const auto d = training_data(points_sampled, points_sampled_value, dim, num_sampled, derivatives,
+                                       num_derivatives, &noise_variance);
           double value = 0.0;
           int info = 0;
           // the reference's Python boundary hard-wires MaternNu2p5 here as well (:57)
-          check(cmoe_log_marginal_likelihood(CMOE_KERNEL_MATERN_NU_2P5, alpha, lengths.data(), X.data(), y.data(),
-                                             noise.data(), derivs.data(), num_derivatives, dim, num_sampled, 0, &value,
-                                             &info), info);
+          check(cmoe_log_marginal_likelihood(CMOE_KERNEL_MATERN_NU_2P5, alpha, lengths.data(), d.X.data(), d.y.data(),
+                                             d.noise.data(), d.derivs.data(), num_derivatives, dim, num_sampled, 0,
+                                             &value, &info), info);
           return value;
         });
   // compute_hyperparameter_grad_log_likelihood(... same arguments ...)   gpp_python_model_selection.cpp:89-140
@@ -1311,15 +1331,13 @@ PYBIND11_MODULE(GPP, m) {
           }
           const double alpha = hyperparameters[0].cast<double>();
           const auto lengths = to_vec(hyperparameters[1].cast<py::list>(), dim);
-          const auto X = to_vec(points_sampled, static_cast<size_t>(dim) * num_sampled);
-          const auto y = to_vec(points_sampled_value, static_cast<size_t>(num_sampled) * (1 + num_derivatives));
-          const auto noise = to_vec(noise_variance, 1 + num_derivatives);
-          const auto derivs = to_ivec(derivatives, num_derivatives);
+          const auto d = training_data(points_sampled, points_sampled_value, dim, num_sampled, derivatives,
+                                       num_derivatives, &noise_variance);
           std::vector<double> grad(static_cast<size_t>(dim) + 2 + num_derivatives);
           int info = 0;
-          check(cmoe_grad_log_marginal_likelihood(CMOE_KERNEL_MATERN_NU_2P5, alpha, lengths.data(), X.data(), y.data(),
-                                                  noise.data(), derivs.data(), num_derivatives, dim, num_sampled, 0,
-                                                  grad.data(), &info), info);
+          check(cmoe_grad_log_marginal_likelihood(CMOE_KERNEL_MATERN_NU_2P5, alpha, lengths.data(), d.X.data(),
+                                                  d.y.data(), d.noise.data(), d.derivs.data(), num_derivatives, dim,
+                                                  num_sampled, 0, grad.data(), &info), info);
           return to_list(grad);
         });
   // evaluate_log_likelihood_at_hyperparameter_list(hyperparameter_list, points_sampled, points_sampled_value, dim,
@@ -1333,22 +1351,9 @@ PYBIND11_MODULE(GPP, m) {
            const py::list& noise_variance, const py::list& derivatives, int num_derivatives, int num_multistarts,
            int /*max_num_threads*/, py::dict status) -> py::list {
           // the reference's order: input lists, covariance constructor, list copy, objective mode, then the driver
-          const auto X = to_vec(points_sampled, static_cast<size_t>(dim) * num_sampled);
-          const auto y = to_vec(points_sampled_value, static_cast<size_t>(num_sampled) * (1 + num_derivatives));
-          to_vec(noise_variance, 1 + num_derivatives);
-          const auto derivs = to_ivec(derivatives, num_derivatives);
-          const double alpha = hyperparameters[0].cast<double>();
-          const auto lengths = to_vec(hyperparameters[1].cast<py::list>(), dim);
-          if (!(alpha > 0.0)) {  // MaternNu2p5's constructor (gpp_covariance.cpp:80-91)
-            PyErr_SetString(g_exc_bounds, "Invalid hyperparameter (alpha).");
-            throw py::error_already_set();
-          }
-          for (double l : lengths) {
-            if (!(l > 0.0)) {
-              PyErr_SetString(g_exc_bounds, "Invalid hyperparameter (length).");
-              throw py::error_already_set();
-            }
-          }
+          const auto d = training_data(points_sampled, points_sampled_value, dim, num_sampled, derivatives,
+                                       num_derivatives, &noise_variance);
+          covariance_hyperparameters(hyperparameters, dim);
           const size_t nh = static_cast<size_t>(dim) + 2 + num_derivatives;
           const auto hypers = to_vec(hyperparameter_list, nh * std::max(num_multistarts, 0));
           if (objective_mode != LogLikelihoodTypes::kLogMarginalLikelihood) {  // leave-one-out is commented out (:323-333)
@@ -1363,9 +1368,9 @@ PYBIND11_MODULE(GPP, m) {
           std::vector<double> values(num_multistarts);
           int info = 0;
           // MaternNu2p5 hard-wired, as the reference's boundary does (:297)
-          check(cmoe_log_marginal_likelihood_list(CMOE_KERNEL_MATERN_NU_2P5, hypers.data(), num_multistarts, X.data(),
-                                                  y.data(), derivs.data(), num_derivatives, dim, num_sampled, 0,
-                                                  values.data(), &info),
+          check(cmoe_log_marginal_likelihood_list(CMOE_KERNEL_MATERN_NU_2P5, hypers.data(), num_multistarts,
+                                                  d.X.data(), d.y.data(), d.derivs.data(), num_derivatives, dim,
+                                                  num_sampled, 0, values.data(), &info),
                 info);
           // found_flag of MultistartOptimize: some value beat the initial -inf with a strict < (gpp_optimization.hpp:1511)
           const bool found = std::any_of(values.begin(), values.end(),
@@ -1397,9 +1402,8 @@ PYBIND11_MODULE(GPP, m) {
         [](const py::list& points_sampled, const py::list& points_sampled_value, int dim, int num_sampled,
            const py::list& derivatives, int num_derivatives, const py::list& initial_positions, int num_walkers,
            int num_steps, bool noisy, bool use_default_prior, uint64_t seed, uint64_t first_step) -> py::tuple {
-          const auto X = to_vec(points_sampled, static_cast<size_t>(dim) * num_sampled);
-          const auto y = to_vec(points_sampled_value, static_cast<size_t>(num_sampled) * (1 + num_derivatives));
-          const auto derivs = to_ivec(derivatives, num_derivatives);
+          const auto d =
+              training_data(points_sampled, points_sampled_value, dim, num_sampled, derivatives, num_derivatives);
           const size_t nh = static_cast<size_t>(dim) + 2 + num_derivatives;
           const auto p0 = to_vec(initial_positions, nh * std::max(num_walkers, 0));
           std::vector<double> pos(p0.size()), lnp(std::max(num_walkers, 0));
@@ -1408,7 +1412,7 @@ PYBIND11_MODULE(GPP, m) {
           check(cmoe_hyperparameter_mcmc(CMOE_KERNEL_MATERN_NU_2P5,
                                          use_default_prior ? CMOE_HYPER_PRIOR_DEFAULT : CMOE_HYPER_PRIOR_NONE,
                                          noisy ? 1 : 0, p0.data(), num_walkers, num_steps, seed, first_step, nullptr,
-                                         X.data(), y.data(), derivs.data(), num_derivatives, dim, num_sampled, 0,
+                                         d.X.data(), d.y.data(), d.derivs.data(), num_derivatives, dim, num_sampled, 0,
                                          pos.data(), lnp.data(), &info),
                 info);
           return py::make_tuple(to_list(pos), to_list(lnp));
@@ -1427,9 +1431,8 @@ PYBIND11_MODULE(GPP, m) {
         [](const py::list& points_sampled, const py::list& points_sampled_value, int dim, int num_sampled,
            const py::list& derivatives, int num_derivatives, const py::list& initial_positions, int num_starts,
            bool noisy, bool use_default_prior, double gtol, int max_iterations) -> py::tuple {
-          const auto X = to_vec(points_sampled, static_cast<size_t>(dim) * num_sampled);
-          const auto y = to_vec(points_sampled_value, static_cast<size_t>(num_sampled) * (1 + num_derivatives));
-          const auto derivs = to_ivec(derivatives, num_derivatives);
+          const auto d =
+              training_data(points_sampled, points_sampled_value, dim, num_sampled, derivatives, num_derivatives);
           const size_t nh = static_cast<size_t>(dim) + 2 + num_derivatives, S = std::max(num_starts, 0);
           const auto p0 = to_vec(initial_positions, nh * S);
           std::vector<double> pos(p0.size()), grads(p0.size()), vals(S);
@@ -1439,9 +1442,9 @@ PYBIND11_MODULE(GPP, m) {
           // MaternNu2p5 hard-wired, as compute_log_likelihood's boundary does
           check(cmoe_hyperparameter_map(CMOE_KERNEL_MATERN_NU_2P5,
                                         use_default_prior ? CMOE_HYPER_PRIOR_DEFAULT : CMOE_HYPER_PRIOR_NONE,
-                                        noisy ? 1 : 0, p0.data(), num_starts, &opts, X.data(), y.data(), derivs.data(),
-                                        num_derivatives, dim, num_sampled, 0, pos.data(), vals.data(), grads.data(),
-                                        iters.data(), evals.data(), status.data(), &info),
+                                        noisy ? 1 : 0, p0.data(), num_starts, &opts, d.X.data(), d.y.data(),
+                                        d.derivs.data(), num_derivatives, dim, num_sampled, 0, pos.data(), vals.data(),
+                                        grads.data(), iters.data(), evals.data(), status.data(), &info),
                 info);
           py::list st;
           for (int v : status) st.append(v);

@@ -184,6 +184,10 @@ inline Centre centre_of(const cmoe_gp& gp) {
   return c;
 }
 void fit_gp(cmoe_gp* gp, bool mean_change);
+// s <- the KernelSpec of (alpha, lengths[dim]) with derivative indices derivs[g]; entries past dim and g are l = 1,
+// 1/l = 0 and index 0.  In place: the list calls fill one per set.
+void fill_kernel_spec(KernelSpec& s, int kernel, int dim, int g, const int* derivs, double alpha,
+                      const double* lengths);
 // bit-identical copy of a fitted GP on another device (peer copies of the factor; no refit)
 cmoe_gp* clone_gp_to_device(const cmoe_gp* gp, int device);
 // Ps <- the m points P (device) in the length-scaled, centred coordinates of gp's covariance build (the Xs argument of

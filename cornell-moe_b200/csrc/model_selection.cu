@@ -570,9 +570,10 @@ std::vector<double> centred_values(const double* points_sampled_value, int N, in
 }
 
 // Uploads the points and y - m and sizes w's buffers for chunks of `chunk` sets (with the gradient's when `grads`).
+// Every buffer lml_stages uses is sized here, so lml_stages allocates nothing and can be captured in a graph.
 void lml_prepare(LmlWork& w, const double* points_sampled, const double* points_sampled_value, int N, int dim, int g,
                  int chunk, bool grads, cudaStream_t s) {
-  const int b = 1 + g, n = N * b;
+  const int b = 1 + g, n = N * b, t = (n + NB - 1) / NB;
   int gx;
   const int nctas = lml_grad_ctas(N, gx);
   const std::vector<double> rc = centred_values(points_sampled_value, N, b);
@@ -581,6 +582,7 @@ void lml_prepare(LmlWork& w, const double* points_sampled, const double* points_
   w.specs.ensure(chunk);
   w.noise.ensure(static_cast<size_t>(chunk) * b);
   w.K.ensure(static_cast<size_t>(chunk) * n * n);
+  w.stage.ensure(static_cast<size_t>(chunk) * t * NB * NB);  // what potrf_batched would grow it to
   w.values.ensure(chunk);
   w.fail.ensure(chunk);
   const size_t smem_solve = (static_cast<size_t>(n) + NB * (NB + 1)) * sizeof(double);
@@ -651,6 +653,19 @@ void check_lml_problem(int kernel, const double* points_sampled, const double* p
     CMOE_REQUIRE(derivatives[k] >= 0 && derivatives[k] < dim, CMOE_ERR_BOUNDS, "derivative index out of range");
   CMOE_REQUIRE(static_cast<long long>(num_sampled) * (1 + num_derivatives) <= kMaxSampleQ, CMOE_ERR_BOUNDS,
                "num_sampled * (1 + num_derivatives) must be <= 8192");
+}
+
+void check_hyper_prior(int prior) {
+  CMOE_REQUIRE(prior == CMOE_HYPER_PRIOR_NONE || prior == CMOE_HYPER_PRIOR_DEFAULT, CMOE_ERR_INVALID_VALUE,
+               "prior must be CMOE_HYPER_PRIOR_NONE or CMOE_HYPER_PRIOR_DEFAULT");
+}
+
+// The drivers that keep all their sets on the device at once need them in one likelihood chunk of per_set bytes each.
+// `what` opens the message ("num_starts = 5000 exceeds").
+void check_one_chunk(int sets, size_t per_set, int n, const std::string& what) {
+  const size_t chunk = chunk_items(kMaxChunkSets, kSampleWorkspaceBytes, per_set);
+  CMOE_REQUIRE(static_cast<size_t>(sets) <= chunk, CMOE_ERR_BOUNDS,
+               what + " one likelihood chunk (" + std::to_string(chunk) + " sets at n = " + std::to_string(n) + ")");
 }
 
 }  // namespace
@@ -733,22 +748,7 @@ void lml_list(int kernel, const double* hyperparameters, int num_sets, const dou
         if (!(h[1 + k] > 0.0))
           throw Error(CMOE_ERR_BOUNDS,
                       "hyperparameter set " + std::to_string(s) + ": Invalid hyperparameter (length).");
-      KernelSpec& sp = specs[s];
-      sp = KernelSpec{};
-      sp.kernel = kernel;
-      sp.dim = dim;
-      sp.g = g;
-      sp.alpha = h[0];
-      for (int k = 0; k < CMOE_MAX_DIM; ++k) {
-        sp.lsq[k] = 1.0;
-        sp.inv_len[k] = 0.0;
-        sp.derivs[k] = 0;
-      }
-      for (int k = 0; k < dim; ++k) {
-        sp.lsq[k] = h[1 + k] * h[1 + k];
-        sp.inv_len[k] = 1.0 / h[1 + k];
-      }
-      for (int k = 0; k < g; ++k) sp.derivs[k] = derivatives[k];
+      fill_kernel_spec(specs[s], kernel, dim, g, derivatives, h[0], h + 1);
       for (int t = 0; t < b; ++t) noise[static_cast<size_t>(s) * b + t] = h[1 + dim + t] + 1.0e-6;
     }
     require_device(device);
@@ -822,8 +822,9 @@ extern "C" int cmoe_grad_log_marginal_likelihood_list_exact(int kernel, const do
 // emcee 2.2.1's EnsembleSampler.sample with the stretch move (a = 2) on GaussianProcessLogLikelihoodMCMC's
 // log-probability (log_likelihood_mcmc.py:277-312), every half-step on the device:
 //   hmc_propose_kernel   one thread per moving walker: draws, z = ((a - 1) u + 1)^2 / a, q = c - z (c - s) rounded as
-//                        numpy rounds it, the box check, the noise pinning, the prior, and the K10 inputs of q
-//   lml_cov_kernel, potrf_batched, lml_solve_kernel   (K10, unchanged) on the half-ensemble's sets
+//                        numpy rounds it, then hyper_trial_set: the box check, the noise pinning, the prior, and the
+//                        K10 inputs of q
+//   lml_stages           K10 without the gradient on the half-ensemble's sets, in the workspace lml_prepare sized
 //   hmc_accept_kernel    one thread per moving walker: lnpdiff = (nh - 1) log z + lnp(q) - lnp(s) and the accept
 // The initial evaluation runs the same kernels with the move switched off.  One step is captured as a CUDA graph and
 // replayed; the step index lives in a device counter that the second half's accept kernel advances.
@@ -835,9 +836,28 @@ constexpr double kStretchA = 2.0;
 constexpr double kLogNoiseFree = -0x1.26bb1bbb55516p+4;  // numpy.log(1e-8), the pinned noise of a noise-free model
 constexpr double kSqrt2Pi = 2.5066282746310002;           // scipy.stats.norm's _norm_pdf_C = sqrt(2 pi)
 
-struct HmcArgs {
-  int Wh, nh, dim, g, kernel, prior, noisy;
+// The model whose log-probability the K12 and K19 kernels evaluate: covariance kernel, the K10 sizes (nh = 2 + dim + g)
+// and derivative indices, the prior and whether the noise is fitted.
+struct HyperModel {
+  int nh, dim, g, kernel, prior, noisy;
   int derivs[CMOE_MAX_DIM];
+};
+
+HyperModel hyper_model(int kernel, int prior, int noisy, int dim, int g, const int* derivatives) {
+  HyperModel m{};
+  m.nh = 2 + dim + g;
+  m.dim = dim;
+  m.g = g;
+  m.kernel = kernel;
+  m.prior = prior;
+  m.noisy = noisy ? 1 : 0;
+  for (int k = 0; k < g; ++k) m.derivs[k] = derivatives[k];
+  return m;
+}
+
+struct HmcArgs {
+  int Wh;
+  HyperModel m;
   uint64_t seed, first_step;
   const double* tz;  // table (NULL: Philox): [num_steps][W] z uniform, partner, accept uniform
   const int* tp;
@@ -930,12 +950,25 @@ __device__ __forceinline__ void hyper_set_inputs(const double* q, bool skip, int
   for (int t = 0; t < 1 + g; ++t) noise[t] = exp(skip ? 0.0 : q[1 + dim + t]) + 1.0e-6;
 }
 
+// Trial set j of the K12 or K19 kernel arguments `a` at log-scale q[nh]: hyper_box_prior on q unless the set is not
+// live, its prior into a.lprior[j] (-inf when the likelihood is skipped), its K10 inputs, and a.fail[j] preset to skip
+// it.  dlp as hyper_box_prior's.
+template <class Args>
+__device__ __forceinline__ void hyper_trial_set(const Args& a, int j, bool live, double* q, double* dlp) {
+  const HyperModel& m = a.m;
+  double lp;
+  const bool need = live && hyper_box_prior(q, m.nh, m.dim, 1 + m.g, m.prior, m.noisy, lp, dlp);
+  a.lprior[j] = need ? lp : -INFINITY;
+  hyper_set_inputs(q, !need, m.kernel, m.dim, m.g, m.derivs, a.specs[j], a.noise + static_cast<size_t>(j) * (1 + m.g));
+  a.fail[j] = need ? 0 : -1;
+}
+
 // Moving walker w = half * Wh + j.  With move == 0 the proposal is the walker itself (the initial evaluation).
 __global__ void __launch_bounds__(kHmcThreads) hmc_propose_kernel(const __grid_constant__ HmcArgs a, int half,
                                                                   int move) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= a.Wh) return;
-  const int nh = a.nh, dim = a.dim, b = 1 + a.g, w = half * a.Wh + j;
+  const int nh = a.m.nh, w = half * a.Wh + j;
   const double* s = a.pos + static_cast<size_t>(w) * nh;
   double* q = a.prop + static_cast<size_t>(j) * nh;
   if (move) {
@@ -960,18 +993,14 @@ __global__ void __launch_bounds__(kHmcThreads) hmc_propose_kernel(const __grid_c
   } else {
     for (int k = 0; k < nh; ++k) q[k] = s[k];
   }
-  double lp;
-  const bool skip = !hyper_box_prior(q, nh, dim, b, a.prior, a.noisy, lp, nullptr);
-  a.lprior[j] = skip ? -INFINITY : lp;
-  hyper_set_inputs(q, skip, a.kernel, dim, a.g, a.derivs, a.specs[j], a.noise + static_cast<size_t>(j) * b);
-  a.fail[j] = skip ? -1 : 0;
+  hyper_trial_set(a, j, true, q, nullptr);
 }
 
 __global__ void __launch_bounds__(kHmcThreads) hmc_accept_kernel(const __grid_constant__ HmcArgs a, int half,
                                                                  int move) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= a.Wh) return;
-  const int nh = a.nh, w = half * a.Wh + j;
+  const int nh = a.m.nh, w = half * a.Wh + j;
   const double lq = a.lprior[j] + a.values[j];  // -inf + -inf for a skipped proposal
   bool take = true;
   if (move) {
@@ -1001,32 +1030,17 @@ void hyper_mcmc(int kernel, int prior, int noisy, const double* initial_position
                 uint64_t seed, uint64_t first_step, const cmoe_mcmc_table* table, const double* points_sampled,
                 const double* points_sampled_value, const int* derivatives, int num_derivatives, int dim,
                 int num_sampled, int device, double* positions, double* log_probabilities) {
-  CMOE_REQUIRE(initial_positions != nullptr && points_sampled != nullptr && points_sampled_value != nullptr &&
-                   positions != nullptr && log_probabilities != nullptr,
+  CMOE_REQUIRE(initial_positions != nullptr && positions != nullptr && log_probabilities != nullptr,
                CMOE_ERR_INVALID_VALUE, "NULL argument");
-  CMOE_REQUIRE(kernel == CMOE_KERNEL_SQUARE_EXPONENTIAL || kernel == CMOE_KERNEL_MATERN_NU_2P5,
-               CMOE_ERR_INVALID_VALUE, "unknown covariance kernel id");
-  CMOE_REQUIRE(prior == CMOE_HYPER_PRIOR_NONE || prior == CMOE_HYPER_PRIOR_DEFAULT, CMOE_ERR_INVALID_VALUE,
-               "prior must be CMOE_HYPER_PRIOR_NONE or CMOE_HYPER_PRIOR_DEFAULT");
-  CMOE_REQUIRE(dim >= 1 && dim <= CMOE_MAX_DIM, CMOE_ERR_BOUNDS, "dim must be in [1, CMOE_MAX_DIM]");
-  CMOE_REQUIRE(num_sampled >= 1, CMOE_ERR_BOUNDS, "num_sampled must be >= 1");
-  CMOE_REQUIRE(num_derivatives >= 0 && num_derivatives <= dim, CMOE_ERR_BOUNDS, "num_derivatives out of range");
-  CMOE_REQUIRE(num_derivatives == 0 || derivatives != nullptr, CMOE_ERR_INVALID_VALUE, "derivatives is NULL");
-  for (int k = 0; k < num_derivatives; ++k)
-    CMOE_REQUIRE(derivatives[k] >= 0 && derivatives[k] < dim, CMOE_ERR_BOUNDS, "derivative index out of range");
+  check_lml_problem(kernel, points_sampled, points_sampled_value, derivatives, num_derivatives, dim, num_sampled);
+  check_hyper_prior(prior);
   const int g = num_derivatives, b = 1 + g, nh = 2 + dim + g, N = num_sampled, W = num_walkers, Wh = W / 2;
-  CMOE_REQUIRE(static_cast<long long>(N) * b <= kMaxSampleQ, CMOE_ERR_BOUNDS,
-               "num_sampled * (1 + num_derivatives) must be <= 8192");
   // EnsembleSampler.__init__'s checks
   CMOE_REQUIRE(W % 2 == 0, CMOE_ERR_BOUNDS, "num_walkers must be even");
   CMOE_REQUIRE(W >= 2 * nh, CMOE_ERR_BOUNDS, "num_walkers must be at least twice the number of hyperparameters");
   CMOE_REQUIRE(num_steps >= 1, CMOE_ERR_BOUNDS, "num_steps must be >= 1");
-  const int n = N * b, nsteps = (n + NB - 1) / NB;
   // the half-ensemble is one K10 chunk of lml_list without the gradient
-  const size_t chunk = chunk_items(kMaxChunkSets, kSampleWorkspaceBytes, lml_set_bytes(n, b));
-  CMOE_REQUIRE(static_cast<size_t>(Wh) <= chunk, CMOE_ERR_BOUNDS,
-               "num_walkers / 2 = " + std::to_string(Wh) + " sets exceed one likelihood chunk (" +
-                   std::to_string(chunk) + " sets at n = " + std::to_string(n) + ")");
+  check_one_chunk(Wh, lml_set_bytes(N * b, b), N * b, "num_walkers / 2 = " + std::to_string(Wh) + " sets exceed");
   for (size_t e = 0; e < static_cast<size_t>(W) * nh; ++e)
     CMOE_REQUIRE(std::isfinite(initial_positions[e]), CMOE_ERR_INVALID_VALUE, "initial position is not finite");
   const size_t tcount = static_cast<size_t>(num_steps) * W;
@@ -1038,19 +1052,11 @@ void hyper_mcmc(int kernel, int prior, int noisy, const double* initial_position
                    "table partner out of range [0, num_walkers / 2)");
   }
   require_device(device);
-  const std::vector<double> rc = centred_values(points_sampled_value, N, b);
 
   LmlWork& w = lml_workspace(device);
   cudaStream_t s = w.stream;
-  // every buffer is sized here, before the capture
-  w.X.upload(points_sampled, static_cast<size_t>(N) * dim, s);
-  w.r.upload(rc.data(), n, s);
-  w.specs.ensure(Wh);
-  w.noise.ensure(static_cast<size_t>(Wh) * b);
-  w.K.ensure(static_cast<size_t>(Wh) * n * n);
-  w.stage.ensure(static_cast<size_t>(Wh) * nsteps * NB * NB);
-  w.values.ensure(Wh);
-  w.fail.ensure(Wh);
+  // every buffer is sized before the capture
+  lml_prepare(w, points_sampled, points_sampled_value, N, dim, g, Wh, false, s);
   DevBuf<double> pos, lnp(W), prop(static_cast<size_t>(Wh) * nh), lprior(Wh), zz(Wh), lu(Wh), tz, tu;
   DevBuf<int> tp;
   DevBuf<unsigned long long> step(1);
@@ -1063,13 +1069,7 @@ void hyper_mcmc(int kernel, int prior, int noisy, const double* initial_position
   step.zero(s);
   HmcArgs a{};
   a.Wh = Wh;
-  a.nh = nh;
-  a.dim = dim;
-  a.g = g;
-  a.kernel = kernel;
-  a.prior = prior;
-  a.noisy = noisy ? 1 : 0;
-  for (int k = 0; k < g; ++k) a.derivs[k] = derivatives[k];
+  a.m = hyper_model(kernel, prior, noisy, dim, g, derivatives);
   a.seed = seed;
   a.first_step = first_step;
   a.tz = table ? tz.p : nullptr;
@@ -1086,21 +1086,14 @@ void hyper_mcmc(int kernel, int prior, int noisy, const double* initial_position
   a.noise = w.noise.p;
   a.fail = w.fail.p;
   a.values = w.values.p;
-  const size_t smem_cov = 2 * static_cast<size_t>(NB) * dim * sizeof(double);
-  const size_t smem_solve = (static_cast<size_t>(n) + NB * (NB + 1)) * sizeof(double);
-  CMOE_CUDA(cudaFuncSetAttribute(lml_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 static_cast<int>(smem_solve)));
   const unsigned blocks = static_cast<unsigned>((Wh + kHmcThreads - 1) / kHmcThreads);
   auto half_step = [&](int half, int move) {
     hmc_propose_kernel<<<blocks, kHmcThreads, 0, s>>>(a, half, move);
-    lml_cov_kernel<<<dim3(nsteps * (nsteps + 1) / 2, 1, Wh), kLmlCovThreads, smem_cov, s>>>(w.specs.p, w.noise.p,
-                                                                                            w.X.p, N, w.K.p);
-    count_launch(2);
+    count_launch();
     CMOE_CUDA(cudaGetLastError());
-    potrf_batched(w.K.p, n, Wh, w.fail.p, w.stage, s);
-    lml_solve_kernel<<<Wh, kLmlSolveThreads, smem_solve, s>>>(w.K.p, n, w.r.p, w.fail.p, w.values.p, nullptr);
+    lml_stages(w, N, dim, g, kernel, Wh, false, false, s);
     hmc_accept_kernel<<<blocks, kHmcThreads, 0, s>>>(a, half, move);
-    count_launch(2);
+    count_launch();
     CMOE_CUDA(cudaGetLastError());
   };
   // run_mcmc evaluates the initial positions first (and pins their noise)
@@ -1142,7 +1135,7 @@ extern "C" int cmoe_hyperparameter_mcmc(int kernel, int prior, int noisy, const 
 // ---- hyper-parameter MAP fit (DESIGN.md K19) ------------------------------------------------------------------------
 // scipy's _minimize_bfgs with an analytic gradient on nll(theta) = -compute_log_likelihood(theta)
 // (log_likelihood_mcmc.py:241-312), every start in lock step.  One round evaluates one trial point of every active start:
-//   map_prep_kernel   one thread per start: the box, the pinning and the prior (hyper_box_prior) and the K10 inputs
+//   map_prep_kernel   one thread per start: the box, the pinning, the prior and the K10 inputs (hyper_trial_set)
 //   lml_stages        (K10/K11, the exact contraction) on all starts; finished or skipped starts have fail = -1
 //   map_step_kernel   one warp per start: the trial's value and gradient, one step of the strong-Wolfe line search
 //                     (scipy's scalar_search_wolfe2 and _zoom), and on acceptance the BFGS update of H and the next
@@ -1170,8 +1163,9 @@ struct MapState {
 };
 
 struct MapArgs {
-  int S, nh, dim, g, kernel, prior, noisy, max_iter;
-  int derivs[CMOE_MAX_DIM];
+  int S;
+  HyperModel m;
+  int max_iter;
   double gtol;
   MapState* st;
   double* x;       // [S][nh] iterates
@@ -1193,17 +1187,11 @@ __global__ void __launch_bounds__(kHmcThreads) map_prep_kernel(const __grid_cons
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s == 0) *a.active = 0;
   if (s >= a.S) return;
-  const int nh = a.nh, b = 1 + a.g;
+  const int nh = a.m.nh;
   double* q = a.q + static_cast<size_t>(s) * nh;
   const double* xt = a.xt + static_cast<size_t>(s) * nh;
   for (int k = 0; k < nh; ++k) q[k] = xt[k];
-  double lp = 1.0;
-  bool need = false;
-  if (a.st[s].phase != kMapDone)
-    need = hyper_box_prior(q, nh, a.dim, b, a.prior, a.noisy, lp, a.dprior + static_cast<size_t>(s) * nh);
-  a.lprior[s] = need ? lp : -INFINITY;
-  hyper_set_inputs(q, !need, a.kernel, a.dim, a.g, a.derivs, a.specs[s], a.noise + static_cast<size_t>(s) * b);
-  a.fail[s] = need ? 0 : -1;
+  hyper_trial_set(a, s, a.st[s].phase != kMapDone, q, a.dprior + static_cast<size_t>(s) * nh);
 }
 
 __device__ __forceinline__ double warp_sum(double v) {
@@ -1315,7 +1303,7 @@ __global__ void __launch_bounds__(kMapWarps * 32) map_step_kernel(const __grid_c
   __syncwarp();
   if (t.phase == kMapDone) return;
   const bool first = t.phase == kMapInit;
-  const int nh = a.nh, dim = a.dim;
+  const int nh = a.m.nh, dim = a.m.dim;
   const size_t off = static_cast<size_t>(s) * nh;
   double* x = a.x + off;
   double* gr = a.gr + off;
@@ -1337,7 +1325,7 @@ __global__ void __launch_bounds__(kMapWarps * 32) map_step_kernel(const __grid_c
   for (int m = 0; m < kMapPer; ++m) {
     const int k = lane + 32 * m;
     double v = 0.0;
-    if (k < nh && lp != -INFINITY && !(a.noisy == 0 && k > dim)) v = -(dp[k] + exp(q[k]) * o[1 + k]);
+    if (k < nh && lp != -INFINITY && !(a.m.noisy == 0 && k > dim)) v = -(dp[k] + exp(q[k]) * o[1 + k]);
     gt[m] = v;
     if (k < nh) dphi = fma(v, p[k], dphi);
   }
@@ -1497,7 +1485,7 @@ __global__ void __launch_bounds__(kMapWarps * 32) map_step_kernel(const __grid_c
 
 __global__ void map_init_kernel(const __grid_constant__ MapArgs a) {
   const size_t e = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  const size_t nh = a.nh;
+  const size_t nh = a.m.nh;
   if (e >= static_cast<size_t>(a.S) * nh * nh) return;
   const size_t r = e % (nh * nh);
   a.H[e] = (r / nh == r % nh) ? 1.0 : 0.0;
@@ -1511,8 +1499,7 @@ void hyper_map(int kernel, int prior, int noisy, const double* starts, int num_s
                    iterations != nullptr && evaluations != nullptr && status != nullptr,
                CMOE_ERR_INVALID_VALUE, "NULL argument");
   check_lml_problem(kernel, points_sampled, points_sampled_value, derivatives, num_derivatives, dim, num_sampled);
-  CMOE_REQUIRE(prior == CMOE_HYPER_PRIOR_NONE || prior == CMOE_HYPER_PRIOR_DEFAULT, CMOE_ERR_INVALID_VALUE,
-               "prior must be CMOE_HYPER_PRIOR_NONE or CMOE_HYPER_PRIOR_DEFAULT");
+  check_hyper_prior(prior);
   CMOE_REQUIRE(noisy == 0 || noisy == 1, CMOE_ERR_INVALID_VALUE, "noisy must be 0 or 1");
   const int g = num_derivatives, b = 1 + g, nh = 2 + dim + g, N = num_sampled, S = num_starts;
   double gtol = 1.0e-5;
@@ -1527,10 +1514,7 @@ void hyper_map(int kernel, int prior, int noisy, const double* starts, int num_s
   // every start is one set of a K11 chunk, with its BFGS state beside it
   const size_t per_set = lml_grad_set_bytes(N, dim, g) + sizeof(MapState) +
                          sizeof(double) * (static_cast<size_t>(nh) * nh + 6 * static_cast<size_t>(nh) + 1);
-  const size_t chunk = chunk_items(kMaxChunkSets, kSampleWorkspaceBytes, per_set);
-  CMOE_REQUIRE(static_cast<size_t>(S) <= chunk, CMOE_ERR_BOUNDS,
-               "num_starts = " + std::to_string(S) + " exceeds one likelihood chunk (" + std::to_string(chunk) +
-                   " sets at n = " + std::to_string(N * b) + ")");
+  check_one_chunk(S, per_set, N * b, "num_starts = " + std::to_string(S) + " exceeds");
   require_device(device);
 
   LmlWork& w = lml_workspace(device);
@@ -1551,14 +1535,8 @@ void hyper_map(int kernel, int prior, int noisy, const double* starts, int num_s
   st.upload(h0.data(), S, s);
   MapArgs a{};
   a.S = S;
-  a.nh = nh;
-  a.dim = dim;
-  a.g = g;
-  a.kernel = kernel;
-  a.prior = prior;
-  a.noisy = noisy;
+  a.m = hyper_model(kernel, prior, noisy, dim, g, derivatives);
   a.max_iter = max_iter;
-  for (int k = 0; k < g; ++k) a.derivs[k] = derivatives[k];
   a.gtol = gtol;
   a.st = st.p;
   a.x = x.p;
