@@ -912,6 +912,35 @@ def ei_gradient_descent(gp, starts, Xp, num_mc, best_so_far, outer, domain_bound
     return vals, pts
 
 
+CONSTANT_LIAR, KRIGING_BELIEVER = 0, 1
+
+
+class EstimationPolicy(ctypes.Structure):
+    """cmoe_estimation_policy: CONSTANT_LIAR (value = the lie) or KRIGING_BELIEVER (value = std_deviation_coef)."""
+    _fields_ = [("policy", ctypes.c_int), ("value", ctypes.c_double), ("noise_variance", ctypes.c_double)]
+
+
+def heuristic_ei(gp, starts, best_so_far, policy, value, noise_variance, outer=None, domain_bounds=None):
+    """cmoe_heuristic_ei: q points by Constant Liar or Kriging Believer.  ``starts`` [q, num_starts, dim] (round r uses
+    block r); ``outer`` gradient-descent parameters, or None for the random search of the screen alone.  Returns
+    (points [q, dim], fantasy_values [q], ei_values [q], found [q]).  The GP is not modified."""
+    starts = _f64(starts)
+    q, ns, dim = starts.shape
+    gd = None if outer is None else GDParams.from_seq(outer)
+    db = _f64(domain_bounds).ravel()
+    pol = EstimationPolicy(int(policy), float(value), float(noise_variance))
+    pts = np.empty((q, dim))
+    fv = np.empty(q)
+    ev = np.empty(q)
+    found = np.empty(q, dtype=np.int32)
+    info = ctypes.c_int()
+    rc = lib().cmoe_heuristic_ei(gp.h, ctypes.byref(pol), None if gd is None else ctypes.byref(gd), _d(db),
+                                 _d(starts), ns, q, ctypes.c_double(best_so_far), _d(pts), _d(fv), _d(ev), _i(found),
+                                 ctypes.byref(info))
+    _check(rc, info.value)
+    return pts, fv, ev, found.astype(bool)
+
+
 def posterior_mean_optimization(gp, initial_guess, params, domain_bounds, num_fidelity=0):
     """cmoe_posterior_mean_optimization: returns (best_point [dim - num_fidelity], -min mu, found)."""
     ps = gp.dim - num_fidelity

@@ -174,7 +174,8 @@ void fit_gp(cmoe_gp* gp, bool mean_change) {
 // O(N^2) append of m points to a fitted GP (the reference refits from scratch and leaves this as a TODO,
 // gpp_math.cpp:1699-1718):  K1 = [K K12; K12^T K22]  =>  L1 = [L 0; (L^-1 K12)^T  chol(K22 - K12^T K^-1 K12)].
 // Everything is built beside the live state and swapped in at the end, so a singular update leaves the handle intact.
-void append_points(cmoe_gp* gp, const double* new_points, const double* new_values, int m) {
+// The new rows' diagonal carries new_noise [1+g] (host), or the GP's own noise when it is NULL.
+void append_points(cmoe_gp* gp, const double* new_points, const double* new_values, int m, const double* new_noise) {
   const KernelSpec& spec = gp->spec;
   const int dim = spec.dim, b = 1 + spec.g, N0 = gp->N, n0 = gp->n, mm = m * b, n1 = n0 + mm;
   cudaStream_t s = gp->stream;
@@ -182,6 +183,8 @@ void append_points(cmoe_gp* gp, const double* new_points, const double* new_valu
   ensure_scaled_points(dXsn, m, dim, s);
   DevBuf<double> K1(static_cast<size_t>(n1) * n1), T(static_cast<size_t>(n0) * mm), S22(static_cast<size_t>(mm) * mm);
   DevBuf<int> dDer(spec.g > 0 ? spec.g : 1), flag(1);
+  DevBuf<double> dNoise;
+  if (new_noise) dNoise.upload(new_noise, b, s);
   dXn.upload(new_points, static_cast<size_t>(m) * dim, s);
   if (spec.g > 0) dDer.upload(spec.derivs, spec.g, s);
   scale_points_kernel<<<(m * dim + 255) / 256, 256, 0, s>>>(spec, centre_of(gp->hX, N0, dim), dXn.p, m, dXsn.p);
@@ -192,7 +195,7 @@ void append_points(cmoe_gp* gp, const double* new_points, const double* new_valu
   build_mix_covariance(spec, gp->dX.p, N0, dXn.p, m, dDer.p, spec.g, T.p, s);
   trsm_lower(gp->dK.p, n0, T.p, n0, mm, false, s);  // T = L^-1 K12
   CMOE_CUDA(cudaMemsetAsync(S22.p, 0, S22.count * sizeof(double), s));
-  build_covariance(spec, dXn.p, dXsn.p, m, gp->dnoise.p, S22.p, s);
+  build_covariance(spec, dXn.p, dXsn.p, m, new_noise ? dNoise.p : gp->dnoise.p, S22.p, s);
   append_schur_kernel<<<mm * (mm + 1) / 2, 256, 0, s>>>(T.p, n0, mm, S22.p);
   append_rows_kernel<<<static_cast<unsigned>((static_cast<size_t>(n0) * mm + 255) / 256), 256, 0, s>>>(T.p, n0, mm, K1.p,
                                                                                                    n1);

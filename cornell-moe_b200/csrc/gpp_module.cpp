@@ -10,6 +10,8 @@
 //     .compute_grad_cholesky_variance_of_points / add_sampled_points / ...   :64-253, 456-463
 //   compute_expected_improvement, compute_grad_expected_improvement, multistart_expected_improvement_optimization,
 //   evaluate_EI_at_point_list                                             gpp_python_expected_improvement.cpp:44-441
+//   heuristic_expected_improvement_optimization, ConstantLiarEstimationPolicy, KrigingBelieverEstimationPolicy
+//                                                                         gpp_python_expected_improvement.cpp:445-659
 //   compute_posterior_mean, compute_grad_posterior_mean, compute_knowledge_gradient, compute_grad_knowledge_gradient,
 //   multistart_knowledge_gradient_optimization, posterior_mean_optimization, evaluate_KG_at_point_list
 //                                                                         gpp_python_knowledge_gradient.cpp:44-397
@@ -473,6 +475,76 @@ py::list evaluate_EI_at_point_list(const GaussianProcess& gp, const py::list& in
   for (double v : vals) found = found || (v > -1.0);
   status["evaluate_EI_at_point_list"] = found;
   return to_list(vals);
+}
+
+// ---- heuristic EI (DESIGN.md K20) -----------------------------------------------------------------------------------
+// The estimation policies of gpp_python_expected_improvement.cpp:445-486, with their positional constructors.
+struct ObjectiveEstimationPolicyInterface {
+  cmoe_estimation_policy p{};
+  virtual ~ObjectiveEstimationPolicyInterface() = default;
+};
+struct ConstantLiarEstimationPolicy : ObjectiveEstimationPolicyInterface {
+  ConstantLiarEstimationPolicy(double lie_value, double lie_noise_variance) {
+    p = {CMOE_ESTIMATION_CONSTANT_LIAR, lie_value, lie_noise_variance};
+  }
+};
+struct KrigingBelieverEstimationPolicy : ObjectiveEstimationPolicyInterface {
+  KrigingBelieverEstimationPolicy(double std_deviation_coef, double kriging_noise_variance) {
+    p = {CMOE_ESTIMATION_KRIGING_BELIEVER, std_deviation_coef, kriging_noise_variance};
+  }
+};
+
+// HeuristicExpectedImprovementOptimizationWrapper (gpp_python_expected_improvement.cpp:278-400, 602-659): q rounds of
+// one-point EI optimisation with the policy's fantasy fed back after each round (cmoe_heuristic_ei).  Round r's starts
+// are the r-th Latin-hypercube block drawn from the uniform engine; the draws do not depend on results, so all q blocks
+// are drawn up front in round order.  The status flag is the AND of the rounds' found flags.
+py::list heuristic_expected_improvement_optimization(const py::object& optimizer_parameters,
+                                                     const py::object& gaussian_process, const py::list& domain_bounds,
+                                                     const ObjectiveEstimationPolicyInterface& estimation_policy,
+                                                     int num_to_sample, double best_so_far, int /*max_num_threads*/,
+                                                     RandomnessSourceContainer& rnd, py::dict& status) {
+  const GaussianProcess& gp = unwrap_gp(gaussian_process);
+  const int dim = gp.dim_, q = num_to_sample;
+  const auto domain_type = optimizer_parameters.attr("domain_type").cast<DomainTypes>();
+  const auto opt_type = optimizer_parameters.attr("optimizer_type").cast<OptimizerTypes>();
+  if (domain_type == DomainTypes::kSimplex) {
+    PyErr_SetString(g_exc_base, "heuristic_expected_improvement_optimization: only the tensor_product domain is "
+                                "implemented");
+    throw py::error_already_set();
+  }
+  if (opt_type != OptimizerTypes::kNull && opt_type != OptimizerTypes::kGradientDescent) {
+    PyErr_SetString(g_exc_base, "ERROR: invalid optimizer choice. Setting all coordinates to 0.0.");
+    throw py::error_already_set();
+  }
+  if (q < 1) {
+    PyErr_SetString(g_exc_bounds, "num_to_sample must be >= 1");
+    throw py::error_already_set();
+  }
+  const auto bounds = full_bounds(domain_bounds, dim);
+  const bool null_opt = opt_type == OptimizerTypes::kNull;
+  cmoe_gd_params gd{};
+  if (!null_opt) gd = gd_of(optimizer_parameters);
+  const int n = null_opt ? optimizer_parameters.attr("num_random_samples").cast<int>() : gd.num_multistarts;
+  if (n < 1) {
+    PyErr_SetString(g_exc_bounds, "num_multistarts must be > 1");
+    throw py::error_already_set();
+  }
+  std::vector<double> starts;
+  for (int r = 0; r < q; ++r) {
+    const auto block = lhc_starts(bounds, dim, 1, n, rnd.uniform_engine);
+    starts.insert(starts.end(), block.begin(), block.end());
+  }
+  std::vector<double> pts(static_cast<size_t>(q) * dim);
+  std::vector<int> found(q);
+  int info = 0;
+  check(cmoe_heuristic_ei(gp.h, &estimation_policy.p, null_opt ? nullptr : &gd, bounds.data(), starts.data(), n, q,
+                          best_so_far, pts.data(), nullptr, nullptr, found.data(), &info),
+        info);
+  bool all = true;
+  for (int f : found) all = all && f != 0;
+  status[null_opt ? "lhc_tensor_product_domain_found_update" : "gradient_descent_tensor_product_domain_found_update"] =
+      all;
+  return to_list(pts);
 }
 
 // ---- posterior mean / KG ----------------------------------------------------------------------------------------------
@@ -1296,8 +1368,9 @@ PYBIND11_MODULE(GPP, m) {
   m.def("posterior_mean_optima_mcmc", &posterior_mean_optima_mcmc, py::arg("gps"), py::arg("num_fidelity"),
         py::arg("optimizer_parameters"), py::arg("domain_bounds"), py::arg("points"), py::arg("num_points"),
         py::arg("shared_discrete_pts"), py::arg("num_shared"), py::arg("include_sampled") = true);
-  // names of the reference module that are outside the hot path (model selection, heuristic EI): present, so that an
-  // unmodified front end fails with the library's own exception class and a clear message rather than AttributeError
+  // names of the reference module whose arguments may match none of the signatures below (model selection): present, so
+  // that an unmodified front end fails with the library's own exception class and a clear message rather than a
+  // TypeError
   // compute_log_likelihood(points_sampled, points_sampled_value, dim, num_sampled, objective_type, hyperparameters,
   //                        derivatives, num_derivatives, noise_variance)   gpp_python_model_selection.cpp:43-87
   m.def("compute_log_likelihood",
@@ -1557,10 +1630,21 @@ PYBIND11_MODULE(GPP, m) {
           return r;
         },
         py::arg("gaussian_process"), py::arg("num_features"), py::arg("kernel_matched") = false);
-  m.def("heuristic_expected_improvement_optimization",
-        [](const py::args&, const py::kwargs&) -> py::object {
-          not_on_path("heuristic_expected_improvement_optimization");
-        });
+  // heuristic_expected_improvement_optimization(optimizer_parameters, gaussian_process, domain_bounds,
+  //     estimation_policy, num_to_sample, best_so_far, max_num_threads, randomness_source, status)
+  //                                                            gpp_python_expected_improvement.cpp:602-659 (DESIGN.md K20)
+  py::class_<ObjectiveEstimationPolicyInterface>(m, "ObjectiveEstimationPolicyInterface");
+  py::class_<ConstantLiarEstimationPolicy, ObjectiveEstimationPolicyInterface>(m, "ConstantLiarEstimationPolicy")
+      .def(py::init<double, double>(), py::arg("lie_value"), py::arg("lie_noise_variance"));
+  py::class_<KrigingBelieverEstimationPolicy, ObjectiveEstimationPolicyInterface>(m, "KrigingBelieverEstimationPolicy")
+      .def(py::init<double, double>(), py::arg("std_deviation_coef"), py::arg("kriging_noise_variance"));
+  m.def("heuristic_expected_improvement_optimization", &heuristic_expected_improvement_optimization);
+  // a call that matches no signature raises the library's own exception
+  m.def("heuristic_expected_improvement_optimization", [](const py::args&, const py::kwargs&) -> py::object {
+    raise_exc(g_exc_base,
+              "heuristic_expected_improvement_optimization: the arguments match no signature of the reference's "
+              "function");
+  });
   m.def("run_cpp_tests", []() -> int { not_on_path("run_cpp_tests"); });
   m.def("device_count", []() { return cmoe_device_count(); });
   m.def("version", []() { return std::string(cmoe_version()); });

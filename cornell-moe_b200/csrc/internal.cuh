@@ -188,6 +188,10 @@ void fit_gp(cmoe_gp* gp, bool mean_change);
 // 1/l = 0 and index 0.  In place: the list calls fill one per set.
 void fill_kernel_spec(KernelSpec& s, int kernel, int dim, int g, const int* derivs, double alpha,
                       const double* lengths);
+// O(N^2) append of m points and their values [m][1+g]; the new rows' diagonal carries new_noise [1+g] (host), or the
+// GP's own noise when it is NULL.  A singular update throws CMOE_ERR_SINGULAR and leaves the handle intact.
+void append_points(cmoe_gp* gp, const double* new_points, const double* new_values, int m,
+                   const double* new_noise = nullptr);
 // bit-identical copy of a fitted GP on another device (peer copies of the factor; no refit)
 cmoe_gp* clone_gp_to_device(const cmoe_gp* gp, int device);
 // Ps <- the m points P (device) in the length-scaled, centred coordinates of gp's covariance build (the Xs argument of
@@ -305,6 +309,14 @@ void posterior_mean_points(const cmoe_gp& gp, const double* P, size_t npts, cons
                            double* gmu, cudaStream_t s);
 
 // ---- multistart.cu -------------------------------------------------------------------------------------------
+constexpr int kTopK = 20;  // hard-coded in the reference (gpp_knowledge_gradient_optimization.hpp:901, gpp_math.hpp:1765)
+// indices of the (up to) kTopK largest values, in the order the reference feeds them to the optimiser
+std::vector<int> top_k_indices(const double* values, int n);
+// closed-form one-point EI (gpp_math.cpp:2196-2253) at nc points [nc][dim] and, if grads is not NULL, its gradient
+// [nc][dim], from cmoe_gp_posterior's mean and variance
+void analytic_ei(const cmoe_gp* gp, const double* pts, int nc, double best_so_far, double* values, double* grads);
+// throws CMOE_ERR_BOUNDS for a tensor-product box [dim][2] with min > max in some dimension
+void validate_bounds(const double* b, int dim);
 // An ensemble (one GP per hyper-parameter sample) is non-empty and its members share dim, g and device.
 void check_ensemble(const cmoe_gp* const* gps, int num_gp);
 // Member m's values v[nc] and gradients g[nc][ps] (g, grads NULL: none) into the ensemble's sums, called in member

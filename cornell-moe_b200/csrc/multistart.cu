@@ -26,8 +26,6 @@ using namespace cmoe;  // NOLINT
 
 namespace {
 
-constexpr int kTopK = 20;  // hard-coded in the reference (gpp_knowledge_gradient_optimization.hpp:901, gpp_math.hpp:1765)
-
 // SimplexIntersectTensorProductDomain::LimitUpdate (gpp_domain.cpp:234-289) for one point: box limited to [0,1]^dim
 // (constructor, :107-139), tensor-product limit first, then half the distance to the diagonal face if the limited step
 // would leave the simplex.
@@ -139,8 +137,9 @@ void gradient_descent_batch(const BatchEval& eval, const cmoe_gd_params& gd, con
   std::copy(x.begin(), x.end(), points_out);
 }
 
-// indices of the (up to) 20 largest values, in the order the reference feeds them to the optimiser
-std::vector<int> top_k_indices(const double* values, int n) {
+}  // namespace
+
+std::vector<int> cmoe::top_k_indices(const double* values, int n) {
   std::priority_queue<std::pair<double, int>> pq;
   const int k = std::min(kTopK, n);
   for (int i = 0; i < n; ++i) {
@@ -158,6 +157,8 @@ std::vector<int> top_k_indices(const double* values, int n) {
   }
   return out;
 }
+
+namespace {
 
 void multistart_common(const BatchEval& eval, const cmoe_gd_params& outer, const double* domain_bounds, int q, int dim,
                        const double* starts, int num_starts, double init_best, double* start_values,
@@ -293,8 +294,9 @@ void make_kg_evaluator(KgEvaluator& ev, const cmoe_gp* const* gps, int num_gp, i
   }
 }
 
-// analytic one-point EI and gradient (gpp_math.cpp:2196-2253) from device posterior quantities
-void analytic_ei(const cmoe_gp* gp, const double* pts, int nc, double best_so_far, double* values, double* grads) {
+}  // namespace
+
+void cmoe::analytic_ei(const cmoe_gp* gp, const double* pts, int nc, double best_so_far, double* values, double* grads) {
   const int dim = gp->spec.dim;
   std::vector<double> mu(nc), var(nc), gmu, gvar;
   int info = 0;
@@ -335,6 +337,8 @@ void analytic_ei(const cmoe_gp* gp, const double* pts, int nc, double best_so_fa
     }
   }
 }
+
+namespace {
 
 // ---- the parallel axis inside the call: starts strided over several GPUs ---------------------------------------------
 // (reference: OpenMP threads over starts, gpp_optimization.hpp:1472-1546).  One worker per device, each with its own
@@ -608,12 +612,12 @@ BatchEval kg_ensemble_eval(KgEvaluator& ev, int q, int dim, int nf, int num_gp) 
   };
 }
 
-void validate_bounds(const double* b, int dim) {
+}  // namespace
+
+void cmoe::validate_bounds(const double* b, int dim) {
   for (int d = 0; d < dim; ++d)
     CMOE_REQUIRE(b[2 * d] <= b[2 * d + 1], CMOE_ERR_BOUNDS, "Tensor product region is EMPTY.");
 }
-
-}  // namespace
 
 extern "C" {
 

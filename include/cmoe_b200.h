@@ -407,6 +407,32 @@ int cmoe_rff_evaluate(int dim, int num_features, int num_functions, const double
 int cmoe_lcb_select(const cmoe_gp* gp, const double* candidates, int num_candidates, int num_to_sample, int* selected,
                     double* mean, double* sd, int* num_satisfied, int* info);
 
+/* ---- heuristic batch EI (DESIGN.md K20) ------------------------------------------------------------------------
+ * Replaces the reference's ComputeHeuristicPointsToSample loop (gpp_python_expected_improvement.cpp:602-659, the
+ * policies :445-486): q rounds of one-point EI optimisation, each point fed back to a private copy of the GP with an
+ * estimated value.  Round r is cmoe_multistart_ei with q = 1, p = 0 and the start block starts[r] on the GP extended
+ * by rounds 0..r-1 (gd == NULL: the random search of the kNull branch, best -1 and strict `<` over the screen); its
+ * restarted descent runs on the device in one launch per round.  After round r the chosen point is appended with the
+ * policy's value and noise_variance on its diagonal:
+ *   Constant Liar      value = policy->value (the lie)
+ *   Kriging Believer   value = mu(x) + policy->value * sqrt(max(sigma^2(x), 0)), mu and sigma^2 (no noise) of round r
+ * best_so_far is held fixed over the rounds.  The caller's GP is never modified.  Outputs: points [q][dim],
+ * fantasy_values [q], ei_values [q] (the chosen point's 1-EI in its round, -1 if no start was found) and found [q]
+ * (each may be NULL except points).  CMOE_ERR_BOUNDS: q < 1, num_starts < 1, a GP with derivative observations,
+ * max_num_steps > 2^20, an empty box, or more than the descent's shared-memory rows (num_sampled + q - 1, about 13500
+ * on an H100).  CMOE_ERR_INVALID_VALUE: a NULL argument, an unknown policy, a non-finite value or noise_variance < 0.
+ * A fantasy that makes the factor singular: CMOE_ERR_SINGULAR, *info = its leading minor. */
+#define CMOE_ESTIMATION_CONSTANT_LIAR 0
+#define CMOE_ESTIMATION_KRIGING_BELIEVER 1
+typedef struct cmoe_estimation_policy {
+  int policy;            /* CMOE_ESTIMATION_* */
+  double value;          /* Constant Liar: the lie; Kriging Believer: std_deviation_coef (finite) */
+  double noise_variance; /* >= 0: noise of each fantasy row */
+} cmoe_estimation_policy;
+int cmoe_heuristic_ei(const cmoe_gp* gp, const cmoe_estimation_policy* policy, const cmoe_gd_params* gd,
+                      const double* domain_bounds, const double* starts, int num_starts, int q, double best_so_far,
+                      double* points, double* fantasy_values, double* ei_values, int* found, int* info);
+
 /* ---- q-EI Monte Carlo, batched over candidates ----------------------------------------------------------------
  * Replaces ExpectedImprovementEvaluator::ComputeExpectedImprovement / ComputeGradExpectedImprovement
  * (gpp_math.cpp:1991-2126); Python boundary compute_expected_improvement / compute_grad_expected_improvement /
